@@ -20,7 +20,8 @@
 //             N = 128 rows of the ring stage; 32 bytes of K per instruction), register accumulators, then the
 //             epilogue: the accumulators are transposed through shared memory so that a thread owns one query, raw
 //             dot products are tested against a register threshold, survivors go to a per-query list in global memory
-//             that a warp-wide radix select cuts back to the best `keep`
+//             that a warp-wide radix select cuts back to the best `keep`.  The fixed-bound pass tests its bound on the
+//             accumulator fragment itself (no transpose) and appends survivors at slots from shared per-query counters.
 // coarse_kernel<CfgTF32>: the SS shape with the rows as the M operand (32 queries per CTA in shared memory), kept for
 // fp32 corpora without shadow memory (mode 2) and rows too wide for the 16-bit kernel's shared memory.
 #include "coarse_tc.h"
@@ -144,9 +145,12 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, uint32_t 
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(rank));
     return r;
 }
-// arrive on an mbarrier of another CTA of the cluster (release at cluster scope: what this thread has observed is published)
+// arrive on an mbarrier of another CTA of the cluster.  Default semantics (release at CTA scope), which compile to the
+// arrive alone: a release at cluster scope adds a GPU-wide memory barrier before every arrive.  The ring stages this
+// releases are read only by wgmma (the async proxy), and those reads are complete once wgmma.wait_group has returned,
+// so there is no generic-proxy access for a cluster-scope release to order before the producer's refill.
 __device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
@@ -679,12 +683,15 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
     }
     constexpr uint32_t kQTrigger = kQListCap - 32;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    // 1024-byte alignment for the 128B swizzle atoms, by an offset of smem_raw itself: the pointers stay visibly shared,
+    // so their accesses compile to STS / LDS rather than generic stores and loads
+    uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t *sB = smem;                                                   // nstages x kQKbPerStage x [128 rows x 128B]
     uint8_t *sQ = sB + (size_t)nstages * kQStageBytes;                    // num_kb x [64 queries x 128B], swizzled
-    uint32_t *sacc = reinterpret_cast<uint32_t *>(sQ + (size_t)num_kb * kQABlockBytes); // [kQM][kQAccStride]
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sacc + kQM * kQAccStride);
+    uint32_t *sacc = reinterpret_cast<uint32_t *>(sQ + (size_t)num_kb * kQABlockBytes); // [kQM][kQAccStride]; not kFixed
+    uint64_t *bars = reinterpret_cast<uint64_t *>(sacc + (kFixed ? 0 : kQM * kQAccStride));
     uint64_t *full = bars, *empty = bars + kQMaxStages;
+    uint32_t *qcount = reinterpret_cast<uint32_t *>(bars + 2 * kQMaxStages); // kFixed: [kQM] appends per query
     // this CTA's candidate lists [kQListCap][kQListStride]
     uint64_t *lists = list_scratch + (size_t)(by * gx + bx) * (kQListCap * kQListStride);
 
@@ -764,6 +771,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                     *reinterpret_cast<uint4 *>(row + ((u ^ (et & 7)) * 16)) = x;
                 }
             }
+            if constexpr (kFixed) qcount[et] = 0;
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy writes of sQ -> tensor-core reads
         asm volatile("bar.sync 1, 128;" ::: "memory");
@@ -783,32 +791,42 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         float nq_norm = 1.0f;
         if constexpr (kOp == 2) nq_norm = live ? *reinterpret_cast<const float *>(q16 + (size_t)q * q16_pitch + dim) : 1.0f;
         if constexpr (kOp == 3) nq_norm = live ? q_norm2[q] : 0.0f; // |q|^2
-        bool ovf = false;
         float smax[kSample ? kSliceSets : 1][kQN / 32]; // kSample: running maxima of the pre-test value per slice (largest = smallest distance)
 #pragma unroll
         for (int x = 0; x < (kSample ? kSliceSets : 1); x++)
 #pragma unroll
             for (int h = 0; h < kQN / 32; h++) smax[x][h] = -__int_as_float(0x7f800000);
-        if constexpr (kFixed) {
-            // fixed admission bound (a distance): keep every row with approximate distance < T
-            const float T = live ? thr_fixed[q] : -__int_as_float(0x7f800000);
-            thr = orderable_key(T);
-            if constexpr (kOp == 0) { // d < T  <=>  dot > 1 - T; slack: the rounding of the two subtractions
-                const float t = 1.0f - T;
-                thr_dot = t - (4e-7f + 2.4e-7f * fabsf(t));
-            } else {
-                thr_dot = 0.5f * (nq_norm - T) - 2e-6f * (fabsf(nq_norm) + fabsf(T));
-            }
-            if (!(T == T)) thr_dot = -__int_as_float(0x7f800000), thr = 0xFFFFFFFFu; // NaN bound: keep everything (-> overflow -> next tier)
-        }
         if (!live) thr_dot = __int_as_float(0x7f800000); // slots without a query: nothing ever passes
+        // kFixed: the bound is tested on the accumulator fragment itself, where this thread holds queries
+        // fq[i2] = 16 ew + lane / 4 + 8 i2 (i2 = 0, 1) against 32 rows of each tile
+        uint32_t fthr[2];
+        float fthr_dot[2], fnq[2];
+        if constexpr (kFixed) {
+#pragma unroll
+            for (int i2 = 0; i2 < 2; i2++) {
+                const uint32_t fq = q_base + 16 * ew + (lane >> 2) + 8 * i2;
+                const bool flive = fq < nq;
+                fnq[i2] = (kOp == 3 && flive) ? q_norm2[fq] : 0.0f; // |q|^2
+                // fixed admission bound (a distance): keep every row with approximate distance < T
+                const float T = flive ? thr_fixed[fq] : -__int_as_float(0x7f800000);
+                fthr[i2] = orderable_key(T);
+                if constexpr (kOp == 0) { // d < T  <=>  dot > 1 - T; slack: the rounding of the two subtractions
+                    const float t = 1.0f - T;
+                    fthr_dot[i2] = t - (4e-7f + 2.4e-7f * fabsf(t));
+                } else {
+                    fthr_dot[i2] = 0.5f * (fnq[i2] - T) - 2e-6f * (fabsf(fnq[i2]) + fabsf(T));
+                }
+                if (!(T == T)) fthr_dot[i2] = -__int_as_float(0x7f800000), fthr[i2] = 0xFFFFFFFFu; // NaN bound: keep everything (-> overflow -> next tier)
+                if (!flive) fthr_dot[i2] = __int_as_float(0x7f800000);
+            }
+        }
         uint32_t s = 0, ph = 0;
         const uint64_t bdesc_first = make_smem_desc(smem_u32(sB)), adesc_first = make_smem_desc(smem_u32(sQ));
         constexpr uint64_t kStageStep = kQStageBytes >> 4, kBlockStep = kQBlockBytes >> 4, kABlockStep = kQABlockBytes >> 4;
         for (uint32_t i = 0; i < my_tiles; i++) {
             const uint32_t tile = (bx + i * gx) * tile_stride;
             float nrm[kQN / 32]; // kOp 2 / 3: lane l holds the norm / squared norm of rows h*32 + l of the tile
-            if constexpr (kOp == 3) {
+            if constexpr (kOp == 3 && !kFixed) {
 #pragma unroll
                 for (int h = 0; h < kQN / 32; h++) {
                     const uint32_t r = tile * kQN + h * 32 + lane;
@@ -820,6 +838,20 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                 for (int h = 0; h < kQN / 32; h++) {
                     const uint32_t r = tile * kQN + h * 32 + lane;
                     nrm[h] = r < n_rows ? __ldg(reinterpret_cast<const float *>(shadow + (size_t)r * row_pitch + dim)) : 1.0f;
+                }
+            }
+            // kFixed: acc[4 j + 2 i2 + c] holds row rbase + 8 j + c of the tile; squared L2 loads the squared norms of
+            // each row pair (j) at once
+            const uint32_t rbase = tile * kQN + 2 * (lane & 3);
+            float2 rn[(kFixed && kOp == 3) ? kQN / 8 : 1];
+            if constexpr (kFixed && kOp == 3) {
+#pragma unroll
+                for (int j = 0; j < kQN / 8; j++) {
+                    const uint32_t r = rbase + 8 * j;
+                    if (r + 1 < n_rows)
+                        rn[j] = __ldg(reinterpret_cast<const float2 *>(row_norm2 + r));
+                    else
+                        rn[j] = make_float2(r < n_rows ? __ldg(row_norm2 + r) : 0.0f, 0.0f);
                 }
             }
             // ===== D[64 queries x 128 rows] (+)= Q[smem] * rows[smem]^T =====
@@ -844,6 +876,64 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
             release(prev);
             wg_fence_operands(acc);
             // accumulator fragment: acc[4j + 2 i2 + c] = (query 16 ew + lane / 4 + 8 i2, row 8 j + 2 (lane % 4) + c)
+            if constexpr (kFixed) {
+                // With a fixed bound only ~k * (rows / sample rows) rows of the whole corpus pass: for each of its two
+                // queries the thread takes the max of its 32 values and ONE compare decides the common case.  The rare
+                // survivors take the exact distance and key comparison and append to the query's list, unordered, at a
+                // slot from the query's shared counter; a count past the capacity is an overflow.
+#pragma unroll
+                for (int i2 = 0; i2 < 2; i2++) {
+                    uint32_t pass = 0; // bit 2 j + c: acc[4 j + 2 i2 + c]
+                    if constexpr (kOp == 0) {
+                        float m8[8];
+#pragma unroll
+                        for (int g = 0; g < 8; g++)
+                            m8[g] = fmaxf(fmaxf(acc[8 * g + 2 * i2], acc[8 * g + 2 * i2 + 1]), fmaxf(acc[8 * g + 4 + 2 * i2], acc[8 * g + 5 + 2 * i2]));
+                        const float mx = fmaxf(fmaxf(fmaxf(m8[0], m8[1]), fmaxf(m8[2], m8[3])), fmaxf(fmaxf(m8[4], m8[5]), fmaxf(m8[6], m8[7])));
+                        if (mx > fthr_dot[i2]) {
+#pragma unroll
+                            for (int j = 0; j < kQN / 8; j++)
+#pragma unroll
+                                for (int c = 0; c < 2; c++)
+                                    if (acc[4 * j + 2 * i2 + c] > fthr_dot[i2]) pass |= 1u << (2 * j + c);
+                        }
+                    } else { // d < d_thr  <=>  dot > |row|^2 / 2 + (|q|^2 - d_thr) / 2, loosened for the rounding of both sides
+#pragma unroll
+                        for (int j = 0; j < kQN / 8; j++)
+#pragma unroll
+                            for (int c = 0; c < 2; c++)
+                                if (acc[4 * j + 2 * i2 + c] > fmaf(c ? rn[j].y : rn[j].x, 0.499999f, fthr_dot[i2])) pass |= 1u << (2 * j + c);
+                    }
+                    if (pass && tile * kQN + kQN > n_rows) { // rows past the end (TMA zero fill / stale shadow bytes)
+#pragma unroll
+                        for (int j = 0; j < kQN / 8; j++)
+#pragma unroll
+                            for (int c = 0; c < 2; c++)
+                                if (rbase + 8 * j + c >= n_rows) pass &= ~(1u << (2 * j + c));
+                    }
+                    while (pass) {
+                        const int b = __ffs(pass) - 1;
+                        pass &= pass - 1;
+                        float raw = 0.0f;
+#pragma unroll
+                        for (int x = 0; x < 32; x++)
+                            if (x == b) raw = acc[4 * (x >> 1) + 2 * i2 + (x & 1)];
+                        const uint32_t row = rbase + 8 * (b >> 1) + (b & 1);
+                        float d;
+                        if constexpr (kOp == 0)
+                            d = 1.0f - raw;
+                        else
+                            d = __fsub_rn(__fadd_rn(fnq[i2], __ldg(row_norm2 + row)), __fmul_rn(2.0f, raw));
+                        const uint32_t key = orderable_key(d);
+                        if (key < fthr[i2]) {
+                            const int qs = 16 * ew + (lane >> 2) + 8 * i2;
+                            const uint32_t slot = atomicAdd(&qcount[qs], 1u);
+                            if (slot < (uint32_t)kQListCap) lists[slot * kQListStride + qs] = ((uint64_t)key << 32) | row;
+                        }
+                    }
+                }
+                continue;
+            }
             asm volatile("bar.sync 1, 128;" ::: "memory"); // the previous tile's reads of sacc are done
 #pragma unroll
             for (int j = 0; j < kQN / 8; j++) {
@@ -874,7 +964,6 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
 #pragma unroll
             for (int h = 0; h < kQN / 32; h++) {
                 const uint32_t row0 = tile * kQN + h * 32;
-                uint32_t pass_pre = 0;
                 if constexpr (kSample) {
                     // largest dot (cosine / inner product) or largest dot - |row|^2 / 2 (squared L2) of the chunk
                     float mx = -__int_as_float(0x7f800000);
@@ -905,31 +994,11 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         if ((int)(i % (uint32_t)kSliceSets) == x) smax[kSample ? x : 0][h] = fmaxf(smax[kSample ? x : 0][h], mx);
                     continue;
                 }
-                if constexpr (kFixed) {
-                    // With a fixed bound only ~k * (rows / sample rows) rows of the whole corpus pass: one 3-input max tree
-                    // over the 32 values (16 instructions) and ONE compare decide the common case
-                    if constexpr (kOp == 0) {
-                        float mx;
-                        float m8[8];
-#pragma unroll
-                        for (int g = 0; g < 8; g++)
-                            m8[g] = fmaxf(fmaxf(__uint_as_float(v[h][4 * g]), __uint_as_float(v[h][4 * g + 1])),
-                                          fmaxf(__uint_as_float(v[h][4 * g + 2]), __uint_as_float(v[h][4 * g + 3])));
-                        mx = fmaxf(fmaxf(fmaxf(m8[0], m8[1]), fmaxf(m8[2], m8[3])), fmaxf(fmaxf(m8[4], m8[5]), fmaxf(m8[6], m8[7])));
-                        if (!(mx > thr_dot)) continue;
-                    } else { // squared L2: the bound depends on the row; the shuffles need the whole warp, so the pass mask
-                             // itself is built here, before the lanes diverge
-#pragma unroll
-                        for (int j = 0; j < 32; j++)
-                            if (__uint_as_float(v[h][j]) > fmaf(__shfl_sync(0xFFFFFFFFu, nrm[h], j), 0.499999f, thr_dot)) pass_pre |= 1u << j;
-                        if (pass_pre == 0) continue;
-                    }
-                }
                 // pre-test on the raw dot product against a slightly loose bound (a few instructions per value);
                 // the few survivors take the exact distance and key comparison below
-                uint32_t pass = pass_pre;
+                uint32_t pass = 0;
 #pragma unroll
-                for (int j = 0; j < ((kFixed && kOp == 3) ? 0 : 32); j++) {
+                for (int j = 0; j < 32; j++) {
                     bool p;
                     if constexpr (kOp == 0)
                         p = __uint_as_float(v[h][j]) > thr_dot;
@@ -963,20 +1032,10 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                     }
                     const uint32_t key = orderable_key(d);
                     if (key < thr) {
-                        if constexpr (kFixed) {
-                            if (cnt < (uint32_t)kQListCap) {
-                                lists[cnt * kQListStride + et] = ((uint64_t)key << 32) | (row0 + j);
-                                cnt++;
-                            } else {
-                                ovf = true; // more rows below the bound than the list holds: the query goes to the next tier
-                            }
-                        } else {
-                            lists[cnt * kQListStride + et] = ((uint64_t)key << 32) | (row0 + j);
-                            cnt++;
-                        }
+                        lists[cnt * kQListStride + et] = ((uint64_t)key << 32) | (row0 + j);
+                        cnt++;
                     }
                 }
-                if constexpr (kFixed) continue;
                 // lists that ran past the trigger are cut back to the best `keep` by the whole warp
                 uint32_t m = __ballot_sync(0xFFFFFFFFu, cnt > kQTrigger);
                 while (m) {
@@ -1008,7 +1067,18 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         // publish: cand_out[q][blockIdx.x][keep], kEmptySlot padded
         __syncwarp();
         if constexpr (kFixed) {
-            if (ovf && live) overflow[q] = 1u;
+            // every append of the CTA is done; warp ew publishes queries 16 ew .. 16 ew + 15.  keep == kQListCap here
+            // (plan_coarse), so a list that did not overflow is published whole.  More rows below the bound than the
+            // list holds: overflow, the query goes to the next tier.
+            asm volatile("bar.sync 1, 128;" ::: "memory");
+            for (int qs = 16 * ew; qs < 16 * ew + 16; qs++) {
+                const uint32_t qq = q_base + qs;
+                if (qq >= nq) break;
+                const uint32_t n = qcount[qs], c = min(n, (uint32_t)kQListCap);
+                uint64_t *dst = cand_out + ((size_t)qq * gx + bx) * keep;
+                for (uint32_t r = lane; r < keep; r += 32) dst[r] = r < c ? lists[r * kQListStride + qs] : kEmptySlot;
+                if (lane == 0 && n > (uint32_t)kQListCap) overflow[qq] = 1u;
+            }
         }
         if constexpr (kSample) { // keep == 8: the slice minima as composites (the row id is not needed by threshold_kernel)
             if (live) {
@@ -1027,7 +1097,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                     }
             }
         }
-        for (int src = 0; src < (kSample ? 0 : 32); src++) {
+        for (int src = 0; src < ((kSample || kFixed) ? 0 : 32); src++) {
             uint32_t c = __shfl_sync(0xFFFFFFFFu, cnt, src);
             const uint32_t qq = q_base + ew * 32 + src;
             if (c > keep) {
@@ -1370,9 +1440,10 @@ static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, bool int_cos, 
     if (int_cos) return epl == 3 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 0> : (const void *)coarse_wgmma_kernel<false, 8, 3, 0>;
     return epl == 3 ? (const void *)coarse_wgmma_kernel<false, 3, 0, 0> : (const void *)coarse_wgmma_kernel<false, 8, 0, 0>;
 }
-// shared memory of coarse_wgmma_kernel besides the ring: the resident queries, the accumulator transpose, the barriers
-static size_t wgmma_fixed_smem(uint32_t num_kb) {
-    return 1024 + (size_t)num_kb * kQABlockBytes + kQAccBytes + 2 * kQMaxStages * 8 + 64;
+// shared memory of coarse_wgmma_kernel besides the ring: the resident queries, the accumulator transpose (the
+// fixed-bound pass, mode 1, tests the accumulators in registers and keeps a counter per query instead), the barriers
+static size_t wgmma_fixed_smem(uint32_t num_kb, int mode = 0) {
+    return 1024 + (size_t)num_kb * kQABlockBytes + (mode == 1 ? kQM * 4 : kQAccBytes) + 2 * kQMaxStages * 8 + 64;
 }
 // the 16/8-bit kernel needs at least two ring stages next to the resident queries (1024 fp16 dimensions fit)
 static bool wgmma_fits_bytes(uint32_t row_bytes) { return wgmma_fixed_smem(coarse_kb(row_bytes)) + 2 * (size_t)kQStageBytes <= kSmemLimit; }
@@ -1429,8 +1500,8 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
         if (p.mode == 1 && kind == CoarseF16) p.keep = kCoarseFixedCap, p.epl = 3; // every row below the bound, up to the list capacity
         if (p.mode == 1 && kind == CoarseDirect16) p.keep = kCoarseFixedCapDirect, p.epl = 8;
         if (p.mode == 2) p.keep = kCoarseSampleSlices, p.epl = 3; // the slice minima
-        p.stages = (uint32_t)std::min<size_t>(kQMaxStages, (kSmemLimit - wgmma_fixed_smem(p.num_kb)) / kQStageBytes);
-        p.smem_bytes = wgmma_fixed_smem(p.num_kb) + (size_t)p.stages * kQStageBytes;
+        p.stages = (uint32_t)std::min<size_t>(kQMaxStages, (kSmemLimit - wgmma_fixed_smem(p.num_kb, p.mode)) / kQStageBytes);
+        p.smem_bytes = wgmma_fixed_smem(p.num_kb, p.mode) + (size_t)p.stages * kQStageBytes;
         // the query groups of a row range form a thread-block cluster (multicast of the row tiles)
         p.csize = 1;
         static int ccap = -1; // VECSIM_B200_CLUSTER caps the cluster size (1 = no clusters)
