@@ -1313,6 +1313,11 @@ __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t
     for (uint32_t i = threadIdx.x; i < k; i += blockDim.x) out[(size_t)q * k + i] = i < n_surv ? surv[i] : kEmptySlot;
     // proof
     bool bad = n_all > kRefineMaxSurv; // more candidates within 2 eps of the k-th than the buffer holds: the next tier answers
+    // a query whose fp16 form is not finite (row_stats_kernel: |q|^2 = NaN) has no error bound.  And a bound that is not a
+    // finite number proves nothing: cut is +-inf or NaN when the k-th approximate key is, or when there are fewer than k
+    // candidates; thr_T is +inf when the sample pass found fewer than k finite distances.
+    if (q_norm2 && !(q_norm2[blockIdx.x] == q_norm2[blockIdx.x])) bad = true;
+    if (!isfinite(cut) || (thr_T && !isfinite(thr_T[blockIdx.x]))) bad = true;
     const bool have_k = n_surv >= k;
     const float ek = have_k ? key_to_float((uint32_t)(surv[k - 1] >> 32)) : 0.0f;
     if (thr_T) {
@@ -1655,7 +1660,10 @@ cudaError_t launch_to_f16_tiled(const void *src, size_t spitch, uint32_t dim, ui
 }
 
 // squared norm of fp32 rows [first, first+n) -> norm2[first + r]; running maxima (as float bits: the values are >= 0,
-// a NaN compares as huge and disables the route) of the squared norm and of |x| into stats[0], stats[1]
+// a NaN compares as huge and disables the route) of the squared norm and of |x| into stats[0], stats[1].
+// A row (in practice a query: rows outside the fp16 range keep their index off the route) whose fp16 form is not finite
+// — a component with |x| >= 65520 rounds to inf, or is NaN — gets norm2 = NaN: its approximate distances are inf or NaN,
+// query_eps does not bound them, and refine_kernel never proves such a query.
 __global__ void __launch_bounds__(256) row_stats_kernel(const uint8_t *__restrict__ rows, size_t pitch, uint32_t dim, uint32_t first,
                                                         uint32_t n, float *__restrict__ norm2, uint32_t *__restrict__ stats) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -1674,7 +1682,7 @@ __global__ void __launch_bounds__(256) row_stats_kernel(const uint8_t *__restric
             m = fmaxf(m, __shfl_xor_sync(0xFFFFFFFFu, m, o));
         }
         if (lane == 0) {
-            norm2[first + r] = s;
+            norm2[first + r] = m < 65520.0f ? s : __int_as_float(0x7fc00000);
             if (stats) {
                 atomicMax(&stats[0], __float_as_uint(s));
                 atomicMax(&stats[1], __float_as_uint(m));

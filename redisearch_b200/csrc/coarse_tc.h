@@ -87,7 +87,8 @@ cudaError_t launch_compact_unproven(const uint32_t *d_ok, uint32_t nq, uint32_t 
 // row i of dst = row d_idx[i] of src (pitch % 16 == 0), squared norms likewise (nullable), for i < *d_count
 cudaError_t launch_gather_queries(const void *d_src, size_t pitch, const float *d_src_n2, const uint32_t *d_idx, const uint32_t *d_count,
                                   uint32_t max_n, void *d_dst, float *d_dst_n2, cudaStream_t s);
-// |row|^2 of fp32 rows [first, first+n) into d_norm2[first..]; d_stats (nullable) = {max |row|^2, max |x|} as float bits
+// |row|^2 of fp32 rows [first, first+n) into d_norm2[first..], NaN for a row whose fp16 form is not finite (a component
+// with |x| >= 65520, or NaN: refine_kernel never proves such a query); d_stats (nullable) = {max |row|^2, max |x|} as float bits
 cudaError_t launch_row_stats(const void *rows, size_t pitch, uint32_t dim, uint32_t first, uint32_t n, float *d_norm2, uint32_t *d_stats,
                              cudaStream_t s);
 

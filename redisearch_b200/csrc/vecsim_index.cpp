@@ -593,7 +593,7 @@ VecSimQueryReply *FlatIndex::topk(const void *q, size_t k, VecSimQueryParams *qp
     if (ok && !multi_ && std::min(k, n) <= (size_t)kMaxFusedK) {
         const uint32_t ke = (uint32_t)std::min(k, n);
         const uint64_t *d_res = nullptr;
-        if (single_query_takes_coarse(ke)) {
+        if (single_query_takes_coarse(ke, reinterpret_cast<const float *>(c->h_query))) {
             // an up-to-date fp16 shadow exists (a batch built it): one pass over 15 GB of it + exact rescoring + proof
             // beats the 31 GB exact scan; same answer (DESIGN.md §4)
             uint64_t *r = nullptr;
@@ -731,10 +731,14 @@ static int coarse_mode() {
 }
 
 // Single queries (and batches below 16) take the tensor-core route only if that costs nothing extra: mode 1, an fp16
-// shadow that is already complete, fp32 cosine, k within the coarse lists.
-bool FlatIndex::single_query_takes_coarse(uint32_t ke) {
+// shadow that is already complete, fp32 cosine, k within the coarse lists.  host_query (nullable): the stored-form query; a
+// raw inner-product / L2 query whose fp16 form is not finite (|x| >= 65520 or NaN) cannot be proven and takes the exact scan.
+bool FlatIndex::single_query_takes_coarse(uint32_t ke, const float *host_query) {
     if (coarse_mode() != 1 || multi_ || coarse_disabled_ || dtype_ != DT_F32) return false;
     if (!unit_rows() && !(shadow_max_abs_ <= 60000.0f)) return false; // fp16 range (also false before the first build)
+    if (!unit_rows() && host_query)
+        for (size_t i = 0; i < dim_; i++)
+            if (!(std::fabs(host_query[i]) < 65520.0f)) return false;
     {
         std::lock_guard<std::mutex> g(mu_);
         if (!d_shadow_ || shadow_rows_ != count_ || !shadow_dirty_.empty() || shadow_cap_ < count_) return false;

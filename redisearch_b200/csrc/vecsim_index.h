@@ -217,7 +217,7 @@ class FlatIndex {
     bool unit_rows() const { return metric_ == VecSimMetric_Cosine && !raw_rows_; }
     std::vector<idType> shadow_dirty_;
     bool ensure_shadow(cudaStream_t st);
-    bool single_query_takes_coarse(uint32_t ke);
+    bool single_query_takes_coarse(uint32_t ke, const float *host_query = nullptr);
     size_t capacity_ = 0; // rows of HBM allocated
     size_t count_ = 0;    // rows in the index (incl. staged)
     size_t resident_ = 0; // rows already copied to HBM

@@ -31,7 +31,8 @@ def _device_batch(vs, torch, index, qs_norm, k):
 @pytest.mark.parametrize("mode", [1, 2])
 @pytest.mark.parametrize("n,dim,nq,k", [(70_000, 128, 40, 10), (66_000, 768, 64, 10), (131_072, 96, 17, 16), (80_000, 104, 33, 5),
                                         (70_000, 128, 128, 10), (300_000, 64, 256, 10), (66_000, 256, 512, 8),
-                                        (66_000, 1024, 70, 10)])
+                                        (66_000, 1024, 70, 10), (70_000, 32, 40, 10), (70_000, 40, 40, 10), (66_000, 776, 64, 10),
+                                        (66_000, 1016, 64, 10)])
 def test_coarse_path_is_exact(n, dim, nq, k, mode):
     import torch
 
@@ -156,11 +157,33 @@ def test_deleted_then_reused_row_ids_do_not_keep_stale_shadow_rows():
     vs.lib().VecSimB200_SetCoarseMode(-1)
 
 
+def _snap_against(x, q, against):
+    """x with every component just short of an fp16 rounding midpoint, on the side where round-to-nearest moves the
+    dot product with q down (against) or up; x's components must lie in the fp16 normal range."""
+    ax = np.abs(x.astype(np.float64))
+    ulp = 2.0 ** (np.floor(np.log2(ax)) - 10)
+    lo = np.floor(ax / ulp) * ulp
+    shrink = (np.sign(x) == np.sign(q)) == against  # the magnitude must round down
+    mag = lo + 0.5 * ulp + np.where(shrink, -1.0, 1.0) * ulp / 1024
+    return np.sign(x) * mag
+
+
 def test_cosine_raw_overwrite_near_the_kth_boundary_keeps_the_proof_sound():
     """brute_force_single.h:139-144 overwrites an existing label with the caller's RAW blob, so a cosine index can hold
     non-unit rows.  Rows of norm ~16 are planted right at the k-th boundary of each query (on both sides of it): their
     fp16 error is ~16x the unit-vector bound, so a proof that assumed unit vectors could pass on a wrong answer.  ids and
     score bits must still equal the reference's."""
+    _raw_overwrite_near_the_kth_boundary("random")
+
+
+def test_cosine_raw_overwrite_with_adversarial_rounding_keeps_the_proof_sound():
+    """The same planted rows with every component just short of an fp16 rounding midpoint: the rows just inside the k-th
+    boundary round outwards and those just outside round inwards, by ~4e-3 each — beyond the unit-vector window
+    2 eps = 2.4e-3, so a bound that lost its norm scaling would pass the proof on a wrong answer."""
+    _raw_overwrite_near_the_kth_boundary("adversarial")
+
+
+def _raw_overwrite_near_the_kth_boundary(rounding):
     import torch
 
     from redisearch_b200 import vecsim as vs
@@ -190,7 +213,12 @@ def test_cosine_raw_overwrite_near_the_kth_boundary_keeps_the_proof_sound():
             u = rng.standard_normal(dim)
             u -= u.dot(q) * q
             u /= np.linalg.norm(u)
-            blob = (scale * (c * q + np.sqrt(max(0.0, 1.0 - c * c)) * u)).astype(np.float32)
+            blob = scale * (c * q + np.sqrt(max(0.0, 1.0 - c * c)) * u)
+            if rounding == "adversarial":
+                blob = _snap_against(blob, q, against=delta < 0)
+                p_ = int(np.argmax(np.abs(q)))  # one component (left off the grid) puts the exact distance back at `want`
+                blob[p_] += ((1.0 - want) - blob @ q) / q[p_]
+            blob = blob.astype(np.float32)
             victim += 1
             assert g.add(blob, victim) == 0  # label exists: in-place overwrite with the raw blob
             p.add(blob, victim)
