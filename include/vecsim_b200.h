@@ -14,8 +14,8 @@
  * distance/top-k computation is a hand-written sm_90a CUDA kernel.  There is no CPU fallback:
  * if no CUDA device is usable VecSimIndex_New returns NULL and logs through the log callback.
  *
- * VecSimB200_* entry points are extensions the reference does not have (batched queries, bulk
- * device ingest, shard merge); INTEGRATION.md shows where a RediSearch maintainer would call them.
+ * VecSimB200_* entry points are extensions the reference does not have (batched top-k and range
+ * queries, bulk device ingest, shard merge); INTEGRATION.md shows where a RediSearch maintainer would call them.
  */
 #ifndef VECSIM_B200_H
 #define VECSIM_B200_H
@@ -435,6 +435,20 @@ int VecSimB200_TopKQueryBatch(VecSimIndex *index, const void *queryBlobs, size_t
  * (a cudaStream_t cast to void*, NULL = the index's own stream) and returns. */
 int VecSimB200_TopKQueryBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, size_t k,
                                     int64_t *d_out_labels, float *d_out_scores, void *stream);
+/* nq range queries in one call.  replies[i] receives exactly what
+ * VecSimIndex_RangeQuery(index, queryBlobs + i*qstride, radii[i], queryParams, order) would return
+ * (same labels, same float scores, same order); the caller frees each with VecSimQueryReply_Free.
+ * Single-value fp32 indexes of >= 65536 rows (dim % 8 == 0, 32..1024; coarse mode 1) answer a batch of
+ * >= 16 queries with one tensor-core pass over the fp16 shadow, exact rescoring and a per-query
+ * completeness proof; every other query is answered by the exact scan, one query at a time.
+ * out_flags (nullable, [nq]): 1 = answered by the tensor-core route, 0 = by the exact scan.
+ * Returns VecSim_QueryReply_OK / _TimedOut (the timeout callback fired: the replies carry that code,
+ * those answered before it fired keep their results, as VecSimIndex_RangeQuery's do); -1 for an order other
+ * than BY_ID / BY_SCORE, a negative radius (no reply is allocated, the index logs a warning, as
+ * VecSimIndex_RangeQuery does) or a CUDA failure. */
+int VecSimB200_RangeQueryBatch(VecSimIndex *index, const void *queryBlobs, size_t qstride, size_t nq,
+                               const double *radii, VecSimQueryParams *queryParams,
+                               VecSimQueryReply_Order order, VecSimQueryReply **replies, uint32_t *out_flags);
 /* Bulk ingest of n host blobs (stride bytes apart) with labels[i] (NULL -> label0+i).  Equivalent
  * to n VecSimIndex_AddVector calls on fresh labels, with one H2D transfer per staging buffer. */
 int VecSimB200_AddVectors(VecSimIndex *index, const void *blobs, size_t stride, size_t n,

@@ -1347,6 +1347,92 @@ __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t
     if (threadIdx.x == 0) ok[q] = s_bad ? 0u : ok_value; // 1 = first tier, 2 = second tier (any non-zero = proven)
 }
 
+// ------------------------------------------------------------------------------------------------
+// Range batches (DESIGN.md §4, "Range queries").  The fixed-bound main pass runs unchanged with the bound
+// T[q] = radius[q] + eps_q: a row it drops has approx >= T, so exact >= T - eps_q > radius — it is not in the answer.
+// Without a list overflow the kept rows therefore hold every row within the radius, and rescoring them with the exact
+// arithmetic of the scan gives the reference's answer.
+// ------------------------------------------------------------------------------------------------
+constexpr uint32_t kRangeWindow = 2048; // list slots packed into shared memory at a time by range_refine_kernel
+
+// T[q] = radius[q] + eps_q, rounded up as threshold_kernel rounds; a radius of +inf or NaN gives a bound that is not
+// finite (the main pass keeps everything and the query is never proven).  Also clears the overflow flags and the
+// result counter of range_refine_kernel.  One thread per query.
+__global__ void range_bound_kernel(const float *__restrict__ radius, uint32_t nq, float eps, const float *__restrict__ q_norm2,
+                                   float max_norm, uint32_t dim, int l2, float *__restrict__ thr, uint32_t *__restrict__ overflow,
+                                   uint32_t *__restrict__ total) {
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q == 0) *total = 0;
+    if (q >= nq) return;
+    const float e = query_eps(eps, q_norm2, q, max_norm, dim, l2 != 0);
+    thr[q] = radius[q] + e * 1.001f + 1e-30f;
+    overflow[q] = 0;
+}
+
+// One CTA per query.  Packs the real candidates of the query's `slots` list entries into shared memory a window at a
+// time, rescores them from the fp32 rows (one warp per row, the scan's own arithmetic) and keeps a row iff
+// d <= radius (the reference's inclusive test, brute_force.h range query).  Kept composites are appended to the front
+// of the query's own list segment: the count kept so far never exceeds the slots already read, so this overwrites
+// only consumed entries.  The segment is then copied to out[off[q], off[q] + cnt[q]) in the dense result buffer, at an
+// offset reserved from *total.  ok[q] = 1 unless a list overflowed, the query's fp16 form is not finite (|q|^2 NaN,
+// row_stats_kernel) or its bound is not finite; an unproven query writes cnt[q] = 0 and skips the rescoring.
+template <int MT>
+__global__ void __launch_bounds__(256) range_refine_kernel(const uint8_t *rows, size_t pitch, uint32_t dim, const uint8_t *queries,
+                                                           size_t qpitch, uint32_t slots, uint64_t *cand, const float *__restrict__ radius,
+                                                           const float *__restrict__ q_norm2, const float *__restrict__ thr,
+                                                           const uint32_t *__restrict__ overflow, uint64_t *__restrict__ out,
+                                                           uint32_t *__restrict__ total, uint32_t *__restrict__ ok, uint32_t *__restrict__ cnt,
+                                                           uint32_t *__restrict__ off) {
+    using Tile = DistTile<DT_F32, MT, 1, 1>;
+    __shared__ uint64_t s_cand[kRangeWindow];
+    __shared__ uint32_t s_n, s_kept, s_base;
+    const uint32_t q = blockIdx.x;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    bool proven = overflow[q] == 0 && isfinite(thr[q]);
+    if (q_norm2 && !(q_norm2[q] == q_norm2[q])) proven = false;
+    if (!proven) { // the same for every thread of the CTA
+        if (threadIdx.x == 0) ok[q] = 0, cnt[q] = 0, off[q] = 0;
+        return;
+    }
+    const float r = radius[q];
+    uint64_t *mine = cand + (size_t)q * slots;
+    const uint8_t *qb[1] = {queries + (size_t)q * qpitch};
+    if (threadIdx.x == 0) s_kept = 0;
+    for (uint32_t w0 = 0; w0 < slots; w0 += kRangeWindow) {
+        const uint32_t wend = min(slots, w0 + kRangeWindow);
+        if (threadIdx.x == 0) s_n = 0;
+        __syncthreads();
+        for (uint32_t i0 = w0; i0 < wend; i0 += blockDim.x) {
+            const uint32_t i = i0 + threadIdx.x;
+            const uint64_t c = i < wend ? mine[i] : kEmptySlot;
+            const uint32_t m = __ballot_sync(0xFFFFFFFFu, c != kEmptySlot);
+            uint32_t base = 0;
+            if (lane == 0 && m) base = atomicAdd(&s_n, (uint32_t)__popc(m));
+            base = __shfl_sync(0xFFFFFFFFu, base, 0);
+            if (c != kEmptySlot) s_cand[base + __popc(m & ((1u << lane) - 1u))] = c;
+        }
+        __syncthreads();
+        const uint32_t n = s_n;
+        for (uint32_t i = warp; i < n; i += blockDim.x / 32) {
+            const uint32_t row = (uint32_t)s_cand[i];
+            const uint8_t *rowb[1] = {rows + (size_t)row * pitch};
+            float d[1];
+            Tile::run(rowb, qb, dim, lane, d);
+            if (lane == 0 && d[0] <= r) mine[atomicAdd(&s_kept, 1u)] = make_composite(d[0], row);
+        }
+        __syncthreads();
+    }
+    const uint32_t kept = s_kept;
+    if (threadIdx.x == 0) {
+        s_base = atomicAdd(total, kept);
+        ok[q] = 1;
+        cnt[q] = kept;
+        off[q] = s_base;
+    }
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < kept; i += blockDim.x) out[s_base + i] = mine[i];
+}
+
 // indices of the queries the first tier left unproven, densely packed: idx[0, *count)
 __global__ void compact_unproven_kernel(const uint32_t *__restrict__ ok, uint32_t nq, uint32_t *__restrict__ idx,
                                         uint32_t *__restrict__ count) {
@@ -1760,6 +1846,25 @@ cudaError_t launch_scatter_rows(const uint64_t *d_src, const uint32_t *d_idx, co
 
 cudaError_t launch_compact_unproven(const uint32_t *d_ok, uint32_t nq, uint32_t *d_idx, uint32_t *d_count, cudaStream_t s) {
     compact_unproven_kernel<<<1, 256, 0, s>>>(d_ok, nq, d_idx, d_count);
+    return cudaGetLastError();
+}
+cudaError_t launch_range_bound(const float *d_radius, uint32_t nq, float eps, const float *d_q_norm2, float max_norm, uint32_t dim, int l2,
+                               float *d_thr, uint32_t *d_overflow, uint32_t *d_total, cudaStream_t s) {
+    if (nq == 0) return cudaSuccess;
+    range_bound_kernel<<<(nq + 255) / 256, 256, 0, s>>>(d_radius, nq, eps, d_q_norm2, max_norm, dim, l2, d_thr, d_overflow, d_total);
+    return cudaGetLastError();
+}
+cudaError_t launch_range_refine(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t slots, uint64_t *d_cand,
+                                const float *d_radius, const float *d_q_norm2, const float *d_thr, const uint32_t *d_overflow, uint64_t *d_out,
+                                uint32_t *d_total, uint32_t *d_ok, uint32_t *d_cnt, uint32_t *d_off, cudaStream_t s) {
+    if (nq == 0) return cudaSuccess;
+    const uint8_t *rows = static_cast<const uint8_t *>(c.rows), *qs = static_cast<const uint8_t *>(d_queries);
+    if (c.metric == MT_L2)
+        range_refine_kernel<MT_L2><<<nq, 256, 0, s>>>(rows, c.pitch, c.dim, qs, qpitch, slots, d_cand, d_radius, d_q_norm2, d_thr, d_overflow,
+                                                      d_out, d_total, d_ok, d_cnt, d_off);
+    else
+        range_refine_kernel<MT_IP><<<nq, 256, 0, s>>>(rows, c.pitch, c.dim, qs, qpitch, slots, d_cand, d_radius, d_q_norm2, d_thr, d_overflow,
+                                                      d_out, d_total, d_ok, d_cnt, d_off);
     return cudaGetLastError();
 }
 cudaError_t launch_gather_queries(const void *d_src, size_t pitch, const float *d_src_n2, const uint32_t *d_idx, const uint32_t *d_count,

@@ -87,6 +87,17 @@ cudaError_t launch_compact_unproven(const uint32_t *d_ok, uint32_t nq, uint32_t 
 // row i of dst = row d_idx[i] of src (pitch % 16 == 0), squared norms likewise (nullable), for i < *d_count
 cudaError_t launch_gather_queries(const void *d_src, size_t pitch, const float *d_src_n2, const uint32_t *d_idx, const uint32_t *d_count,
                                   uint32_t max_n, void *d_dst, float *d_dst_n2, cudaStream_t s);
+// range batches: bound of the fixed-bound main pass, d_thr[q] = d_radius[q] + eps_q (rounded up); clears d_overflow[q] and
+// *d_total
+cudaError_t launch_range_bound(const float *d_radius, uint32_t nq, float eps, const float *d_q_norm2, float max_norm, uint32_t dim, int l2,
+                               float *d_thr, uint32_t *d_overflow, uint32_t *d_total, cudaStream_t s);
+// range batches, one CTA per query over its `slots` list entries of the main pass (d_cand, overwritten): exact rescoring and
+// the inclusive test d <= d_radius[q].  Query q's hits go to d_out[d_off[q], d_off[q] + d_cnt[q]) (composites, unordered;
+// d_out holds nq * slots); d_ok[q] = 1 if the answer is proven complete, else 0 with d_cnt[q] = 0.  d_q_norm2 == NULL: unit
+// rows.
+cudaError_t launch_range_refine(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t slots, uint64_t *d_cand,
+                                const float *d_radius, const float *d_q_norm2, const float *d_thr, const uint32_t *d_overflow, uint64_t *d_out,
+                                uint32_t *d_total, uint32_t *d_ok, uint32_t *d_cnt, uint32_t *d_off, cudaStream_t s);
 // |row|^2 of fp32 rows [first, first+n) into d_norm2[first..], NaN for a row whose fp16 form is not finite (a component
 // with |x| >= 65520, or NaN: refine_kernel never proves such a query); d_stats (nullable) = {max |row|^2, max |x|} as float bits
 cudaError_t launch_row_stats(const void *rows, size_t pitch, uint32_t dim, uint32_t first, uint32_t n, float *d_norm2, uint32_t *d_stats,

@@ -240,6 +240,20 @@ int VecSimB200_TopKQueryBatch(VecSimIndex *index, const void *queryBlobs, size_t
                               VecSimQueryParams *queryParams, size_t *out_labels, double *out_scores) {
     return IX(index)->topk_batch(queryBlobs, qstride, nq, k, queryParams, out_labels, out_scores);
 }
+int VecSimB200_RangeQueryBatch(VecSimIndex *index, const void *queryBlobs, size_t qstride, size_t nq, const double *radii,
+                               VecSimQueryParams *queryParams, VecSimQueryReply_Order order, VecSimQueryReply **replies, uint32_t *out_flags) {
+    // the argument checks of VecSimIndex_RangeQuery, for the whole batch before anything is allocated
+    if (order != BY_ID && order != BY_SCORE) {
+        IX(index)->log("warning", "Possible order values are only 'BY_ID' or 'BY_SCORE'");
+        return -1;
+    }
+    for (size_t i = 0; i < nq; i++)
+        if (radii[i] < 0) {
+            IX(index)->log("warning", "radius must be non-negative");
+            return -1;
+        }
+    return IX(index)->range_batch(queryBlobs, qstride, nq, radii, queryParams, order, replies, out_flags);
+}
 int VecSimB200_TopKQueryBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, size_t k,
                                     int64_t *d_out_labels, float *d_out_scores, void *stream) {
     return IX(index)->topk_batch_device(d_queries, nq, k, d_out_labels, d_out_scores, static_cast<cudaStream_t>(stream));

@@ -818,6 +818,17 @@ bool FlatIndex::ensure_shadow(cudaStream_t st) {
     return true;
 }
 
+void FlatIndex::disable_coarse() {
+    std::lock_guard<std::mutex> g(mu_);
+    coarse_disabled_ = true;
+    cudaFree(d_shadow_);
+    cudaFree(d_norm2_);
+    d_shadow_ = nullptr;
+    d_norm2_ = nullptr;
+    shadow_cap_ = shadow_rows_ = 0;
+    shadow_dirty_.clear();
+}
+
 // Enqueue on `st`: the `ke` best composites of each of `nq` device-resident stored-form queries into
 // d_out [nq][ke].  Cosine fp32 batches take the tensor-core coarse pass + exact rescoring + proof, with
 // the exact scan as an on-device fallback for unverified queries; everything else takes the exact
@@ -911,14 +922,7 @@ bool FlatIndex::batch_scan(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t
     if (coarse && !unit && !(shadow_max_abs_ <= 60000.0f)) {
         // values outside the fp16 range (or NaN): this index stays on the exact scan; give the shadow's HBM back
         coarse = false;
-        std::lock_guard<std::mutex> g(mu_);
-        coarse_disabled_ = true;
-        cudaFree(d_shadow_);
-        cudaFree(d_norm2_);
-        d_shadow_ = nullptr;
-        d_norm2_ = nullptr;
-        shadow_cap_ = shadow_rows_ = 0;
-        shadow_dirty_.clear();
+        disable_coarse();
     }
     last_batch_coarse_ = coarse;
     last_batch_path_ = coarse ? 1 : 0;
@@ -1210,6 +1214,150 @@ VecSimQueryReply *FlatIndex::range(const void *q, double radius, VecSimQueryPara
     if (timed_out(tctx)) rep->code = VecSim_QueryReply_TimedOut; // brute_force.h:306-309 keeps partial results
     finish_reply(rep, order);
     return rep;
+}
+
+// Range batches (DESIGN.md §4, "Range queries"): an eligible fp32 batch takes ONE fixed-bound main pass over the fp16 shadow
+// with the bound radius + eps per query, exact rescoring of the kept rows and a per-query proof; every other batch, and every
+// query whose proof fails, is answered by range() one query at a time.
+int FlatIndex::range_batch(const void *qs, size_t qstride, size_t nq, const double *radii, VecSimQueryParams *qp, VecSimQueryReply_Order order,
+                           VecSimQueryReply **replies, uint32_t *out_flags) {
+    void *tctx = qp ? qp->timeoutCtx : nullptr;
+    last_mode_ = RANGE_QUERY;
+    for (size_t i = 0; i < nq; i++) {
+        replies[i] = nullptr;
+        if (out_flags) out_flags[i] = 0;
+    }
+    if (nq == 0) return VecSim_QueryReply_OK;
+    const auto all_timed_out = [&]() {
+        for (size_t i = 0; i < nq; i++) {
+            if (!replies[i]) replies[i] = new VecSimQueryReply();
+            replies[i]->results.clear();
+            replies[i]->code = VecSim_QueryReply_TimedOut;
+        }
+        return (int)VecSim_QueryReply_TimedOut;
+    };
+    if (timed_out(tctx)) return all_timed_out();
+    if (!flush()) return -1;
+    const size_t n = count_;
+    const CorpusView v = view();
+    // k plays no part in a range query: any k the planner accepts
+    bool route = n > 0 && nq <= 0xFFFFFFFFu && coarse_mode() == 1 && dtype_ == DT_F32 && !multi_ && !coarse_disabled_ && coarse_fixed_enabled() &&
+                 coarse_supported(v, (uint32_t)nq, 1, CoarseF16) && (nq >= 16 || single_query_takes_coarse(1));
+    std::unique_ptr<QueryCtx> c;
+    if (route) {
+        c = checkout();
+        route = c && ensure_shadow(c->stream);
+    }
+    if (route && !unit_rows() && !(shadow_max_abs_ <= 60000.0f)) { // values outside the fp16 range: exact scans from now on
+        disable_coarse();
+        route = false;
+    }
+    if (route) {
+        const uint32_t nq32 = (uint32_t)nq;
+        cudaStream_t st = c->stream;
+        LaunchCounters lc;
+        const bool unit = unit_rows();
+        // stored-form queries, then the radii as float (the reference compares score <= DistType(radius))
+        const size_t qpitch = (stored_bytes_ + 15) & ~(size_t)15, radii_off = qpitch * nq;
+        bool ok = c->need_query(radii_off + nq * sizeof(float));
+        if (ok) {
+            memset(c->h_query, 0, radii_off);
+            float *hr = reinterpret_cast<float *>(c->h_query + radii_off);
+            for (size_t i = 0; i < nq; i++) {
+                preprocess_query(static_cast<const uint8_t *>(qs) + i * qstride, c->h_query + i * qpitch);
+                hr[i] = (float)radii[i];
+            }
+            ok = cudaMemcpyAsync(c->d_query, c->h_query, radii_off + nq * sizeof(float), cudaMemcpyHostToDevice, st) == cudaSuccess;
+        }
+        const float *d_radius = reinterpret_cast<const float *>(c->d_query + radii_off);
+        const CoarsePlan cp = plan_coarse(v, nq32, CoarseF16, 1, 0, 1, 1);
+        const size_t slots = (size_t)cp.grid_x * cp.keep, nA = nq * slots;
+        const size_t q16_pitch = (dim_ * 2 + 15) & ~(size_t)15, q16_elems = (nq * q16_pitch + 7) / 8;
+        const size_t flag_elems = (nq + 1) / 2 + 1; // nq uint32 / float values
+        const size_t qn_elems = unit ? 0 : flag_elems, res_elems = (3 * nq + 1 + 1) / 2 + 1;
+        ok = ok && c->need_cand(2 * nA + q16_elems + cp.scratch_elems + qn_elems + 2 * flag_elems + res_elems) && c->need_ids(3 * nq + 1);
+        uint64_t *cand = c->d_cand, *hits = cand + nA, *q16 = hits + nA, *list_scratch = q16 + q16_elems, *tail = list_scratch + cp.scratch_elems;
+        float *d_qn2 = unit ? nullptr : reinterpret_cast<float *>(tail); // |q|^2 per query
+        tail += qn_elems;
+        float *d_thr = reinterpret_cast<float *>(tail);                         // bound of the main pass per query
+        uint32_t *d_ovf = reinterpret_cast<uint32_t *>(tail + flag_elems);     // a list of the main pass ran full
+        uint32_t *d_res = reinterpret_cast<uint32_t *>(tail + 2 * flag_elems); // [ok nq][count nq][offset nq][hits in total]
+        uint32_t *d_total = d_res + 3 * nq;
+        ok = ok && launch_to_f16(c->d_query, qpitch, (uint32_t)dim_, 0, nq32, q16, q16_pitch, st) == cudaSuccess;
+        if (!unit) ok = ok && launch_row_stats(c->d_query, qpitch, (uint32_t)dim_, 0, nq32, d_qn2, nullptr, st) == cudaSuccess;
+        ok = ok && launch_range_bound(d_radius, nq32, kCoarseEpsF16, d_qn2, shadow_max_norm_, (uint32_t)dim_, mkind_ == MT_L2 ? 1 : 0, d_thr, d_ovf,
+                                      d_total, st) == cudaSuccess;
+        const CoarseOperands ops{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
+        cudaEventRecord(c->ev_start, st);
+        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_thr, d_ovf) == cudaSuccess;
+        cudaEventRecord(c->ev_stop, st);
+        ok = ok && launch_range_refine(v, c->d_query, qpitch, nq32, (uint32_t)slots, cand, d_radius, d_qn2, d_thr, d_ovf, hits, d_total, d_res,
+                                       d_res + nq, d_res + 2 * nq, st) == cudaSuccess;
+        ok = ok && cudaMemcpyAsync(c->h_ids, d_res, (3 * nq + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st) == cudaSuccess;
+        lc.launches += unit ? 4 : 5;
+        launches_total_ += lc.launches;
+        coarse_batches_++;
+        if (ok) {
+            const int w = wait_polling(st, tctx);
+            if (w == 1) { // deadline passed while the pass was running
+                c->abandoned = true;
+                *c->h_abort = 1;
+                checkin(std::move(c));
+                return all_timed_out();
+            }
+            ok = w == 0;
+        }
+        const uint32_t *h_ok = c->h_ids, *h_cnt = h_ok + nq, *h_off = h_cnt + nq;
+        if (ok) {
+            float ms = 0;
+            if (cudaEventElapsedTime(&ms, c->ev_start, c->ev_stop) == cudaSuccess) {
+                std::lock_guard<std::mutex> g(stats_mu_);
+                scan_us_ += ms * 1000.0;
+                scan_launches_++;
+                scan_bytes_ += (uint64_t)n * stored_bytes_;
+            }
+            const uint32_t total = h_ok[3 * nq]; // only the occupied part of the result buffer crosses PCIe
+            ok = c->need_out(total) && cudaMemcpyAsync(c->h_out, hits, (size_t)total * 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+                 cudaStreamSynchronize(st) == cudaSuccess;
+        }
+        if (ok) {
+            for (size_t i = 0; i < nq; i++) {
+                if (!h_ok[i]) continue;
+                auto *rep = new VecSimQueryReply();
+                rep->results.reserve(h_cnt[i]);
+                for (uint32_t j = 0; j < h_cnt[i]; j++) {
+                    const uint64_t comp = c->h_out[(size_t)h_off[i] + j];
+                    rep->results.push_back({id_to_label_[(uint32_t)comp], (double)key_to_float((uint32_t)(comp >> 32))});
+                }
+                finish_reply(rep, order);
+                replies[i] = rep;
+                if (out_flags) out_flags[i] = 1;
+            }
+        }
+        checkin(std::move(c));
+        if (!ok) {
+            log("warning", "vecsim_b200: range batch failed on device");
+            for (size_t i = 0; i < nq; i++) {
+                delete replies[i];
+                replies[i] = nullptr;
+                if (out_flags) out_flags[i] = 0;
+            }
+            return -1;
+        }
+    } else if (c) {
+        checkin(std::move(c));
+    }
+    // queries the route did not answer (or the whole batch): one exact scan each
+    for (size_t i = 0; i < nq; i++)
+        if (!replies[i]) replies[i] = range(static_cast<const uint8_t *>(qs) + i * qstride, radii[i], qp, order);
+    last_mode_ = RANGE_QUERY;
+    const bool late = timed_out(tctx); // as range(): the replies keep what was found
+    int rc = VecSim_QueryReply_OK;
+    for (size_t i = 0; i < nq; i++) {
+        if (late) replies[i]->code = VecSim_QueryReply_TimedOut;
+        if (replies[i]->code == VecSim_QueryReply_TimedOut) rc = VecSim_QueryReply_TimedOut;
+    }
+    return rc;
 }
 
 double FlatIndex::distance_from(size_t label, const void *blob) {

@@ -130,6 +130,11 @@ class FlatIndex {
                    double *out_scores);
     int topk_batch_device(const void *d_q, size_t nq, size_t k, int64_t *d_labels, float *d_scores, cudaStream_t s);
     VecSimQueryReply *range(const void *q, double radius, VecSimQueryParams *qp, VecSimQueryReply_Order order);
+    // nq range queries, replies[i] = what range(qs + i * qstride, radii[i], qp, order) returns.  Eligible fp32 batches take
+    // the fixed-bound tensor-core pass + exact rescoring + proof (DESIGN.md §4); out_flags[i] (nullable) = 1 for a query
+    // answered there, 0 for one answered by range().  Arguments are validated by the caller.
+    int range_batch(const void *qs, size_t qstride, size_t nq, const double *radii, VecSimQueryParams *qp, VecSimQueryReply_Order order,
+                    VecSimQueryReply **replies, uint32_t *out_flags);
     double distance_from(size_t label, const void *stored_form_blob);
     bool prefer_adhoc(size_t subset, size_t k, bool initial);
 
@@ -217,6 +222,7 @@ class FlatIndex {
     bool unit_rows() const { return metric_ == VecSimMetric_Cosine && !raw_rows_; }
     std::vector<idType> shadow_dirty_;
     bool ensure_shadow(cudaStream_t st);
+    void disable_coarse(); // rows outside the fp16 range: exact scans from now on, the shadow's HBM is given back
     bool single_query_takes_coarse(uint32_t ke, const float *host_query = nullptr);
     size_t capacity_ = 0; // rows of HBM allocated
     size_t count_ = 0;    // rows in the index (incl. staged)

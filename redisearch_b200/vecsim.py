@@ -137,6 +137,7 @@ SIGNATURES = [
     ("VecSim_GetSharedMemory", _SZ, []),
     ("VecSimB200_TopKQueryBatch", C.c_int, [_P, _P, _SZ, _SZ, _SZ, C.POINTER(VecSimQueryParams), _P, _P]),
     ("VecSimB200_TopKQueryBatchDevice", C.c_int, [_P, _P, _SZ, _SZ, _P, _P, _P]),
+    ("VecSimB200_RangeQueryBatch", C.c_int, [_P, _P, _SZ, _SZ, _P, C.POINTER(VecSimQueryParams), C.c_int, _P, _P]),
     ("VecSimB200_AddVectors", C.c_int, [_P, _P, _SZ, _SZ, _P, _SZ]),
     ("VecSimB200_AddVectorsDevice", C.c_int, [_P, _P, _SZ, _SZ]),
     ("VecSimB200_Reserve", C.c_int, [_P, _SZ]),
@@ -263,6 +264,20 @@ class VecSimIndex:
         scores = np.empty((nq, k), dtype=np.float64)
         rc = self.L.VecSimB200_TopKQueryBatch(self.h, _ptr(qs), qs.strides[0], nq, k, params, _ptr(labels), _ptr(scores))
         return labels, scores, rc
+
+    def range_batch(self, qs: np.ndarray, radii, order=BY_SCORE, params=None):
+        """nq range queries in one call: ([(ids, scores, code) per query], rc, flags); flags[i] = 1 if query i was answered
+        by the tensor-core route.  rc == -1 (invalid order, negative radius, device failure): no replies, an empty list."""
+        qs = np.ascontiguousarray(qs)
+        nq = qs.shape[0]
+        radii = np.ascontiguousarray(np.broadcast_to(np.asarray(radii, dtype=np.float64), (nq,)))
+        reps = (C.c_void_p * max(1, nq))()
+        flags = np.zeros(nq, dtype=np.uint32)
+        rc = self.L.VecSimB200_RangeQueryBatch(self.h, _ptr(qs), qs.strides[0], nq, _ptr(radii), params, order, C.cast(reps, C.c_void_p),
+                                               _ptr(flags))
+        if rc == -1:
+            return [], rc, flags
+        return [self._drain(reps[i]) for i in range(nq)], rc, flags
 
     def topk_filtered(self, q: np.ndarray, k: int, doc_ids, n=None):
         """k nearest among the listed labels.  doc_ids: ascending uint32 numpy array, or a device pointer (int) with n."""
