@@ -425,14 +425,18 @@ size_t VecSim_GetSharedMemory(void);                                      /* 0, 
  * ---------------------------------------------------------------------------------------------- */
 /* nq queries in one corpus pass.  queryBlobs: nq host blobs, qstride bytes apart.  Results are
  * written to out_labels / out_scores ([nq][k], row-major, ascending (score,label)); entries past
- * the number of hits carry label SIZE_MAX and score NaN.  Returns VecSim_QueryReply_OK /
- * _TimedOut, or -1 on a CUDA failure. */
+ * the number of hits carry label SIZE_MAX and score NaN.  A multi-value index answers the k best
+ * labels, each scored by its best row, as VecSimIndex_TopKQuery does (k <= 128: a tensor-core row route
+ * + label stage, queries it cannot prove and corpora of >= 65536 rows no such route serves one at a
+ * time; the label-aware exact scan below that size; k > 128: one query at a time).  Returns
+ * VecSim_QueryReply_OK / _TimedOut, or -1 on a CUDA failure. */
 int VecSimB200_TopKQueryBatch(VecSimIndex *index, const void *queryBlobs, size_t qstride, size_t nq,
                               size_t k, VecSimQueryParams *queryParams, size_t *out_labels,
                               double *out_scores);
 /* Same, but queries and results are DEVICE pointers (fp/int data as the index type; labels are
- * int64, scores float).  Nothing crosses PCIe; the call only enqueues on `stream`
- * (a cudaStream_t cast to void*, NULL = the index's own stream) and returns. */
+ * int64, -1 for empty entries, scores float).  Nothing crosses PCIe; the call only enqueues on `stream`
+ * (a cudaStream_t cast to void*, NULL = the index's own stream) and returns.  k <= 128, single- and
+ * multi-value indexes; -1 for a larger k. */
 int VecSimB200_TopKQueryBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, size_t k,
                                     int64_t *d_out_labels, float *d_out_scores, void *stream);
 /* nq range queries in one call.  replies[i] receives exactly what
@@ -543,8 +547,10 @@ int VecSimB200_TopKFilteredBatch(VecSimIndex *index, const void *const *queryBlo
  * -1 = environment default (VECSIM_B200_COARSE, 1 unless set). */
 void VecSimB200_SetCoarseMode(int mode);
 /* Debug: after a VecSimB200_TopKQueryBatchDevice call, per-query flags (1 = answered by the tensor-core path on the first
- * tier's 24-entry candidate lists, 2 = by the second tier's 128-entry lists, 0 = fell back to the exact scan).  Returns -1
- * if the last batch did not take the coarse path. */
+ * tier's 24-entry candidate lists, 2 = by the second tier's 128-entry lists, 0 = fell back to the exact scan).  Multi-value
+ * index: 1 / 2 / 0 as before for its row stage, with the label check passed; 3 = fewer than k labels among the rows the row
+ * stage selected, the label-aware exact scan answered (DESIGN.md §4.4).  Returns -1 if the last batch did not take the coarse
+ * path. */
 int VecSimB200_LastCoarseFlags(VecSimIndex *index, uint32_t *out_ok, size_t nq);
 /* Debug: which route the last top-k query (single or batched) took: 0 = exact CUDA-core scan, 1 = tensor-core coarse pass + exact
  * rescoring + proof (fp32 cosine), 2 = tensor-core direct, k <= 128 (csrc/coarse_tc.cu): fp16 / bf16 corpora, inner

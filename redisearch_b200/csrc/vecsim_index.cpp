@@ -50,6 +50,7 @@ QueryCtx::~QueryCtx() {
     cudaFreeHost(h_ids);
     cudaFree(d_dist);
     cudaFreeHost(h_dist);
+    cudaFree(d_lab);
     if (ev_start) cudaEventDestroy(ev_start);
     if (ev_stop) cudaEventDestroy(ev_stop);
     if (stream) cudaStreamDestroy(stream);
@@ -133,6 +134,18 @@ bool QueryCtx::need_ids(size_t n) {
     CU_OK(cudaMalloc(&d_dist, cap * 4));
     CU_OK(cudaMallocHost(&h_dist, cap * 4));
     ids_cap = cap;
+    return true;
+}
+
+bool QueryCtx::need_lab(size_t elems) {
+    if (elems <= lab_cap) return true;
+    cudaStreamSynchronize(stream);
+    cudaFree(d_lab);
+    d_lab = nullptr;
+    lab_cap = 0;
+    const size_t cap = std::max<size_t>(elems, 64 * 1024);
+    CU_OK(cudaMalloc(&d_lab, cap * sizeof(uint64_t)));
+    lab_cap = cap;
     return true;
 }
 
@@ -386,10 +399,13 @@ int FlatIndex::add(const void *blob, size_t label) {
     preprocess_storage(blob, slot);
     const idType id = (idType)count_++;
     id_to_label_.push_back(label);
-    if (multi_)
-        label_to_ids_[label].push_back(id);
-    else
+    if (multi_) {
+        auto &ids = label_to_ids_[label];
+        label_rows_changed(ids.size(), ids.size() + 1);
+        ids.push_back(id);
+    } else {
         label_to_id_[label] = id;
+    }
     labels_dirty_ = true;
     l2i_dirty_ = true;
     return 1;
@@ -415,10 +431,13 @@ int FlatIndex::add_bulk_device(const void *d_src, size_t n, size_t label0) {
     for (size_t i = 0; i < n; i++) {
         const idType id = (idType)(count_ + i);
         id_to_label_.push_back(label0 + i);
-        if (multi_)
-            label_to_ids_[label0 + i].push_back(id);
-        else
+        if (multi_) {
+            auto &ids = label_to_ids_[label0 + i];
+            label_rows_changed(ids.size(), ids.size() + 1);
+            ids.push_back(id);
+        } else {
             label_to_id_[label0 + i] = id;
+        }
     }
     count_ += n;
     resident_ = count_;
@@ -435,6 +454,7 @@ int FlatIndex::remove(size_t label) {
         if (it == label_to_ids_.end()) return 0;
         victims = it->second;
         label_to_ids_.erase(it);
+        label_rows_changed(victims.size(), 0);
     } else {
         auto it = label_to_id_.find(label);
         if (it == label_to_id_.end()) return 0;
@@ -473,6 +493,19 @@ int FlatIndex::remove(size_t label) {
     labels_dirty_ = true;
     l2i_dirty_ = true;
     return removed;
+}
+
+void FlatIndex::label_rows_changed(size_t from, size_t to) {
+    if (from) {
+        auto it = rows_per_label_.find(from);
+        if (it != rows_per_label_.end() && --it->second == 0) rows_per_label_.erase(it);
+    }
+    if (to) rows_per_label_[to]++;
+}
+
+size_t FlatIndex::max_rows_per_label() const {
+    std::lock_guard<std::mutex> g(mu_);
+    return rows_per_label_.empty() ? 0 : rows_per_label_.rbegin()->first;
 }
 
 bool FlatIndex::read_rows(size_t first, size_t n, void *host_dst) {
@@ -832,9 +865,15 @@ void FlatIndex::disable_coarse() {
 // Enqueue on `st`: the `ke` best composites of each of `nq` device-resident stored-form queries into
 // d_out [nq][ke].  Cosine fp32 batches take the tensor-core coarse pass + exact rescoring + proof, with
 // the exact scan as an on-device fallback for unverified queries; everything else takes the exact
-// fused scan.  ev_start/ev_stop of `c` bracket the dominant scan kernel.
+// fused scan.  ev_start/ev_stop of `c` bracket the dominant scan kernel.  A multi-value index selects labels instead
+// (batch_scan_labels).
 bool FlatIndex::batch_scan(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t nq, uint32_t ke, cudaStream_t st,
                            LaunchCounters &lc, uint64_t **d_result) {
+    return multi_ ? batch_scan_labels(c, d_q, qpitch, nq, ke, st, lc, d_result) : batch_scan_rows(c, d_q, qpitch, nq, ke, st, lc, d_result);
+}
+
+bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t nq, uint32_t ke, cudaStream_t st,
+                                LaunchCounters &lc, uint64_t **d_result, bool tc_only) {
     const CorpusView v = view();
     const ScanPlan sp = plan_scan_topk(v, nq, ke);
     const int cmode = coarse_mode();
@@ -842,7 +881,7 @@ bool FlatIndex::batch_scan(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t
     // orders of magnitude), so the batch is one kernel + the usual final selection — no shadow, no rescoring
     const bool is16 = dtype_ == DT_F16 || dtype_ == DT_BF16, is8 = dtype_ == DT_I8 || dtype_ == DT_U8;
     const CoarseKind dkind = is16 ? CoarseDirect16 : CoarseDirect8;
-    if (cmode != 0 && !multi_ && nq >= 16 && (is16 || is8) && coarse_supported(v, nq, ke, dkind)) {
+    if (cmode != 0 && nq >= 16 && (is16 || is8) && coarse_supported(v, nq, ke, dkind)) {
         // int8 / uint8: s8 / u8 wgmma dot products are exact integers and the epilogue applies the reference's own
         // float expression, so that route is bit-exact
         const CoarseOperands ops{v.rows, v.pitch, d_q, qpitch, (dtype_ == DT_BF16 || dtype_ == DT_I8) ? 1 : 0, mkind_ == MT_COS ? 1 : 0, nullptr, nullptr};
@@ -912,7 +951,7 @@ bool FlatIndex::batch_scan(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t
     // cosine: unit vectors, constant error bound, either operand kind.  L2 / raw inner product (fp32): the fp16 route only,
     // error bound from the row and query norms
     const bool unit = unit_rows();
-    const bool eligible = cmode != 0 && !multi_ && !coarse_disabled_ && dtype_ == DT_F32 && (unit || cmode == 1) &&
+    const bool eligible = cmode != 0 && !coarse_disabled_ && dtype_ == DT_F32 && (unit || cmode == 1) &&
                           (nq >= 16 || single_query_takes_coarse(ke));
     bool coarse = eligible && coarse_supported(v, nq, ke, kind);
     if (eligible && kind == CoarseF16 && (!coarse || !ensure_shadow(st))) { // rows too wide for the 16-bit kernel's shared memory, or no HBM for the shadow
@@ -926,6 +965,10 @@ bool FlatIndex::batch_scan(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t
     }
     last_batch_coarse_ = coarse;
     last_batch_path_ = coarse ? 1 : 0;
+    if (!coarse && tc_only) {
+        *d_result = nullptr;
+        return true;
+    }
     if (!coarse) {
         if (!c.need_cand(sp.cand_elems) || !c.need_out((size_t)nq * ke)) return false;
         cudaEventRecord(c.ev_start, st);
@@ -1032,6 +1075,56 @@ bool FlatIndex::batch_scan(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t
     return ok;
 }
 
+// Multi-value index (DESIGN.md §4.4).  Rows are ordered by (score, row id) and a label by its best row.  If a tensor-core route
+// applies, it selects the K = min(128, kl * m, n) best rows of each query (m = most rows any label owns) and label_select takes
+// their first kl distinct labels; that is exact when the K rows hold kl distinct labels, which K >= kl * m guarantees unless
+// K was capped at 128.  Queries with fewer labels, and whole batches no tensor-core route serves, run the label-aware exact
+// scan.  Nothing returns to the host in between.
+// host_fallback (the host API): the label-aware exact scan runs only for corpora too small for the tensor-core routes.  Elsewhere
+// it is slower than one query at a time (DESIGN.md §4.4), so the caller answers those queries with topk(): the ones whose
+// c.d_last_ok flag is 3 after a row route, or all of them when *d_result comes back NULL.
+bool FlatIndex::batch_scan_labels(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t nq, uint32_t kl, cudaStream_t st, LaunchCounters &lc,
+                                  uint64_t **d_result, bool host_fallback) {
+    const CorpusView v = view();
+    const uint32_t K = (uint32_t)std::min<size_t>(std::min<size_t>(kMaxFusedK, (size_t)kl * max_rows_per_label()), v.n_rows);
+    const ScanPlan sp = plan_scan_topk(v, nq, kl, true);
+    const size_t nO = (size_t)nq * kl, flag_elems = (nq + 1) / 2 + 1;
+    // [label answers nq x kl][exact answers nq x kl][lists of the exact scan][label check per query][reported flags]
+    if (!c.need_lab(2 * nO + sp.cand_elems + 2 * flag_elems)) return false;
+    uint64_t *out1 = c.d_lab, *out2 = out1 + nO, *cand = out2 + nO;
+    uint32_t *lab_ok = reinterpret_cast<uint32_t *>(cand + sp.cand_elems), *flags = reinterpret_cast<uint32_t *>(cand + sp.cand_elems + flag_elems);
+    uint64_t *rows = nullptr;
+    if (!batch_scan_rows(c, d_q, qpitch, nq, K, st, lc, &rows, true)) return false;
+    bool ok = true;
+    if (rows) {
+        // rows: [nq][K] in c.d_out; the label answers are blended back into it
+        ok = launch_label_select(rows, nq, K, d_id_to_label_, kl, c.d_last_ok, out1, lab_ok, flags, st, &lc) == cudaSuccess;
+        c.d_last_ok = flags;
+        c.last_ok_n = nq;
+        if (host_fallback) {
+            ok = ok && cudaMemcpyAsync(c.d_out, out1, nO * 8, cudaMemcpyDeviceToDevice, st) == cudaSuccess;
+        } else {
+            ok = ok && launch_scan_topk(v, d_q, qpitch, nq, kl, sp, cand, st, &lc, lab_ok, c.d_abort, d_id_to_label_) == cudaSuccess;
+            ok = ok && launch_final_select_labels(cand, nq, sp.lists_per_query * kl, kl, d_id_to_label_, out2, st, &lc) == cudaSuccess;
+            ok = ok && launch_blend(lab_ok, out1, out2, nq, kl, c.d_out, st, &lc) == cudaSuccess;
+            cudaEventRecord(c.ev_stop, st); // the timed span runs from the row stage's main pass through the label-aware scan
+        }
+    } else if (host_fallback && v.n_rows >= 65536) {
+        c.d_last_ok = nullptr;
+        *d_result = nullptr;
+        return true;
+    } else {
+        c.d_last_ok = nullptr;
+        if (!c.need_out(nO)) return false;
+        cudaEventRecord(c.ev_start, st);
+        ok = launch_scan_topk(v, d_q, qpitch, nq, kl, sp, cand, st, &lc, nullptr, c.d_abort, d_id_to_label_) == cudaSuccess;
+        cudaEventRecord(c.ev_stop, st);
+        ok = ok && launch_final_select_labels(cand, nq, sp.lists_per_query * kl, kl, d_id_to_label_, c.d_out, st, &lc) == cudaSuccess;
+    }
+    *d_result = c.d_out;
+    return ok;
+}
+
 int FlatIndex::topk_batch(const void *qs, size_t qstride, size_t nq, size_t k, VecSimQueryParams *qp, size_t *out_labels,
                           double *out_scores) {
     void *tctx = qp ? qp->timeoutCtx : nullptr;
@@ -1046,23 +1139,28 @@ int FlatIndex::topk_batch(const void *qs, size_t qstride, size_t nq, size_t k, V
     const size_t n = count_;
     if (n == 0) return VecSim_QueryReply_OK;
     if (timed_out(tctx)) return VecSim_QueryReply_TimedOut;
-    if (multi_ || std::min(k, n) > (size_t)kMaxFusedK) { // generic path, one query at a time
+    const auto one_query = [&](size_t i) { // the generic path for query i
+        VecSimQueryReply *r = topk(static_cast<const uint8_t *>(qs) + i * qstride, k, qp, BY_SCORE);
+        const int code = r->code;
+        for (size_t j = 0; j < k; j++) {
+            out_labels[i * k + j] = j < r->results.size() ? r->results[j].id : SIZE_MAX;
+            out_scores[i * k + j] = j < r->results.size() ? r->results[j].score : nan;
+        }
+        delete r;
+        return code;
+    };
+    if (multi_ ? k > (size_t)kMaxFusedK : std::min(k, n) > (size_t)kMaxFusedK) { // generic path, one query at a time
         for (size_t i = 0; i < nq; i++) {
-            VecSimQueryReply *r = topk(static_cast<const uint8_t *>(qs) + i * qstride, k, qp, BY_SCORE);
-            const int code = r->code;
-            for (size_t j = 0; j < r->results.size() && j < k; j++) {
-                out_labels[i * k + j] = r->results[j].id;
-                out_scores[i * k + j] = r->results[j].score;
-            }
-            delete r;
+            const int code = one_query(i);
             if (code != VecSim_QueryReply_OK) return code;
         }
         return VecSim_QueryReply_OK;
     }
+    if (multi_ && !sync_labels_to_device()) return -1;
     auto c = checkout();
     if (!c) return -1;
     const size_t qpitch = (stored_bytes_ + 15) & ~(size_t)15;
-    const uint32_t ke = (uint32_t)std::min(k, n);
+    const uint32_t ke = (uint32_t)std::min(k, multi_ ? label_count() : n); // a multi-value index answers labels
     const CorpusView v = view();
     LaunchCounters lc;
     bool ok = c->need_query(qpitch * nq);
@@ -1072,8 +1170,18 @@ int FlatIndex::topk_batch(const void *qs, size_t qstride, size_t nq, size_t k, V
         ok = cudaMemcpyAsync(c->d_query, c->h_query, qpitch * nq, cudaMemcpyHostToDevice, c->stream) == cudaSuccess;
     }
     uint64_t *d_res = nullptr;
-    ok = ok && batch_scan(*c, c->d_query, qpitch, (uint32_t)nq, ke, c->stream, lc, &d_res);
-    ok = ok && cudaMemcpyAsync(c->h_out, c->d_out, nq * ke * 8, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess;
+    // multi-value: queries the label stage could not prove, or all of them, are answered one at a time below (batch_scan_labels)
+    bool per_query_all = false;
+    const uint32_t *d_flags = nullptr;
+    if (multi_) {
+        ok = ok && c->need_ids(nq) && batch_scan_labels(*c, c->d_query, qpitch, (uint32_t)nq, ke, c->stream, lc, &d_res, true);
+        per_query_all = ok && !d_res;
+        d_flags = c->d_last_ok;
+        ok = ok && (!d_flags || cudaMemcpyAsync(c->h_ids, d_flags, nq * 4, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess);
+    } else {
+        ok = ok && batch_scan(*c, c->d_query, qpitch, (uint32_t)nq, ke, c->stream, lc, &d_res);
+    }
+    ok = ok && (per_query_all || cudaMemcpyAsync(c->h_out, c->d_out, nq * ke * 8, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess);
     launches_total_ += lc.launches;
     if (ok) {
         const int w = wait_polling(c->stream, tctx); // a full exact-scan fallback no longer holds a timed-out caller
@@ -1085,6 +1193,15 @@ int FlatIndex::topk_batch(const void *qs, size_t qstride, size_t nq, size_t k, V
         }
         ok = w == 0;
     }
+    if (per_query_all && ok) { // the stream is idle: wait_polling above saw the query upload finish
+        checkin(std::move(c));
+        for (size_t i = 0; i < nq; i++) {
+            const int code = one_query(i);
+            if (code != VecSim_QueryReply_OK) return code;
+        }
+        return VecSim_QueryReply_OK;
+    }
+    std::vector<size_t> open; // multi-value queries whose label check failed (flag 3)
     if (ok) {
         float ms = 0;
         if (cudaEventElapsedTime(&ms, c->ev_start, c->ev_stop) == cudaSuccess) {
@@ -1093,6 +1210,9 @@ int FlatIndex::topk_batch(const void *qs, size_t qstride, size_t nq, size_t k, V
             scan_launches_++;
             scan_bytes_ += (uint64_t)n * stored_bytes_;
         }
+        if (d_flags)
+            for (size_t i = 0; i < nq; i++)
+                if (c->h_ids[i] == 3u) open.push_back(i);
         std::vector<VecSimQueryResult> tmp;
         VecSimQueryReply rr;
         for (size_t i = 0; i < nq; i++) {
@@ -1111,6 +1231,15 @@ int FlatIndex::topk_batch(const void *qs, size_t qstride, size_t nq, size_t k, V
     }
     checkin(std::move(c));
     if (!ok) return -1;
+    const int path = last_batch_path_; // LastBatchPath reports the batch's row stage, not the per-query answers below
+    for (size_t i : open) {
+        const int code = one_query(i);
+        if (code != VecSim_QueryReply_OK) {
+            last_batch_path_ = path;
+            return code;
+        }
+    }
+    last_batch_path_ = path;
     if (timed_out(tctx)) return VecSim_QueryReply_TimedOut;
     return VecSim_QueryReply_OK;
 }
@@ -1119,7 +1248,7 @@ int FlatIndex::topk_batch_device(const void *d_q, size_t nq, size_t k, int64_t *
     if (nq == 0 || k == 0) return 0;
     if (!flush() || !sync_labels_to_device()) return -1;
     const size_t n = count_;
-    if (multi_ || k > (size_t)kMaxFusedK) return -1;
+    if (k > (size_t)kMaxFusedK) return -1;
     // Scratch of this entry point is stream-ordered: one dedicated context, reused call after call.
     // Callers enqueue on one stream (or synchronise between streams), as with any async API.
     std::lock_guard<std::mutex> dg(dev_mu_);
@@ -1128,7 +1257,7 @@ int FlatIndex::topk_batch_device(const void *d_q, size_t nq, size_t k, int64_t *
     if (!c) return -1;
     collect_dev_timing_locked(); // the previous call's scan events (stream-ordered before this call)
     const size_t qpitch = (stored_bytes_ + 15) & ~(size_t)15;
-    const uint32_t ke = (uint32_t)std::min(k, std::max<size_t>(n, 1));
+    const uint32_t ke = (uint32_t)std::min(k, std::max<size_t>(multi_ ? label_count() : n, 1));
     cudaStream_t st = s ? s : cudaStreamLegacy; // NULL = the legacy default stream, as everywhere in CUDA
     LaunchCounters lc;
     bool ok = true;

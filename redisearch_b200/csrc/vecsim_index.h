@@ -69,6 +69,8 @@ struct QueryCtx {
     uint32_t *d_ids = nullptr, *h_ids = nullptr;
     float *d_dist = nullptr, *h_dist = nullptr;
     size_t ids_cap = 0;
+    uint64_t *d_lab = nullptr; // label stage of a multi-value batch (its flags stay readable after the call)
+    size_t lab_cap = 0;
     bool abandoned = false; // a timed-out caller left while kernels were still running on `stream`: synchronise before reuse
     // raised by the host when a caller times out: the exact-scan kernel polls it (mapped pinned memory) and winds down, so the GPU
     // does not finish a pass nobody waits for
@@ -81,6 +83,7 @@ struct QueryCtx {
     bool need_out(size_t elems);
     bool need_scores(size_t n);
     bool need_ids(size_t n);
+    bool need_lab(size_t elems);
 };
 
 class FlatIndex;
@@ -195,8 +198,15 @@ class FlatIndex {
     // kMaxFusedK; returns the number found or -1.
     long select_from_scores(QueryCtx &c, uint32_t n, bool has_cursor, uint64_t cursor, size_t want);
     bool upload_query(QueryCtx &c, const uint8_t *stored_q, size_t nq);
+    // [nq][ke] best composites of a batch: rows of a single-value index, labels (score, best row) of a multi-value one
     bool batch_scan(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t nq, uint32_t ke, cudaStream_t st, LaunchCounters &lc,
                     uint64_t **d_result);
+    // row-level routes; tc_only: only a tensor-core route runs, else nothing is launched and *d_result = NULL
+    bool batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t nq, uint32_t ke, cudaStream_t st, LaunchCounters &lc,
+                         uint64_t **d_result, bool tc_only = false);
+    // multi-value index: the first kl distinct labels per query (DESIGN.md §4.4); needs d_id_to_label_ in sync
+    bool batch_scan_labels(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t nq, uint32_t kl, cudaStream_t st, LaunchCounters &lc,
+                           uint64_t **d_result, bool host_fallback = false);
     void finish_reply(VecSimQueryReply *rep, VecSimQueryReply_Order order) const;
 
     DType dtype_;
@@ -234,6 +244,11 @@ class FlatIndex {
     std::vector<size_t> id_to_label_;
     std::unordered_map<size_t, idType> label_to_id_;
     std::unordered_map<size_t, std::vector<idType>> label_to_ids_;
+    // multi-value index: rows per label -> number of labels with that many rows; its largest key is m, the most rows any label
+    // owns, which sizes the row stage of a batch (DESIGN.md §4.4)
+    std::map<size_t, size_t> rows_per_label_;
+    void label_rows_changed(size_t from, size_t to); // a label went from `from` to `to` rows (0 = absent); caller holds mu_
+    size_t max_rows_per_label() const;
     uint64_t *d_id_to_label_ = nullptr;
     size_t d_labels_cap_ = 0;
     bool labels_dirty_ = true;
@@ -251,7 +266,7 @@ class FlatIndex {
     std::atomic<uint64_t> launches_total_{0};
     std::atomic<uint64_t> coarse_batches_{0};
     bool last_batch_coarse_ = false;
-    int last_batch_path_ = 0; // 0 exact scan, 1 tensor-core coarse pass + proof, 2 tensor-core direct (16-bit corpora)
+    int last_batch_path_ = 0; // 0 exact scan, 1 tensor-core coarse pass + proof, 2 tensor-core direct (16-bit corpora); multi-value: the row stage's
   public:
     int last_batch_path() const { return last_batch_path_; }
   private:

@@ -45,10 +45,8 @@ struct ListState {
     uint32_t *wpos;  // [1]
 };
 
-// All 32 lanes; cand is warp-uniform.  Replaces the current worst entry, then rescans.
-__device__ __forceinline__ void list_admit(const ListState &ls, uint32_t k, uint64_t cand, int lane) {
-    if (lane == 0) ls.slots[*ls.wpos] = cand;
-    __syncwarp();
+// All 32 lanes: finds the worst entry again after a slot changed.
+__device__ __forceinline__ void list_rescan(const ListState &ls, uint32_t k, int lane) {
     uint64_t best = 0;
     uint32_t pos = 0;
     for (uint32_t p = lane; p < k; p += 32) {
@@ -74,6 +72,79 @@ __device__ __forceinline__ void list_admit(const ListState &ls, uint32_t k, uint
     __syncwarp();
 }
 
+// All 32 lanes; cand is warp-uniform.  Replaces the current worst entry, then rescans.
+__device__ __forceinline__ void list_admit(const ListState &ls, uint32_t k, uint64_t cand, int lane) {
+    if (lane == 0) ls.slots[*ls.wpos] = cand;
+    __syncwarp();
+    list_rescan(ls, k, lane);
+}
+
+// Label-aware list of a multi-value index (DESIGN.md §4.4): the list holds distinct labels, lab[p] = label of slots[p] (~0 for
+// an empty slot), each at the best composite seen for it.  A candidate whose label is already listed replaces that entry only if
+// it is smaller; a new label evicts the worst entry.  All 32 lanes; cand and label are warp-uniform, cand < *ls.worst.
+__device__ __forceinline__ void list_admit_label(const ListState &ls, uint64_t *lab, uint32_t k, uint64_t cand, uint64_t label, int lane) {
+    int hit = -1;
+    for (uint32_t p0 = 0; p0 < k; p0 += 32) {
+        const unsigned m = __ballot_sync(0xffffffffu, p0 + lane < k && lab[p0 + lane] == label);
+        if (m) {
+            hit = (int)(p0 + __ffs(m) - 1);
+            break;
+        }
+    }
+    if (hit >= 0) {
+        const uint64_t cur = ls.slots[hit];
+        __syncwarp();
+        if (cand >= cur) return;
+        if (lane == 0) ls.slots[hit] = cand;
+        __syncwarp();
+        list_rescan(ls, k, lane);
+        return;
+    }
+    if (lane == 0) lab[*ls.wpos] = label;
+    list_admit(ls, k, cand, lane);
+}
+
+// One CTA.  buf[0, n): composites in ascending order, kEmptySlot entries last (n <= 32 * blockDim.x).  Writes the first k
+// composites whose label (id_to_label[row]) does not occur earlier in buf to out[0, k), kEmptySlot after them, and returns the
+// number of distinct labels in buf to every thread.  Scratch in shared memory: lab [n], cnt [blockDim.x + 1].
+__device__ uint32_t first_distinct_labels(const uint64_t *buf, uint32_t n, const uint64_t *__restrict__ id_to_label, uint32_t k,
+                                          uint64_t *out, uint64_t *lab, uint32_t *cnt) {
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) lab[i] = buf[i] == kEmptySlot ? kEmptySlot : id_to_label[(uint32_t)buf[i]];
+    __syncthreads();
+    // each thread owns a contiguous chunk of positions: its first occurrences as a bit mask, then one exclusive scan of the counts
+    const uint32_t per = (n + blockDim.x - 1) / blockDim.x, i0 = min(n, threadIdx.x * per), i1 = min(n, i0 + per);
+    uint32_t mine = 0;
+    for (uint32_t i = i0; i < i1; i++) {
+        if (buf[i] == kEmptySlot) break;
+        const uint64_t l = lab[i];
+        bool first = true;
+        for (uint32_t j = 0; j < i && first; j++) first = lab[j] != l;
+        if (first) mine |= 1u << (i - i0);
+    }
+    cnt[threadIdx.x] = __popc(mine);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t s = 0;
+        for (uint32_t t = 0; t < blockDim.x; t++) {
+            const uint32_t c = cnt[t];
+            cnt[t] = s;
+            s += c;
+        }
+        cnt[blockDim.x] = s;
+    }
+    __syncthreads();
+    uint32_t r = cnt[threadIdx.x];
+    for (uint32_t i = i0; i < i1; i++)
+        if ((mine >> (i - i0)) & 1u) {
+            if (r < k) out[r] = buf[i];
+            r++;
+        }
+    const uint32_t total = cnt[blockDim.x];
+    for (uint32_t p = total + threadIdx.x; p < k; p += blockDim.x) out[p] = kEmptySlot;
+    __syncthreads(); // lab / cnt may be reused
+    return total;
+}
+
 // ------------------------------------------------------------------------------------------------
 // fused scan + top-k
 // ------------------------------------------------------------------------------------------------
@@ -89,9 +160,11 @@ struct ScanArgs {
     const uint32_t *q_ok; // optional: queries already answered (coarse path verified) are skipped
     const uint32_t *abort; // optional (mapped host memory): non-zero = the caller has left (timeout), stop scanning
     uint32_t poll_mask;    // the flag is read every poll_mask + 1 tiles of a warp
+    const uint64_t *id_to_label; // LAB: row -> label; the lists hold distinct labels (multi-value index)
 };
 
-template <int DT, int MT, int RT, int QT, bool QSMEM>
+// LAB: label-aware lists (list_admit_label), a label per slot in shared memory after the slots
+template <int DT, int MT, int RT, int QT, bool QSMEM, bool LAB>
 __global__ void __launch_bounds__(kScanThreads) scan_topk_kernel(const ScanArgs a) {
     extern __shared__ __align__(16) uint8_t smem[];
     using Tile = DistTile<DT, MT, RT, QT>;
@@ -106,7 +179,8 @@ __global__ void __launch_bounds__(kScanThreads) scan_topk_kernel(const ScanArgs 
     const size_t qs_bytes = QSMEM ? (size_t)WQ * QT * a.q_smem_pitch : 0;
     uint8_t *qs = smem;
     uint64_t *slots = reinterpret_cast<uint64_t *>(smem + qs_bytes);
-    uint64_t *worst = slots + (size_t)kScanWarps * QT * k;
+    uint64_t *slab = slots + (size_t)kScanWarps * QT * k; // LAB only
+    uint64_t *worst = slab + (LAB ? (size_t)kScanWarps * QT * k : 0);
     uint32_t *wpos = reinterpret_cast<uint32_t *>(worst + kScanWarps * QT);
 
     if (QSMEM) {
@@ -121,6 +195,8 @@ __global__ void __launch_bounds__(kScanThreads) scan_topk_kernel(const ScanArgs 
     {
         uint64_t *my = slots + (size_t)warp * QT * k;
         for (uint32_t p = lane; p < QT * k; p += 32) my[p] = kEmptySlot;
+        if (LAB)
+            for (uint32_t p = lane; p < QT * k; p += 32) slab[(size_t)warp * QT * k + p] = kEmptySlot;
         if (lane < QT) {
             worst[warp * QT + lane] = kEmptySlot;
             wpos[warp * QT + lane] = 0;
@@ -175,7 +251,11 @@ __global__ void __launch_bounds__(kScanThreads) scan_topk_kernel(const ScanArgs 
                     const uint64_t c = shfl_u64(comp, src);
                     const uint32_t js = __shfl_sync(0xffffffffu, j, src);
                     ListState ls{slots + ((size_t)warp * QT + js) * k, worst + warp * QT + js, wpos + warp * QT + js};
-                    if (c < *ls.worst) list_admit(ls, k, c, lane);
+                    if (LAB) {
+                        if (c < *ls.worst) list_admit_label(ls, slab + ((size_t)warp * QT + js) * k, k, c, a.id_to_label[(uint32_t)c], lane);
+                    } else if (c < *ls.worst) {
+                        list_admit(ls, k, c, lane);
+                    }
                 }
             }
         }
@@ -227,6 +307,63 @@ __global__ void __launch_bounds__(kScanThreads) final_select_kernel(const uint64
     }
     bitonic_sort_smem(sortbuf, sortn);
     for (uint32_t p = threadIdx.x; p < k; p += blockDim.x) out[(size_t)blockIdx.x * k + p] = sortbuf[p];
+}
+
+// The same over label-aware lists (multi-value index): each warp keeps the k best distinct labels of its share, and the first k
+// distinct labels of the sorted union are the answer (per-list dedup, DESIGN.md §4.4).  out: (score, best row) composites.
+__global__ void __launch_bounds__(kScanThreads) final_select_labels_kernel(const uint64_t *__restrict__ cand, uint32_t m, uint32_t k,
+                                                                           const uint64_t *__restrict__ id_to_label,
+                                                                           uint64_t *__restrict__ out) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t sortn = next_pow2(kScanWarps * k);
+    uint64_t *sortbuf = reinterpret_cast<uint64_t *>(smem); // [sortn]; first 8*k double as the lists
+    uint64_t *lab = sortbuf + sortn;                        // [sortn]: labels of the lists, then of the sorted entries
+    uint64_t *worst = lab + sortn;
+    uint32_t *wpos = reinterpret_cast<uint32_t *>(worst + kScanWarps);
+    uint32_t *cnt = wpos + kScanWarps; // [kScanThreads + 1]
+    const uint64_t *src = cand + (size_t)blockIdx.x * m;
+
+    for (uint32_t p = threadIdx.x; p < sortn; p += blockDim.x) sortbuf[p] = lab[p] = kEmptySlot;
+    if (threadIdx.x < kScanWarps) {
+        worst[threadIdx.x] = kEmptySlot;
+        wpos[threadIdx.x] = 0;
+    }
+    __syncthreads();
+    ListState ls{sortbuf + (size_t)warp * k, worst + warp, wpos + warp};
+    for (uint32_t base = warp * 32; base < m; base += kScanThreads) {
+        const uint32_t i = base + lane;
+        const uint64_t c = (i < m) ? src[i] : kEmptySlot;
+        unsigned pending = __ballot_sync(0xffffffffu, c < *ls.worst);
+        while (pending) {
+            const int s = __ffs(pending) - 1;
+            pending &= pending - 1;
+            const uint64_t cc = shfl_u64(c, s);
+            if (cc < *ls.worst) list_admit_label(ls, lab + (size_t)warp * k, k, cc, id_to_label[(uint32_t)cc], lane);
+        }
+    }
+    bitonic_sort_smem(sortbuf, sortn);
+    first_distinct_labels(sortbuf, sortn, id_to_label, k, out + (size_t)blockIdx.x * k, lab, cnt);
+}
+
+// Label stage after a row-level route (DESIGN.md §4.4), one CTA per query: rows[q] holds the query's K best rows, ascending.  The
+// first kl distinct labels go to out[q] ([nq][kl], kEmptySlot after them).  The selection is proven iff the K rows hold at least
+// kl distinct labels: lab_ok[q] = 1, flags[q] = the row stage's flag (row_ok[q], 1 without one); otherwise lab_ok[q] = 0 and
+// flags[q] = 3 (the label-aware exact scan answers the query).
+__global__ void __launch_bounds__(128) label_select_kernel(const uint64_t *__restrict__ rows, uint32_t K, const uint64_t *__restrict__ id_to_label,
+                                                           uint32_t kl, const uint32_t *__restrict__ row_ok, uint64_t *__restrict__ out,
+                                                           uint32_t *__restrict__ lab_ok, uint32_t *__restrict__ flags) {
+    __shared__ uint64_t buf[kMaxFusedK], lab[kMaxFusedK];
+    __shared__ uint32_t cnt[129];
+    const uint32_t q = blockIdx.x;
+    for (uint32_t i = threadIdx.x; i < K; i += blockDim.x) buf[i] = rows[(size_t)q * K + i];
+    __syncthreads();
+    const uint32_t distinct = first_distinct_labels(buf, K, id_to_label, kl, out + (size_t)q * kl, lab, cnt);
+    if (threadIdx.x == 0) {
+        const bool pass = distinct >= kl;
+        lab_ok[q] = pass ? 1u : 0u;
+        flags[q] = pass ? (row_ok ? row_ok[q] : 1u) : 3u;
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -426,43 +563,57 @@ static int occupancy(K kernel, size_t smem) {
 
 constexpr size_t kMaxQuerySmem = 96 * 1024; // beyond this the batched scan reads queries through L1
 
-ScanPlan plan_scan_topk(const CorpusView &c, uint32_t nq, uint32_t k) {
+constexpr size_t kMaxScanSmem = 227 * 1024; // opt-in shared memory per CTA on sm_90
+
+ScanPlan plan_scan_topk(const CorpusView &c, uint32_t nq, uint32_t k, bool labels) {
     ScanPlan p{};
     p.qt = (nq == 1) ? 1 : 8;
+    p.labels = labels;
     uint32_t groups = (nq + p.qt - 1) / p.qt;
     p.wq = groups >= 8 ? 8 : groups >= 4 ? 4 : groups >= 2 ? 2 : 1;
+    const uint32_t qsp = round16(query_blob_bytes(c));
     p.grid_y = (groups + p.wq - 1) / p.wq;
     const uint32_t wr = kScanWarps / p.wq;
-    const uint32_t qsp = round16(query_blob_bytes(c));
+    // label-aware lists (multi-value index) carry a 64-bit label per slot: at k = 128 and 8 queries per warp that is 64 KB more,
+    // 226 KB with 96 KB of staged queries; queries that would not fit are read through L1
+    const size_t lists = (size_t)kScanWarps * p.qt * k * (labels ? 16 : 8) + (size_t)kScanWarps * p.qt * 12;
     size_t qs = (size_t)p.wq * p.qt * qsp;
-    if (qs > kMaxQuerySmem) qs = 0;
-    p.smem_bytes = qs + (size_t)kScanWarps * p.qt * k * 8 + (size_t)kScanWarps * p.qt * 12;
+    if (qs > kMaxQuerySmem || qs + lists > kMaxScanSmem) qs = 0;
+    p.q_smem = qs != 0;
+    p.smem_bytes = qs + lists;
     // persistent grid: resident CTAs only, split evenly over the query slices
     const int sms = device_sm_count();
     const uint32_t rt = 4;
     const uint32_t ntiles = (c.n_rows + rt - 1) / rt;
     uint32_t want = (ntiles + wr - 1) / wr;
-    uint32_t resident = (uint32_t)sms * 2u; // refined at launch time from the occupancy API
+    uint32_t resident = (uint32_t)sms * 2u;
+    if (labels) // as many CTAs as the shared memory of an SM holds (228 KB, 1 KB reserved per CTA): one at k = 128
+        resident = (uint32_t)sms * (uint32_t)std::max<size_t>(1, std::min<size_t>(2, (228 * 1024) / (p.smem_bytes + 1024)));
     p.grid_x = std::max(1u, std::min(want, std::max(1u, resident / p.grid_y)));
     p.lists_per_query = p.grid_x * wr;
     p.cand_elems = (size_t)nq * p.lists_per_query * k;
     return p;
 }
 
-template <int DT, int MT, int RT, int QT, bool QSMEM>
+template <int DT, int MT, int RT, int QT, bool QSMEM, bool LAB>
 static cudaError_t launch_scan_inst(const ScanArgs &a, const ScanPlan &plan, cudaStream_t s) {
-    auto kern = scan_topk_kernel<DT, MT, RT, QT, QSMEM>;
+    auto kern = scan_topk_kernel<DT, MT, RT, QT, QSMEM, LAB>;
     cudaError_t e = ensure_smem(kern, plan.smem_bytes);
     if (e != cudaSuccess) return e;
     kern<<<dim3(plan.grid_x, plan.grid_y), kScanThreads, plan.smem_bytes, s>>>(a);
     return cudaGetLastError();
 }
 
+template <int DT, int MT, bool LAB>
+static cudaError_t launch_scan_dml(const ScanArgs &a, const ScanPlan &plan, cudaStream_t s) {
+    if (plan.qt == 1) return launch_scan_inst<DT, MT, 4, 1, true, LAB>(a, plan, s);
+    if (plan.q_smem) return launch_scan_inst<DT, MT, 4, 8, true, LAB>(a, plan, s);
+    return launch_scan_inst<DT, MT, 4, 8, false, LAB>(a, plan, s);
+}
+
 template <int DT, int MT>
-static cudaError_t launch_scan_dm(const ScanArgs &a, const ScanPlan &plan, bool qsmem, cudaStream_t s) {
-    if (plan.qt == 1) return launch_scan_inst<DT, MT, 4, 1, true>(a, plan, s);
-    if (qsmem) return launch_scan_inst<DT, MT, 4, 8, true>(a, plan, s);
-    return launch_scan_inst<DT, MT, 4, 8, false>(a, plan, s);
+static cudaError_t launch_scan_dm(const ScanArgs &a, const ScanPlan &plan, cudaStream_t s) {
+    return plan.labels ? launch_scan_dml<DT, MT, true>(a, plan, s) : launch_scan_dml<DT, MT, false>(a, plan, s);
 }
 
 #define RSB_DISPATCH_DM(dtype, metric, CALL)                                                         \
@@ -504,8 +655,9 @@ cudaError_t launch_blend(const uint32_t *d_ok, const uint64_t *d_a, const uint64
 
 cudaError_t launch_scan_topk(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t k,
                              const ScanPlan &plan, uint64_t *d_cand, cudaStream_t s, LaunchCounters *ctr,
-                             const uint32_t *d_q_ok, const uint32_t *d_abort) {
+                             const uint32_t *d_q_ok, const uint32_t *d_abort, const uint64_t *d_id_to_label) {
     if (nq == 0 || k == 0 || k > (uint32_t)kMaxFusedK || c.n_rows == 0) return cudaErrorInvalidValue;
+    if (plan.labels != (d_id_to_label != nullptr)) return cudaErrorInvalidValue;
     ScanArgs a{};
     a.rows = static_cast<const uint8_t *>(c.rows);
     a.pitch = c.pitch;
@@ -522,9 +674,9 @@ cudaError_t launch_scan_topk(const CorpusView &c, const void *d_queries, size_t 
     a.q_ok = d_q_ok;
     a.abort = d_abort;
     a.poll_mask = nq >= 16 ? 15u : 255u; // a batched tile costs ~100x a single-query tile: keep the reaction time in milliseconds
-    const bool qsmem = (size_t)plan.wq * plan.qt * a.q_smem_pitch <= kMaxQuerySmem;
+    a.id_to_label = d_id_to_label;
     cudaError_t e = cudaErrorInvalidValue;
-#define CALL_SCAN(DT, MT) e = launch_scan_dm<DT, MT>(a, plan, qsmem, s)
+#define CALL_SCAN(DT, MT) e = launch_scan_dm<DT, MT>(a, plan, s)
     RSB_DISPATCH_DM(c.dtype, c.metric, CALL_SCAN)
 #undef CALL_SCAN
     if (ctr) ctr->launches++;
@@ -536,6 +688,28 @@ cudaError_t launch_final_select(const uint64_t *d_cand, uint32_t nq, uint32_t m_
     if (k == 0 || k > (uint32_t)kMaxFusedK) return cudaErrorInvalidValue;
     const size_t smem = (size_t)next_pow2(kScanWarps * k) * 8 + kScanWarps * 12;
     final_select_kernel<<<nq, kScanThreads, smem, s>>>(d_cand, m_per_query, k, d_out, d_nq_dev);
+    if (ctr) ctr->launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_final_select_labels(const uint64_t *d_cand, uint32_t nq, uint32_t m_per_query, uint32_t k, const uint64_t *d_id_to_label,
+                                       uint64_t *d_out, cudaStream_t s, LaunchCounters *ctr) {
+    if (k == 0 || k > (uint32_t)kMaxFusedK || !d_id_to_label) return cudaErrorInvalidValue;
+    if (nq == 0) return cudaSuccess;
+    const size_t smem = (size_t)next_pow2(kScanWarps * k) * 16 + kScanWarps * 12 + (kScanThreads + 1) * 4;
+    cudaError_t e = ensure_smem(final_select_labels_kernel, smem);
+    if (e != cudaSuccess) return e;
+    final_select_labels_kernel<<<nq, kScanThreads, smem, s>>>(d_cand, m_per_query, k, d_id_to_label, d_out);
+    if (ctr) ctr->launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_label_select(const uint64_t *d_rows, uint32_t nq, uint32_t K, const uint64_t *d_id_to_label, uint32_t kl,
+                                const uint32_t *d_row_ok, uint64_t *d_out, uint32_t *d_lab_ok, uint32_t *d_flags, cudaStream_t s,
+                                LaunchCounters *ctr) {
+    if (K == 0 || K > (uint32_t)kMaxFusedK || kl == 0 || kl > K || !d_id_to_label) return cudaErrorInvalidValue;
+    if (nq == 0) return cudaSuccess;
+    label_select_kernel<<<nq, 128, 0, s>>>(d_rows, K, d_id_to_label, kl, d_row_ok, d_out, d_lab_ok, d_flags);
     if (ctr) ctr->launches++;
     return cudaGetLastError();
 }

@@ -34,12 +34,28 @@ struct ScanPlan {
     uint32_t grid_x, grid_y, wq, qt, lists_per_query;
     size_t smem_bytes;
     size_t cand_elems; // uint64 elements needed in d_cand
+    bool labels;       // label-aware lists (multi-value index)
+    bool q_smem;       // the queries are staged in shared memory
 };
-ScanPlan plan_scan_topk(const CorpusView &c, uint32_t nq, uint32_t k);
+// labels: plan the label-aware variant (lists of distinct labels, a label per slot in shared memory)
+ScanPlan plan_scan_topk(const CorpusView &c, uint32_t nq, uint32_t k, bool labels = false);
 // d_queries: nq device blobs, qpitch bytes apart, already in stored form (normalised etc.).
+// d_id_to_label (label-aware plans only, else NULL): row -> label; each list then holds the k best distinct labels it has seen,
+// each at its best (score, row) composite (DESIGN.md §4.4), to be reduced with launch_final_select_labels.
 cudaError_t launch_scan_topk(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq,
                              uint32_t k, const ScanPlan &plan, uint64_t *d_cand, cudaStream_t s,
-                             LaunchCounters *ctr, const uint32_t *d_q_ok = nullptr, const uint32_t *d_abort = nullptr);
+                             LaunchCounters *ctr, const uint32_t *d_q_ok = nullptr, const uint32_t *d_abort = nullptr,
+                             const uint64_t *d_id_to_label = nullptr);
+// label-aware lists -> per query the first k distinct labels of the sorted union, as (score, best row) composites, ascending,
+// kEmptySlot-padded
+cudaError_t launch_final_select_labels(const uint64_t *d_cand, uint32_t nq, uint32_t m_per_query, uint32_t k, const uint64_t *d_id_to_label,
+                                       uint64_t *d_out, cudaStream_t s, LaunchCounters *ctr);
+// Label stage after a row-level route: d_rows [nq][K] ascending composites -> d_out [nq][kl], the first kl distinct labels.
+// d_lab_ok[q] = 1 iff the K rows hold at least kl distinct labels (the selection is then exact); d_flags[q] = d_row_ok[q] (1 if
+// d_row_ok is NULL) when it holds, else 3.
+cudaError_t launch_label_select(const uint64_t *d_rows, uint32_t nq, uint32_t K, const uint64_t *d_id_to_label, uint32_t kl,
+                                const uint32_t *d_row_ok, uint64_t *d_out, uint32_t *d_lab_ok, uint32_t *d_flags, cudaStream_t s,
+                                LaunchCounters *ctr);
 // out[q] = ok[q] ? a[q] : b[q] for [nq][k] composite arrays
 cudaError_t launch_blend(const uint32_t *d_ok, const uint64_t *d_a, const uint64_t *d_b, uint32_t nq, uint32_t k, uint64_t *d_out,
                          cudaStream_t s, LaunchCounters *ctr);
