@@ -519,7 +519,8 @@ int VecSimB200_ShardGroup_TopKBatch(VecSimB200_ShardGroup *g, VecSimIndex *shard
  * object with the reference's QueryIterator vtable (iterator_api.h:46-151) — a device AND / OR result or a host iterator; it
  * is NOT freed.  The k best are kept in the reference's heap order (cmpVecSimResByScore :35-44) and written ordered by
  * (score, docId).  *out_mode = VecSearchMode the query ended in (also VecSimIndex's LAST_SEARCH_MODE), *out_iterations =
- * batches run.  Returns a VecSimQueryReply_Code, or -1.  Exact score ties at the k-th place in ad-hoc mode resolve towards
+ * batches run.  Multi-value indexes are served in every mode (ad-hoc mode through VecSimB200_TopKFiltered's fold).
+ * Returns a VecSimQueryReply_Code, or -1 (also for labels too sparse for ad-hoc mode).  Exact score ties at the k-th place in ad-hoc mode resolve towards
  * the smaller docId (the reference's min-max heap evicts the smaller docId among tied worst entries). */
 int VecSimB200_HybridTopK(VecSimIndex *index, const void *queryBlob, size_t k, void *child_iterator, VecSimQueryParams *queryParams,
                           size_t *out_labels, double *out_scores, size_t *out_count, int *out_mode, size_t *out_iterations);
@@ -528,13 +529,18 @@ int VecSimB200_HybridTopK(VecSimIndex *index, const void *queryBlob, size_t k, v
  * keep the k best in a heap with strict `<` admission, skip NaN = deleted) — in one call.  doc_ids: the filter's
  * ascending docIds (= vector labels), on the host or on the device (ids_on_device != 0, e.g.
  * II_ResultSet_DeviceDocIds of the filter's AND/OR).  Writes up to k (label, distance) pairs ordered by
- * (distance asc, docId asc) and their number.  Returns 0; -2 if the index cannot serve it (multi-value index, or
- * labels too sparse for the dense docId -> row table) — the caller then stays on VecSimIndex_GetDistanceFrom_Unsafe. */
+ * (distance asc, docId asc) and their number.  Multi-value indexes are served: a docId's distance is getDistanceFrom_Unsafe's
+ * fold over its rows (brute_force_multi.h:224-241, dist = (dist < d) ? dist : d from +inf in insertion order, so a NaN in the
+ * label's last row makes it NaN and the docId is skipped).  Returns 0; -2 if the labels are too sparse for the dense docId ->
+ * rows table (a label >= 2^32 - 1, or beyond 4 x rows + 2^24) or n exceeds the 32-bit id range — the caller then stays on
+ * VecSimIndex_GetDistanceFrom_Unsafe. */
 int VecSimB200_TopKFiltered(VecSimIndex *index, const void *queryBlob, size_t k, const uint32_t *doc_ids, size_t n, int ids_on_device,
                             size_t *out_labels, double *out_scores, size_t *out_count);
 /* The same for nq hybrid queries in one call (k <= 128): queryBlobs[i] with the DEVICE-resident ascending docId list
  * d_doc_ids[i] of counts[i] entries (its filter's AND / OR result).  Every query's kernel chain is enqueued on its own stream
- * before anything is waited for.  out_labels / out_scores are [nq][k], out_counts[i] the entries written for query i. */
+ * before anything is waited for.  out_labels / out_scores are [nq][k], out_counts[i] the entries written for query i.
+ * Multi-value indexes as in VecSimB200_TopKFiltered.  Returns 0; -2 for sparse labels, k > 128 or a list beyond the 32-bit id
+ * range. */
 int VecSimB200_TopKFilteredBatch(VecSimIndex *index, const void *const *queryBlobs, size_t nq, size_t k, const uint32_t *const *d_doc_ids,
                                  const size_t *counts, size_t *out_labels, double *out_scores, size_t *out_counts);
 /* Batched fp32 queries (cosine, and in mode 1 also L2 and raw inner product; nq >= 16, k <= 16, dim % 8 == 0,

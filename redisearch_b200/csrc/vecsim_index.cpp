@@ -231,6 +231,7 @@ FlatIndex::~FlatIndex() {
     cudaFree(d_norm2_);
     cudaFree(d_stats_);
     cudaFree(d_label_to_id_);
+    cudaFree(d_label_rows_);
     cudaFree(d_id_to_label_);
     cudaFreeHost(h_stage_);
 }
@@ -1709,16 +1710,37 @@ bool FlatIndex::sync_label_table() {
     for (size_t i = 0; i < count_; i++) max_label = std::max(max_label, id_to_label_[i]);
     if (max_label > 4 * count_ + (1u << 24) || max_label >= 0xFFFFFFFFull) return false; // sparse labels: no dense table
     const size_t size = max_label + 1;
-    std::vector<uint32_t> tab(size, 0xFFFFFFFFu);
-    for (size_t i = 0; i < count_; i++) tab[id_to_label_[i]] = (uint32_t)i;
-    if (size > l2i_cap_) {
+    // single-value: row of each label (0xFFFFFFFF = absent); multi-value: CSR offsets [size + 1] over `rows`
+    const size_t entries = multi_ ? size + 1 : size;
+    std::vector<uint32_t> tab(entries, multi_ ? 0u : 0xFFFFFFFFu);
+    std::vector<uint32_t> rows;
+    if (multi_) {
+        for (const auto &kv : label_to_ids_) tab[kv.first + 1] = (uint32_t)kv.second.size();
+        for (size_t l = 0; l < size; l++) tab[l + 1] += tab[l];
+        rows.resize(count_);
+        for (const auto &kv : label_to_ids_)
+            std::copy(kv.second.begin(), kv.second.end(), rows.begin() + tab[kv.first]);
+    } else {
+        for (size_t i = 0; i < count_; i++) tab[id_to_label_[i]] = (uint32_t)i;
+    }
+    if (entries > l2i_cap_) {
         cudaFree(d_label_to_id_);
         d_label_to_id_ = nullptr;
-        const size_t cap = size + size / 4 + 1024;
+        const size_t cap = entries + entries / 4 + 1024;
         CU_OK(cudaMalloc(&d_label_to_id_, cap * 4));
         l2i_cap_ = cap;
     }
-    CU_OK(cudaMemcpy(d_label_to_id_, tab.data(), size * 4, cudaMemcpyHostToDevice));
+    CU_OK(cudaMemcpy(d_label_to_id_, tab.data(), entries * 4, cudaMemcpyHostToDevice));
+    if (multi_) {
+        if (rows.size() > label_rows_cap_ || !d_label_rows_) {
+            cudaFree(d_label_rows_);
+            d_label_rows_ = nullptr;
+            const size_t cap = rows.size() + rows.size() / 4 + 1024;
+            CU_OK(cudaMalloc(&d_label_rows_, cap * 4));
+            label_rows_cap_ = cap;
+        }
+        CU_OK(cudaMemcpy(d_label_rows_, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice));
+    }
     l2i_size_ = size;
     l2i_dirty_ = false;
     return true;
@@ -1729,7 +1751,7 @@ int FlatIndex::topk_filtered(const void *q, size_t k, const uint32_t *doc_ids, s
     *out_count = 0;
     last_mode_ = HYBRID_ADHOC_BF;
     if (k == 0 || n == 0) return 0;
-    if (multi_ || n > 0xFFFFFFF0ull) return -2;
+    if (n > 0xFFFFFFF0ull) return -2;
     if (!flush()) return -1;
     if (count_ == 0) return 0;
     if (!sync_label_table()) return -2;
@@ -1749,8 +1771,13 @@ int FlatIndex::topk_filtered(const void *q, size_t k, const uint32_t *doc_ids, s
         ok = cudaMemcpyAsync(c->d_ids + n, doc_ids, n * 4, cudaMemcpyHostToDevice, c->stream) == cudaSuccess;
         d_labels = c->d_ids + n;
     }
-    ok = ok && launch_map_labels(d_labels, (uint32_t)n, d_label_to_id_, (uint32_t)l2i_size_, c->d_ids, c->stream, &lc) == cudaSuccess;
-    ok = ok && launch_gather_distances(view(), c->d_query, c->d_ids, (uint32_t)n, c->d_scores, c->stream, &lc) == cudaSuccess;
+    if (multi_) { // one score per docId: the min fold over its rows (DESIGN.md §4.4)
+        ok = ok && launch_gather_min_distances(view(), c->d_query, d_labels, (uint32_t)n, d_label_to_id_, (uint32_t)l2i_size_, d_label_rows_,
+                                               c->d_scores, c->stream, &lc) == cudaSuccess;
+    } else {
+        ok = ok && launch_map_labels(d_labels, (uint32_t)n, d_label_to_id_, (uint32_t)l2i_size_, c->d_ids, c->stream, &lc) == cudaSuccess;
+        ok = ok && launch_gather_distances(view(), c->d_query, c->d_ids, (uint32_t)n, c->d_scores, c->stream, &lc) == cudaSuccess;
+    }
     launches_total_ += lc.launches;
     if (!ok) {
         checkin(std::move(c));
@@ -1793,7 +1820,7 @@ int FlatIndex::topk_filtered_batch(const void *const *queries, size_t nq, size_t
     for (size_t i = 0; i < nq; i++) out_counts[i] = 0;
     last_mode_ = HYBRID_ADHOC_BF;
     if (k == 0 || nq == 0) return 0;
-    if (multi_ || k > (size_t)kMaxFusedK) return -2;
+    if (k > (size_t)kMaxFusedK) return -2;
     if (!flush()) return -1;
     if (count_ == 0) return 0;
     if (!sync_label_table()) return -2;
@@ -1833,8 +1860,13 @@ int FlatIndex::topk_filtered_batch(const void *const *queries, size_t nq, size_t
                 ok = upload_query(c, c.h_query, 1);
             }
             const uint32_t *d_labels = d_doc_ids[qi];
-            ok = ok && launch_map_labels(d_labels, (uint32_t)n, d_label_to_id_, (uint32_t)l2i_size_, c.d_ids, c.stream, &lc) == cudaSuccess;
-            ok = ok && launch_gather_distances(view(), c.d_query, c.d_ids, (uint32_t)n, c.d_scores, c.stream, &lc) == cudaSuccess;
+            if (multi_) {
+                ok = ok && launch_gather_min_distances(view(), c.d_query, d_labels, (uint32_t)n, d_label_to_id_, (uint32_t)l2i_size_,
+                                                       d_label_rows_, c.d_scores, c.stream, &lc) == cudaSuccess;
+            } else {
+                ok = ok && launch_map_labels(d_labels, (uint32_t)n, d_label_to_id_, (uint32_t)l2i_size_, c.d_ids, c.stream, &lc) == cudaSuccess;
+                ok = ok && launch_gather_distances(view(), c.d_query, c.d_ids, (uint32_t)n, c.d_scores, c.stream, &lc) == cudaSuccess;
+            }
             ok = ok && launch_select_scores(c.d_scores, (uint32_t)n, nullptr, (uint32_t)j.want, c.d_cand, c.stream, &lc) == cudaSuccess;
             ok = ok && launch_final_select(c.d_cand, 1, lists * (uint32_t)j.want, (uint32_t)j.want, c.d_out, c.stream, &lc) == cudaSuccess;
             ok = ok && cudaMemcpyAsync(c.h_out, c.d_out, j.want * 8, cudaMemcpyDeviceToHost, c.stream) == cudaSuccess;

@@ -252,9 +252,13 @@ class FlatIndex {
     uint64_t *d_id_to_label_ = nullptr;
     size_t d_labels_cap_ = 0;
     bool labels_dirty_ = true;
-    // dense label -> row id table on the device (labels are RediSearch docIds: small integers), for topk_filtered
+    // dense label -> row id table on the device (labels are RediSearch docIds: small integers), for topk_filtered.  A multi-value
+    // index keeps a CSR table instead: d_label_to_id_ holds offsets [l2i_size_ + 1], d_label_rows_ the rows [count_] of each label
+    // in label_to_ids_ order (the order the reference's min fold visits them).  l2i_size_ = largest label + 1.
     uint32_t *d_label_to_id_ = nullptr;
     size_t l2i_size_ = 0, l2i_cap_ = 0;
+    uint32_t *d_label_rows_ = nullptr;
+    size_t label_rows_cap_ = 0;
     bool l2i_dirty_ = true;
     bool sync_label_table();
 

@@ -7,6 +7,7 @@
 //   select_scores_kernel cursor-select over a score array             (N*4 bytes per pass)
 //   range_compact_kernel scores <= radius -> compacted composites
 //   gather_kernel        distances of listed rows (ad-hoc / hybrid)
+//   gather_min_kernel    min fold over each listed label's rows (hybrid, multi-value index)
 //   unpack / merge       reply formatting, G-way shard merge
 //
 // Replaces, on device: BruteForceIndex::topKQuery (VS/algorithms/brute_force/brute_force.h:243-291),
@@ -473,6 +474,45 @@ __global__ void __launch_bounds__(kScanThreads) gather_kernel(const uint8_t *row
     }
 }
 
+// Ad-hoc gather of a multi-value index: one warp per listed label.  The label's rows are
+// label_rows[offsets[l], offsets[l + 1]) in the order the host's label -> ids vector holds them; out[w] is
+// getDistanceFrom_Unsafe's fold over them (brute_force_multi.h:224-241): dist = +inf, then
+// dist = (dist < d) ? dist : d row by row.  Unlike fminf, a NaN row resets dist to NaN and the next
+// row replaces it, so only a NaN in the LAST row survives.  Absent label (out of range or no rows) -> NaN.
+template <int DT, int MT>
+__global__ void __launch_bounds__(kScanThreads) gather_min_kernel(const uint8_t *rows, size_t pitch, uint32_t dim,
+                                                                  const uint8_t *query, uint32_t q_smem_pitch,
+                                                                  const uint32_t *labels, uint32_t count,
+                                                                  const uint32_t *__restrict__ offsets, uint32_t n_labels,
+                                                                  const uint32_t *__restrict__ label_rows, float *out) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    using Tile = DistTile<DT, MT, 1, 1>;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (uint32_t i = threadIdx.x; i < (q_smem_pitch >> 4); i += blockDim.x)
+        reinterpret_cast<uint4 *>(smem)[i] = reinterpret_cast<const uint4 *>(query)[i];
+    __syncthreads();
+    const uint8_t *qb[1] = {smem};
+    for (uint32_t w = blockIdx.x * kScanWarps + warp; w < count; w += gridDim.x * kScanWarps) {
+        const uint32_t l = labels[w];
+        uint32_t r = 0, e = 0;
+        if (l < n_labels) {
+            r = offsets[l];
+            e = offsets[l + 1];
+        }
+        float dist = r < e ? __uint_as_float(0x7F800000u) : __uint_as_float(0x7FC00000u);
+        uint32_t id = r < e ? label_rows[r] : 0u; // the next row id is loaded while this row is scored
+#pragma unroll 1
+        for (; r < e; r++) {
+            const uint8_t *rowb[1] = {rows + (size_t)id * pitch};
+            if (r + 1 < e) id = label_rows[r + 1];
+            float d[1];
+            Tile::run(rowb, qb, dim, lane, d);
+            if (lane == 0) dist = (dist < d[0]) ? dist : d[0];
+        }
+        if (lane == 0) out[w] = dist;
+    }
+}
+
 // ------------------------------------------------------------------------------------------------
 // reply formatting and shard merge
 // ------------------------------------------------------------------------------------------------
@@ -815,6 +855,33 @@ cudaError_t launch_gather_distances(const CorpusView &c, const void *d_query, co
 #define CALL_GATHER(DT, MT) e = launch_gather_inst<DT, MT>(c, d_query, d_ids, count, d_out, s)
     RSB_DISPATCH_DM(c.dtype, c.metric, CALL_GATHER)
 #undef CALL_GATHER
+    if (ctr) ctr->launches++;
+    return e;
+}
+
+template <int DT, int MT>
+static cudaError_t launch_gather_min_inst(const CorpusView &c, const void *d_query, const uint32_t *d_labels, uint32_t count,
+                                          const uint32_t *d_offsets, uint32_t n_labels, const uint32_t *d_label_rows, float *d_out,
+                                          cudaStream_t s) {
+    auto kern = gather_min_kernel<DT, MT>;
+    const uint32_t qsp = round16(query_blob_bytes(c));
+    cudaError_t e = ensure_smem(kern, qsp);
+    if (e != cudaSuccess) return e;
+    const uint32_t want = (count + kScanWarps - 1) / kScanWarps;
+    const uint32_t grid = std::max(1u, std::min(want, (uint32_t)(device_sm_count() * occupancy(kern, qsp))));
+    kern<<<grid, kScanThreads, qsp, s>>>(static_cast<const uint8_t *>(c.rows), c.pitch, c.dim, static_cast<const uint8_t *>(d_query), qsp,
+                                         d_labels, count, d_offsets, n_labels, d_label_rows, d_out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_gather_min_distances(const CorpusView &c, const void *d_query, const uint32_t *d_labels, uint32_t count,
+                                        const uint32_t *d_offsets, uint32_t n_labels, const uint32_t *d_label_rows, float *d_out,
+                                        cudaStream_t s, LaunchCounters *ctr) {
+    if (count == 0) return cudaSuccess;
+    cudaError_t e = cudaErrorInvalidValue;
+#define CALL_GATHER_MIN(DT, MT) e = launch_gather_min_inst<DT, MT>(c, d_query, d_labels, count, d_offsets, n_labels, d_label_rows, d_out, s)
+    RSB_DISPATCH_DM(c.dtype, c.metric, CALL_GATHER_MIN)
+#undef CALL_GATHER_MIN
     if (ctr) ctr->launches++;
     return e;
 }

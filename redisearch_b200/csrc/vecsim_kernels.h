@@ -82,6 +82,11 @@ cudaError_t launch_range_compact(const float *d_scores, uint32_t n, float radius
 // d_ids[i] == 0xFFFFFFFF -> NaN.
 cudaError_t launch_gather_distances(const CorpusView &c, const void *d_query, const uint32_t *d_ids,
                                     uint32_t count, float *d_out, cudaStream_t s, LaunchCounters *ctr);
+// Multi-value index: d_out[i] = the reference's min fold (brute_force_multi.h:224-241) over the rows of label d_labels[i],
+// label_rows[offsets[l], offsets[l + 1]) in insertion order (CSR, offsets has n_labels + 1 entries); NaN for an absent label.
+cudaError_t launch_gather_min_distances(const CorpusView &c, const void *d_query, const uint32_t *d_labels, uint32_t count,
+                                        const uint32_t *d_offsets, uint32_t n_labels, const uint32_t *d_label_rows, float *d_out,
+                                        cudaStream_t s, LaunchCounters *ctr);
 
 // filter-set plumbing of the fused hybrid query: docId -> row id through a dense table; selected positions -> docIds
 cudaError_t launch_map_labels(const uint32_t *d_labels, uint32_t n, const uint32_t *d_table, uint32_t table_size, uint32_t *d_ids,
