@@ -428,7 +428,9 @@ size_t VecSim_GetSharedMemory(void);                                      /* 0, 
  * the number of hits carry label SIZE_MAX and score NaN.  A multi-value index answers the k best
  * labels, each scored by its best row, as VecSimIndex_TopKQuery does (k <= 128: a tensor-core row route
  * + label stage, queries it cannot prove and corpora of >= 65536 rows no such route serves one at a
- * time; the label-aware exact scan below that size; k > 128: one query at a time).  Returns
+ * time; the label-aware exact scan below that size; k > 128: one query at a time).  int8 / uint8 corpora with inner
+ * product, cosine or L2 (nq >= 16, >= 65536 rows, dim % 16 == 0, 32 <= dim <= 2048, k <= 128, coarse mode 1 or 2) take the
+ * s8 / u8 tensor-core route, bit-exact with the reference (ids, score bits and tie order).  Returns
  * VecSim_QueryReply_OK / _TimedOut, or -1 on a CUDA failure. */
 int VecSimB200_TopKQueryBatch(VecSimIndex *index, const void *queryBlobs, size_t qstride, size_t nq,
                               size_t k, VecSimQueryParams *queryParams, size_t *out_labels,
@@ -561,8 +563,8 @@ int VecSimB200_LastCoarseFlags(VecSimIndex *index, uint32_t *out_ok, size_t nq);
 /* Debug: which route the last top-k query (single or batched) took: 0 = exact CUDA-core scan, 1 = tensor-core coarse pass + exact
  * rescoring + proof (fp32 cosine), 2 = tensor-core direct, k <= 128 (csrc/coarse_tc.cu): fp16 / bf16 corpora, inner
  * product or cosine — the fp32-accumulated products of the stored 16-bit values are the distances; int8 / uint8 corpora,
- * inner product or cosine — s8 / u8 wgmma integer dot products are exact and the reference's float expression is applied
- * to them, bit-exact. */
+ * inner product, cosine or L2 — s8 / u8 wgmma integer dot products are exact and the reference's float expression is applied
+ * to them (L2: float(|row|^2 + |q|^2 - 2 dot), evaluated in int32 from exact squared norms), bit-exact. */
 int VecSimB200_LastBatchPath(VecSimIndex *index);
 /* Library/ABI version and the SM arch the kernels were compiled for ("sm_90a"). */
 const char *VecSimB200_Version(void);

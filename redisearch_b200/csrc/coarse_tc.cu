@@ -649,6 +649,10 @@ __device__ __forceinline__ uint32_t select_keep(uint64_t *lists, int q, uint32_t
 //            (IP.cpp:264-271).  The integer dot products are exact, so kOp 1/2 reproduce the reference bit for bit.
 //   kOp = 3  16-bit float operands, squared L2 from the GEMM: (|q|^2 + |row|^2) - 2 dot, with the squared norms of
 //            the fp32 rows / queries in row_norm2 / q_norm2 (coarse stage of the fp32 L2 route)
+//   kOp = 4  int8 / uint8 operands, squared L2: (float)(|row|^2 + |q|^2 - 2 dot) evaluated in int32, with the exact int32
+//            squared norms in row_norm2 / q_norm2 (the pointers carry int32).  The integer is the reference's exact sum
+//            (L2.cpp:148-174), rounded once to float as it is, so kOp 4 is bit-exact too.  Each term is at most
+//            65025 * dim <= 1.4e8 at the widest 8-bit dim (2048): no int32 overflow.
 //   kFixed   the admission threshold of every query is FIXED for the whole pass (thr_fixed[q], a distance, from the sample
 //            pass): every row with approximate distance < thr_fixed[q] is kept — no running threshold, no list compaction;
 //            a list that runs full sets overflow[q] (the query goes to the next tier).  fp32 route only (kOp 0 / 3).
@@ -669,7 +673,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                     uint64_t *__restrict__ list_scratch, uint64_t *__restrict__ cand_out, const uint32_t *__restrict__ nq_dev,
                     uint32_t tile_stride, const float *__restrict__ thr_fixed, uint32_t *__restrict__ overflow) {
     constexpr bool kFixed = kMode == 1, kSample = kMode == 2;
-    constexpr bool kInt = kOp == 1 || kOp == 2;
+    constexpr bool kInt = kOp == 1 || kOp == 2 || kOp == 4;
     using Acc = typename std::conditional<kInt, uint32_t, float>::type;
     // bx = row range, by = query group
     const uint32_t bx = blockIdx.x, by = blockIdx.y, gx = gridDim.x;
@@ -791,6 +795,12 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         float nq_norm = 1.0f;
         if constexpr (kOp == 2) nq_norm = live ? *reinterpret_cast<const float *>(q16 + (size_t)q * q16_pitch + dim) : 1.0f;
         if constexpr (kOp == 3) nq_norm = live ? q_norm2[q] : 0.0f; // |q|^2
+        // kOp 4: the exact int32 |q|^2, and the pre-test bound on the int32 distance e: a row can only pass the key test
+        // (float)e < T if e < T, and every stored T is an integer (a rounded integer), so e < thr_e = T is exact.
+        // INT_MIN: slots without a query never pass (e >= 0)
+        const int *irn2 = reinterpret_cast<const int *>(row_norm2);
+        int nq_int = 0, thr_e = live ? INT_MAX : INT_MIN;
+        if constexpr (kOp == 4) nq_int = live ? reinterpret_cast<const int *>(q_norm2)[q] : 0;
         float smax[kSample ? kSliceSets : 1][kQN / 32]; // kSample: running maxima of the pre-test value per slice (largest = smallest distance)
 #pragma unroll
         for (int x = 0; x < (kSample ? kSliceSets : 1); x++)
@@ -826,6 +836,14 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         for (uint32_t i = 0; i < my_tiles; i++) {
             const uint32_t tile = (bx + i * gx) * tile_stride;
             float nrm[kQN / 32]; // kOp 2 / 3: lane l holds the norm / squared norm of rows h*32 + l of the tile
+            int inrm[kQN / 32];  // kOp 4: the same, int32
+            if constexpr (kOp == 4) {
+#pragma unroll
+                for (int h = 0; h < kQN / 32; h++) {
+                    const uint32_t r = tile * kQN + h * 32 + lane;
+                    inrm[h] = r < n_rows ? __ldg(irn2 + r) : 0;
+                }
+            }
             if constexpr (kOp == 3 && !kFixed) {
 #pragma unroll
                 for (int h = 0; h < kQN / 32; h++) {
@@ -1006,6 +1024,8 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         p = (float)(int)v[h][j] > thr_dot;
                     else if constexpr (kOp == 2)
                         p = (float)(int)v[h][j] > __shfl_sync(0xFFFFFFFFu, nrm[h], j) * thr_dot - 0.01f;
+                    else if constexpr (kOp == 4)
+                        p = __shfl_sync(0xFFFFFFFFu, inrm[h], j) + nq_int - 2 * (int)v[h][j] < thr_e;
                     else // d < d_thr  <=>  dot > |row|^2 / 2 + (|q|^2 - d_thr) / 2, loosened for the rounding of both sides
                         p = __uint_as_float(v[h][j]) > fmaf(__shfl_sync(0xFFFFFFFFu, nrm[h], j), 0.499999f, thr_dot);
                     if (p) pass |= 1u << j;
@@ -1027,6 +1047,8 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         const uint32_t r = row0 + j; // rare path: re-read the norm (L1/L2 hit) instead of a divergent shuffle
                         const float nr = __ldg(reinterpret_cast<const float *>(shadow + (size_t)r * row_pitch + dim));
                         d = __fsub_rn(1.0f, __fdiv_rn((float)(int)raw, __fmul_rn(nr, nq_norm)));
+                    } else if constexpr (kOp == 4) {
+                        d = __int2float_rn(__ldg(irn2 + row0 + j) + nq_int - 2 * (int)raw); // rare path: re-read, as kOp 2
                     } else {
                         d = __fsub_rn(__fadd_rn(nq_norm, __ldg(row_norm2 + row0 + j)), __fmul_rn(2.0f, __uint_as_float(raw)));
                     }
@@ -1056,6 +1078,8 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         else if constexpr (kOp == 2) {
                             const float tq = t * nq_norm;
                             thr_dot = tq - fabsf(tq) * 4e-6f;
+                        } else if constexpr (kOp == 4) {
+                            thr_e = __float2int_ru(key_to_float(thr)); // a finite distance in [0, 2^28]
                         } else {
                             const float dthr = key_to_float(thr);
                             thr_dot = 0.5f * (nq_norm - dthr) - 2e-6f * (fabsf(nq_norm) + fabsf(dthr));
@@ -1508,27 +1532,29 @@ static bool make_map(CUtensorMap *m, CUtensorMapDataType dt, const void *base, u
 static constexpr size_t kSmemLimit = 232448; // 227 KB opt-in maximum of dynamic shared memory per CTA on sm_90
 
 template <int V>
-static const void *wgmma_kernel_fn_v(CoarseKind kind, uint32_t epl, bool int_cos, int mode) {
+static const void *wgmma_kernel_fn_v(CoarseKind kind, uint32_t epl, int epi, int mode) {
     if (kind == CoarseDirect16) {
         if (mode == 1) return (const void *)coarse_wgmma_kernel<true, 8, 0, 1, V>; // fixed bound, lists of 256
         if (mode == 2) return (const void *)coarse_wgmma_kernel<true, 3, 0, 2, V>; // sample pass
         return epl == 3 ? (const void *)coarse_wgmma_kernel<true, 3, 0, 0, V> : (const void *)coarse_wgmma_kernel<true, 8, 0, 0, V>;
     }
     if (kind == CoarseDirect8) {
-        if (int_cos) return epl == 3 ? (const void *)coarse_wgmma_kernel<true, 3, 2, 0, V> : (const void *)coarse_wgmma_kernel<true, 8, 2, 0, V>;
+        if (epi == 2) return epl == 3 ? (const void *)coarse_wgmma_kernel<true, 3, 4, 0, V> : (const void *)coarse_wgmma_kernel<true, 8, 4, 0, V>;
+        if (epi == 1) return epl == 3 ? (const void *)coarse_wgmma_kernel<true, 3, 2, 0, V> : (const void *)coarse_wgmma_kernel<true, 8, 2, 0, V>;
         return epl == 3 ? (const void *)coarse_wgmma_kernel<true, 3, 1, 0, V> : (const void *)coarse_wgmma_kernel<true, 8, 1, 0, V>;
     }
     return nullptr;
 }
-// variant: 16-bit corpora 1 = bf16, 8-bit corpora 1 = int8 (the fp32 route's shadow is always fp16)
-static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, bool int_cos, int mode = 0, uint32_t variant = 0) {
+// variant: 16-bit corpora 1 = bf16, 8-bit corpora 1 = int8 (the fp32 route's shadow is always fp16); epi: CoarseOperands::epilogue
+static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, int epi, int mode = 0, uint32_t variant = 0) {
+    const bool l2 = epi != 0;
     if (kind == CoarseDirect16 || kind == CoarseDirect8)
-        return variant ? wgmma_kernel_fn_v<1>(kind, epl, int_cos, mode) : wgmma_kernel_fn_v<0>(kind, epl, int_cos, mode);
+        return variant ? wgmma_kernel_fn_v<1>(kind, epl, epi, mode) : wgmma_kernel_fn_v<0>(kind, epl, epi, mode);
     // fp32 route (shadow rows): the flag selects the squared-L2 epilogue; epl 8 = lists of up to 128 (second tier);
     // mode 1 = fixed admission bound (lists of 96, no compaction), mode 2 = the sample pass (slice minima only)
-    if (mode == 1) return int_cos ? (const void *)coarse_wgmma_kernel<false, 3, 3, 1> : (const void *)coarse_wgmma_kernel<false, 3, 0, 1>;
-    if (mode == 2) return int_cos ? (const void *)coarse_wgmma_kernel<false, 3, 3, 2> : (const void *)coarse_wgmma_kernel<false, 3, 0, 2>;
-    if (int_cos) return epl == 3 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 0> : (const void *)coarse_wgmma_kernel<false, 8, 3, 0>;
+    if (mode == 1) return l2 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 1> : (const void *)coarse_wgmma_kernel<false, 3, 0, 1>;
+    if (mode == 2) return l2 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 2> : (const void *)coarse_wgmma_kernel<false, 3, 0, 2>;
+    if (l2) return epl == 3 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 0> : (const void *)coarse_wgmma_kernel<false, 8, 3, 0>;
     return epl == 3 ? (const void *)coarse_wgmma_kernel<false, 3, 0, 0> : (const void *)coarse_wgmma_kernel<false, 8, 0, 0>;
 }
 // shared memory of coarse_wgmma_kernel besides the ring: the resident queries, the accumulator transpose (the
@@ -1553,8 +1579,8 @@ bool coarse_supported(const CorpusView &c, uint32_t nq, uint32_t k, CoarseKind k
         if (k > 128 || nq < 1 || c.n_rows < 65536) return false;
         return encode_fn() != nullptr;
     }
-    if (kind == CoarseDirect8) { // int8 / uint8 corpora, inner product or cosine: exact integer dot products on s8 / u8 wgmma
-        if ((c.dtype != DT_I8 && c.dtype != DT_U8) || (c.metric != MT_IP && c.metric != MT_COS)) return false;
+    if (kind == CoarseDirect8) { // int8 / uint8 corpora, inner product, cosine or L2: exact integer dot products on s8 / u8 wgmma
+        if (c.dtype != DT_I8 && c.dtype != DT_U8) return false;
         if (c.dim % 16 != 0 || c.dim < 32 || c.pitch % 16 != 0 || !wgmma_fits_bytes(c.dim)) return false;
         if (k > 128 || nq < 1 || c.n_rows < 65536) return false;
         return encode_fn() != nullptr;
@@ -1605,8 +1631,8 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
                 p.csize = cs;
                 break;
             }
-        const void *kfn = wgmma_kernel_fn(kind, p.epl, kind == CoarseF16 ? c.metric == MT_L2 : c.metric == MT_COS, p.mode,
-                                          (c.dtype == DT_BF16 || c.dtype == DT_I8) ? 1u : 0u);
+        const int epi = kind == CoarseF16 ? (c.metric == MT_L2 ? 1 : 0) : c.metric == MT_COS ? 1 : (kind == CoarseDirect8 && c.metric == MT_L2) ? 2 : 0;
+        const void *kfn = wgmma_kernel_fn(kind, p.epl, epi, p.mode, (c.dtype == DT_BF16 || c.dtype == DT_I8) ? 1u : 0u);
         if (p.csize > 1) {
             cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes);
             cudaLaunchConfig_t cfg{};
@@ -1664,7 +1690,7 @@ cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim
         if (p.mode == 1 && (!d_thr_fixed || !d_overflow)) return cudaErrorInvalidValue;
         // operand variant: 16-bit 1 = bf16 (else fp16); 8-bit 1 = int8 (else uint8); the fp16 shadow of the fp32 route: 0
         const uint32_t ev = (p.kind == CoarseDirect16 || p.kind == CoarseDirect8) && o.elem_variant ? 1u : 0u;
-        const void *kfn = wgmma_kernel_fn(p.kind, p.epl, o.int_cosine != 0, p.mode, ev); // (CoarseF16: the flag selects the L2 epilogue)
+        const void *kfn = wgmma_kernel_fn(p.kind, p.epl, o.epilogue, p.mode, ev);
         cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes);
         if (e != cudaSuccess) {
             fprintf(stderr, "vecsim_b200: coarse pass: %zu bytes of shared memory refused: %s\n", p.smem_bytes, cudaGetErrorString(e));
@@ -1781,6 +1807,39 @@ cudaError_t launch_row_stats(const void *rows, size_t pitch, uint32_t dim, uint3
     if (n == 0) return cudaSuccess;
     const uint32_t grid = std::max(1u, std::min((n + 7) / 8, (uint32_t)device_sm_count() * 8));
     row_stats_kernel<<<grid, 256, 0, s>>>(static_cast<const uint8_t *>(rows), pitch, dim, first, n, d_norm2, d_stats);
+    return cudaGetLastError();
+}
+
+// exact int32 squared norm of int8 / uint8 rows [first, first+n) -> norm2[first + r]; one warp per row, 16 bytes per lane
+// and step (dim % 16 == 0, pitch % 16 == 0).  At most 65025 * 2048 < 2^31.
+template <bool kSigned>
+__global__ void __launch_bounds__(256) int_norm2_kernel(const uint8_t *__restrict__ rows, size_t pitch, uint32_t dim, uint32_t first,
+                                                        uint32_t n, int32_t *__restrict__ norm2) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (uint32_t r = blockIdx.x * 8 + warp; r < n; r += gridDim.x * 8) {
+        const uint8_t *x = rows + (size_t)(first + r) * pitch;
+        int s = 0;
+        for (uint32_t i = lane * 16; i < dim; i += 32 * 16) {
+            const uint4 w = *reinterpret_cast<const uint4 *>(x + i);
+            const uint32_t u[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+            for (int t = 0; t < 4; t++) s = kSigned ? __dp4a((int)u[t], (int)u[t], s) : (int)__dp4a(u[t], u[t], (uint32_t)s);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, o);
+        if (lane == 0) norm2[first + r] = s;
+    }
+}
+cudaError_t launch_int_norm2(const void *rows, size_t pitch, uint32_t dim, uint32_t first, uint32_t n, bool is_signed, int32_t *d_norm2,
+                             cudaStream_t s) {
+    if (n == 0) return cudaSuccess;
+    if (dim % 16 != 0 || pitch % 16 != 0 || dim > 2048) return cudaErrorInvalidValue;
+    const uint32_t grid = std::max(1u, std::min((n + 7) / 8, (uint32_t)device_sm_count() * 8));
+    const uint8_t *r = static_cast<const uint8_t *>(rows);
+    if (is_signed)
+        int_norm2_kernel<true><<<grid, 256, 0, s>>>(r, pitch, dim, first, n, d_norm2);
+    else
+        int_norm2_kernel<false><<<grid, 256, 0, s>>>(r, pitch, dim, first, n, d_norm2);
     return cudaGetLastError();
 }
 

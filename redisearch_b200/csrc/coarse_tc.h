@@ -44,10 +44,10 @@ struct CoarseOperands {
     const void *queries;
     size_t qpitch;
     int elem_variant; // CoarseDirect16: 1 = bfloat16 (else IEEE half); CoarseDirect8: 1 = int8 (else uint8)
-    int int_cosine;   // CoarseDirect8: cosine (rows carry their fp32 norm after the payload) instead of inner product;
-                      // CoarseF16: squared-L2 epilogue (needs the two arrays below)
-    const float *row_norm2; // CoarseF16 / L2: |row|^2 per row (fp32 rows)
-    const float *q_norm2;   //                 |q|^2 per query
+    int epilogue;     // CoarseDirect8: 0 inner product, 1 cosine (rows carry their fp32 norm after the payload), 2 squared L2
+                      // (needs the two arrays below, as int32); CoarseF16: 1 = squared-L2 epilogue (needs the two arrays below)
+    const float *row_norm2; // CoarseF16 / L2: |row|^2 per row (fp32 rows); CoarseDirect8 / L2: exact int32 |row|^2 per row
+    const float *q_norm2;   //                 |q|^2 per query;                CoarseDirect8 / L2: exact int32 |q|^2 per query
 };
 bool coarse_supported(const CorpusView &c, uint32_t nq, uint32_t k, CoarseKind kind);
 // keep_override != 0 (CoarseF16 only): candidates per list instead of the default for k
@@ -101,6 +101,10 @@ cudaError_t launch_range_refine(const CorpusView &c, const void *d_queries, size
 // |row|^2 of fp32 rows [first, first+n) into d_norm2[first..], NaN for a row whose fp16 form is not finite (a component
 // with |x| >= 65520, or NaN: refine_kernel never proves such a query); d_stats (nullable) = {max |row|^2, max |x|} as float bits
 cudaError_t launch_row_stats(const void *rows, size_t pitch, uint32_t dim, uint32_t first, uint32_t n, float *d_norm2, uint32_t *d_stats,
+                             cudaStream_t s);
+// exact int32 |x|^2 of int8 (is_signed) / uint8 rows [first, first+n) into d_norm2[first..] (dim <= 2048: no overflow); serves
+// the corpus rows and the query batch of the 8-bit L2 route
+cudaError_t launch_int_norm2(const void *rows, size_t pitch, uint32_t dim, uint32_t first, uint32_t n, bool is_signed, int32_t *d_norm2,
                              cudaStream_t s);
 
 } // namespace rsb200

@@ -378,7 +378,7 @@ int FlatIndex::add(const void *blob, size_t label) {
             } else {
                 if (cudaMemcpy(d_rows_ + (size_t)id * pitch_, tmp.data(), pitch_, cudaMemcpyHostToDevice) != cudaSuccess)
                     return 0;
-                if (d_shadow_) shadow_dirty_.push_back(id);
+                if (keeps_row_copies()) shadow_dirty_.push_back(id);
             }
             // the overwritten row is the caller's RAW blob: a cosine index may now hold a non-unit row, so the coarse
             // proof must stop assuming unit vectors (it switches to the norm-scaled bound of the inner-product route)
@@ -473,7 +473,7 @@ int FlatIndex::remove(size_t label) {
             const size_t last_label = id_to_label_[last];
             cudaMemcpyAsync(d_rows_ + (size_t)id * pitch_, d_rows_ + (size_t)last * pitch_, pitch_,
                             cudaMemcpyDeviceToDevice, copy_stream_);
-            if (d_shadow_) shadow_dirty_.push_back(id);
+            if (keeps_row_copies()) shadow_dirty_.push_back(id);
             id_to_label_[id] = last_label;
             if (multi_) {
                 auto &v = label_to_ids_[last_label];
@@ -783,9 +783,24 @@ bool FlatIndex::single_query_takes_coarse(uint32_t ke, const float *host_query) 
 // Bring the fp16 shadow copy of the rows up to date on `st` (rows appended, overwritten or moved by a
 // swap-delete since the last coarse batch).  Returns false if HBM for the shadow cannot be had; the
 // caller then runs the TF32 variant on the fp32 rows.
+// int8 / uint8 L2 indexes keep no shadow, only the exact int32 |row|^2 of every row, under the same bookkeeping.
 bool FlatIndex::ensure_shadow(cudaStream_t st) {
     std::lock_guard<std::mutex> g(mu_);
-    if (shadow_cap_ < count_ || !d_shadow_) {
+    const bool inorm = int_l2();
+    if (inorm && (shadow_cap_ < count_ || !d_norm2_)) {
+        const size_t cap = std::max(capacity_, count_);
+        cudaFree(d_norm2_);
+        d_norm2_ = nullptr;
+        shadow_cap_ = shadow_rows_ = 0;
+        shadow_dirty_.clear();
+        if (cudaMalloc(&d_norm2_, cap * sizeof(int32_t)) != cudaSuccess) {
+            cudaGetLastError();
+            d_norm2_ = nullptr;
+            return false;
+        }
+        shadow_cap_ = cap;
+    }
+    if (!inorm && (shadow_cap_ < count_ || !d_shadow_)) {
         const size_t cap = std::max(capacity_, count_);
         uint8_t *nu = nullptr;
         if (cudaMalloc(&nu, coarse_shadow_bytes((uint32_t)cap, (uint32_t)dim_)) != cudaSuccess) {
@@ -800,8 +815,8 @@ bool FlatIndex::ensure_shadow(cudaStream_t st) {
         shadow_rows_ = 0;
         shadow_dirty_.clear();
     }
-    if (!unit_rows() && !d_norm2_) { // L2 / raw inner product / cosine after a raw overwrite: the error bound (and the L2
-                                     // epilogue) need |row|^2 of every row
+    if (!inorm && !unit_rows() && !d_norm2_) { // L2 / raw inner product / cosine after a raw overwrite: the error bound (and the L2
+                                               // epilogue) need |row|^2 of every row
         if (!d_stats_ && (cudaMalloc(&d_stats_, 8) != cudaSuccess || cudaMemset(d_stats_, 0, 8) != cudaSuccess)) {
             cudaGetLastError();
             return false;
@@ -814,6 +829,13 @@ bool FlatIndex::ensure_shadow(cudaStream_t st) {
         shadow_dirty_.clear();
     }
     if (shadow_rows_ > count_) shadow_rows_ = count_;
+    // rows [first, first + n) into every copy this index keeps
+    const auto refresh = [&](uint32_t first, uint32_t n) {
+        if (inorm) return launch_int_norm2(d_rows_, pitch_, (uint32_t)dim_, first, n, dtype_ == DT_I8, reinterpret_cast<int32_t *>(d_norm2_), st) ==
+                          cudaSuccess;
+        if (launch_to_f16_tiled(d_rows_, pitch_, (uint32_t)dim_, first, n, d_shadow_, st) != cudaSuccess) return false;
+        return !d_norm2_ || launch_row_stats(d_rows_, pitch_, (uint32_t)dim_, first, n, d_norm2_, d_stats_, st) == cudaSuccess;
+    };
     bool launched = false;
     if (shadow_dirty_.size() > 256) {
         shadow_rows_ = 0;
@@ -821,27 +843,22 @@ bool FlatIndex::ensure_shadow(cudaStream_t st) {
     }
     for (idType id : shadow_dirty_)
         if (id < shadow_rows_) {
-            if (launch_to_f16_tiled(d_rows_, pitch_, (uint32_t)dim_, id, 1, d_shadow_, st) != cudaSuccess) return false;
-            if (d_norm2_ && launch_row_stats(d_rows_, pitch_, (uint32_t)dim_, id, 1, d_norm2_, d_stats_, st) != cudaSuccess) return false;
+            if (!refresh(id, 1)) return false;
             launched = true;
         }
     shadow_dirty_.clear();
     if (shadow_rows_ < count_) {
-        if (launch_to_f16_tiled(d_rows_, pitch_, (uint32_t)dim_, (uint32_t)shadow_rows_, (uint32_t)(count_ - shadow_rows_), d_shadow_,
-                                st) != cudaSuccess)
-            return false;
-        if (d_norm2_ && launch_row_stats(d_rows_, pitch_, (uint32_t)dim_, (uint32_t)shadow_rows_, (uint32_t)(count_ - shadow_rows_), d_norm2_,
-                                         d_stats_, st) != cudaSuccess)
-            return false;
+        if (!refresh((uint32_t)shadow_rows_, (uint32_t)(count_ - shadow_rows_))) return false;
         shadow_rows_ = count_;
         launched = true;
     }
     // other query streams may read the shadow as soon as the lock is released
     if (launched) {
+        const bool stats = d_norm2_ && !inorm;
         uint32_t h[2] = {0, 0};
-        if (d_norm2_ && cudaMemcpyAsync(h, d_stats_, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) return false;
+        if (stats && cudaMemcpyAsync(h, d_stats_, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) return false;
         if (cudaStreamSynchronize(st) != cudaSuccess) return false;
-        if (d_norm2_) { // running maxima over every row ever converted (deletes do not lower them: conservative)
+        if (stats) { // running maxima over every row ever converted (deletes do not lower them: conservative)
             float n2, ma;
             memcpy(&n2, &h[0], 4);
             memcpy(&ma, &h[1], 4);
@@ -882,10 +899,13 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
     // orders of magnitude), so the batch is one kernel + the usual final selection — no shadow, no rescoring
     const bool is16 = dtype_ == DT_F16 || dtype_ == DT_BF16, is8 = dtype_ == DT_I8 || dtype_ == DT_U8;
     const CoarseKind dkind = is16 ? CoarseDirect16 : CoarseDirect8;
-    if (cmode != 0 && nq >= 16 && (is16 || is8) && coarse_supported(v, nq, ke, dkind)) {
+    // int8 / uint8 L2: the int32 |row|^2 table is brought up to date on `st` first (no HBM for it: the exact scan)
+    if (cmode != 0 && nq >= 16 && (is16 || is8) && coarse_supported(v, nq, ke, dkind) && (!int_l2() || ensure_shadow(st))) {
         // int8 / uint8: s8 / u8 wgmma dot products are exact integers and the epilogue applies the reference's own
-        // float expression, so that route is bit-exact
-        const CoarseOperands ops{v.rows, v.pitch, d_q, qpitch, (dtype_ == DT_BF16 || dtype_ == DT_I8) ? 1 : 0, mkind_ == MT_COS ? 1 : 0, nullptr, nullptr};
+        // float expression, so that route is bit-exact.  L2: |row|^2 + |q|^2 - 2 dot in int32, rounded once to float, is the
+        // reference's float(sum of squared differences) bit for bit
+        CoarseOperands ops{v.rows, v.pitch, d_q, qpitch, (dtype_ == DT_BF16 || dtype_ == DT_I8) ? 1 : 0,
+                           mkind_ == MT_COS ? 1 : int_l2() ? 2 : 0, nullptr, nullptr};
         last_batch_coarse_ = true;
         last_batch_path_ = 2;
         c.d_last_ok = nullptr;
@@ -938,9 +958,18 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
             return ok;
         }
         const size_t nA = (size_t)nq * cp.grid_x * cp.keep;
-        if (!c.need_cand(nA + cp.scratch_elems) || !c.need_out((size_t)nq * ke)) return false;
+        const size_t qn_elems = int_l2() ? ((size_t)nq + 1) / 2 : 0; // int8 / uint8 L2: |q|^2 per query, after the list scratch
+        if (!c.need_cand(nA + cp.scratch_elems + qn_elems) || !c.need_out((size_t)nq * ke)) return false;
+        bool ok = true;
+        if (int_l2()) {
+            int32_t *d_qn = reinterpret_cast<int32_t *>(c.d_cand + nA + cp.scratch_elems);
+            ok = launch_int_norm2(d_q, qpitch, v.dim, 0, nq, dtype_ == DT_I8, d_qn, st) == cudaSuccess;
+            ops.row_norm2 = reinterpret_cast<const float *>(d_norm2_); // int32 values (CoarseOperands)
+            ops.q_norm2 = reinterpret_cast<const float *>(d_qn);
+            lc.launches++;
+        }
         cudaEventRecord(c.ev_start, st);
-        bool ok = launch_coarse(ops, v.n_rows, v.dim, nq, cp, c.d_cand, c.d_cand + nA, st) == cudaSuccess;
+        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq, cp, c.d_cand, c.d_cand + nA, st) == cudaSuccess;
         cudaEventRecord(c.ev_stop, st);
         ok = ok && launch_final_select(c.d_cand, nq, (uint32_t)(cp.grid_x * cp.keep), ke, c.d_out, st, &lc) == cudaSuccess;
         lc.launches++;

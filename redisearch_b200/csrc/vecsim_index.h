@@ -221,7 +221,9 @@ class FlatIndex {
     // valid except shadow_dirty_
     uint8_t *d_shadow_ = nullptr;
     size_t shadow_cap_ = 0, shadow_rows_ = 0;
-    // L2 / raw inner-product indexes: |row|^2 per row and the running maxima the error bound needs
+    // L2 / raw inner-product indexes: |row|^2 per row and the running maxima the error bound needs.  int8 / uint8 L2 indexes keep
+    // the exact int32 |row|^2 here (stored as int32, no shadow, no maxima) for the integer tensor-core route; the same
+    // shadow_rows_ / shadow_dirty_ / shadow_cap_ bookkeeping tracks it
     float *d_norm2_ = nullptr;
     uint32_t *d_stats_ = nullptr;
     float shadow_max_norm_ = 0.0f, shadow_max_abs_ = std::numeric_limits<float>::infinity();
@@ -231,6 +233,10 @@ class FlatIndex {
     std::atomic<bool> raw_rows_{false};
     bool unit_rows() const { return metric_ == VecSimMetric_Cosine && !raw_rows_; }
     std::vector<idType> shadow_dirty_;
+    // a per-row copy (the fp16 shadow and / or |row|^2) exists: in-place overwrites and swap-deletes go to shadow_dirty_
+    bool keeps_row_copies() const { return d_shadow_ || d_norm2_; }
+    bool int_l2() const { return (dtype_ == DT_I8 || dtype_ == DT_U8) && mkind_ == MT_L2; }
+    // fp32: the fp16 shadow (+ |row|^2 unless unit rows); int8 / uint8 L2: only the int32 |row|^2 table
     bool ensure_shadow(cudaStream_t st);
     void disable_coarse(); // rows outside the fp16 range: exact scans from now on, the shadow's HBM is given back
     bool single_query_takes_coarse(uint32_t ke, const float *host_query = nullptr);
