@@ -430,15 +430,19 @@ size_t VecSim_GetSharedMemory(void);                                      /* 0, 
  * + label stage, queries it cannot prove and corpora of >= 65536 rows no such route serves one at a
  * time; the label-aware exact scan below that size; k > 128: one query at a time).  int8 / uint8 corpora with inner
  * product, cosine or L2 (nq >= 16, >= 65536 rows, dim % 16 == 0, 32 <= dim <= 2048, k <= 128, coarse mode 1 or 2) take the
- * s8 / u8 tensor-core route, bit-exact with the reference (ids, score bits and tie order).  Returns
+ * s8 / u8 tensor-core route, bit-exact with the reference (ids, score bits and tie order).  Single-value indexes with
+ * 128 < min(k, rows) <= 1024: batches the fp32 route serves (fp32, coarse mode 1 with the fixed bound, nq >= 16, >= 65536
+ * rows, dim % 8 == 0, 32..1024, rows inside the fp16 range) run as one batch, the queries it cannot prove finishing on the
+ * exact batched top-k on the device (DESIGN.md §4.5); every other such batch, and k > 1024, one query at a time.  Returns
  * VecSim_QueryReply_OK / _TimedOut, or -1 on a CUDA failure. */
 int VecSimB200_TopKQueryBatch(VecSimIndex *index, const void *queryBlobs, size_t qstride, size_t nq,
                               size_t k, VecSimQueryParams *queryParams, size_t *out_labels,
                               double *out_scores);
 /* Same, but queries and results are DEVICE pointers (fp/int data as the index type; labels are
  * int64, -1 for empty entries, scores float).  Nothing crosses PCIe; the call only enqueues on `stream`
- * (a cudaStream_t cast to void*, NULL = the index's own stream) and returns.  k <= 128, single- and
- * multi-value indexes; -1 for a larger k. */
+ * (a cudaStream_t cast to void*, NULL = the index's own stream) and returns.  Single-value indexes: k <= 1024 (above 128
+ * the fp32 route where it applies, otherwise the exact batched top-k on the device, DESIGN.md §4.5); multi-value indexes:
+ * k <= 128; -1 for a larger k. */
 int VecSimB200_TopKQueryBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, size_t k,
                                     int64_t *d_out_labels, float *d_out_scores, void *stream);
 /* nq range queries in one call.  replies[i] receives exactly what
@@ -506,11 +510,12 @@ void VecSimB200_ShardGroup_Free(VecSimB200_ShardGroup *g);
 int VecSimB200_ShardGroup_Rank(const VecSimB200_ShardGroup *g);
 int VecSimB200_ShardGroup_Size(const VecSimB200_ShardGroup *g);
 /* Collective, enqueued on `stream`, nothing synchronised: d_queries = nq stored-form (normalised) query blobs on this
- * rank's device; every rank receives the merged [nq][k] labels (int64, -1 = empty) and distances. */
+ * rank's device; every rank receives the merged [nq][k] labels (int64, -1 = empty) and distances.  k as in
+ * VecSimB200_TopKQueryBatchDevice: up to 1024 on single-value shards, 128 on multi-value shards; -1 beyond. */
 int VecSimB200_ShardGroup_TopKBatchDevice(VecSimB200_ShardGroup *g, VecSimIndex *shard, const void *d_queries, size_t nq, size_t k,
                                           int64_t *d_out_labels, float *d_out_scores, void *stream);
 /* Collective, host buffers end to end (raw query blobs in as for VecSimIndex_TopKQuery; H2D, shard scan, all-gather,
- * merge, D2H inside the call).  Empty slots: label SIZE_MAX, score NaN.  Returns 0 / -1. */
+ * merge, D2H inside the call).  Empty slots: label SIZE_MAX, score NaN.  The same limits on k.  Returns 0 / -1. */
 int VecSimB200_ShardGroup_TopKBatch(VecSimB200_ShardGroup *g, VecSimIndex *shard, const void *queryBlobs, size_t qstride, size_t nq,
                                     size_t k, size_t *out_labels, double *out_scores);
 /* The whole HybridIterator state machine of src/iterators/hybrid_reader.c in one call: mode choice (:668-691:
@@ -555,7 +560,7 @@ int VecSimB200_TopKFilteredBatch(VecSimIndex *index, const void *const *queryBlo
  * -1 = environment default (VECSIM_B200_COARSE, 1 unless set). */
 void VecSimB200_SetCoarseMode(int mode);
 /* Debug: after a VecSimB200_TopKQueryBatchDevice call, per-query flags (1 = answered by the tensor-core path on the first
- * tier's 24-entry candidate lists, 2 = by the second tier's 128-entry lists, 0 = fell back to the exact scan).  Multi-value
+ * tier's candidate lists, 2 = by the second tier's 128-entry lists, 0 = fell back to the exact scan).  Multi-value
  * index: 1 / 2 / 0 as before for its row stage, with the label check passed; 3 = fewer than k labels among the rows the row
  * stage selected, the label-aware exact scan answered (DESIGN.md §4.4).  Returns -1 if the last batch did not take the coarse
  * path. */

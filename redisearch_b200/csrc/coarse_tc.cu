@@ -1178,7 +1178,8 @@ __global__ void __launch_bounds__(256) to_f16_kernel(const uint8_t *__restrict__
 //   q_index (nullable): second tier — CTA i works on query q_index[i] of the original batch (its lists are stored at
 //   position i); nq_dev (nullable) = number of live CTAs.
 // ------------------------------------------------------------------------------------------------
-constexpr uint32_t kRefineMaxSurv = 2048;
+constexpr uint32_t kRefineMaxSurv = 2048;     // survivors rescored per query, k <= kCoarseMaxK
+constexpr uint32_t kRefineMaxSurvWide = 4096; // the same for k > kCoarseMaxK (32 KB)
 
 // |approx - exact| bound of one query (see above); q_norm2 == NULL: unit vectors
 __device__ __forceinline__ float query_eps(float eps, const float *q_norm2, uint32_t pos, float max_norm, uint32_t dim, bool l2) {
@@ -1256,7 +1257,7 @@ __global__ void __launch_bounds__(256) threshold_kernel(const uint64_t *__restri
 // thr_T == NULL: adaptive lists (a full list's worst kept approximate distance bounds what its row range dropped).
 // thr_T != NULL: lists of the fixed-bound pass — every list holds ALL rows of its range with approx < thr_T[pos] unless
 //                overflow[pos] is set; what was dropped has approx >= thr_T[pos].
-template <int MT>
+template <int MT, uint32_t kSurv>
 __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t pitch, uint32_t dim, const uint8_t *queries,
                                                      size_t qpitch, uint32_t nq, uint32_t lists_per_query, uint32_t keep, uint32_t k,
                                                      const uint64_t *__restrict__ cand, float eps, const float *__restrict__ q_norm2,
@@ -1265,7 +1266,7 @@ __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t
                                                      const float *__restrict__ thr_T, const uint32_t *__restrict__ overflow,
                                                      uint32_t smem_cap) {
     using Tile = DistTile<DT_F32, MT, 1, 1>;
-    __shared__ uint64_t surv[kRefineMaxSurv];
+    __shared__ uint64_t surv[kSurv];
     __shared__ uint32_t hist[256];
     __shared__ uint32_t ctl[4];
     __shared__ uint32_t s_nsurv, s_bad, s_ncomp;
@@ -1315,11 +1316,11 @@ __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t
         base = __shfl_sync(0xFFFFFFFFu, base, 0);
         if (take) {
             const uint32_t pos = base + __popc(m & ((1u << lane) - 1u));
-            if (pos < kRefineMaxSurv) surv[pos] = c;
+            if (pos < kSurv) surv[pos] = c;
         }
     }
     __syncthreads();
-    const uint32_t n_all = s_nsurv, n_surv = min(n_all, kRefineMaxSurv);
+    const uint32_t n_all = s_nsurv, n_surv = min(n_all, kSurv);
     // exact distances of the survivors (one warp per row)
     const uint8_t *qb[1] = {queries + (size_t)q * qpitch};
     for (uint32_t i = warp; i < n_surv; i += 8) {
@@ -1336,7 +1337,7 @@ __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t
     bitonic_sort_smem(surv, n_sort);
     for (uint32_t i = threadIdx.x; i < k; i += blockDim.x) out[(size_t)q * k + i] = i < n_surv ? surv[i] : kEmptySlot;
     // proof
-    bool bad = n_all > kRefineMaxSurv; // more candidates within 2 eps of the k-th than the buffer holds: the next tier answers
+    bool bad = n_all > kSurv; // more candidates within 2 eps of the k-th than the buffer holds: the next tier answers
     // a query whose fp16 form is not finite (row_stats_kernel: |q|^2 = NaN) has no error bound.  And a bound that is not a
     // finite number proves nothing: cut is +-inf or NaN when the k-th approximate key is, or when there are fewer than k
     // candidates; thr_T is +inf when the sample pass found fewer than k finite distances.
@@ -1552,6 +1553,8 @@ static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, int epi, int m
         return variant ? wgmma_kernel_fn_v<1>(kind, epl, epi, mode) : wgmma_kernel_fn_v<0>(kind, epl, epi, mode);
     // fp32 route (shadow rows): the flag selects the squared-L2 epilogue; epl 8 = lists of up to 128 (second tier);
     // mode 1 = fixed admission bound (lists of 96, no compaction), mode 2 = the sample pass (slice minima only)
+    // (epl 8: lists of 256, k > kCoarseMaxK)
+    if (mode == 1 && epl == 8) return l2 ? (const void *)coarse_wgmma_kernel<false, 8, 3, 1> : (const void *)coarse_wgmma_kernel<false, 8, 0, 1>;
     if (mode == 1) return l2 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 1> : (const void *)coarse_wgmma_kernel<false, 3, 0, 1>;
     if (mode == 2) return l2 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 2> : (const void *)coarse_wgmma_kernel<false, 3, 0, 2>;
     if (l2) return epl == 3 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 0> : (const void *)coarse_wgmma_kernel<false, 8, 3, 0>;
@@ -1590,7 +1593,8 @@ bool coarse_supported(const CorpusView &c, uint32_t nq, uint32_t k, CoarseKind k
     if (kind == CoarseTF32 && c.metric != MT_IP) return false;
     if (c.dim % 8 != 0 || c.dim < 32 || c.dim > 1024) return false;
     if (c.pitch % 16 != 0) return false;
-    if (k > kCoarseMaxK || nq < 1) return false; // batch_scan decides whether a small batch is worth the route
+    // k above kCoarseMaxK: the fp16 route's two-pass first tier only (batch_scan_rows)
+    if (k > (kind == CoarseF16 ? kCoarseMaxKWide : kCoarseMaxK) || nq < 1) return false; // batch_scan decides whether a small batch is worth the route
     if (c.n_rows < 65536) return false; // tiny corpora: the exact kernel is already fast
     if (kind == CoarseF16 && !wgmma_fits(c.dim)) return false; // wider rows: the TF32 variant
     if (kind == CoarseTF32 && fixed_smem((c.dim + CfgTF32::kBlockK - 1) / CfgTF32::kBlockK) + 3 * kStageBytes > kSmemLimit) return false;
@@ -1614,7 +1618,8 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
         p.keep = kind == CoarseF16 ? (keep_override ? keep_override : (k <= kCoarseTier1MaxK ? kCoarseKeep : kCoarseKeepWide))
                                    : (k <= 32 ? 32u : 128u);
         p.epl = p.keep <= 32 ? 3 : 8;
-        if (p.mode == 1 && kind == CoarseF16) p.keep = kCoarseFixedCap, p.epl = 3; // every row below the bound, up to the list capacity
+        if (p.mode == 1 && kind == CoarseF16) // every row below the bound, up to the list capacity
+            p.keep = k > kCoarseMaxK ? kCoarseFixedCapWide : kCoarseFixedCap, p.epl = k > kCoarseMaxK ? 8 : 3;
         if (p.mode == 1 && kind == CoarseDirect16) p.keep = kCoarseFixedCapDirect, p.epl = 8;
         if (p.mode == 2) p.keep = kCoarseSampleSlices, p.epl = 3; // the slice minima
         p.stages = (uint32_t)std::min<size_t>(kQMaxStages, (kSmemLimit - wgmma_fixed_smem(p.num_kb, p.mode)) / kQStageBytes);
@@ -1859,15 +1864,27 @@ cudaError_t launch_refine(const CorpusView &c, const void *d_queries, size_t qpi
     if (nq == 0) return cudaSuccess;
     const uint32_t okv = d_q_index ? 2u : 1u;
     const uint8_t *rows = static_cast<const uint8_t *>(c.rows), *qs = static_cast<const uint8_t *>(d_queries);
-    // candidates packed in shared memory: as many slots as the lists have, up to 20 KB worth
-    const uint32_t smem_cap = std::min<uint32_t>(lists_per_query * keep, 2560);
+    // candidates packed in shared memory: as many slots as the lists have, up to 20 KB worth (k > kCoarseMaxK: 64 KB, two CTAs
+    // per SM next to the 32 KB survivor buffer)
+    const bool wide = k > kCoarseMaxK;
+    if (k > kCoarseMaxKWide) return cudaErrorInvalidValue;
+    const uint32_t max_cap = wide ? 8192 : 2560;
+    const uint32_t smem_cap = std::min<uint32_t>(lists_per_query * keep, max_cap);
     const size_t smem = (size_t)smem_cap * 8;
-    if (c.metric == MT_L2)
-        refine_kernel<MT_L2><<<nq, 256, smem, s>>>(rows, c.pitch, c.dim, qs, qpitch, nq, lists_per_query, keep, k, d_cand, eps, d_q_norm2,
-                                                   max_norm, d_ok, okv, d_out, d_q_index, d_nq_dev, d_thr_T, d_overflow, smem_cap);
-    else
-        refine_kernel<MT_IP><<<nq, 256, smem, s>>>(rows, c.pitch, c.dim, qs, qpitch, nq, lists_per_query, keep, k, d_cand, eps, d_q_norm2,
-                                                   max_norm, d_ok, okv, d_out, d_q_index, d_nq_dev, d_thr_T, d_overflow, smem_cap);
+    const auto kern = c.metric == MT_L2 ? (wide ? refine_kernel<MT_L2, kRefineMaxSurvWide> : refine_kernel<MT_L2, kRefineMaxSurv>)
+                                        : (wide ? refine_kernel<MT_IP, kRefineMaxSurvWide> : refine_kernel<MT_IP, kRefineMaxSurv>);
+    // the 48 KB a launch gets without opting in cover static + dynamic shared memory (the wide survivor buffer alone is 32 KB).
+    // Opt in to the largest packing this instantiation can ask for, the same value every time: concurrent launches of the same
+    // kernel from other host threads never see the limit lowered under them
+    cudaFuncAttributes fa{};
+    cudaError_t e = cudaFuncGetAttributes(&fa, kern);
+    if (e != cudaSuccess) return e;
+    if (fa.sharedSizeBytes + (size_t)max_cap * 8 > 48 * 1024) {
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(max_cap * 8));
+        if (e != cudaSuccess) return e;
+    }
+    kern<<<nq, 256, smem, s>>>(rows, c.pitch, c.dim, qs, qpitch, nq, lists_per_query, keep, k, d_cand, eps, d_q_norm2, max_norm, d_ok, okv,
+                               d_out, d_q_index, d_nq_dev, d_thr_T, d_overflow, smem_cap);
     return cudaGetLastError();
 }
 

@@ -9,7 +9,9 @@ namespace rsb200 {
 constexpr uint32_t kCoarseKeep = 24;       // candidates kept per (CTA row range, query), first tier
 constexpr uint32_t kCoarseKeepWide = 128;  // second tier (queries the first proof left open) and first tier of k > 16
 constexpr uint32_t kCoarseTier1MaxK = 16;  // largest k the 24-entry lists serve
-constexpr uint32_t kCoarseMaxK = 128;      // largest k served by the coarse path
+constexpr uint32_t kCoarseMaxK = 128;      // largest k served by the coarse path (TF32, direct 16/8-bit routes, tier 1 at small k)
+constexpr uint32_t kCoarseMaxKWide = 1024; // largest k of the fp32 route's two-pass first tier (DESIGN.md §4.5)
+constexpr uint32_t kCoarseFixedCapWide = 256; // list capacity of the fp32 main pass for k > kCoarseMaxK
 constexpr uint32_t kCoarseSampleSlices = 32; // minima the sample pass publishes per (query, row range)
 constexpr uint32_t kCoarseFixedCapDirect = 256; // list capacity of the fixed-bound pass on 16-bit corpora (k up to 128)
 constexpr uint32_t kCoarseFixedCap = 96;   // list capacity of the fixed-bound main pass (rows below the bound per row range)

@@ -18,6 +18,7 @@ namespace rsb200 {
 constexpr uint64_t kEmptySlot = 0xFFFFFFFFFFFFFFFFull; // sorts after every real candidate
 constexpr uint32_t kNaNKey = 0xFFFFFFFEu;              // NaN distances sort after +inf
 constexpr int kMaxFusedK = 128;                        // largest k the fused per-warp lists take
+constexpr int kMaxWideK = 1024;                        // largest k of a batch on the device (chunks of kMaxFusedK beyond it)
 
 // float -> uint32 whose unsigned order equals the float order (-inf < ... < -0 == +0 < ... < +inf
 // < NaN).

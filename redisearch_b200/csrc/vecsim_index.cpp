@@ -981,8 +981,10 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
     // cosine: unit vectors, constant error bound, either operand kind.  L2 / raw inner product (fp32): the fp16 route only,
     // error bound from the row and query norms
     const bool unit = unit_rows();
+    // k > kCoarseMaxK (DESIGN.md §4.5): the fp16 route's two-pass first tier, for batches of 16 queries and more
+    const bool wide = ke > kCoarseMaxK;
     const bool eligible = cmode != 0 && !coarse_disabled_ && dtype_ == DT_F32 && (unit || cmode == 1) &&
-                          (nq >= 16 || single_query_takes_coarse(ke));
+                          (nq >= 16 || (!wide && single_query_takes_coarse(ke))) && (!wide || coarse_fixed_enabled());
     bool coarse = eligible && coarse_supported(v, nq, ke, kind);
     if (eligible && kind == CoarseF16 && (!coarse || !ensure_shadow(st))) { // rows too wide for the 16-bit kernel's shared memory, or no HBM for the shadow
         kind = CoarseTF32;
@@ -998,6 +1000,17 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
     if (!coarse && tc_only) {
         *d_result = nullptr;
         return true;
+    }
+    // the exact top-k of k > kMaxFusedK: whole batches no route serves here, the queries the route leaves open below
+    const WidePlan wp = wide ? plan_topk_wide(v.n_rows, nq) : WidePlan{};
+    if (!coarse && wide) {
+        if (!c.need_scores(wp.score_elems) || !c.need_cand(wp.cand_elems) || !c.need_out((size_t)nq * ke)) return false;
+        cudaEventRecord(c.ev_start, st);
+        const bool ok = launch_topk_wide(v, d_q, qpitch, nq, ke, nullptr, nullptr, wp, c.d_scores, c.d_cand, c.d_out, c.d_abort, st, &lc) ==
+                        cudaSuccess;
+        cudaEventRecord(c.ev_stop, st);
+        *d_result = c.d_out;
+        return ok;
     }
     if (!coarse) {
         if (!c.need_cand(sp.cand_elems) || !c.need_out((size_t)nq * ke)) return false;
@@ -1021,11 +1034,22 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
     if (two_pass) {
         // expected rows below T per (query, row range) = k / (sample fraction * ranges): aim at 24 of the 96 slots
         const CoarsePlan probe = plan_coarse(v, nq, kind, ke, 0, 1, 1);
-        double f = (double)ke / (24.0 * probe.grid_x);
-        f = std::min(0.25, std::max(0.01, f));
-        // small corpora: the sample must still hold a few times k slice minima (4 per visited tile)
-        const uint32_t stride = (uint32_t)std::max(1.0, std::min(std::floor(1.0 / f), std::floor(probe.tiles / (2.0 * ke))));
-        cps = plan_coarse(v, nq, kind, ke, 0, stride, 2);
+        if (wide) {
+            // k in the hundreds: ranges x 32 slice minima barely hold k values.  The sample pass keeps adaptive lists of 128 per
+            // (query, row range) instead; their union holds at least k distinct rows at or below its k-th smallest
+            // approximate distance, so threshold_kernel's bound stands.  Aim at 128 of the 256 slots of the main pass.
+            double f = (double)ke / (128.0 * probe.grid_x);
+            f = std::min(0.25, std::max(0.01, f));
+            // small corpora: the sample must still hold about 4 k rows (128 per visited tile)
+            const uint32_t stride = (uint32_t)std::max(1.0, std::min(std::floor(1.0 / f), std::floor(probe.tiles / (ke / 32.0))));
+            cps = plan_coarse(v, nq, kind, ke, kCoarseKeepWide, stride, 0);
+        } else {
+            double f = (double)ke / (24.0 * probe.grid_x);
+            f = std::min(0.25, std::max(0.01, f));
+            // small corpora: the sample must still hold a few times k slice minima (4 per visited tile)
+            const uint32_t stride = (uint32_t)std::max(1.0, std::min(std::floor(1.0 / f), std::floor(probe.tiles / (2.0 * ke))));
+            cps = plan_coarse(v, nq, kind, ke, 0, stride, 2);
+        }
         cp = probe;
     }
     const size_t per_query = (size_t)cp.grid_x * cp.keep;
@@ -1044,11 +1068,15 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
     const size_t qn_elems = unit ? 0 : (nq + 1) / 2 + 1; // |q|^2 per query (floats)
     const size_t scratch = std::max(std::max(cp.scratch_elems, two_pass ? cps.scratch_elems : 0), tier2 ? cp2.scratch_elems : 0);
     const size_t flag_elems = (nq + 1) / 2 + 1; // nq uint32 / float values
-    const size_t total = nA + nS + nA2 + 2 * nO + sp.cand_elems + (tier2 ? 2 : 1) * (q16_elems + qn_elems) + scratch + 5 * flag_elems + 16;
-    if (!c.need_cand(total) || !c.need_out(nO)) return false;
-    uint64_t *coarse_cand = c.d_cand, *cand_s = coarse_cand + nA, *cand_t2 = cand_s + nS, *out1 = cand_t2 + nA2, *out2 = out1 + nO,
-             *cand2 = out2 + nO;
-    uint64_t *q16 = cand2 + sp.cand_elems;
+    // k > kMaxFusedK: the exact fallback's chunk-select lists take the place of the fused scan's
+    const size_t fb_elems = wide ? wp.cand_elems : sp.cand_elems;
+    const size_t nO12 = wide ? 0 : nO; // k > kMaxFusedK: the tiers write the answer rows in place, no out1 / out2
+    const size_t total = nA + nS + nA2 + 2 * nO12 + fb_elems + (tier2 ? 2 : 1) * (q16_elems + qn_elems) + scratch + 5 * flag_elems + 16;
+    if (!c.need_cand(total) || !c.need_out(nO) || (wide && !c.need_scores(wp.score_elems))) return false;
+    uint64_t *coarse_cand = c.d_cand, *cand_s = coarse_cand + nA, *cand_t2 = cand_s + nS, *out1 = cand_t2 + nA2, *out2 = out1 + nO12,
+             *cand2 = out2 + nO12;
+    uint64_t *q16 = cand2 + fb_elems;
+    if (wide) out1 = c.d_out; // both tiers and the exact fallback write their rows of the answer in place (no blend)
     uint64_t *q16_t2 = q16 + q16_elems;
     uint64_t *list_scratch = q16_t2 + (tier2 ? q16_elems : 0);
     uint64_t *tail = list_scratch + scratch;
@@ -1095,6 +1123,15 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
         ok = ok && launch_refine(v, d_q, qpitch, nq, cp2.grid_x, cp2.keep, ke, cand_t2, eps, d_qn2_t2, shadow_max_norm_, d_ok, out1, d_idx, d_n2,
                                  st) == cudaSuccess;
         lc.launches += 4;
+    }
+    if (wide) {
+        // exact fallback of the open queries, entirely on device; with none open, every launch exits at once
+        ok = ok && launch_compact_unproven(d_ok, nq, d_idx, d_n2, st) == cudaSuccess;
+        ok = ok && launch_topk_wide(v, d_q, qpitch, nq, ke, d_idx, d_n2, wp, c.d_scores, cand2, c.d_out, c.d_abort, st, &lc) == cudaSuccess;
+        lc.launches++;
+        coarse_batches_++;
+        *d_result = c.d_out;
+        return ok;
     }
     // exact fallback, entirely on device: CTAs whose queries are all verified exit at once
     ok = ok && launch_scan_topk(v, d_q, qpitch, nq, ke, sp, cand2, st, &lc, d_ok, c.d_abort) == cudaSuccess;
@@ -1179,7 +1216,9 @@ int FlatIndex::topk_batch(const void *qs, size_t qstride, size_t nq, size_t k, V
         delete r;
         return code;
     };
-    if (multi_ ? k > (size_t)kMaxFusedK : std::min(k, n) > (size_t)kMaxFusedK) { // generic path, one query at a time
+    // single-value, kMaxFusedK < min(k, n) <= kMaxWideK: batches the fp32 route serves run as one batch (DESIGN.md §4.5)
+    const bool wide = !multi_ && std::min(k, n) > (size_t)kMaxFusedK && std::min(k, n) <= (size_t)kMaxWideK;
+    if (multi_ ? k > (size_t)kMaxFusedK : (std::min(k, n) > (size_t)kMaxFusedK && !wide)) { // generic path, one query at a time
         for (size_t i = 0; i < nq; i++) {
             const int code = one_query(i);
             if (code != VecSim_QueryReply_OK) return code;
@@ -1208,6 +1247,10 @@ int FlatIndex::topk_batch(const void *qs, size_t qstride, size_t nq, size_t k, V
         per_query_all = ok && !d_res;
         d_flags = c->d_last_ok;
         ok = ok && (!d_flags || cudaMemcpyAsync(c->h_ids, d_flags, nq * 4, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess);
+    } else if (wide) {
+        // no route for this batch: the host API keeps answering it one query at a time (d_res comes back NULL)
+        ok = ok && batch_scan_rows(*c, c->d_query, qpitch, (uint32_t)nq, ke, c->stream, lc, &d_res, true);
+        per_query_all = ok && !d_res;
     } else {
         ok = ok && batch_scan(*c, c->d_query, qpitch, (uint32_t)nq, ke, c->stream, lc, &d_res);
     }
@@ -1278,7 +1321,7 @@ int FlatIndex::topk_batch_device(const void *d_q, size_t nq, size_t k, int64_t *
     if (nq == 0 || k == 0) return 0;
     if (!flush() || !sync_labels_to_device()) return -1;
     const size_t n = count_;
-    if (k > (size_t)kMaxFusedK) return -1;
+    if (k > (size_t)(multi_ ? kMaxFusedK : kMaxWideK)) return -1; // single-value, k > kMaxFusedK: DESIGN.md §4.5
     // Scratch of this entry point is stream-ordered: one dedicated context, reused call after call.
     // Callers enqueue on one stream (or synchronise between streams), as with any async API.
     std::lock_guard<std::mutex> dg(dev_mu_);

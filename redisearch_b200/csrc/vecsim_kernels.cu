@@ -276,17 +276,14 @@ __global__ void __launch_bounds__(kScanThreads) scan_topk_kernel(const ScanArgs 
 // ------------------------------------------------------------------------------------------------
 // candidates -> k smallest per query, ascending
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kScanThreads) final_select_kernel(const uint64_t *__restrict__ cand, uint32_t m,
-                                                                    uint32_t k, uint64_t *__restrict__ out,
-                                                                    const uint32_t *__restrict__ nq_dev) {
+// One CTA: the k smallest of src[0, m), ascending, into out[0, k).
+__device__ __forceinline__ void final_select_cta(const uint64_t *__restrict__ src, uint32_t m, uint32_t k, uint64_t *__restrict__ out) {
     extern __shared__ __align__(16) uint8_t smem[];
-    if (nq_dev && blockIdx.x >= *nq_dev) return; // second tier: only the first *nq_dev positions hold lists
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t sortn = next_pow2(kScanWarps * k);
     uint64_t *sortbuf = reinterpret_cast<uint64_t *>(smem); // [sortn]; first 8*k double as the lists
     uint64_t *worst = sortbuf + sortn;
     uint32_t *wpos = reinterpret_cast<uint32_t *>(worst + kScanWarps);
-    const uint64_t *src = cand + (size_t)blockIdx.x * m;
 
     for (uint32_t p = threadIdx.x; p < sortn; p += blockDim.x) sortbuf[p] = kEmptySlot;
     if (threadIdx.x < kScanWarps) {
@@ -307,7 +304,14 @@ __global__ void __launch_bounds__(kScanThreads) final_select_kernel(const uint64
         }
     }
     bitonic_sort_smem(sortbuf, sortn);
-    for (uint32_t p = threadIdx.x; p < k; p += blockDim.x) out[(size_t)blockIdx.x * k + p] = sortbuf[p];
+    for (uint32_t p = threadIdx.x; p < k; p += blockDim.x) out[p] = sortbuf[p];
+}
+
+__global__ void __launch_bounds__(kScanThreads) final_select_kernel(const uint64_t *__restrict__ cand, uint32_t m,
+                                                                    uint32_t k, uint64_t *__restrict__ out,
+                                                                    const uint32_t *__restrict__ nq_dev) {
+    if (nq_dev && blockIdx.x >= *nq_dev) return; // second tier: only the first *nq_dev positions hold lists
+    final_select_cta(cand + (size_t)blockIdx.x * m, m, k, out + (size_t)blockIdx.x * k);
 }
 
 // The same over label-aware lists (multi-value index): each warp keeps the k best distinct labels of its share, and the first k
@@ -396,10 +400,9 @@ __global__ void __launch_bounds__(kScanThreads) scan_scores_kernel(const uint8_t
     }
 }
 
-// k smallest composites > cursor over a score array -> per-warp lists
-__global__ void __launch_bounds__(kScanThreads) select_scores_kernel(const float *__restrict__ scores, uint32_t n,
-                                                                     const uint64_t *__restrict__ cursor, uint32_t k,
-                                                                     uint64_t *__restrict__ cand) {
+// k smallest composites > cursor over a score array -> per-warp lists (blockIdx.x, warp) of cand
+__device__ __forceinline__ void select_scores_cta(const float *__restrict__ scores, uint32_t n, const uint64_t *__restrict__ cursor,
+                                                  uint32_t k, uint64_t *__restrict__ cand) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint64_t *slots = reinterpret_cast<uint64_t *>(smem);
@@ -434,6 +437,102 @@ __global__ void __launch_bounds__(kScanThreads) select_scores_kernel(const float
     __syncwarp();
     uint64_t *dst = cand + (size_t)gw * k;
     for (uint32_t p = lane; p < k; p += 32) dst[p] = ls.slots[p];
+}
+
+__global__ void __launch_bounds__(kScanThreads) select_scores_kernel(const float *__restrict__ scores, uint32_t n,
+                                                                     const uint64_t *__restrict__ cursor, uint32_t k,
+                                                                     uint64_t *__restrict__ cand) {
+    select_scores_cta(scores, n, cursor, k, cand);
+}
+
+// ------------------------------------------------------------------------------------------------
+// exact top-k of a batch for kMaxFusedK < k <= kMaxWideK (DESIGN.md §4.5): the unfused path of one query (all scores, then
+// cursor selects of up to 128) with a query dimension.  The batch's positions are taken G at a time (a group); slot y of the
+// group is position base + y, whose query is pos[base + y] (base + y without pos).  Only positions below *count (nq without
+// count) are live: a CTA of a dead slot leaves at once, so a group whose positions are all answered reads nothing.
+// ------------------------------------------------------------------------------------------------
+struct WideGroup {
+    const uint32_t *pos;   // nullable
+    const uint32_t *count; // nullable
+    uint32_t nq, base;
+};
+// live positions of the group from `base` on (0 = none)
+__device__ __forceinline__ uint32_t wide_live(const WideGroup &g) {
+    const uint32_t n = g.count ? min(*g.count, g.nq) : g.nq;
+    return n > g.base ? n - g.base : 0u;
+}
+__device__ __forceinline__ uint32_t wide_query(const WideGroup &g, uint32_t slot) {
+    return g.pos ? g.pos[g.base + slot] : g.base + slot;
+}
+
+struct WideScanArgs {
+    const uint8_t *rows;
+    size_t pitch;
+    uint32_t n_rows, dim, wq, slots; // slots: positions in the group (scores holds slots x n_rows)
+    const uint8_t *queries;
+    size_t qpitch;
+    WideGroup g;
+    float *scores;
+    const uint32_t *abort; // as ScanArgs
+    uint32_t poll_mask;
+};
+
+// scores[slot][row] for the group's live slots: warp (qg, rg) of CTA y scores 8 slots against its row tiles (the arithmetic of
+// scan_scores_kernel, which is that of the fused scan, query by query).  The wq query groups of a CTA share its rows through L1.
+template <int DT, int MT>
+__global__ void __launch_bounds__(kScanThreads) scan_scores_wide_kernel(const WideScanArgs a) {
+    constexpr int RT = 4, QT = 8;
+    using Tile = DistTile<DT, MT, RT, QT>;
+    using Map = typename Tile::Map;
+    const uint32_t live = min(wide_live(a.g), a.slots);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t WQ = a.wq, WR = kScanWarps / WQ, qg = warp % WQ, rg = warp / WQ;
+    const uint32_t s0 = (blockIdx.y * WQ + qg) * QT;
+    if (s0 >= live) return;
+    const uint8_t *qb[QT];
+#pragma unroll
+    for (int j = 0; j < QT; j++) qb[j] = a.queries + (size_t)wide_query(a.g, min(s0 + j, live - 1)) * a.qpitch;
+    const uint32_t ntiles = (a.n_rows + RT - 1) / RT;
+    float *my_scores = a.scores + (size_t)s0 * a.n_rows;
+    const uint32_t my_live = live - s0;
+    uint32_t since_poll = 0;
+    for (uint32_t t = blockIdx.x * WR + rg; t < ntiles; t += gridDim.x * WR) {
+        if (a.abort && (since_poll++ & a.poll_mask) == a.poll_mask) {
+            uint32_t f = 0;
+            if (lane == 0) f = *reinterpret_cast<const volatile uint32_t *>(a.abort);
+            if (__shfl_sync(0xffffffffu, f, 0)) break; // the caller has left: the scores are never read
+        }
+        const uint32_t r0 = t * RT;
+        const uint8_t *rowb[RT];
+#pragma unroll
+        for (int i = 0; i < RT; i++) rowb[i] = a.rows + (size_t)min(r0 + i, a.n_rows - 1) * a.pitch;
+        float d[Map::kPerLane];
+        Tile::run(rowb, qb, a.dim, lane, d);
+#pragma unroll
+        for (int t2 = 0; t2 < Map::kPerLane; t2++) {
+            const int idx = Map::value_index(lane, t2);
+            const uint32_t row = r0 + idx / QT, j = idx % QT;
+            if (Map::primary(lane) && row < a.n_rows && j < my_live) my_scores[(size_t)j * a.n_rows + row] = d[t2];
+        }
+    }
+}
+
+// chunk select of slot blockIdx.y: its scores, its cursor = the last composite of the previous chunk in its answer row
+__global__ void __launch_bounds__(kScanThreads) select_scores_wide_kernel(const float *__restrict__ scores, uint32_t n, const WideGroup g,
+                                                                          const uint64_t *__restrict__ out, uint32_t out_k, uint32_t first,
+                                                                          uint32_t k, uint64_t *__restrict__ cand) {
+    const uint32_t y = blockIdx.y;
+    if (y >= wide_live(g)) return;
+    const uint64_t *cursor = first ? out + (size_t)wide_query(g, y) * out_k + first - 1 : nullptr;
+    select_scores_cta(scores + (size_t)y * n, n, cursor, k, cand + (size_t)y * gridDim.x * kScanWarps * k);
+}
+
+// slot blockIdx.x: its lists -> its answer row, entries [first, first + k)
+__global__ void __launch_bounds__(kScanThreads) final_select_wide_kernel(const uint64_t *__restrict__ cand, uint32_t m, const WideGroup g,
+                                                                         uint64_t *__restrict__ out, uint32_t out_k, uint32_t first, uint32_t k) {
+    const uint32_t y = blockIdx.x;
+    if (y >= wide_live(g)) return;
+    final_select_cta(cand + (size_t)y * m, m, k, out + (size_t)wide_query(g, y) * out_k + first);
 }
 
 __global__ void range_compact_kernel(const float *__restrict__ scores, uint32_t n, float radius,
@@ -792,6 +891,71 @@ cudaError_t launch_select_scores(const float *d_scores, uint32_t n, const uint64
     select_scores_kernel<<<select_grid(n), kScanThreads, smem, s>>>(d_scores, n, d_cursor, k, d_cand);
     if (ctr) ctr->launches++;
     return cudaGetLastError();
+}
+
+constexpr size_t kWideScoreBytes = size_t(1) << 30; // HBM for the scores of one group of the batched exact top-k
+
+WidePlan plan_topk_wide(uint32_t n_rows, uint32_t nq) {
+    WidePlan p{};
+    const size_t n = std::max<uint32_t>(n_rows, 1);
+    // at most 65,535 slots: the chunk select puts a group's slots on gridDim.y
+    p.group = (uint32_t)std::max<size_t>(1, std::min<size_t>(std::min<size_t>(nq, 65535), kWideScoreBytes / (n * 4)));
+    // the chunk selects of a group keep about two CTAs per SM busy in all: fewer lists per slot the more slots there are
+    p.sel_grid = std::max(1u, std::min(select_grid(n_rows), (uint32_t)device_sm_count() * 2u / p.group));
+    p.score_elems = (size_t)p.group * n_rows;
+    p.cand_elems = (size_t)p.group * p.sel_grid * kScanWarps * kMaxFusedK;
+    return p;
+}
+
+template <int DT, int MT>
+static cudaError_t launch_scores_wide_inst(const WideScanArgs &a, cudaStream_t s) {
+    auto kern = scan_scores_wide_kernel<DT, MT>;
+    const uint32_t groups = (a.slots + 7) / 8, grid_y = (groups + a.wq - 1) / a.wq, wr = kScanWarps / a.wq;
+    const uint32_t want = ((a.n_rows + 3) / 4 + wr - 1) / wr;
+    const uint32_t resident = (uint32_t)(device_sm_count() * occupancy(kern, 0));
+    const uint32_t grid_x = std::max(1u, std::min(want, std::max(1u, resident / grid_y)));
+    kern<<<dim3(grid_x, grid_y), kScanThreads, 0, s>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_topk_wide(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t k, const uint32_t *d_pos,
+                             const uint32_t *d_count, const WidePlan &p, float *d_scores, uint64_t *d_cand, uint64_t *d_out,
+                             const uint32_t *d_abort, cudaStream_t s, LaunchCounters *ctr) {
+    if (k == 0 || k > (uint32_t)kMaxWideK || k > c.n_rows || p.group == 0) return cudaErrorInvalidValue;
+    if (nq == 0) return cudaSuccess;
+    WideScanArgs a{};
+    a.rows = static_cast<const uint8_t *>(c.rows);
+    a.pitch = c.pitch;
+    a.n_rows = c.n_rows;
+    a.dim = c.dim;
+    a.queries = static_cast<const uint8_t *>(d_queries);
+    a.qpitch = qpitch;
+    a.scores = d_scores;
+    a.abort = d_abort;
+    a.poll_mask = 15u;
+    const size_t fsmem = (size_t)next_pow2(kScanWarps * kMaxFusedK) * 8 + kScanWarps * 12;
+    const size_t ssmem = (size_t)kScanWarps * kMaxFusedK * 8 + kScanWarps * 12;
+    for (uint32_t base = 0; base < nq; base += p.group) {
+        const WideGroup g{d_pos, d_count, nq, base};
+        a.g = g;
+        a.slots = std::min(p.group, nq - base);
+        const uint32_t groups8 = (a.slots + 7) / 8;
+        a.wq = groups8 >= 8 ? 8 : groups8 >= 4 ? 4 : groups8 >= 2 ? 2 : 1;
+        cudaError_t e = cudaErrorInvalidValue;
+#define CALL_SCORES_WIDE(DT, MT) e = launch_scores_wide_inst<DT, MT>(a, s)
+        RSB_DISPATCH_DM(c.dtype, c.metric, CALL_SCORES_WIDE)
+#undef CALL_SCORES_WIDE
+        if (e != cudaSuccess) return e;
+        if (ctr) ctr->launches++;
+        for (uint32_t first = 0; first < k; first += kMaxFusedK) {
+            const uint32_t chunk = std::min<uint32_t>(kMaxFusedK, k - first);
+            select_scores_wide_kernel<<<dim3(p.sel_grid, a.slots), kScanThreads, ssmem, s>>>(d_scores, c.n_rows, g, d_out, k, first, chunk, d_cand);
+            final_select_wide_kernel<<<a.slots, kScanThreads, fsmem, s>>>(d_cand, p.sel_grid * kScanWarps * chunk, g, d_out, k, first, chunk);
+            if ((e = cudaGetLastError()) != cudaSuccess) return e;
+            if (ctr) ctr->launches += 2;
+        }
+    }
+    return cudaSuccess;
 }
 
 cudaError_t launch_range_compact(const float *d_scores, uint32_t n, float radius, uint64_t *d_out, uint32_t *d_count,

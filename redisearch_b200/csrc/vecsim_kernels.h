@@ -74,6 +74,21 @@ cudaError_t launch_scan_scores(const CorpusView &c, const void *d_query, float *
 uint32_t plan_select_scores_lists(uint32_t n);
 cudaError_t launch_select_scores(const float *d_scores, uint32_t n, const uint64_t *d_cursor, uint32_t k,
                                  uint64_t *d_cand, cudaStream_t s, LaunchCounters *ctr);
+
+// ---- exact top-k of a batch for kMaxFusedK < k <= kMaxWideK (DESIGN.md §4.5) --------------------
+// The unfused path of one query with a query dimension: per group of `group` batch positions one scan of all their scores
+// (score_elems floats of HBM) and ceil(k / 128) cursor selects of up to 128 (cand_elems uint64 of lists).
+struct WidePlan {
+    uint32_t group, sel_grid;
+    size_t score_elems, cand_elems;
+};
+WidePlan plan_topk_wide(uint32_t n_rows, uint32_t nq);
+// Batch positions p < *d_count (nq when d_count is NULL; read on the device) get the exact answer of query d_pos[p] (p when
+// d_pos is NULL) in d_out[query][0, k), ascending composites, as the single-query path computes them.  Rows of other queries are
+// left alone.  1 + 2 ceil(k / 128) launches per group; a launch whose positions are all dead exits at once.  k <= n_rows.
+cudaError_t launch_topk_wide(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t k, const uint32_t *d_pos,
+                             const uint32_t *d_count, const WidePlan &p, float *d_scores, uint64_t *d_cand, uint64_t *d_out,
+                             const uint32_t *d_abort, cudaStream_t s, LaunchCounters *ctr);
 // Append composite(score,id) of every score <= radius to d_out (capacity n), count in *d_count.
 cudaError_t launch_range_compact(const float *d_scores, uint32_t n, float radius, uint64_t *d_out,
                                  uint32_t *d_count, cudaStream_t s, LaunchCounters *ctr);
