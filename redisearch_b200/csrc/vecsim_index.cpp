@@ -1,5 +1,6 @@
 // Host logic of the device FLAT index.  See vecsim_index.h for the reference files mirrored.
 #include "vecsim_index.h"
+#include "batch_scratch.h"
 #include "host_numeric.h"
 #include "topk_common.cuh"
 #include "coarse_tc.h"
@@ -68,86 +69,31 @@ bool QueryCtx::init() {
     d_abort = static_cast<const uint32_t *>(dp);
     return true;
 }
+template <class T> bool QueryCtx::grow(T *&d, size_t &cap, size_t new_cap, T **h) {
+    cudaStreamSynchronize(stream);
+    cudaFree(d);
+    d = nullptr;
+    if (h) {
+        cudaFreeHost(*h);
+        *h = nullptr;
+    }
+    cap = 0;
+    CU_OK(cudaMalloc(&d, new_cap * sizeof(T)));
+    if (h) CU_OK(cudaMallocHost(h, new_cap * sizeof(T)));
+    cap = new_cap;
+    return true;
+}
 bool QueryCtx::need_query(size_t bytes) {
-    if (bytes <= query_cap) return true;
-    cudaStreamSynchronize(stream);
-    cudaFree(d_query);
-    cudaFreeHost(h_query);
-    d_query = nullptr;
-    h_query = nullptr;
-    query_cap = 0;
-    const size_t cap = std::max<size_t>(bytes, 64 * 1024);
-    CU_OK(cudaMalloc(&d_query, cap));
-    CU_OK(cudaMallocHost(&h_query, cap));
-    query_cap = cap;
-    return true;
+    return bytes <= query_cap || grow(d_query, query_cap, std::max<size_t>(bytes, 64 * 1024), &h_query);
 }
-bool QueryCtx::need_cand(size_t elems) {
-    if (elems <= cand_cap) return true;
-    cudaStreamSynchronize(stream);
-    cudaFree(d_cand);
-    d_cand = nullptr;
-    cand_cap = 0;
-    const size_t cap = std::max<size_t>(elems, 64 * 1024);
-    CU_OK(cudaMalloc(&d_cand, cap * sizeof(uint64_t)));
-    cand_cap = cap;
-    return true;
-}
-bool QueryCtx::need_out(size_t elems) {
-    if (elems <= out_cap) return true;
-    cudaStreamSynchronize(stream);
-    cudaFree(d_out);
-    cudaFreeHost(h_out);
-    d_out = nullptr;
-    h_out = nullptr;
-    out_cap = 0;
-    const size_t cap = std::max<size_t>(elems, 4096);
-    CU_OK(cudaMalloc(&d_out, cap * sizeof(uint64_t)));
-    CU_OK(cudaMallocHost(&h_out, cap * sizeof(uint64_t)));
-    out_cap = cap;
-    return true;
-}
-bool QueryCtx::need_scores(size_t n) {
-    if (n <= scores_cap) return true;
-    cudaStreamSynchronize(stream);
-    cudaFree(d_scores);
-    d_scores = nullptr;
-    scores_cap = 0;
-    const size_t cap = n + n / 8 + 1024;
-    CU_OK(cudaMalloc(&d_scores, cap * sizeof(float)));
-    scores_cap = cap;
-    return true;
-}
-bool QueryCtx::need_ids(size_t n) {
-    if (n <= ids_cap) return true;
-    cudaStreamSynchronize(stream);
-    cudaFree(d_ids);
-    cudaFreeHost(h_ids);
-    cudaFree(d_dist);
-    cudaFreeHost(h_dist);
-    d_ids = h_ids = nullptr;
-    d_dist = h_dist = nullptr;
-    ids_cap = 0;
+bool QueryCtx::need_cand(size_t elems) { return elems <= cand_cap || grow(d_cand, cand_cap, std::max<size_t>(elems, 64 * 1024)); }
+bool QueryCtx::need_out(size_t elems) { return elems <= out_cap || grow(d_out, out_cap, std::max<size_t>(elems, 4096), &h_out); }
+bool QueryCtx::need_scores(size_t n) { return n <= scores_cap || grow(d_scores, scores_cap, n + n / 8 + 1024); }
+bool QueryCtx::need_ids(size_t n) { // ids and distances share one capacity
     const size_t cap = std::max<size_t>(n, 1024);
-    CU_OK(cudaMalloc(&d_ids, cap * 4));
-    CU_OK(cudaMallocHost(&h_ids, cap * 4));
-    CU_OK(cudaMalloc(&d_dist, cap * 4));
-    CU_OK(cudaMallocHost(&h_dist, cap * 4));
-    ids_cap = cap;
-    return true;
+    return n <= ids_cap || (grow(d_ids, ids_cap, cap, &h_ids) && grow(d_dist, ids_cap, cap, &h_dist));
 }
-
-bool QueryCtx::need_lab(size_t elems) {
-    if (elems <= lab_cap) return true;
-    cudaStreamSynchronize(stream);
-    cudaFree(d_lab);
-    d_lab = nullptr;
-    lab_cap = 0;
-    const size_t cap = std::max<size_t>(elems, 64 * 1024);
-    CU_OK(cudaMalloc(&d_lab, cap * sizeof(uint64_t)));
-    lab_cap = cap;
-    return true;
-}
+bool QueryCtx::need_lab(size_t elems) { return elems <= lab_cap || grow(d_lab, lab_cap, std::max<size_t>(elems, 64 * 1024)); }
 
 // ------------------------------------------------------------------------------------------------
 // construction
@@ -287,6 +233,24 @@ int FlatIndex::wait_polling(cudaStream_t s, void *timeout_ctx) const {
         if (cb(timeout_ctx) != 0) return 1;
         std::this_thread::sleep_for(std::chrono::microseconds(50));
     }
+}
+
+int FlatIndex::wait_or_abandon(QueryCtx &c, void *timeout_ctx) const {
+    const int w = wait_polling(c.stream, timeout_ctx);
+    if (w == 1) { // the next checkout synchronises before the buffers are reused
+        c.abandoned = true;
+        *c.h_abort = 1;
+    }
+    return w;
+}
+
+void FlatIndex::record_scan(const QueryCtx *c, uint64_t bytes) {
+    float ms = 0;
+    if (c && cudaEventElapsedTime(&ms, c->ev_start, c->ev_stop) != cudaSuccess) return;
+    std::lock_guard<std::mutex> g(stats_mu_);
+    scan_us_ += ms * 1000.0;
+    scan_launches_++;
+    scan_bytes_ += bytes;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -536,25 +500,26 @@ bool FlatIndex::sync_labels_to_device() {
 // ------------------------------------------------------------------------------------------------
 // queries
 // ------------------------------------------------------------------------------------------------
-bool FlatIndex::upload_query(QueryCtx &c, const uint8_t *stored_q, size_t nq) {
-    const size_t qp = (stored_bytes_ + 15) & ~(size_t)15;
-    if (!c.need_query(qp * nq)) return false;
-    if (stored_q != c.h_query) {
-        for (size_t i = 0; i < nq; i++) {
-            memcpy(c.h_query + i * qp, stored_q + i * stored_bytes_, stored_bytes_);
-            memset(c.h_query + i * qp + stored_bytes_, 0, qp - stored_bytes_);
-        }
+bool FlatIndex::stage_queries(QueryCtx &c, const void *blobs, size_t stride, size_t nq, bool raw, const void *tail, size_t tail_bytes) {
+    const size_t qp = query_pitch(), bytes = qp * nq + tail_bytes;
+    if (!c.need_query(bytes)) return false;
+    memset(c.h_query, 0, qp * nq);
+    for (size_t i = 0; i < nq; i++) {
+        const uint8_t *blob = static_cast<const uint8_t *>(blobs) + i * stride;
+        if (raw)
+            preprocess_query(blob, c.h_query + i * qp);
+        else
+            memcpy(c.h_query + i * qp, blob, stored_bytes_);
     }
-    CU_OK(cudaMemcpyAsync(c.d_query, c.h_query, qp * nq, cudaMemcpyHostToDevice, c.stream));
+    if (tail_bytes) memcpy(c.h_query + qp * nq, tail, tail_bytes);
+    CU_OK(cudaMemcpyAsync(c.d_query, c.h_query, bytes, cudaMemcpyHostToDevice, c.stream));
     return true;
 }
 
-namespace {
-struct KeyedResult {
-    uint32_t key;
-    size_t label;
-};
-} // namespace
+// composite (score key << 32 | row) -> the row's label (from `id_to_label`) and its score
+static VecSimQueryResult decode(uint64_t comp, const std::vector<size_t> &id_to_label) {
+    return {id_to_label[(uint32_t)comp], (double)key_to_float((uint32_t)(comp >> 32))};
+}
 
 // reply ordering: (score asc, label asc) — the order the reference's heap drains in
 // (vecsim_stl.h:64-84) — or by label (vec_utils.cpp:100-103).
@@ -615,13 +580,8 @@ VecSimQueryReply *FlatIndex::topk(const void *q, size_t k, VecSimQueryParams *qp
     }
     auto c = checkout();
     if (!c) return rep;
-    const size_t qpitch = (stored_bytes_ + 15) & ~(size_t)15;
-    bool ok = c->need_query(qpitch);
-    if (ok) {
-        memset(c->h_query, 0, qpitch);
-        preprocess_query(q, c->h_query);
-        ok = upload_query(*c, c->h_query, 1);
-    }
+    const size_t qpitch = query_pitch();
+    bool ok = stage_queries(*c, q, 0, 1, true);
     const CorpusView v = view();
     LaunchCounters lc;
     if (ok && !multi_ && std::min(k, n) <= (size_t)kMaxFusedK) {
@@ -647,10 +607,8 @@ VecSimQueryReply *FlatIndex::topk(const void *q, size_t k, VecSimQueryParams *qp
         }
         ok = ok && cudaMemcpyAsync(c->h_out, d_res, ke * 8, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess;
         if (ok) {
-            const int w = wait_polling(c->stream, tctx);
+            const int w = wait_or_abandon(*c, tctx);
             if (w == 1) { // deadline passed while the scan was running
-                c->abandoned = true;
-                *c->h_abort = 1; // the kernels still running on its stream wind down
                 launches_total_ += lc.launches;
                 checkin(std::move(c));
                 rep->code = VecSim_QueryReply_TimedOut;
@@ -659,18 +617,9 @@ VecSimQueryReply *FlatIndex::topk(const void *q, size_t k, VecSimQueryParams *qp
             ok = w == 0;
         }
         if (ok) {
-            float ms = 0;
-            if (cudaEventElapsedTime(&ms, c->ev_start, c->ev_stop) == cudaSuccess) {
-                std::lock_guard<std::mutex> g(stats_mu_);
-                scan_us_ += ms * 1000.0;
-                scan_launches_++;
-                scan_bytes_ += (uint64_t)n * stored_bytes_;
-            }
-            for (uint32_t i = 0; i < ke; i++) {
-                const uint64_t comp = c->h_out[i];
-                if (comp == kEmptySlot) break;
-                rep->results.push_back({id_to_label_[(uint32_t)comp], (double)key_to_float((uint32_t)(comp >> 32))});
-            }
+            record_scan(c.get(), (uint64_t)n * stored_bytes_);
+            for (uint32_t i = 0; i < ke && c->h_out[i] != kEmptySlot; i++)
+                rep->results.push_back(decode(c->h_out[i], id_to_label_));
         }
     } else if (ok) {
         // k > kMaxFusedK or multi-value: materialise all scores, then cursor-select in chunks.
@@ -695,23 +644,16 @@ VecSimQueryReply *FlatIndex::topk(const void *q, size_t k, VecSimQueryParams *qp
                     break;
                 }
                 for (long i = 0; i < got && rep->results.size() < want_labels; i++) {
-                    const uint64_t comp = c->h_out[i];
-                    const size_t label = id_to_label_[(uint32_t)comp];
-                    if (multi_ && !seen.insert(label).second) continue; // best score per label comes first
-                    rep->results.push_back({label, (double)key_to_float((uint32_t)(comp >> 32))});
+                    const VecSimQueryResult r = decode(c->h_out[i], id_to_label_);
+                    if (multi_ && !seen.insert(r.id).second) continue; // best score per label comes first
+                    rep->results.push_back(r);
                 }
                 scanned += (size_t)got;
                 if ((size_t)got < want) break;
                 has_cursor = true;
                 cursor = c->h_out[got - 1];
             }
-            float ms = 0;
-            if (ok && cudaEventElapsedTime(&ms, c->ev_start, c->ev_stop) == cudaSuccess) {
-                std::lock_guard<std::mutex> g(stats_mu_);
-                scan_us_ += ms * 1000.0;
-                scan_launches_++;
-                scan_bytes_ += (uint64_t)n * stored_bytes_;
-            }
+            if (ok) record_scan(c.get(), (uint64_t)n * stored_bytes_);
         }
     }
     launches_total_ += lc.launches;
@@ -890,6 +832,14 @@ bool FlatIndex::batch_scan(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t
     return multi_ ? batch_scan_labels(c, d_q, qpitch, nq, ke, st, lc, d_result) : batch_scan_rows(c, d_q, qpitch, nq, ke, st, lc, d_result);
 }
 
+// Row-tile stride of a sample pass that visits a fraction f = ke / (aim * row ranges) of the tiles, 1 % <= f <= 25 %: about `aim`
+// slots per (query, row range) of the main pass then fall below the bound it yields.  Small corpora: at least tiles_per_k * ke
+// tiles are visited, so that the sample still holds a few times k candidates.
+static uint32_t sample_stride(const CoarsePlan &probe, uint32_t ke, double aim, double tiles_per_k) {
+    const double f = std::min(0.25, std::max(0.01, (double)ke / (aim * probe.grid_x)));
+    return (uint32_t)std::max(1.0, std::min(std::floor(1.0 / f), std::floor(probe.tiles / (tiles_per_k * ke))));
+}
+
 bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t nq, uint32_t ke, cudaStream_t st,
                                 LaunchCounters &lc, uint64_t **d_result, bool tc_only) {
     const CorpusView v = view();
@@ -917,22 +867,32 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
         // adaptive kernel.  (int8 distances are small integers with massive ties: they stay on the adaptive lists.)
         const CoarsePlan probe = plan_coarse(v, nq, dkind, ke, 0, 1, 1);
         if (is16 && probe.mode == 1 && coarse_fixed_enabled()) {
-            double f = (double)ke / (64.0 * probe.grid_x); // aim at 64 of the 256 slots per (query, row range)
-            f = std::min(0.25, std::max(0.01, f));
-            // small corpora: the sample must still hold a few times k slice minima (4 per visited tile)
-            const uint32_t stride = (uint32_t)std::max(1.0, std::min(std::floor(1.0 / f), std::floor(probe.tiles / (2.0 * ke))));
-            const CoarsePlan cps = plan_coarse(v, nq, dkind, ke, 0, stride, 2);
+            // aim at 64 of the 256 slots per (query, row range); the sample holds a few times k slice minima (4 per visited tile)
+            const CoarsePlan cps = plan_coarse(v, nq, dkind, ke, 0, sample_stride(probe, ke, 64.0, 2.0), 2);
             const bool tier2 = coarse_tier2_enabled();
-            const size_t nM = (size_t)nq * probe.grid_x * probe.keep, nS = (size_t)nq * cps.grid_x * cps.keep, nO = (size_t)nq * ke;
-            const size_t nA2 = tier2 ? (size_t)nq * cp.grid_x * cp.keep : 0;
+            const size_t nO = (size_t)nq * ke;
             const size_t scratch = std::max(std::max(probe.scratch_elems, cps.scratch_elems), tier2 ? cp.scratch_elems : 0);
-            const size_t qcopy = tier2 ? ((size_t)nq * qpitch + 7) / 8 : 0, flag_elems = (nq + 1) / 2 + 1;
-            if (!c.need_cand(nM + nS + nA2 + nO + scratch + qcopy + 5 * flag_elems + 16) || !c.need_out(nO)) return false;
-            uint64_t *cand_m = c.d_cand, *cand_s = cand_m + nM, *cand_t2 = cand_s + nS, *out2 = cand_t2 + nA2, *list_scratch = out2 + nO;
-            uint64_t *q_t2 = list_scratch + scratch, *tail = q_t2 + qcopy;
-            uint32_t *d_ok = reinterpret_cast<uint32_t *>(tail), *d_idx = reinterpret_cast<uint32_t *>(tail + flag_elems);
-            uint32_t *d_n2 = reinterpret_cast<uint32_t *>(tail + 2 * flag_elems), *d_ovf = reinterpret_cast<uint32_t *>(tail + 4 * flag_elems);
-            float *d_thr = reinterpret_cast<float *>(tail + 3 * flag_elems);
+            uint64_t *cand_m, *cand_s, *cand_t2, *out2, *list_scratch;
+            uint8_t *q_t2;
+            uint32_t *d_ok, *d_idx, *d_n2, *d_ovf;
+            float *d_thr;
+            const auto layout = [&](void *base) {
+                BatchScratch s(base);
+                cand_m = s.take<uint64_t>((size_t)nq * probe.grid_x * probe.keep);
+                cand_s = s.take<uint64_t>((size_t)nq * cps.grid_x * cps.keep);
+                cand_t2 = s.take<uint64_t>(tier2 ? (size_t)nq * cp.grid_x * cp.keep : 0);
+                out2 = s.take<uint64_t>(nO);
+                list_scratch = s.take<uint64_t>(scratch);
+                q_t2 = s.take<uint8_t>(tier2 ? (size_t)nq * qpitch : 0); // tier 2: the open queries, packed to the front
+                d_ok = s.take<uint32_t>(nq);
+                d_idx = s.take<uint32_t>(nq); // tier 2: indices of the open queries
+                d_n2 = s.take<uint32_t>(1);   //         and their count
+                d_thr = s.take<float>(nq);    // fixed bound per query
+                d_ovf = s.take<uint32_t>(nq); // a list of the main pass ran full
+                return s.words();
+            };
+            if (!c.need_cand(layout(nullptr)) || !c.need_out(nO)) return false;
+            layout(c.d_cand);
             c.d_last_ok = d_ok;
             c.last_ok_n = nq;
             bool ok = launch_coarse(ops, v.n_rows, v.dim, nq, cps, cand_s, list_scratch, st) == cudaSuccess;
@@ -957,21 +917,28 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
             *d_result = c.d_out;
             return ok;
         }
-        const size_t nA = (size_t)nq * cp.grid_x * cp.keep;
-        const size_t qn_elems = int_l2() ? ((size_t)nq + 1) / 2 : 0; // int8 / uint8 L2: |q|^2 per query, after the list scratch
-        if (!c.need_cand(nA + cp.scratch_elems + qn_elems) || !c.need_out((size_t)nq * ke)) return false;
+        uint64_t *cand, *list_scratch;
+        int32_t *d_qn;
+        const auto layout = [&](void *base) {
+            BatchScratch s(base);
+            cand = s.take<uint64_t>((size_t)nq * cp.grid_x * cp.keep);
+            list_scratch = s.take<uint64_t>(cp.scratch_elems);
+            d_qn = s.take<int32_t>(int_l2() ? nq : 0); // int8 / uint8 L2: |q|^2 per query
+            return s.words();
+        };
+        if (!c.need_cand(layout(nullptr)) || !c.need_out((size_t)nq * ke)) return false;
+        layout(c.d_cand);
         bool ok = true;
         if (int_l2()) {
-            int32_t *d_qn = reinterpret_cast<int32_t *>(c.d_cand + nA + cp.scratch_elems);
             ok = launch_int_norm2(d_q, qpitch, v.dim, 0, nq, dtype_ == DT_I8, d_qn, st) == cudaSuccess;
             ops.row_norm2 = reinterpret_cast<const float *>(d_norm2_); // int32 values (CoarseOperands)
             ops.q_norm2 = reinterpret_cast<const float *>(d_qn);
             lc.launches++;
         }
         cudaEventRecord(c.ev_start, st);
-        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq, cp, c.d_cand, c.d_cand + nA, st) == cudaSuccess;
+        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq, cp, cand, list_scratch, st) == cudaSuccess;
         cudaEventRecord(c.ev_stop, st);
-        ok = ok && launch_final_select(c.d_cand, nq, (uint32_t)(cp.grid_x * cp.keep), ke, c.d_out, st, &lc) == cudaSuccess;
+        ok = ok && launch_final_select(cand, nq, (uint32_t)(cp.grid_x * cp.keep), ke, c.d_out, st, &lc) == cudaSuccess;
         lc.launches++;
         coarse_batches_++;
         *d_result = c.d_out;
@@ -1037,22 +1004,15 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
         if (wide) {
             // k in the hundreds: ranges x 32 slice minima barely hold k values.  The sample pass keeps adaptive lists of 128 per
             // (query, row range) instead; their union holds at least k distinct rows at or below its k-th smallest
-            // approximate distance, so threshold_kernel's bound stands.  Aim at 128 of the 256 slots of the main pass.
-            double f = (double)ke / (128.0 * probe.grid_x);
-            f = std::min(0.25, std::max(0.01, f));
-            // small corpora: the sample must still hold about 4 k rows (128 per visited tile)
-            const uint32_t stride = (uint32_t)std::max(1.0, std::min(std::floor(1.0 / f), std::floor(probe.tiles / (ke / 32.0))));
-            cps = plan_coarse(v, nq, kind, ke, kCoarseKeepWide, stride, 0);
+            // approximate distance, so threshold_kernel's bound stands.  Aim at 128 of the 256 slots of the main pass; the sample
+            // holds about 4 k rows (128 per visited tile).
+            cps = plan_coarse(v, nq, kind, ke, kCoarseKeepWide, sample_stride(probe, ke, 128.0, 1 / 32.0), 0);
         } else {
-            double f = (double)ke / (24.0 * probe.grid_x);
-            f = std::min(0.25, std::max(0.01, f));
-            // small corpora: the sample must still hold a few times k slice minima (4 per visited tile)
-            const uint32_t stride = (uint32_t)std::max(1.0, std::min(std::floor(1.0 / f), std::floor(probe.tiles / (2.0 * ke))));
-            cps = plan_coarse(v, nq, kind, ke, 0, stride, 2);
+            // the sample holds a few times k slice minima (4 per visited tile)
+            cps = plan_coarse(v, nq, kind, ke, 0, sample_stride(probe, ke, 24.0, 2.0), 2);
         }
         cp = probe;
     }
-    const size_t per_query = (size_t)cp.grid_x * cp.keep;
     // second tier (fp16 route): the queries whose first-tier proof failed (a list of the main pass overflowed: more than 96
     // rows of one range within the bound — clustered corpora) are packed to the front and run once more with adaptive
     // lists of 128 per row range.  Nothing is known on the host: the tier's kernels read the count of open queries from
@@ -1060,34 +1020,39 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
     const bool tier2 = kind == CoarseF16 && coarse_tier2_enabled();
     CoarsePlan cp2{};
     if (tier2) cp2 = plan_coarse(v, nq, kind, ke, kCoarseKeepWide);
-    const size_t nA = (size_t)nq * per_query, nO = (size_t)nq * ke;
-    const size_t nS = two_pass ? (size_t)nq * cps.grid_x * cps.keep : 0;
-    const size_t nA2 = tier2 ? (size_t)nq * cp2.grid_x * cp2.keep : 0;
+    const size_t nO = (size_t)nq * ke;
     const size_t q16_pitch = (dim_ * 2 + 15) & ~(size_t)15;
-    const size_t q16_elems = kind == CoarseF16 ? ((size_t)nq * q16_pitch + 7) / 8 : 0;
-    const size_t qn_elems = unit ? 0 : (nq + 1) / 2 + 1; // |q|^2 per query (floats)
+    const size_t q16_bytes = kind == CoarseF16 ? (size_t)nq * q16_pitch : 0;
     const size_t scratch = std::max(std::max(cp.scratch_elems, two_pass ? cps.scratch_elems : 0), tier2 ? cp2.scratch_elems : 0);
-    const size_t flag_elems = (nq + 1) / 2 + 1; // nq uint32 / float values
-    // k > kMaxFusedK: the exact fallback's chunk-select lists take the place of the fused scan's
-    const size_t fb_elems = wide ? wp.cand_elems : sp.cand_elems;
     const size_t nO12 = wide ? 0 : nO; // k > kMaxFusedK: the tiers write the answer rows in place, no out1 / out2
-    const size_t total = nA + nS + nA2 + 2 * nO12 + fb_elems + (tier2 ? 2 : 1) * (q16_elems + qn_elems) + scratch + 5 * flag_elems + 16;
-    if (!c.need_cand(total) || !c.need_out(nO) || (wide && !c.need_scores(wp.score_elems))) return false;
-    uint64_t *coarse_cand = c.d_cand, *cand_s = coarse_cand + nA, *cand_t2 = cand_s + nS, *out1 = cand_t2 + nA2, *out2 = out1 + nO12,
-             *cand2 = out2 + nO12;
-    uint64_t *q16 = cand2 + fb_elems;
+    uint64_t *coarse_cand, *cand_s, *cand_t2, *out1, *out2, *cand2, *list_scratch;
+    uint8_t *q16, *q16_t2;
+    float *d_qn2, *d_qn2_t2, *d_thr;
+    uint32_t *d_ok, *d_idx, *d_n2, *d_ovf;
+    const auto layout = [&](void *base) {
+        BatchScratch s(base);
+        coarse_cand = s.take<uint64_t>((size_t)nq * cp.grid_x * cp.keep);
+        cand_s = s.take<uint64_t>(two_pass ? (size_t)nq * cps.grid_x * cps.keep : 0);
+        cand_t2 = s.take<uint64_t>(tier2 ? (size_t)nq * cp2.grid_x * cp2.keep : 0);
+        out1 = s.take<uint64_t>(nO12);
+        out2 = s.take<uint64_t>(nO12);
+        // k > kMaxFusedK: the exact fallback's chunk-select lists take the place of the fused scan's
+        cand2 = s.take<uint64_t>(wide ? wp.cand_elems : sp.cand_elems);
+        q16 = s.take<uint8_t>(q16_bytes);
+        q16_t2 = s.take<uint8_t>(tier2 ? q16_bytes : 0);
+        list_scratch = s.take<uint64_t>(scratch);
+        d_qn2 = s.take<float>(unit ? 0 : nq); // |q|^2 per query
+        d_qn2_t2 = s.take<float>(unit || !tier2 ? 0 : nq);
+        d_ok = s.take<uint32_t>(nq);
+        d_idx = s.take<uint32_t>(nq); // tier 2: indices of the open queries
+        d_n2 = s.take<uint32_t>(1);   //         and their count
+        d_thr = s.take<float>(nq);    // fixed bound per query
+        d_ovf = s.take<uint32_t>(nq); // a list of the main pass ran full
+        return s.words();
+    };
+    if (!c.need_cand(layout(nullptr)) || !c.need_out(nO) || (wide && !c.need_scores(wp.score_elems))) return false;
+    layout(c.d_cand);
     if (wide) out1 = c.d_out; // both tiers and the exact fallback write their rows of the answer in place (no blend)
-    uint64_t *q16_t2 = q16 + q16_elems;
-    uint64_t *list_scratch = q16_t2 + (tier2 ? q16_elems : 0);
-    uint64_t *tail = list_scratch + scratch;
-    float *d_qn2 = unit ? nullptr : reinterpret_cast<float *>(tail);
-    float *d_qn2_t2 = (unit || !tier2) ? nullptr : reinterpret_cast<float *>(tail + qn_elems);
-    tail += (tier2 ? 2 : 1) * qn_elems;
-    uint32_t *d_ok = reinterpret_cast<uint32_t *>(tail);
-    uint32_t *d_idx = reinterpret_cast<uint32_t *>(tail + flag_elems); // tier 2: indices of the open queries
-    uint32_t *d_n2 = reinterpret_cast<uint32_t *>(tail + 2 * flag_elems); //         and their count
-    float *d_thr = reinterpret_cast<float *>(tail + 3 * flag_elems);       // fixed bound per query
-    uint32_t *d_ovf = reinterpret_cast<uint32_t *>(tail + 4 * flag_elems); // a list of the main pass ran full
     c.d_last_ok = d_ok;
     c.last_ok_n = nq;
     CoarseOperands ops{v.rows, v.pitch, d_q, qpitch, 0, 0, nullptr, nullptr};
@@ -1155,11 +1120,21 @@ bool FlatIndex::batch_scan_labels(QueryCtx &c, const void *d_q, size_t qpitch, u
     const CorpusView v = view();
     const uint32_t K = (uint32_t)std::min<size_t>(std::min<size_t>(kMaxFusedK, (size_t)kl * max_rows_per_label()), v.n_rows);
     const ScanPlan sp = plan_scan_topk(v, nq, kl, true);
-    const size_t nO = (size_t)nq * kl, flag_elems = (nq + 1) / 2 + 1;
-    // [label answers nq x kl][exact answers nq x kl][lists of the exact scan][label check per query][reported flags]
-    if (!c.need_lab(2 * nO + sp.cand_elems + 2 * flag_elems)) return false;
-    uint64_t *out1 = c.d_lab, *out2 = out1 + nO, *cand = out2 + nO;
-    uint32_t *lab_ok = reinterpret_cast<uint32_t *>(cand + sp.cand_elems), *flags = reinterpret_cast<uint32_t *>(cand + sp.cand_elems + flag_elems);
+    const size_t nO = (size_t)nq * kl;
+    uint64_t *out1, *out2, *cand;
+    uint32_t *lab_ok, *flags;
+    const auto layout = [&](void *base) {
+        BatchScratch s(base);
+        out1 = s.take<uint64_t>(nO);              // label answers
+        out2 = s.take<uint64_t>(nO);              // exact answers
+        cand = s.take<uint64_t>(sp.cand_elems);   // lists of the exact scan
+        lab_ok = s.take<uint32_t>(nq);            // label check per query
+        flags = s.take<uint32_t>(nq);             // reported flags
+        return s.words();
+    };
+    // d_lab, not d_cand: the row stage below lays out its own scratch there
+    if (!c.need_lab(layout(nullptr))) return false;
+    layout(c.d_lab);
     uint64_t *rows = nullptr;
     if (!batch_scan_rows(c, d_q, qpitch, nq, K, st, lc, &rows, true)) return false;
     bool ok = true;
@@ -1228,16 +1203,10 @@ int FlatIndex::topk_batch(const void *qs, size_t qstride, size_t nq, size_t k, V
     if (multi_ && !sync_labels_to_device()) return -1;
     auto c = checkout();
     if (!c) return -1;
-    const size_t qpitch = (stored_bytes_ + 15) & ~(size_t)15;
+    const size_t qpitch = query_pitch();
     const uint32_t ke = (uint32_t)std::min(k, multi_ ? label_count() : n); // a multi-value index answers labels
-    const CorpusView v = view();
     LaunchCounters lc;
-    bool ok = c->need_query(qpitch * nq);
-    if (ok) {
-        memset(c->h_query, 0, qpitch * nq);
-        for (size_t i = 0; i < nq; i++) preprocess_query(static_cast<const uint8_t *>(qs) + i * qstride, c->h_query + i * qpitch);
-        ok = cudaMemcpyAsync(c->d_query, c->h_query, qpitch * nq, cudaMemcpyHostToDevice, c->stream) == cudaSuccess;
-    }
+    bool ok = stage_queries(*c, qs, qstride, nq, true);
     uint64_t *d_res = nullptr;
     // multi-value: queries the label stage could not prove, or all of them, are answered one at a time below (batch_scan_labels)
     bool per_query_all = false;
@@ -1257,10 +1226,8 @@ int FlatIndex::topk_batch(const void *qs, size_t qstride, size_t nq, size_t k, V
     ok = ok && (per_query_all || cudaMemcpyAsync(c->h_out, c->d_out, nq * ke * 8, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess);
     launches_total_ += lc.launches;
     if (ok) {
-        const int w = wait_polling(c->stream, tctx); // a full exact-scan fallback no longer holds a timed-out caller
+        const int w = wait_or_abandon(*c, tctx); // a full exact-scan fallback no longer holds a timed-out caller
         if (w == 1) {
-            c->abandoned = true;
-                *c->h_abort = 1; // the kernels still running on its stream wind down
             checkin(std::move(c));
             return VecSim_QueryReply_TimedOut;
         }
@@ -1276,25 +1243,15 @@ int FlatIndex::topk_batch(const void *qs, size_t qstride, size_t nq, size_t k, V
     }
     std::vector<size_t> open; // multi-value queries whose label check failed (flag 3)
     if (ok) {
-        float ms = 0;
-        if (cudaEventElapsedTime(&ms, c->ev_start, c->ev_stop) == cudaSuccess) {
-            std::lock_guard<std::mutex> g(stats_mu_);
-            scan_us_ += ms * 1000.0;
-            scan_launches_++;
-            scan_bytes_ += (uint64_t)n * stored_bytes_;
-        }
+        record_scan(c.get(), (uint64_t)n * stored_bytes_);
         if (d_flags)
             for (size_t i = 0; i < nq; i++)
                 if (c->h_ids[i] == 3u) open.push_back(i);
-        std::vector<VecSimQueryResult> tmp;
         VecSimQueryReply rr;
         for (size_t i = 0; i < nq; i++) {
             rr.results.clear();
-            for (uint32_t j = 0; j < ke; j++) {
-                const uint64_t comp = c->h_out[i * ke + j];
-                if (comp == kEmptySlot) break;
-                rr.results.push_back({id_to_label_[(uint32_t)comp], (double)key_to_float((uint32_t)(comp >> 32))});
-            }
+            for (uint32_t j = 0; j < ke && c->h_out[i * ke + j] != kEmptySlot; j++)
+                rr.results.push_back(decode(c->h_out[i * ke + j], id_to_label_));
             finish_reply(&rr, BY_SCORE);
             for (size_t j = 0; j < rr.results.size(); j++) {
                 out_labels[i * k + j] = rr.results[j].id;
@@ -1329,7 +1286,7 @@ int FlatIndex::topk_batch_device(const void *d_q, size_t nq, size_t k, int64_t *
     QueryCtx *c = dev_ctx_.get();
     if (!c) return -1;
     collect_dev_timing_locked(); // the previous call's scan events (stream-ordered before this call)
-    const size_t qpitch = (stored_bytes_ + 15) & ~(size_t)15;
+    const size_t qpitch = query_pitch();
     const uint32_t ke = (uint32_t)std::min(k, std::max<size_t>(multi_ ? label_count() : n, 1));
     cudaStream_t st = s ? s : cudaStreamLegacy; // NULL = the legacy default stream, as everywhere in CUDA
     LaunchCounters lc;
@@ -1372,14 +1329,8 @@ VecSimQueryReply *FlatIndex::range(const void *q, double radius, VecSimQueryPara
     }
     auto c = checkout();
     if (!c) return rep;
-    const size_t qpitch = (stored_bytes_ + 15) & ~(size_t)15;
     LaunchCounters lc;
-    bool ok = c->need_query(qpitch) && c->need_scores(n) && c->need_cand(n);
-    if (ok) {
-        memset(c->h_query, 0, qpitch);
-        preprocess_query(q, c->h_query);
-        ok = upload_query(*c, c->h_query, 1);
-    }
+    bool ok = c->need_scores(n) && c->need_cand(n) && stage_queries(*c, q, 0, 1, true);
     const CorpusView v = view();
     ok = ok && launch_scan_scores(v, c->d_query, c->d_scores, c->stream, &lc) == cudaSuccess;
     ok = ok && launch_range_compact(c->d_scores, (uint32_t)n, (float)radius, c->d_cand, c->d_count, c->stream, &lc) == cudaSuccess;
@@ -1403,10 +1354,7 @@ VecSimQueryReply *FlatIndex::range(const void *q, double radius, VecSimQueryPara
                 for (auto &kv : best) rep->results.push_back({kv.first, (double)key_to_float(kv.second)});
             } else {
                 rep->results.reserve(m);
-                for (uint32_t i = 0; i < m; i++) {
-                    const uint64_t comp = c->h_out[i];
-                    rep->results.push_back({id_to_label_[(uint32_t)comp], (double)key_to_float((uint32_t)(comp >> 32))});
-                }
+                for (uint32_t i = 0; i < m; i++) rep->results.push_back(decode(c->h_out[i], id_to_label_));
             }
         }
     }
@@ -1460,30 +1408,30 @@ int FlatIndex::range_batch(const void *qs, size_t qstride, size_t nq, const doub
         LaunchCounters lc;
         const bool unit = unit_rows();
         // stored-form queries, then the radii as float (the reference compares score <= DistType(radius))
-        const size_t qpitch = (stored_bytes_ + 15) & ~(size_t)15, radii_off = qpitch * nq;
-        bool ok = c->need_query(radii_off + nq * sizeof(float));
-        if (ok) {
-            memset(c->h_query, 0, radii_off);
-            float *hr = reinterpret_cast<float *>(c->h_query + radii_off);
-            for (size_t i = 0; i < nq; i++) {
-                preprocess_query(static_cast<const uint8_t *>(qs) + i * qstride, c->h_query + i * qpitch);
-                hr[i] = (float)radii[i];
-            }
-            ok = cudaMemcpyAsync(c->d_query, c->h_query, radii_off + nq * sizeof(float), cudaMemcpyHostToDevice, st) == cudaSuccess;
-        }
-        const float *d_radius = reinterpret_cast<const float *>(c->d_query + radii_off);
+        const size_t qpitch = query_pitch();
+        const std::vector<float> radii_f(radii, radii + nq);
+        bool ok = stage_queries(*c, qs, qstride, nq, true, radii_f.data(), nq * sizeof(float));
+        const float *d_radius = reinterpret_cast<const float *>(c->d_query + qpitch * nq);
         const CoarsePlan cp = plan_coarse(v, nq32, CoarseF16, 1, 0, 1, 1);
-        const size_t slots = (size_t)cp.grid_x * cp.keep, nA = nq * slots;
-        const size_t q16_pitch = (dim_ * 2 + 15) & ~(size_t)15, q16_elems = (nq * q16_pitch + 7) / 8;
-        const size_t flag_elems = (nq + 1) / 2 + 1; // nq uint32 / float values
-        const size_t qn_elems = unit ? 0 : flag_elems, res_elems = (3 * nq + 1 + 1) / 2 + 1;
-        ok = ok && c->need_cand(2 * nA + q16_elems + cp.scratch_elems + qn_elems + 2 * flag_elems + res_elems) && c->need_ids(3 * nq + 1);
-        uint64_t *cand = c->d_cand, *hits = cand + nA, *q16 = hits + nA, *list_scratch = q16 + q16_elems, *tail = list_scratch + cp.scratch_elems;
-        float *d_qn2 = unit ? nullptr : reinterpret_cast<float *>(tail); // |q|^2 per query
-        tail += qn_elems;
-        float *d_thr = reinterpret_cast<float *>(tail);                         // bound of the main pass per query
-        uint32_t *d_ovf = reinterpret_cast<uint32_t *>(tail + flag_elems);     // a list of the main pass ran full
-        uint32_t *d_res = reinterpret_cast<uint32_t *>(tail + 2 * flag_elems); // [ok nq][count nq][offset nq][hits in total]
+        const size_t slots = (size_t)cp.grid_x * cp.keep, q16_pitch = (dim_ * 2 + 15) & ~(size_t)15;
+        uint64_t *cand, *hits, *list_scratch;
+        uint8_t *q16;
+        float *d_qn2, *d_thr;
+        uint32_t *d_ovf, *d_res;
+        const auto layout = [&](void *base) {
+            BatchScratch s(base);
+            cand = s.take<uint64_t>(nq * slots);
+            hits = s.take<uint64_t>(nq * slots);
+            q16 = s.take<uint8_t>(nq * q16_pitch);
+            list_scratch = s.take<uint64_t>(cp.scratch_elems);
+            d_qn2 = s.take<float>(unit ? 0 : nq);  // |q|^2 per query
+            d_thr = s.take<float>(nq);             // bound of the main pass per query
+            d_ovf = s.take<uint32_t>(nq);          // a list of the main pass ran full
+            d_res = s.take<uint32_t>(3 * nq + 1);  // [ok nq][count nq][offset nq][hits in total]
+            return s.words();
+        };
+        ok = ok && c->need_cand(layout(nullptr)) && c->need_ids(3 * nq + 1);
+        layout(c->d_cand);
         uint32_t *d_total = d_res + 3 * nq;
         ok = ok && launch_to_f16(c->d_query, qpitch, (uint32_t)dim_, 0, nq32, q16, q16_pitch, st) == cudaSuccess;
         if (!unit) ok = ok && launch_row_stats(c->d_query, qpitch, (uint32_t)dim_, 0, nq32, d_qn2, nullptr, st) == cudaSuccess;
@@ -1500,10 +1448,8 @@ int FlatIndex::range_batch(const void *qs, size_t qstride, size_t nq, const doub
         launches_total_ += lc.launches;
         coarse_batches_++;
         if (ok) {
-            const int w = wait_polling(st, tctx);
+            const int w = wait_or_abandon(*c, tctx);
             if (w == 1) { // deadline passed while the pass was running
-                c->abandoned = true;
-                *c->h_abort = 1;
                 checkin(std::move(c));
                 return all_timed_out();
             }
@@ -1511,13 +1457,7 @@ int FlatIndex::range_batch(const void *qs, size_t qstride, size_t nq, const doub
         }
         const uint32_t *h_ok = c->h_ids, *h_cnt = h_ok + nq, *h_off = h_cnt + nq;
         if (ok) {
-            float ms = 0;
-            if (cudaEventElapsedTime(&ms, c->ev_start, c->ev_stop) == cudaSuccess) {
-                std::lock_guard<std::mutex> g(stats_mu_);
-                scan_us_ += ms * 1000.0;
-                scan_launches_++;
-                scan_bytes_ += (uint64_t)n * stored_bytes_;
-            }
+            record_scan(c.get(), (uint64_t)n * stored_bytes_);
             const uint32_t total = h_ok[3 * nq]; // only the occupied part of the result buffer crosses PCIe
             ok = c->need_out(total) && cudaMemcpyAsync(c->h_out, hits, (size_t)total * 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
                  cudaStreamSynchronize(st) == cudaSuccess;
@@ -1527,10 +1467,7 @@ int FlatIndex::range_batch(const void *qs, size_t qstride, size_t nq, const doub
                 if (!h_ok[i]) continue;
                 auto *rep = new VecSimQueryReply();
                 rep->results.reserve(h_cnt[i]);
-                for (uint32_t j = 0; j < h_cnt[i]; j++) {
-                    const uint64_t comp = c->h_out[(size_t)h_off[i] + j];
-                    rep->results.push_back({id_to_label_[(uint32_t)comp], (double)key_to_float((uint32_t)(comp >> 32))});
-                }
+                for (uint32_t j = 0; j < h_cnt[i]; j++) rep->results.push_back(decode(c->h_out[(size_t)h_off[i] + j], id_to_label_));
                 finish_reply(rep, order);
                 replies[i] = rep;
                 if (out_flags) out_flags[i] = 1;
@@ -1581,7 +1518,7 @@ double FlatIndex::distance_from(size_t label, const void *blob) {
     auto c = checkout();
     if (!c) return nan;
     LaunchCounters lc;
-    bool ok = c->need_ids(ids.size()) && upload_query(*c, static_cast<const uint8_t *>(blob), 1);
+    bool ok = c->need_ids(ids.size()) && stage_queries(*c, blob, 0, 1, false);
     if (ok) {
         for (size_t i = 0; i < ids.size(); i++) c->h_ids[i] = ids[i];
         ok = cudaMemcpyAsync(c->d_ids, c->h_ids, ids.size() * 4, cudaMemcpyHostToDevice, c->stream) == cudaSuccess;
@@ -1635,7 +1572,7 @@ bool FlatIndex::prefer_adhoc(size_t subset, size_t k, bool initial) {
 BatchIter *FlatIndex::batch_new(const void *q, VecSimQueryParams *qp) {
     auto *it = new BatchIter();
     it->index = this;
-    it->query.assign((stored_bytes_ + 15) & ~(size_t)15, 0);
+    it->query.assign(query_pitch(), 0);
     preprocess_query(q, it->query.data()); // forced copy, brute_force.h:371-372
     it->timeout_ctx = qp ? qp->timeoutCtx : nullptr;
     it->label_count = label_count();
@@ -1658,16 +1595,11 @@ VecSimQueryReply *FlatIndex::batch_next(BatchIter *it, size_t n_res, VecSimQuery
         if (!it->ctx) return rep;
         if (it->n_rows) {
             LaunchCounters lc;
-            bool ok = it->ctx->need_scores(it->n_rows) && upload_query(*it->ctx, it->query.data(), 1);
-            // upload_query copies stored_bytes_ from a tightly packed source
+            bool ok = it->ctx->need_scores(it->n_rows) && stage_queries(*it->ctx, it->query.data(), 0, 1, false);
             ok = ok && launch_scan_scores(view(), it->ctx->d_query, it->ctx->d_scores, it->ctx->stream, &lc) == cudaSuccess;
             ok = ok && cudaStreamSynchronize(it->ctx->stream) == cudaSuccess;
             launches_total_ += lc.launches;
-            {
-                std::lock_guard<std::mutex> g(stats_mu_);
-                scan_launches_++;
-                scan_bytes_ += (uint64_t)it->n_rows * stored_bytes_;
-            }
+            record_scan(nullptr, (uint64_t)it->n_rows * stored_bytes_);
             if (!ok) return rep;
         }
         it->scored = true;
@@ -1686,11 +1618,11 @@ VecSimQueryReply *FlatIndex::batch_next(BatchIter *it, size_t n_res, VecSimQuery
         for (long i = 0; i < got; i++) {
             const uint64_t comp = it->ctx->h_out[i];
             if (produced < want_labels) {
-                const size_t label = it->id_to_label_snap[(uint32_t)comp];
+                const VecSimQueryResult r = decode(comp, it->id_to_label_snap);
                 it->has_cursor = true;
                 it->cursor = comp;
-                if (multi_ && !it->seen.insert(label).second) continue;
-                rep->results.push_back({label, (double)key_to_float((uint32_t)(comp >> 32))});
+                if (multi_ && !it->seen.insert(r.id).second) continue;
+                rep->results.push_back(r);
                 produced++;
             } else {
                 break; // leave the rest for the next call: cursor stays on the last consumed entry
@@ -1750,7 +1682,7 @@ void FlatIndex::adhoc_distances(AdhocCtx *a, const size_t *labels, double *out, 
     if (ids.empty()) return;
     bool ok = c.need_ids(ids.size());
     if (ok && !a->query_on_device) {
-        ok = upload_query(c, a->query.data(), 1);
+        ok = stage_queries(c, a->query.data(), 0, 1, false);
         a->query_on_device = ok;
     }
     if (ok) {
@@ -1831,14 +1763,8 @@ int FlatIndex::topk_filtered(const void *q, size_t k, const uint32_t *doc_ids, s
     if (!sync_label_table()) return -2;
     auto c = checkout();
     if (!c) return -1;
-    const size_t qpitch = (stored_bytes_ + 15) & ~(size_t)15;
     LaunchCounters lc;
-    bool ok = c->need_query(qpitch) && c->need_ids(2 * n + 256) && c->need_scores(n);
-    if (ok) {
-        memset(c->h_query, 0, qpitch);
-        preprocess_query(q, c->h_query);
-        ok = upload_query(*c, c->h_query, 1);
-    }
+    bool ok = c->need_ids(2 * n + 256) && c->need_scores(n) && stage_queries(*c, q, 0, 1, true);
     // d_ids: [0,n) row ids, [n,2n) the labels when they arrive from the host
     const uint32_t *d_labels = doc_ids;
     if (ok && !ids_on_device) {
@@ -1898,7 +1824,6 @@ int FlatIndex::topk_filtered_batch(const void *const *queries, size_t nq, size_t
     if (!flush()) return -1;
     if (count_ == 0) return 0;
     if (!sync_label_table()) return -2;
-    const size_t qpitch = (stored_bytes_ + 15) & ~(size_t)15;
     constexpr size_t kWave = 16; // contexts in flight at once
     int rc = 0;
     for (size_t q0 = 0; q0 < nq && rc == 0; q0 += kWave) {
@@ -1926,13 +1851,8 @@ int FlatIndex::topk_filtered_batch(const void *const *queries, size_t nq, size_t
             QueryCtx &c = *j.c;
             j.want = std::min(k, n);
             const uint32_t lists = plan_select_scores_lists((uint32_t)n);
-            bool ok = c.need_query(qpitch) && c.need_ids(2 * n + 256) && c.need_scores(n) && c.need_out(j.want + 1) &&
-                      c.need_cand((size_t)lists * j.want);
-            if (ok) {
-                memset(c.h_query, 0, qpitch);
-                preprocess_query(queries[qi], c.h_query);
-                ok = upload_query(c, c.h_query, 1);
-            }
+            bool ok = c.need_ids(2 * n + 256) && c.need_scores(n) && c.need_out(j.want + 1) && c.need_cand((size_t)lists * j.want) &&
+                      stage_queries(c, queries[qi], 0, 1, true);
             const uint32_t *d_labels = d_doc_ids[qi];
             if (multi_) {
                 ok = ok && launch_gather_min_distances(view(), c.d_query, d_labels, (uint32_t)n, d_label_to_id_, (uint32_t)l2i_size_,
@@ -2152,14 +2072,7 @@ void set_coarse_mode(int mode) { g_coarse_mode.store(mode); }
 // dev_mu_ held.  Folds the CUDA-event timing of the last topk_batch_device scan into the stats.
 void FlatIndex::collect_dev_timing_locked() {
     if (!dev_timing_pending_ || !dev_ctx_) return;
-    float ms = 0;
-    if (cudaEventSynchronize(dev_ctx_->ev_stop) == cudaSuccess &&
-        cudaEventElapsedTime(&ms, dev_ctx_->ev_start, dev_ctx_->ev_stop) == cudaSuccess) {
-        std::lock_guard<std::mutex> g(stats_mu_);
-        scan_us_ += ms * 1000.0;
-        scan_launches_++;
-        scan_bytes_ += dev_timing_bytes_;
-    }
+    if (cudaEventSynchronize(dev_ctx_->ev_stop) == cudaSuccess) record_scan(dev_ctx_.get(), dev_timing_bytes_);
     dev_timing_pending_ = false;
 }
 

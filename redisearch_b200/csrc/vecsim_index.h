@@ -84,6 +84,10 @@ struct QueryCtx {
     bool need_scores(size_t n);
     bool need_ids(size_t n);
     bool need_lab(size_t elems);
+
+  private:
+    // once the stream is idle: frees d (and its pinned mirror *h), then allocates new_cap elements for each; cap = new_cap on success
+    template <class T> bool grow(T *&d, size_t &cap, size_t new_cap, T **h = nullptr);
 };
 
 class FlatIndex;
@@ -194,10 +198,17 @@ class FlatIndex {
     // the reference checks it per vector (brute_force.h:265-269); a device pass cannot be interrupted, but the caller
     // is released as soon as the deadline passes.  0 = done, 1 = timed out (the stream is still busy), -1 = CUDA error.
     int wait_polling(cudaStream_t s, void *timeout_ctx) const;
+    // wait_polling on c's stream; on a timeout c is marked abandoned and its running kernels are told to wind down (h_abort)
+    int wait_or_abandon(QueryCtx &c, void *timeout_ctx) const;
+    // a scan over `bytes` of rows into the stats, timed by c's events (c == NULL: untimed)
+    void record_scan(const QueryCtx *c, uint64_t bytes);
     // k smallest composites (> cursor) over ctx->d_scores[0..n) into ctx->h_out, chunked by
     // kMaxFusedK; returns the number found or -1.
     long select_from_scores(QueryCtx &c, uint32_t n, bool has_cursor, uint64_t cursor, size_t want);
-    bool upload_query(QueryCtx &c, const uint8_t *stored_q, size_t nq);
+    size_t query_pitch() const { return (stored_bytes_ + 15) & ~(size_t)15; } // bytes between staged queries
+    // nq query blobs, `stride` bytes apart -> c.d_query, query_pitch() apart and zero-padded, then `tail_bytes` of `tail`.  raw:
+    // the blobs are put in stored form (preprocess_query); else they are in stored form already
+    bool stage_queries(QueryCtx &c, const void *blobs, size_t stride, size_t nq, bool raw, const void *tail = nullptr, size_t tail_bytes = 0);
     // [nq][ke] best composites of a batch: rows of a single-value index, labels (score, best row) of a multi-value one
     bool batch_scan(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t nq, uint32_t ke, cudaStream_t st, LaunchCounters &lc,
                     uint64_t **d_result);

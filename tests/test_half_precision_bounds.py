@@ -710,6 +710,33 @@ def test_ties_overflowing_a_row_range_resolve_by_label_on_the_second_tier(vtype)
 
 
 @pytest.mark.gpu
+def test_clustered_corpus_overflowing_a_row_range_reaches_the_second_tier():
+    """Clusters of near-duplicates, as in test_vecsim_coarse.py's clustered corpus, but 300 of them per query, in three row tiles
+    of one row range of the main pass that the sample pass does not visit: more rows fall below the bound than that range's list
+    of 256 holds, so every query of an odd-sized batch (nq = 17, k = 7) is gathered into the second tier (flag 2)."""
+    vtype, n, dim, nq, k = F16, 70_000, 128, 17, 7
+    stride, gx = _sample_stride(n, k, nq)
+    bases = [b for b in range(1, gx) if all((b + j * gx) % stride for j in range(3))][:nq]
+    assert len(bases) == nq and (bases[-1] + 2 * gx + 1) * 128 <= n
+    rng = np.random.default_rng(23)
+    rows = ol.synth_rows(vtype, 31, 0, n, dim)
+    centers = rng.uniform(-1, 1, (nq, dim)).astype(np.float32)
+    for b, center in zip(bases, centers):
+        for t in (b, b + gx, b + 2 * gx):
+            rows[t * 128:t * 128 + 100] = to16(center[None, :] + 2e-3 * rng.standard_normal((100, dim)).astype(np.float32), vtype)
+    qs = to16(centers + 2e-3 * rng.standard_normal((nq, dim)).astype(np.float32), vtype)
+    g = new_index(vtype, dim, COS, rows)
+    bl, bs, f = route_batch(g, qs, k, host_too=True)
+    assert _vs().lib().VecSimB200_LastBatchPath(g.h) == 2
+    assert f is not None and (f == 2).all(), f
+    e_all, b_all = _exact_many(g, stored_rows(g, n), qs, vtype, COS, bound_tensor_core)
+    worst = 0.0
+    for i in range(nq):
+        worst = max(worst, check_answer(bl[i].astype(np.int64), bs[i], e_all[i], b_all[i], k))
+    _report(f"tensor-core clustered corpus on the second tier {TNAME[vtype]}", worst)
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize("vtype", [F16, BF16])
 def test_duplicates_across_the_k_boundary_on_the_route(vtype):
     """Exact duplicates of rows (as the 8-bit route's test plants them) and a query equal to one of them: ties at every k

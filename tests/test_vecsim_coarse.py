@@ -32,7 +32,7 @@ def _device_batch(vs, torch, index, qs_norm, k):
 @pytest.mark.parametrize("n,dim,nq,k", [(70_000, 128, 40, 10), (66_000, 768, 64, 10), (131_072, 96, 17, 16), (80_000, 104, 33, 5),
                                         (70_000, 128, 128, 10), (300_000, 64, 256, 10), (66_000, 256, 512, 8),
                                         (66_000, 1024, 70, 10), (70_000, 32, 40, 10), (70_000, 40, 40, 10), (66_000, 776, 64, 10),
-                                        (66_000, 1016, 64, 10)])
+                                        (66_000, 1016, 64, 10), (70_000, 128, 401, 9)])
 def test_coarse_path_is_exact(n, dim, nq, k, mode):
     import torch
 
