@@ -21,7 +21,9 @@
 //             epilogue: the accumulators are transposed through shared memory so that a thread owns one query, raw
 //             dot products are tested against a register threshold, survivors go to a per-query list in global memory
 //             that a warp-wide radix select cuts back to the best `keep`.  The fixed-bound pass tests its bound on the
-//             accumulator fragment itself (no transpose) and appends survivors at slots from shared per-query counters.
+//             accumulator fragment itself (no transpose) and appends survivors at slots from shared per-query counters;
+//             it runs a second such warpgroup (warps 8-11), the two taking the CTA's tiles alternately so that one's
+//             drain and bound test overlap the other's MMAs.
 // coarse_kernel<CfgTF32>: the SS shape with the rows as the M operand (32 queries per CTA in shared memory), kept for
 // fp32 corpora without shadow memory (mode 2) and rows too wide for the 16-bit kernel's shared memory.
 #include "coarse_tc.h"
@@ -556,6 +558,49 @@ __host__ __device__ constexpr uint32_t coarse_kb(uint32_t bytes_per_row) {
 }
 constexpr int kQAccStride = kQN + 4;                            // accumulator transpose [64 queries][132 words]
 constexpr uint32_t kQAccBytes = kQM * kQAccStride * 4;
+// The fixed-bound pass (mode 1) runs two consumer warpgroups that take the CTA's tiles alternately: one warpgroup's
+// drain and bound test run under the other's MMAs instead of leaving the tensor pipe idle at every tile boundary
+// (DESIGN.md §4.2: 5,022 -> 4,294 clk per tile at 10M x 768).  The other modes keep one: their epilogue transposes
+// through shared memory and compacts lists, which a second warpgroup would have to double.
+__host__ __device__ constexpr int coarse_consumers(int mode) { return mode == 1 ? 2 : 1; }
+// warp 0 produces, warps 1-3 idle, warps 4.. are the consumer warpgroups
+__host__ __device__ constexpr int coarse_threads(int mode) { return 128 * (1 + coarse_consumers(mode)); }
+
+// bar.sync / bar.arrive on a named barrier (ids 1-3 in coarse_wgmma_kernel; 0 is __syncthreads)
+template <int kId, int kCount>
+__device__ __forceinline__ void named_sync() {
+    asm volatile("bar.sync %0, %1;" ::"n"(kId), "n"(kCount) : "memory");
+}
+template <int kId, int kCount>
+__device__ __forceinline__ void named_arrive() {
+    asm volatile("bar.arrive %0, %1;" ::"n"(kId), "n"(kCount) : "memory");
+}
+
+// Cycle account of the fixed-bound pass (tools/coarse_cycles.py), compiled only with -DCOARSE_CYCLE_ACCOUNT: per CTA and
+// role (consumer warpgroup 0, 1, producer), clock64() sums of the phases below.  Without the macro every call is empty
+// and the kernels compile to the same code as without the calls.
+enum : int { kCaPass, kCaWait, kCaIssue, kCaWait1, kCaEpilogue, kCaHandoff, kCaTiles, kCaSlots };
+#ifdef COARSE_CYCLE_ACCOUNT
+constexpr int kCaMaxCtas = 1024;
+__device__ unsigned long long g_coarse_cycles[kCaMaxCtas][3][kCaSlots];
+struct CycleAccount {
+    unsigned long long v[kCaSlots] = {};
+    __device__ __forceinline__ long long now() const { return clock64(); }
+    __device__ __forceinline__ void add(int slot, long long t0) { v[slot] += (unsigned long long)(clock64() - t0); }
+    __device__ __forceinline__ void count(int slot) { v[slot]++; }
+    __device__ __forceinline__ void flush(uint32_t cta, int role) {
+        if (cta < (uint32_t)kCaMaxCtas)
+            for (int i = 0; i < kCaSlots; i++) g_coarse_cycles[cta][role][i] = v[i];
+    }
+};
+#else
+struct CycleAccount {
+    __device__ __forceinline__ long long now() const { return 0; }
+    __device__ __forceinline__ void add(int, long long) {}
+    __device__ __forceinline__ void count(int) {}
+    __device__ __forceinline__ void flush(uint32_t, int) {}
+};
+#endif
 
 // Cut list `q` (c entries, keep < c <= 32 * kEpl) back to its `keep` smallest, unordered, in slots [0, keep); returns the
 // key of the worst kept entry (the new admission threshold).  Warp-wide radix select on the 32-bit key — 32 rounds
@@ -665,7 +710,7 @@ __device__ __forceinline__ uint32_t select_keep(uint64_t *lists, int q, uint32_t
 //   kVar     operand type: 16-bit operands 1 = bfloat16 (else IEEE half); 8-bit 1 = int8 (else uint8).  A template parameter so
 //            that the MMA sequence of a stage is one straight run of wgmma instructions (no branch between them)
 template <bool kDirect, int kEpl, int kOp, int kMode, int kVar = 0>
-__global__ void __launch_bounds__(kCoarseThreads, 1)
+__global__ void __launch_bounds__(coarse_threads(kMode), 1)
 coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t *__restrict__ shadow, size_t row_pitch,
                     const uint8_t *__restrict__ q16, size_t q16_pitch, const float *__restrict__ row_norm2,
                     const float *__restrict__ q_norm2, uint32_t n_rows, uint32_t nq, uint32_t dim, uint32_t row_bytes,
@@ -674,6 +719,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                     uint32_t tile_stride, const float *__restrict__ thr_fixed, uint32_t *__restrict__ overflow) {
     constexpr bool kFixed = kMode == 1, kSample = kMode == 2;
     constexpr bool kInt = kOp == 1 || kOp == 2 || kOp == 4;
+    constexpr int kCons = coarse_consumers(kMode), kConsThreads = 128 * kCons;
     using Acc = typename std::conditional<kInt, uint32_t, float>::type;
     // bx = row range, by = query group
     const uint32_t bx = blockIdx.x, by = blockIdx.y, gx = gridDim.x;
@@ -719,15 +765,20 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
     const uint16_t cmask = (uint16_t)((1u << csize) - 1u);
     if (csize > 1) cluster_sync_all(); // peers must see initialised barriers before anything is signalled remotely
 
+    CycleAccount ca;
+    const uint32_t cta = by * gx + bx;
     if (warp == 0) {
         // ===== producer: row tiles [128 rows x 128 bytes] per K block, kQKbPerStage K blocks per stage =====
         uint32_t s = 0, ph = 0;
         const uint32_t slice = kQStageBytes / csize; // num_kb is a multiple of kQKbPerStage: every stage is full
+        const long long t_pass = ca.now();
         for (uint32_t i = 0; i < my_tiles; i++) {
             const uint32_t tile = (bx + i * gx) * tile_stride;
             for (uint32_t kb0 = 0; kb0 < num_kb; kb0 += kQKbPerStage) {
                 const uint32_t kbn = min((uint32_t)kQKbPerStage, num_kb - kb0);
+                const long long t_wait = ca.now();
                 mbar_wait_spin(&empty[s], ph ^ 1);
+                ca.add(kCaWait, t_wait);
                 if (elect_one_sync()) {
                     const uint32_t bytes = kbn * kQBlockBytes;
                     mbar_expect_tx(&full[s], bytes);
@@ -757,13 +808,17 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                 if (++s == nstages) s = 0, ph ^= 1;
             }
         }
+        ca.add(kCaPass, t_pass);
+        if (kFixed && lane == 0) ca.flush(cta, 2);
     } else if (warp >= 4) {
-        const int ew = warp - 4;          // warp of the warpgroup: accumulator rows (queries) 16 ew .. 16 ew + 15
-        const int et = threadIdx.x - 128; // 0..127; the query slot in the epilogue (slots >= kQM own no query)
+        const int cw = kCons > 1 ? (warp - 4) >> 2 : 0; // consumer warpgroup (0 .. kCons - 1)
+        const int ew = kCons > 1 ? (warp - 4) & 3 : warp - 4; // warp of the warpgroup: accumulator rows (queries) 16 ew .. 16 ew + 15
+        // 0..127 within the warpgroup; the query slot in the epilogue (slots >= kQM own no query)
+        const int et = kCons > 1 ? (threadIdx.x - 128) & 127 : threadIdx.x - 128;
         const uint32_t q = q_base + et;
         const bool live = et < kQM && q < nq;
         // ===== queries -> shared memory (zero padded to num_kb * 128 bytes and to 64 queries) =====
-        if (et < kQM) {
+        if (cw == 0 && et < kQM) {
             const uint4 *src = reinterpret_cast<const uint4 *>(q16 + (size_t)q * q16_pitch);
             for (uint32_t kb = 0; kb < num_kb; kb++) {
                 // row `et` of a K-major 128B-swizzled operand tile: chunk u at et*128 + ((u ^ (et & 7)) * 16)
@@ -778,7 +833,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
             if constexpr (kFixed) qcount[et] = 0;
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy writes of sQ -> tensor-core reads
-        asm volatile("bar.sync 1, 128;" ::: "memory");
+        named_sync<1, kConsThreads>();
         // stage `st` of the ring has been read by this CTA's MMAs: one arrival on its `empty` barrier in every CTA of
         // the cluster (each producer multicasts into all of them)
         auto release = [&](uint32_t st) {
@@ -833,8 +888,19 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         uint32_t s = 0, ph = 0;
         const uint64_t bdesc_first = make_smem_desc(smem_u32(sB)), adesc_first = make_smem_desc(smem_u32(sQ));
         constexpr uint64_t kStageStep = kQStageBytes >> 4, kBlockStep = kQBlockBytes >> 4, kABlockStep = kQABlockBytes >> 4;
-        for (uint32_t i = 0; i < my_tiles; i++) {
+        // kCons warpgroups take tiles i = cw, cw + kCons, ...; a warpgroup steps its ring position past the stages of
+        // the tiles the others take.  MMA issue stays in ring order: a warpgroup waits on a stage's `full` barrier only
+        // once every earlier stage has been waited on, so that barrier is never more than one phase ahead of the wait.
+        const uint32_t stages_per_tile = num_kb / kQKbPerStage;
+        auto skip = [&](uint32_t n) {
+            for (s += n; s >= nstages; s -= nstages) ph ^= 1;
+        };
+        if (kCons > 1) skip(stages_per_tile * cw);
+        const long long t_pass = ca.now();
+        for (uint32_t i = cw; i < my_tiles; i += kCons) {
             const uint32_t tile = (bx + i * gx) * tile_stride;
+            if (kCons > 1 && i >= (uint32_t)kCons) skip(stages_per_tile * (kCons - 1));
+            ca.count(kCaTiles);
             float nrm[kQN / 32]; // kOp 2 / 3: lane l holds the norm / squared norm of rows h*32 + l of the tile
             int inrm[kQN / 32];  // kOp 4: the same, int32
             if constexpr (kOp == 4) {
@@ -872,11 +938,26 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         rn[j] = make_float2(r < n_rows ? __ldg(row_norm2 + r) : 0.0f, 0.0f);
                 }
             }
+            if constexpr (kCons > 1) {
+                static_assert(kCons == 2, "the hand-off pairs two warpgroups");
+                // hand-off: the warpgroup of tile i - 1 has issued its last MMAs (warpgroup cw waits on barrier 2 + cw)
+                const long long t_handoff = ca.now();
+                if (i != 0) {
+                    if (cw == 0)
+                        named_sync<2, 2 * 128>();
+                    else
+                        named_sync<3, 2 * 128>();
+                }
+                ca.add(kCaHandoff, t_handoff);
+            }
             // ===== D[64 queries x 128 rows] (+)= Q[smem] * rows[smem]^T =====
             Acc acc[64];
             uint32_t prev = 0;
             for (uint32_t kb0 = 0; kb0 < num_kb; kb0 += kQKbPerStage) {
+                const long long t_wait = ca.now();
                 mbar_wait_spin(&full[s], ph);
+                const long long t_issue = ca.now();
+                ca.add(kCaWait, t_wait);
                 wg_fence(); // the accumulator registers are handed to the MMA pipe for this stage's run
                 const uint64_t bd = bdesc_first + (uint64_t)s * kStageStep, ad = adesc_first + (uint64_t)kb0 * kABlockStep;
                 // x = 4 j + kk: K block j of the stage, 32-byte step kk inside its swizzled rows
@@ -885,11 +966,23 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                     wgmma_n128<kInt, kVar>(acc, ad + (x >> 2) * kABlockStep + 2 * (x & 3), bd + (x >> 2) * kBlockStep + 2 * (x & 3),
                                            (kb0 | (uint32_t)x) != 0);
                 wg_commit();
+                if constexpr (kCons > 1) { // the tile's last MMAs are issued: the other warpgroup may start the next tile
+                    if (kb0 + kQKbPerStage >= num_kb && i + 1 < my_tiles) {
+                        if (cw == 0)
+                            named_arrive<3, 2 * 128>();
+                        else
+                            named_arrive<2, 2 * 128>();
+                    }
+                }
+                ca.add(kCaIssue, t_issue);
+                const long long t_wait1 = ca.now();
                 wg_wait<1>(); // the previous stage's MMAs have retired (nothing to wait for on the first): its slot may be refilled
+                ca.add(kCaWait1, t_wait1);
                 if (kb0 != 0) release(prev);
                 prev = s;
                 if (++s == nstages) s = 0, ph ^= 1;
             }
+            const long long t_epilogue = ca.now();
             wg_wait<0>();
             release(prev);
             wg_fence_operands(acc);
@@ -950,6 +1043,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         }
                     }
                 }
+                ca.add(kCaEpilogue, t_epilogue);
                 continue;
             }
             asm volatile("bar.sync 1, 128;" ::: "memory"); // the previous tile's reads of sacc are done
@@ -1088,14 +1182,18 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                 }
             }
         }
+        ca.add(kCaPass, t_pass);
+        if (kFixed && et == 0) ca.flush(cta, cw);
         // publish: cand_out[q][blockIdx.x][keep], kEmptySlot padded
         __syncwarp();
         if constexpr (kFixed) {
-            // every append of the CTA is done; warp ew publishes queries 16 ew .. 16 ew + 15.  keep == kQListCap here
-            // (plan_coarse), so a list that did not overflow is published whole.  More rows below the bound than the
-            // list holds: overflow, the query goes to the next tier.
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            for (int qs = 16 * ew; qs < 16 * ew + 16; qs++) {
+            // every append of the CTA is done; consumer warp pw publishes queries per * pw .. per * pw + per - 1.
+            // keep == kQListCap here (plan_coarse), so a list that did not overflow is published whole.  More rows below
+            // the bound than the list holds: overflow, the query goes to the next tier.
+            named_sync<1, kConsThreads>();
+            constexpr int per = kQM / (4 * kCons);
+            const int pw = 4 * cw + ew;
+            for (int qs = per * pw; qs < per * pw + per; qs++) {
                 const uint32_t qq = q_base + qs;
                 if (qq >= nq) break;
                 const uint32_t n = qcount[qs], c = min(n, (uint32_t)kQListCap);
@@ -1622,6 +1720,7 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
             p.keep = k > kCoarseMaxK ? kCoarseFixedCapWide : kCoarseFixedCap, p.epl = k > kCoarseMaxK ? 8 : 3;
         if (p.mode == 1 && kind == CoarseDirect16) p.keep = kCoarseFixedCapDirect, p.epl = 8;
         if (p.mode == 2) p.keep = kCoarseSampleSlices, p.epl = 3; // the slice minima
+        p.threads = (uint32_t)coarse_threads(p.mode);
         p.stages = (uint32_t)std::min<size_t>(kQMaxStages, (kSmemLimit - wgmma_fixed_smem(p.num_kb, p.mode)) / kQStageBytes);
         p.smem_bytes = wgmma_fixed_smem(p.num_kb, p.mode) + (size_t)p.stages * kQStageBytes;
         // the query groups of a row range form a thread-block cluster (multicast of the row tiles)
@@ -1643,7 +1742,7 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
             cudaLaunchConfig_t cfg{};
             cudaLaunchAttribute at[1];
             cfg.gridDim = dim3(1, p.grid_y, 1);
-            cfg.blockDim = dim3(kCoarseThreads);
+            cfg.blockDim = dim3(p.threads); // a block size the kernel cannot take reports no cluster: csize would fall to 1
             cfg.dynamicSmemBytes = p.smem_bytes;
             at[0].id = cudaLaunchAttributeClusterDimension;
             at[0].val.clusterDim.x = 1, at[0].val.clusterDim.y = p.csize, at[0].val.clusterDim.z = 1;
@@ -1669,6 +1768,7 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
     p.grid_x = std::max(1u, std::min(p.tiles, sms / p.grid_y));
     p.keep = kCoarseKeep;
     const size_t fixed_bytes = fixed_smem(p.num_kb);
+    p.threads = kCoarseThreads;
     p.stages = (uint32_t)std::min<size_t>(kMaxStages, (kSmemLimit - fixed_bytes) / kStageBytes);
     p.cand_elems = (size_t)nq * p.grid_x * p.keep;
     p.smem_bytes = fixed_bytes + (size_t)p.stages * kStageBytes;
@@ -1684,8 +1784,8 @@ static cudaError_t launch_coarse_t(const void *rows, size_t pitch, uint32_t n_ro
     if (!make_map(&mq, dt, d_queries, dim, nq, qpitch, Cfg::kBlockK, Cfg::kTileN)) return cudaErrorInvalidValue;
     cudaError_t e = cudaFuncSetAttribute(coarse_kernel<Cfg>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes);
     if (e != cudaSuccess) return e;
-    coarse_kernel<Cfg><<<dim3(p.grid_x, p.grid_y), kCoarseThreads, p.smem_bytes, s>>>(ma, mq, n_rows, nq, p.num_kb, p.tiles, p.keep,
-                                                                                     p.stages, d_cand);
+    coarse_kernel<Cfg><<<dim3(p.grid_x, p.grid_y), p.threads, p.smem_bytes, s>>>(ma, mq, n_rows, nq, p.num_kb, p.tiles, p.keep, p.stages,
+                                                                                d_cand);
     return cudaGetLastError();
 }
 
@@ -1714,7 +1814,7 @@ cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim
         cudaLaunchConfig_t cfg{};
         cudaLaunchAttribute at[1];
         cfg.gridDim = dim3(p.grid_x, p.grid_y, 1);
-        cfg.blockDim = dim3(kCoarseThreads);
+        cfg.blockDim = dim3(p.threads);
         cfg.dynamicSmemBytes = p.smem_bytes;
         cfg.stream = s;
         at[0].id = cudaLaunchAttributeClusterDimension;
@@ -1735,6 +1835,16 @@ cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim
     }
     return launch_coarse_t<CfgTF32>(o.rows, o.pitch, n_rows, dim, o.queries, o.qpitch, nq, p, d_cand, s);
 }
+
+#ifdef COARSE_CYCLE_ACCOUNT
+// the cycle account of the last fixed-bound pass, [cta][role][kCaSlots] as unsigned 64-bit, into host memory; returns
+// the slots per (cta, role)
+extern "C" int VecSimB200_CoarseCycles(unsigned long long *host, int max_ctas) {
+    const size_t bytes = (size_t)std::min(max_ctas, kCaMaxCtas) * 3 * kCaSlots * sizeof(unsigned long long);
+    if (cudaMemcpyFromSymbol(host, g_coarse_cycles, bytes) != cudaSuccess) return -1;
+    return kCaSlots;
+}
+#endif
 
 // fp32 rows -> the tiled fp16 shadow: [tile of 128 rows][K block of 64 halves][128 rows x 128 B, 128B-swizzled],
 // i.e. exactly the bytes a SWIZZLE_128B tensor-map load would have produced in shared memory, so that

@@ -30,6 +30,7 @@ struct CoarsePlan {
     CoarseKind kind;
     uint32_t grid_x, grid_y, num_kb, tiles, keep;
     uint32_t stages; // depth of the row-tile ring in shared memory
+    uint32_t threads; // block size of the kernel the plan launches
     uint32_t epl;    // candidate-list entries per lane of the compacting warp (3 or 8)
     uint32_t tile_stride; // 1 = every row tile; n = every n-th (the sample pass)
     int mode;        // CoarseF16: 0 adaptive top-`keep` lists, 1 fixed admission bound per query (main pass), 2 sample pass (slice minima)
