@@ -224,6 +224,20 @@ II_ResultSet *II_IntersectEx(II_PostingList *const *lists, const int *modes, siz
 II_ResultSet *II_IntersectPhrase(II_PostingList *const *lists, const int *modes, size_t n, int32_t max_slop, int in_order);
 size_t II_ResultSet_Len(const II_ResultSet *rs);
 void II_ResultSet_Free(II_ResultSet *rs);
+/* The same nq ANDs with no host wait at all: each is enqueued on one of the library's streams and `stream` (a cudaStream_t cast
+ * to void*, NULL = the legacy default stream) is made to wait, through events, for every one of them.  out[i] = a result set whose
+ * length is still pending on the device, or NULL (an empty child, no list or more than 32 lists: the caller passes cap 0 for it);
+ * returns how many were built.  Its docIds (II_ResultSet_DeviceDocIds) and u32 count (II_ResultSet_DeviceLen) are valid in
+ * `stream` order; II_ResultSet_Capacity is the host bound on the count (the shortest list's length).  Every other accessor (Len,
+ * Fetch, TopN, Score, the iterators, ...) first waits for the set and then behaves as on a set from II_IntersectBatch. */
+size_t II_IntersectBatchDevice(size_t nq, II_PostingList *const *const *lists, const size_t *n_lists, void *stream, II_ResultSet **out);
+const uint32_t *II_ResultSet_DeviceLen(const II_ResultSet *rs); /* u32 hit count, valid in stream order */
+size_t II_ResultSet_Capacity(const II_ResultSet *rs);           /* host upper bound on the count */
+/* Free rs once the work enqueued on `stream` so far is done, without waiting: the library's stream waits for an event recorded
+ * on `stream` before the memory goes back to the pool.  II_ResultSet_Free releases the memory in the library's own stream order,
+ * so kernels of the caller's stream still reading the docIds would see it handed out again; use this after enqueuing a consumer
+ * on another stream. */
+void II_ResultSet_FreeAfter(II_ResultSet *rs, void *stream);
 
 /* ---- scoring ------------------------------------------------------------------------------------ */
 typedef enum {

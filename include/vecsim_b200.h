@@ -550,6 +550,28 @@ int VecSimB200_TopKFiltered(VecSimIndex *index, const void *queryBlob, size_t k,
  * range. */
 int VecSimB200_TopKFilteredBatch(VecSimIndex *index, const void *const *queryBlobs, size_t nq, size_t k, const uint32_t *const *d_doc_ids,
                                  const size_t *counts, size_t *out_labels, double *out_scores, size_t *out_counts);
+/* nq filtered KNN queries, device pointers end to end, enqueued on `stream` (a cudaStream_t cast to void*, NULL = the legacy
+ * default stream); the call returns without waiting for the device.
+ * d_queries: nq stored-form query blobs, laid out as for VecSimB200_TopKQueryBatchDevice (cosine normalised, int8 / uint8 cosine
+ * with its norm appended).  d_doc_ids[i]: device pointer to query i's ascending filter docIds; d_counts (nullable) [i]: device
+ * pointer to its u32 count, read in stream order (NULL, or a NULL entry: caps[i] is the exact count); caps[i]: a host upper bound on
+ * that count (II_ResultSet_Capacity of an AND from II_IntersectBatchDevice; 0 = an empty filter, its pointers are not read).  The
+ * three pointer arrays are host arrays.
+ * Out: [nq][k] int64 labels (-1 = empty) and float distances (NaN = empty), ascending by (distance, docId); d_out_counts (nullable)
+ * [nq] u32 entries per query.  Every row is exactly what VecSimB200_TopKFiltered answers for that query and filter: absent or
+ * deleted docIds score NaN and are skipped, multi-value indexes take its fold, and distance bits are the same.
+ * Single- and multi-value indexes, k <= 1024.  The launches do not depend on nq: one ragged gather over the caps, 2 ceil(k / 128)
+ * segmented selects and one unpack (DESIGN.md §4.6).
+ * Host waits: none once the index has no pending mutation.  After rows or labels changed, the first call flushes staged rows and
+ * rebuilds the docId -> rows table, which waits for those copies; a call needing more scratch than any before it grows the
+ * index's device scratch, which waits for the device.  The scratch is shared with VecSimB200_TopKQueryBatchDevice and reused call
+ * after call in stream order: enqueue both on one stream (or synchronise between streams), and do not mutate the index while a
+ * batch is in flight.
+ * Returns 0 (also for nq == 0 or k == 0: nothing is enqueued); -1 for k > 1024 or a CUDA failure; -2, before anything is enqueued,
+ * for labels too sparse for the dense table or a cap beyond the 32-bit id range (the same rules as VecSimB200_TopKFiltered). */
+int VecSimB200_TopKFilteredBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, size_t k, const uint32_t *const *d_doc_ids,
+                                       const uint32_t *const *d_counts, const size_t *caps, int64_t *d_out_labels, float *d_out_scores,
+                                       uint32_t *d_out_counts, void *stream);
 /* Batched fp32 queries (cosine, and in mode 1 also L2 and raw inner product; nq >= 16, k <= 16, dim % 8 == 0,
  * >= 65536 rows) take a wgmma coarse
  * pass + exact rescoring from the fp32 rows + a per-query completeness proof, with the exact scan as

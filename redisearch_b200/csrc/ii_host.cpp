@@ -199,7 +199,14 @@ struct II_ResultSet {
     std::vector<uint8_t> child_tag; // RSResultData tag per child (aggregate order)
     size_t estimated = 0;           // num_estimated by the reference's rule: min over the children (AND), their sum (OR)
     std::unique_ptr<UnionOrder> h_order; // host copy of d_order (EXPLAINSCORE walks one hit's children in aggregate order)
+    // II_IntersectBatchDevice: the hit count is known only on the device until settle(); `ready` completes with the AND's kernels
+    bool pending = false;
+    cudaEvent_t ready = nullptr;
     ~II_ResultSet() {
+        if (ready) { // allocated on another stream, whose AND may still be writing: the frees below wait for it
+            cudaStreamWaitEvent(ctx().stream, ready, 0);
+            cudaEventDestroy(ready);
+        }
         dfree(d_docs);
         dfree(d_freqs);
         dfree(d_scores);
@@ -1539,6 +1546,84 @@ size_t II_IntersectBatch(size_t nq, II_PostingList *const *const *lists, const s
     return built;
 }
 
+// The same ANDs with no host wait: round-robin over a pool of streams of their own, each set's count left in its d_len, and
+// `stream` made to wait for every stream used.  A set stays `pending` until an accessor needs its length on the host (settle).
+size_t II_IntersectBatchDevice(size_t nq, II_PostingList *const *const *lists, const size_t *n_lists, void *stream, II_ResultSet **out) {
+    constexpr size_t kSlots = 16;
+    struct Pool {
+        std::mutex mu;
+        Ctx slot[kSlots];
+        cudaEvent_t done[kSlots] = {};
+    };
+    static Pool pool;
+    std::lock_guard<std::mutex> g(pool.mu);
+    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : cudaStreamLegacy;
+    bool used[kSlots] = {false};
+    size_t built = 0;
+    for (size_t qi = 0; qi < nq; qi++) {
+        out[qi] = nullptr;
+        const size_t sl = qi % kSlots, n = n_lists[qi];
+        if (n == 0 || n > (size_t)kIIMaxLists) continue;
+        CtxScope scope(&pool.slot[sl]); // the set's memory is allocated and, on failure, freed in this stream's order
+        Ctx &c = pool.slot[sl];
+        if (!c.init()) continue;
+        std::unique_ptr<II_ResultSet> rs(new II_ResultSet());
+        bool empty = false;
+        if (!intersect_enqueue(c, lists[qi], n, rs.get(), &empty) || empty) continue;
+        if (cudaEventCreateWithFlags(&rs->ready, cudaEventDisableTiming) != cudaSuccess || cudaEventRecord(rs->ready, c.stream) != cudaSuccess)
+            continue;
+        rs->pending = true;
+        used[sl] = true;
+        out[qi] = rs.release();
+        built++;
+    }
+    for (size_t sl = 0; sl < kSlots; sl++) {
+        if (!used[sl]) continue;
+        if (!pool.done[sl] && cudaEventCreateWithFlags(&pool.done[sl], cudaEventDisableTiming) != cudaSuccess) continue;
+        // the wait takes the event's state now: re-recording it for the next batch does not move this wait
+        if (cudaEventRecord(pool.done[sl], pool.slot[sl].stream) == cudaSuccess) cudaStreamWaitEvent(st, pool.done[sl], 0);
+    }
+    return built;
+}
+
+namespace {
+// a pending set (II_IntersectBatchDevice): wait for its AND, then its length is on the host as for every other set
+void settle(const II_ResultSet *crs) {
+    if (!crs || !crs->pending) return;
+    static std::mutex mu;
+    static cudaStream_t s = nullptr; // of its own: the copy queues behind nothing but the set's AND
+    std::lock_guard<std::mutex> g(mu);
+    auto *rs = const_cast<II_ResultSet *>(crs);
+    if (!rs->pending) return;
+    if (!s && cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) return;
+    uint32_t len = 0;
+    if (cudaStreamWaitEvent(s, rs->ready, 0) != cudaSuccess || cudaMemcpyAsync(&len, rs->d_len, 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+        cudaStreamSynchronize(s) != cudaSuccess)
+        return;
+    rs->len = len;
+    rs->pending = false;
+}
+} // namespace
+
+const uint32_t *II_ResultSet_DeviceLen(const II_ResultSet *rs) { return rs->d_len; }
+size_t II_ResultSet_Capacity(const II_ResultSet *rs) { return rs->cap; }
+
+void II_ResultSet_FreeAfter(II_ResultSet *rs, void *stream) {
+    if (!rs) return;
+    Ctx &c = ctx();
+    std::lock_guard<std::mutex> g(c.mu);
+    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : cudaStreamLegacy;
+    cudaEvent_t ev = nullptr;
+    if (c.init() && cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) == cudaSuccess) {
+        // the frees of the destructor run in c.stream order: after everything enqueued on `stream` so far (and the AND itself)
+        if (cudaEventRecord(ev, st) == cudaSuccess) cudaStreamWaitEvent(c.stream, ev, 0);
+        cudaEventDestroy(ev);
+    } else {
+        cudaStreamSynchronize(st);
+    }
+    delete rs;
+}
+
 II_ResultSet *II_Union(II_PostingList *const *lists, size_t n, int quick_exit) {
     if (n == 0 || n > (size_t)kIIMaxUnionLists) return nullptr;
     Ctx &c = ctx();
@@ -1559,7 +1644,10 @@ II_ResultSet *II_Union(II_PostingList *const *lists, size_t n, int quick_exit) {
     return rs;
 }
 
-size_t II_ResultSet_Len(const II_ResultSet *rs) { return rs->len; }
+size_t II_ResultSet_Len(const II_ResultSet *rs) {
+    settle(rs);
+    return rs->len;
+}
 size_t II_ResultSet_NumChildren(const II_ResultSet *rs) { return rs->n_children; }
 void II_ResultSet_ChildOrder(const II_ResultSet *rs, uint32_t *child_order) {
     for (uint32_t i = 0; i < rs->n_children; i++) child_order[i] = rs->child_order[i];
@@ -1573,6 +1661,7 @@ void II_ResultSet_Free(II_ResultSet *rs) { delete rs; }
 // with slop / in-order needs them up front; GetSlop builds them on demand).
 II_PostingList *II_ResultSet_IntoChild(II_ResultSet *rs, const II_TermParams *terms, double weight, int with_positions) {
     if (!rs) return nullptr;
+    settle(rs);
     auto ns = std::make_shared<NestedSet>();
     ns->rs.reset(rs);
     Ctx &c = ctx();
@@ -1627,6 +1716,7 @@ double II_CalculateIDF_BM25(size_t total_docs, size_t term_docs) { // :103-110
 
 int II_Score(II_ResultSet *rs, II_Scorer scorer, const II_TermParams *terms, double agg_weight, const II_IndexStats *stats,
              const II_DocTable *docs, double min_score, uint64_t tanh_factor) {
+    settle(rs);
     Ctx &c = ctx();
     std::lock_guard<std::mutex> g(c.mu);
     if (!c.init() || !rs) return -1;
@@ -1655,6 +1745,7 @@ int II_Score(II_ResultSet *rs, II_Scorer scorer, const II_TermParams *terms, dou
 
 // HAMMING (src/ext/default.c:475-497): the scorer looks at the query payload and the document payload only
 int II_ScoreHamming(II_ResultSet *rs, const II_DocTable *docs, const void *qdata, size_t qdatalen) {
+    settle(rs);
     Ctx &c = ctx();
     std::lock_guard<std::mutex> g(c.mu);
     if (!c.init() || !rs) return -1;
@@ -1682,6 +1773,7 @@ int II_ScoreHamming(II_ResultSet *rs, const II_DocTable *docs, const void *qdata
 }
 
 int II_ResultSet_Fetch(const II_ResultSet *rs, uint64_t *doc_ids, double *scores, uint32_t *child_freqs) {
+    settle(rs);
     const size_t m = rs->len;
     if (m == 0) return 0;
     if (doc_ids) {
@@ -1707,6 +1799,7 @@ int II_ResultSet_Fetch(const II_ResultSet *rs, uint64_t *doc_ids, double *scores
 }
 
 size_t II_ResultSet_TopN(const II_ResultSet *rs, size_t n, uint64_t *doc_ids, double *scores) {
+    settle(rs);
     Ctx &c = ctx();
     std::unique_lock<std::mutex> g(c.mu);
     if (!c.init() || rs->len == 0 || n == 0) return 0;
@@ -2245,6 +2338,7 @@ void ri_free(II_QueryIterator *b) { delete RI(b); }
 } // namespace
 
 II_QueryIterator *II_NewResultIterator(II_ResultSet *rs, double weight) {
+    settle(rs);
     if (!rs) return nullptr;
     auto *it = new ResultIter();
     memset(&it->base, 0, sizeof(it->base));

@@ -180,6 +180,11 @@ FlatIndex::~FlatIndex() {
     cudaFree(d_label_rows_);
     cudaFree(d_id_to_label_);
     cudaFreeHost(h_stage_);
+    for (TableSlot &t : table_ring_) {
+        cudaEventSynchronize(t.ev);
+        cudaEventDestroy(t.ev);
+        cudaFreeHost(t.h);
+    }
 }
 
 CorpusView FlatIndex::view() const {
@@ -1893,6 +1898,87 @@ int FlatIndex::topk_filtered_batch(const void *const *queries, size_t nq, size_t
         }
     }
     return rc;
+}
+
+// The same batch with device pointers end to end (DESIGN.md §4.6): no filter length comes back to the host.  One ragged gather over
+// the flat space of the caps, 2 ceil(k / 128) segmented selects, one unpack: 2 + 2 ceil(k / 128) launches whatever nq.  Selection is
+// by (distance, position in the filter) as in topk_filtered, so every row equals its answer.
+int FlatIndex::topk_filtered_batch_device(const void *d_q, size_t nq, size_t k, const uint32_t *const *d_doc_ids,
+                                          const uint32_t *const *d_counts, const size_t *caps, int64_t *d_labels, float *d_scores,
+                                          uint32_t *d_counts_out, cudaStream_t s) {
+    last_mode_ = HYBRID_ADHOC_BF;
+    if (nq == 0 || k == 0) return 0;
+    if (k > (size_t)kMaxWideK || nq > 0x7FFFFFFFull) return -1;
+    size_t total = 0, max_cap = 0;
+    uint64_t blocks = 0;
+    for (size_t i = 0; i < nq; i++) {
+        if (caps[i] > 0xFFFFFFF0ull) return -2;
+        total += caps[i];
+        max_cap = std::max(max_cap, caps[i]);
+        blocks += ragged_blocks(caps[i]);
+    }
+    if (!flush()) return -1;
+    if (!sync_label_table()) return -2;
+    const uint32_t nq32 = (uint32_t)nq, chunk = (uint32_t)std::min<size_t>(k, kMaxFusedK);
+    const uint32_t parts = plan_ragged_select_parts(max_cap, nq32);
+    std::lock_guard<std::mutex> dg(dev_mu_);
+    if (!dev_ctx_) dev_ctx_ = checkout();
+    QueryCtx *c = dev_ctx_.get();
+    if (!c) return -1;
+    const size_t tab_elems = 4 * nq + 2; // [docId pointers nq][count pointers nq][score offsets nq + 1][first CTAs nq + 1]
+    uint64_t *tab, *cand, *out;
+    float *scores;
+    const auto layout = [&](void *base) {
+        BatchScratch sc(base);
+        tab = sc.take<uint64_t>(tab_elems);
+        scores = sc.take<float>(total);
+        cand = sc.take<uint64_t>((size_t)nq * parts * 8 * chunk); // 8 lists (one per warp) per select CTA
+        out = sc.take<uint64_t>(nq * k);
+        return sc.words();
+    };
+    if (!c->need_cand(layout(nullptr))) return -1;
+    layout(c->d_cand);
+    // a staging slot whose previous upload has executed (a never-recorded event counts as complete), else a new one
+    TableSlot *slot = nullptr;
+    for (TableSlot &t : table_ring_)
+        if (t.cap >= tab_elems && cudaEventQuery(t.ev) == cudaSuccess) {
+            slot = &t;
+            break;
+        }
+    cudaGetLastError(); // cudaErrorNotReady of a slot in flight is no failure
+    if (!slot) {
+        TableSlot t;
+        t.cap = std::max<size_t>(2 * tab_elems, 1024);
+        if (cudaMallocHost(&t.h, t.cap * 8) != cudaSuccess) return -1;
+        if (cudaEventCreateWithFlags(&t.ev, cudaEventDisableTiming) != cudaSuccess) {
+            cudaFreeHost(t.h);
+            return -1;
+        }
+        table_ring_.push_back(t);
+        slot = &table_ring_.back();
+    }
+    uint64_t *h = slot->h, off = 0, blk = 0;
+    for (size_t i = 0; i < nq; i++) {
+        h[i] = (uint64_t)(uintptr_t)d_doc_ids[i];
+        h[nq + i] = d_counts ? (uint64_t)(uintptr_t)d_counts[i] : 0;
+        h[2 * nq + i] = off;
+        h[3 * nq + 1 + i] = blk;
+        off += caps[i];
+        blk += ragged_blocks(caps[i]);
+    }
+    h[3 * nq] = off;
+    h[4 * nq + 1] = blk;
+    cudaStream_t st = s ? s : cudaStreamLegacy; // NULL = the legacy default stream, as everywhere in CUDA
+    bool ok = cudaMemcpyAsync(tab, h, tab_elems * 8, cudaMemcpyHostToDevice, st) == cudaSuccess;
+    ok = ok && cudaEventRecord(slot->ev, st) == cudaSuccess;
+    const RaggedBatch b{reinterpret_cast<const uint32_t *const *>(tab), reinterpret_cast<const uint32_t *const *>(tab + nq), tab + 2 * nq, nq32};
+    LaunchCounters lc;
+    ok = ok && launch_gather_ragged(view(), d_q, query_pitch(), b, tab + 3 * nq + 1, blocks, d_label_to_id_, (uint32_t)l2i_size_,
+                                    multi_ ? d_label_rows_ : nullptr, scores, st, &lc) == cudaSuccess;
+    ok = ok && launch_topk_ragged(b, scores, (uint32_t)k, parts, cand, out, st, &lc) == cudaSuccess;
+    ok = ok && launch_unpack_ragged(b, out, (uint32_t)k, d_labels, d_scores, d_counts_out, st, &lc) == cudaSuccess;
+    launches_total_ += lc.launches;
+    return ok ? 0 : -1;
 }
 
 // ------------------------------------------------------------------------------------------------

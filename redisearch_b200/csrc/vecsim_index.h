@@ -155,6 +155,9 @@ class FlatIndex {
                       double *out_scores, size_t *out_count);
     int topk_filtered_batch(const void *const *queries, size_t nq, size_t k, const uint32_t *const *d_doc_ids, const size_t *counts,
                             size_t *out_labels, double *out_scores, size_t *out_counts);
+    // the same, device pointers end to end and stream-ordered: VecSimB200_TopKFilteredBatchDevice
+    int topk_filtered_batch_device(const void *d_q, size_t nq, size_t k, const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts,
+                                   const size_t *caps, int64_t *d_labels, float *d_scores, uint32_t *d_counts_out, cudaStream_t s);
 
     VecSimIndexBasicInfo basic_info() const;
     VecSimIndexStatsInfo stats_info() const;
@@ -291,8 +294,16 @@ class FlatIndex {
   public:
     int last_batch_path() const { return last_batch_path_; }
   private:
-    std::unique_ptr<QueryCtx> dev_ctx_; // scratch of topk_batch_device (stream-ordered)
+    std::unique_ptr<QueryCtx> dev_ctx_; // scratch of topk_batch_device / topk_filtered_batch_device (stream-ordered)
     std::mutex dev_mu_;
+    // pinned staging of topk_filtered_batch_device's pointer tables (under dev_mu_): a slot is reused once the event recorded after
+    // its upload has completed; while every slot is still in flight a new one is added, so the host never waits for the upload
+    struct TableSlot {
+        uint64_t *h = nullptr;
+        size_t cap = 0; // uint64 elements
+        cudaEvent_t ev = nullptr;
+    };
+    std::vector<TableSlot> table_ring_;
     bool dev_timing_pending_ = false;
     uint64_t dev_timing_bytes_ = 0;
     void collect_dev_timing_locked();

@@ -400,9 +400,9 @@ __global__ void __launch_bounds__(kScanThreads) scan_scores_kernel(const uint8_t
     }
 }
 
-// k smallest composites > cursor over a score array -> per-warp lists (blockIdx.x, warp) of cand
+// k smallest composites > cursor over a score array -> per-warp lists (part, warp) of cand; the array is shared by `parts` CTAs
 __device__ __forceinline__ void select_scores_cta(const float *__restrict__ scores, uint32_t n, const uint64_t *__restrict__ cursor,
-                                                  uint32_t k, uint64_t *__restrict__ cand) {
+                                                  uint32_t k, uint64_t *__restrict__ cand, uint32_t part, uint32_t parts) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint64_t *slots = reinterpret_cast<uint64_t *>(smem);
@@ -417,7 +417,7 @@ __device__ __forceinline__ void select_scores_cta(const float *__restrict__ scor
     const bool has_cursor = cursor != nullptr;
     const uint64_t lo = has_cursor ? *cursor : 0;
     ListState ls{slots + (size_t)warp * k, worst + warp, wpos + warp};
-    const uint32_t gw = blockIdx.x * kScanWarps + warp, nw = gridDim.x * kScanWarps;
+    const uint32_t gw = part * kScanWarps + warp, nw = parts * kScanWarps;
     for (uint64_t base = (uint64_t)gw * 32; base < n; base += (uint64_t)nw * 32) {
         const uint32_t i = (uint32_t)base + lane;
         bool valid = i < n;
@@ -442,7 +442,7 @@ __device__ __forceinline__ void select_scores_cta(const float *__restrict__ scor
 __global__ void __launch_bounds__(kScanThreads) select_scores_kernel(const float *__restrict__ scores, uint32_t n,
                                                                      const uint64_t *__restrict__ cursor, uint32_t k,
                                                                      uint64_t *__restrict__ cand) {
-    select_scores_cta(scores, n, cursor, k, cand);
+    select_scores_cta(scores, n, cursor, k, cand, blockIdx.x, gridDim.x);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -524,7 +524,7 @@ __global__ void __launch_bounds__(kScanThreads) select_scores_wide_kernel(const 
     const uint32_t y = blockIdx.y;
     if (y >= wide_live(g)) return;
     const uint64_t *cursor = first ? out + (size_t)wide_query(g, y) * out_k + first - 1 : nullptr;
-    select_scores_cta(scores + (size_t)y * n, n, cursor, k, cand + (size_t)y * gridDim.x * kScanWarps * k);
+    select_scores_cta(scores + (size_t)y * n, n, cursor, k, cand + (size_t)y * gridDim.x * kScanWarps * k, blockIdx.x, gridDim.x);
 }
 
 // slot blockIdx.x: its lists -> its answer row, entries [first, first + k)
@@ -609,6 +609,130 @@ __global__ void __launch_bounds__(kScanThreads) gather_min_kernel(const uint8_t 
             if (lane == 0) dist = (dist < d[0]) ? dist : d[0];
         }
         if (lane == 0) out[w] = dist;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// batched filtered KNN (DESIGN.md §4.6): nq filter lists of ragged lengths known only on the device.  Query q owns the flat score
+// range [off[q], off[q + 1]) sized by its host cap; only its first min(*counts[q], cap) entries are live.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t ragged_count(const RaggedBatch &b, uint32_t q) {
+    const uint32_t cap = (uint32_t)(b.off[q + 1] - b.off[q]);
+    const uint32_t *c = b.counts[q];
+    return c ? min(*c, cap) : cap;
+}
+
+struct GatherRaggedArgs {
+    const uint8_t *rows;
+    size_t pitch;
+    uint32_t dim;
+    const uint8_t *queries;
+    size_t qpitch;
+    uint32_t q_smem_pitch;
+    RaggedBatch b;
+    const uint64_t *blk; // [nq + 1] first CTA of each query (prefix of ragged_blocks over the caps)
+    const uint32_t *table; // single-value: docId -> row (0xFFFFFFFF absent); multi-value: CSR offsets [table_size + 1]
+    uint32_t table_size;
+    const uint32_t *label_rows; // multi-value: rows of each label in insertion order
+    float *scores;
+};
+
+// One CTA = kRaggedPerBlock consecutive entries of ONE query (its blob stays in shared memory), one warp per entry, with the
+// arithmetic of gather_kernel (single-value) / gather_min_kernel's fold (multi-value).  A CTA past its query's device count
+// leaves after reading the count.
+template <int DT, int MT, bool MULTI>
+__global__ void __launch_bounds__(kScanThreads) gather_ragged_kernel(const GatherRaggedArgs a) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    using Tile = DistTile<DT, MT, 1, 1>;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint64_t bid = blockIdx.x;
+    uint32_t lo = 0, hi = a.b.nq; // blk[lo] <= bid < blk[hi]: lo is this CTA's query
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (a.blk[mid] <= bid) lo = mid;
+        else hi = mid;
+    }
+    const uint32_t q = lo;
+    const uint32_t e0 = (uint32_t)(bid - a.blk[q]) * kRaggedPerBlock;
+    const uint32_t n = ragged_count(a.b, q);
+    if (e0 >= n) return;
+    const uint32_t e1 = min(n, e0 + kRaggedPerBlock);
+    const uint8_t *query = a.queries + (size_t)q * a.qpitch;
+    for (uint32_t i = threadIdx.x; i < (a.q_smem_pitch >> 4); i += blockDim.x)
+        reinterpret_cast<uint4 *>(smem)[i] = reinterpret_cast<const uint4 *>(query)[i];
+    __syncthreads();
+    const uint8_t *qb[1] = {smem};
+    const uint32_t *ids = a.b.doc_ids[q];
+    float *out = a.scores + a.b.off[q];
+    for (uint32_t w = e0 + warp; w < e1; w += kScanWarps) {
+        const uint32_t l = ids[w];
+        if (MULTI) {
+            uint32_t r = 0, e = 0;
+            if (l < a.table_size) {
+                r = a.table[l];
+                e = a.table[l + 1];
+            }
+            float dist = r < e ? __uint_as_float(0x7F800000u) : __uint_as_float(0x7FC00000u);
+            uint32_t id = r < e ? a.label_rows[r] : 0u;
+#pragma unroll 1
+            for (; r < e; r++) {
+                const uint8_t *rowb[1] = {a.rows + (size_t)id * a.pitch};
+                if (r + 1 < e) id = a.label_rows[r + 1];
+                float d[1];
+                Tile::run(rowb, qb, a.dim, lane, d);
+                if (lane == 0) dist = (dist < d[0]) ? dist : d[0];
+            }
+            if (lane == 0) out[w] = dist;
+        } else {
+            const uint32_t id = l < a.table_size ? a.table[l] : 0xFFFFFFFFu;
+            if (id == 0xFFFFFFFFu) {
+                if (lane == 0) out[w] = __uint_as_float(0x7FC00000u);
+                continue;
+            }
+            const uint8_t *rowb[1] = {a.rows + (size_t)id * a.pitch};
+            float d[1];
+            Tile::run(rowb, qb, a.dim, lane, d);
+            if (lane == 0) out[w] = d[0];
+        }
+    }
+}
+
+// chunk select of query blockIdx.x / parts over its live scores; cursor = the last composite of the previous chunk in its row
+__global__ void __launch_bounds__(kScanThreads) select_scores_ragged_kernel(const RaggedBatch b, const float *__restrict__ scores,
+                                                                            uint32_t parts, const uint64_t *__restrict__ out, uint32_t out_k,
+                                                                            uint32_t first, uint32_t k, uint64_t *__restrict__ cand) {
+    const uint32_t q = blockIdx.x / parts, part = blockIdx.x - q * parts;
+    const uint64_t *cursor = first ? out + (size_t)q * out_k + first - 1 : nullptr;
+    select_scores_cta(scores + b.off[q], ragged_count(b, q), cursor, k, cand + (size_t)q * parts * kScanWarps * k, part, parts);
+}
+
+// query blockIdx.x: its lists -> its answer row, entries [first, first + k)
+__global__ void __launch_bounds__(kScanThreads) final_select_ragged_kernel(const uint64_t *__restrict__ cand, uint32_t m,
+                                                                           uint64_t *__restrict__ out, uint32_t out_k, uint32_t first,
+                                                                           uint32_t k) {
+    final_select_cta(cand + (size_t)blockIdx.x * m, m, k, out + (size_t)blockIdx.x * out_k + first);
+}
+
+// [nq][k] composites (position in the filter, ascending) -> docId labels and distances; NaN distances and empty slots -> -1 / NaN.
+// They sort after every real entry, so a row's real entries are a prefix: counts[q] = its length.
+__global__ void unpack_ragged_kernel(const RaggedBatch b, const uint64_t *__restrict__ comp, uint32_t k, int64_t *__restrict__ labels,
+                                     float *__restrict__ scores, uint32_t *__restrict__ counts) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)b.nq * k) return;
+    const uint32_t q = (uint32_t)(i / k), j = (uint32_t)(i - (size_t)q * k);
+    const uint64_t c = comp[i];
+    const bool real = c < ((uint64_t)kNaNKey << 32);
+    if (real) {
+        labels[i] = (int64_t)b.doc_ids[q][(uint32_t)c];
+        scores[i] = key_to_float((uint32_t)(c >> 32));
+    } else {
+        labels[i] = -1;
+        scores[i] = __uint_as_float(0x7FC00000u);
+    }
+    if (counts) {
+        const bool next_real = j + 1 < k && comp[i + 1] < ((uint64_t)kNaNKey << 32);
+        if (real && !next_real) counts[q] = j + 1;
+        if (j == 0 && !real) counts[q] = 0;
     }
 }
 
@@ -1048,6 +1172,77 @@ cudaError_t launch_gather_min_distances(const CorpusView &c, const void *d_query
 #undef CALL_GATHER_MIN
     if (ctr) ctr->launches++;
     return e;
+}
+
+template <int DT, int MT, bool MULTI>
+static cudaError_t launch_gather_ragged_inst(const GatherRaggedArgs &a, uint64_t n_blocks, cudaStream_t s) {
+    auto kern = gather_ragged_kernel<DT, MT, MULTI>;
+    cudaError_t e = ensure_smem(kern, a.q_smem_pitch);
+    if (e != cudaSuccess) return e;
+    kern<<<(uint32_t)n_blocks, kScanThreads, a.q_smem_pitch, s>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_gather_ragged(const CorpusView &c, const void *d_queries, size_t qpitch, const RaggedBatch &b, const uint64_t *d_blk,
+                                 uint64_t n_blocks, const uint32_t *d_table, uint32_t table_size, const uint32_t *d_label_rows, float *d_scores,
+                                 cudaStream_t s, LaunchCounters *ctr) {
+    if (n_blocks == 0 || b.nq == 0) return cudaSuccess;
+    if (n_blocks > 0x7FFFFFFFull) return cudaErrorInvalidValue;
+    GatherRaggedArgs a{};
+    a.rows = static_cast<const uint8_t *>(c.rows);
+    a.pitch = c.pitch;
+    a.dim = c.dim;
+    a.queries = static_cast<const uint8_t *>(d_queries);
+    a.qpitch = qpitch;
+    a.q_smem_pitch = round16(query_blob_bytes(c));
+    a.b = b;
+    a.blk = d_blk;
+    a.table = d_table;
+    a.table_size = table_size;
+    a.label_rows = d_label_rows;
+    a.scores = d_scores;
+    cudaError_t e = cudaErrorInvalidValue;
+#define CALL_GATHER_RAGGED(DT, MT)                                                                       \
+    e = d_label_rows ? launch_gather_ragged_inst<DT, MT, true>(a, n_blocks, s) : launch_gather_ragged_inst<DT, MT, false>(a, n_blocks, s)
+    RSB_DISPATCH_DM(c.dtype, c.metric, CALL_GATHER_RAGGED)
+#undef CALL_GATHER_RAGGED
+    if (ctr) ctr->launches++;
+    return e;
+}
+
+uint32_t plan_ragged_select_parts(size_t max_cap, uint32_t nq) {
+    // about two CTAs per SM over the whole batch, never more CTAs for a query than its largest list can feed
+    const uint32_t budget = std::max(1u, (uint32_t)device_sm_count() * 2u / std::max(1u, nq));
+    return std::max(1u, std::min(select_grid((uint32_t)std::min<size_t>(max_cap, 0xFFFFFFFFu)), budget));
+}
+
+cudaError_t launch_topk_ragged(const RaggedBatch &b, const float *d_scores, uint32_t k, uint32_t parts, uint64_t *d_cand, uint64_t *d_out,
+                               cudaStream_t s, LaunchCounters *ctr) {
+    if (k == 0 || k > (uint32_t)kMaxWideK || parts == 0) return cudaErrorInvalidValue;
+    if (b.nq == 0) return cudaSuccess;
+    const uint64_t sel_ctas = (uint64_t)b.nq * parts;
+    if (sel_ctas > 0x7FFFFFFFull) return cudaErrorInvalidValue;
+    for (uint32_t first = 0; first < k; first += kMaxFusedK) {
+        const uint32_t chunk = std::min<uint32_t>(kMaxFusedK, k - first);
+        const size_t ssmem = (size_t)kScanWarps * chunk * 8 + kScanWarps * 12;
+        const size_t fsmem = (size_t)next_pow2(kScanWarps * chunk) * 8 + kScanWarps * 12;
+        select_scores_ragged_kernel<<<(uint32_t)sel_ctas, kScanThreads, ssmem, s>>>(b, d_scores, parts, d_out, k, first, chunk, d_cand);
+        final_select_ragged_kernel<<<b.nq, kScanThreads, fsmem, s>>>(d_cand, parts * kScanWarps * chunk, d_out, k, first, chunk);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+        if (ctr) ctr->launches += 2;
+    }
+    return cudaSuccess;
+}
+
+cudaError_t launch_unpack_ragged(const RaggedBatch &b, const uint64_t *d_comp, uint32_t k, int64_t *d_labels, float *d_scores,
+                                 uint32_t *d_counts, cudaStream_t s, LaunchCounters *ctr) {
+    const size_t total = (size_t)b.nq * k;
+    if (total == 0) return cudaSuccess;
+    if ((total + 255) / 256 > 0x7FFFFFFFull) return cudaErrorInvalidValue;
+    unpack_ragged_kernel<<<(uint32_t)((total + 255) / 256), 256, 0, s>>>(b, d_comp, k, d_labels, d_scores, d_counts);
+    if (ctr) ctr->launches++;
+    return cudaGetLastError();
 }
 
 cudaError_t launch_unpack_results(const uint64_t *d_comp, uint32_t nq, uint32_t k, const uint64_t *d_id_to_label,

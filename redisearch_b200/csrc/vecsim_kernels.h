@@ -103,6 +103,33 @@ cudaError_t launch_gather_min_distances(const CorpusView &c, const void *d_query
                                         const uint32_t *d_offsets, uint32_t n_labels, const uint32_t *d_label_rows, float *d_out,
                                         cudaStream_t s, LaunchCounters *ctr);
 
+// ---- batched filtered KNN: ragged filter lists whose lengths are known only on the device (DESIGN.md §4.6) ----------------------
+// The tables live in device memory.  Query q's scores are scores[off[q], off[q + 1]) (off = prefix sums of the host caps); only the
+// first min(*counts[q], cap) entries are live (the whole cap when counts[q] is NULL).
+struct RaggedBatch {
+    const uint32_t *const *doc_ids; // [nq] query q's ascending docIds
+    const uint32_t *const *counts;  // [nq] query q's u32 count, or NULL
+    const uint64_t *off;            // [nq + 1]
+    uint32_t nq;
+};
+constexpr uint32_t kRaggedPerBlock = 128; // filter entries per gather CTA
+inline uint64_t ragged_blocks(size_t cap) { return (cap + kRaggedPerBlock - 1) / kRaggedPerBlock; }
+// distances of every live entry: one launch of n_blocks CTAs, d_blk [nq + 1] = prefix of ragged_blocks over the caps.  Single-value
+// index (d_label_rows NULL): d_table maps docId -> row as launch_map_labels; multi-value: CSR offsets over d_label_rows and the fold
+// of launch_gather_min_distances.  d_queries: nq stored-form blobs qpitch bytes apart.
+cudaError_t launch_gather_ragged(const CorpusView &c, const void *d_queries, size_t qpitch, const RaggedBatch &b, const uint64_t *d_blk,
+                                 uint64_t n_blocks, const uint32_t *d_table, uint32_t table_size, const uint32_t *d_label_rows, float *d_scores,
+                                 cudaStream_t s, LaunchCounters *ctr);
+// CTAs per query of the segmented select (their lists: parts * 8 per query and chunk)
+uint32_t plan_ragged_select_parts(size_t max_cap, uint32_t nq);
+// d_out [nq][k] = each query's k smallest (score, position) composites over its live scores, ascending, kEmptySlot-padded;
+// k <= kMaxWideK in cursor chunks of kMaxFusedK: 2 ceil(k / 128) launches.  d_cand: nq * parts * 8 * min(k, 128) elements.
+cudaError_t launch_topk_ragged(const RaggedBatch &b, const float *d_scores, uint32_t k, uint32_t parts, uint64_t *d_cand, uint64_t *d_out,
+                               cudaStream_t s, LaunchCounters *ctr);
+// d_out -> int64 docIds (-1) and float distances (NaN) for empty or NaN entries; d_counts (nullable) [nq] real entries per query
+cudaError_t launch_unpack_ragged(const RaggedBatch &b, const uint64_t *d_comp, uint32_t k, int64_t *d_labels, float *d_scores,
+                                 uint32_t *d_counts, cudaStream_t s, LaunchCounters *ctr);
+
 // filter-set plumbing of the fused hybrid query: docId -> row id through a dense table; selected positions -> docIds
 cudaError_t launch_map_labels(const uint32_t *d_labels, uint32_t n, const uint32_t *d_table, uint32_t table_size, uint32_t *d_ids,
                               cudaStream_t s, LaunchCounters *ctr);

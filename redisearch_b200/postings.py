@@ -95,6 +95,10 @@ SIGNATURES = [
     ("II_NewResultIterator", _QI, [_P, C.c_double]),
     ("II_IntersectEx", _P, [_P, _P, _SZ]),
     ("II_IntersectBatch", _SZ, [_SZ, _P, _P, _P]),
+    ("II_IntersectBatchDevice", _SZ, [_SZ, _P, _P, _P, _P]),
+    ("II_ResultSet_DeviceLen", _P, [_P]),
+    ("II_ResultSet_Capacity", _SZ, [_P]),
+    ("II_ResultSet_FreeAfter", None, [_P, _P]),
     ("II_IndexWriter_New", _P, [C.c_int]),
     ("II_IndexWriter_NewNumeric", _P, [C.c_int]),
     ("II_IndexWriter_Add", _SZ, [_P, C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint64, _P, C.c_uint32]),
@@ -369,11 +373,44 @@ class ResultSet:
             self.L.II_ResultSet_Free(self.h)
             self.h = None
 
+    def free_after(self, stream=None):
+        """II_ResultSet_FreeAfter: released once the work enqueued on `stream` (a torch.cuda.Stream, a raw cudaStream_t or None =
+        the legacy default stream) so far is done; the host does not wait."""
+        if self.h:
+            self.L.II_ResultSet_FreeAfter(self.h, _stream_handle(stream))
+            self.h = None
+
     def __del__(self):
         try:
             self.close()
         except Exception:
             pass
+
+
+def _stream_handle(stream):
+    if stream is None:
+        return None
+    return C.c_void_p(int(getattr(stream, "cuda_stream", stream)) or None)
+
+
+def intersect_batch_device(batch, stream=None):
+    """II_IntersectBatchDevice: batch[i] = the posting lists of query i's AND.  Enqueued without a host wait; `stream` waits for
+    every AND.  Returns [(ResultSet or None, device docId pointer, device count pointer, cap)] per query; a None set has cap 0."""
+    nq = len(batch)
+    arrays = [_list_array(lists) if lists else None for lists in batch]
+    lists_pp = (C.c_void_p * max(1, nq))(*[C.cast(a, C.c_void_p) if a is not None else None for a in arrays])
+    n_lists = (C.c_size_t * max(1, nq))(*[len(lists) for lists in batch])
+    out = (C.c_void_p * max(1, nq))()
+    L = lib()
+    L.II_IntersectBatchDevice(nq, lists_pp, n_lists, _stream_handle(stream), out)
+    res = []
+    for i in range(nq):
+        if not out[i]:
+            res.append((None, None, None, 0))
+            continue
+        rs = ResultSet(out[i])
+        res.append((rs, L.II_ResultSet_DeviceDocIds(rs.h), L.II_ResultSet_DeviceLen(rs.h), L.II_ResultSet_Capacity(rs.h)))
+    return res
 
 
 def intersect(lists) -> ResultSet:

@@ -121,6 +121,7 @@ SIGNATURES = [
     ("VecSimIndex_StatsInfo", VecSimIndexStatsInfo, [_P]),
     ("VecSimIndex_DebugInfo", VecSimIndexDebugInfo, [_P]),
     ("VecSimB200_TopKFilteredBatch", C.c_int, [_P, _P, _SZ, _SZ, _P, _P, _P, _P, _P]),
+    ("VecSimB200_TopKFilteredBatchDevice", C.c_int, [_P, _P, _SZ, _SZ, _P, _P, _P, _P, _P, _P, _P]),
     ("VecSimIndex_DebugInfoIterator", _P, [_P]),
     ("VecSimDebugInfoIterator_NumberOfFields", _SZ, [_P]),
     ("VecSimDebugInfoIterator_HasNextField", C.c_bool, [_P]),
@@ -291,6 +292,36 @@ class VecSimIndex:
         else:
             rc = self.L.VecSimB200_TopKFiltered(self.h, _ptr(q), k, C.c_void_p(int(doc_ids)), n, 1, _ptr(labels), _ptr(scores), C.byref(cnt))
         return labels[:cnt.value], scores[:cnt.value], rc
+
+    def topk_filtered_batch_device(self, d_queries, k, doc_ids, caps, counts=None, out_labels=None, out_scores=None, out_counts=None,
+                                   stream=None):
+        """VecSimB200_TopKFilteredBatchDevice, enqueued on `stream` (a torch.cuda.Stream, a raw cudaStream_t or None = the legacy
+        default stream) without waiting.  d_queries: a [nq, query_pitch] CUDA tensor of stored-form blobs (or a device pointer);
+        doc_ids / counts: per query a device pointer (int) or None; caps: per query the host bound.  Outputs are torch CUDA tensors
+        ([nq, k] int64 / float32, [nq] int32 holding the u32 counts), allocated when not given.  Returns (labels, scores, counts, rc)."""
+        import torch
+
+        nq = len(caps)
+        dev = torch.device("cuda")
+        if out_labels is None:
+            out_labels = torch.empty((nq, k), dtype=torch.int64, device=dev)
+        if out_scores is None:
+            out_scores = torch.empty((nq, k), dtype=torch.float32, device=dev)
+        if out_counts is None:
+            out_counts = torch.empty(nq, dtype=torch.int32, device=dev)
+        n = max(1, nq)
+        ids = (C.c_void_p * n)(*[int(p) if p else None for p in doc_ids])
+        cnt = (C.c_void_p * n)(*[int(p) if p else None for p in counts]) if counts is not None else None
+        cap_arr = (C.c_size_t * n)(*[int(c) for c in caps])
+        qp = d_queries.data_ptr() if hasattr(d_queries, "data_ptr") else int(d_queries)
+        sh = None if stream is None else C.c_void_p(int(getattr(stream, "cuda_stream", stream)) or None)
+        rc = self.L.VecSimB200_TopKFilteredBatchDevice(self.h, C.c_void_p(qp), nq, k, ids, cnt, cap_arr, C.c_void_p(out_labels.data_ptr()),
+                                                       C.c_void_p(out_scores.data_ptr()), C.c_void_p(out_counts.data_ptr()), sh)
+        return out_labels, out_scores, out_counts, rc
+
+    def query_pitch(self) -> int:
+        """bytes between the stored-form query blobs of a device batch"""
+        return (self.L.VecSimParams_GetQueryBlobSize(self.vtype, self.dim, self.metric) + 15) // 16 * 16
 
     def distance_from(self, label: int, blob: np.ndarray) -> float:
         blob = np.ascontiguousarray(blob)
