@@ -238,6 +238,28 @@ size_t II_ResultSet_Capacity(const II_ResultSet *rs);           /* host upper bo
  * so kernels of the caller's stream still reading the docIds would see it handed out again; use this after enqueuing a consumer
  * on another stream. */
 void II_ResultSet_FreeAfter(II_ResultSet *rs, void *stream);
+/* nq ORs with no host wait: out[i] = II_Union(lists[i], n_lists[i], quick_exit) as a set whose count is pending on the device, or
+ * NULL when query i has no list or all its lists are empty.  Once settled (any host accessor: Len, Fetch, TopN, Score, ChildOrder,
+ * IntoChild, the result iterator) every set is indistinguishable from II_Union's: docIds, count, per-hit child freq rows, aggregate
+ * child order, num_estimated, cap.  II_ResultSet_DeviceDocIds / DeviceLen / Capacity are valid in `stream` order as for
+ * II_IntersectBatchDevice, and `stream` waits, through an event, for everything the call enqueued.  The whole batch takes 4
+ * launches (quick_exit) or 6, whatever nq and the number of lists; nothing reads a count back.  Returns 0, or -1 before anything is
+ * enqueued (a query with more than 1024 lists, a NULL list, or a list carrying a nested set, II_ResultSet_IntoChild);
+ * *built (may be NULL) = the sets created. */
+int II_UnionBatchDevice(size_t nq, II_PostingList *const *const *lists, const size_t *n_lists, int quick_exit, void *stream,
+                        II_ResultSet **out, size_t *built);
+typedef struct {
+    double min, max;
+    int min_inclusive, max_inclusive;
+} II_NumericRange;
+/* nq numeric range filters with no host wait.  Query i: the leaves the host's range-tree walk picked for its filter, and the
+ * filter.  out[i] = the ascending docIds, one per document, of the documents with at least one value in the range in any of
+ * those leaves (NumericFilter::value_in_range, bit for bit) — the set II_Union(quick) over II_NumericList_Filter of each leaf
+ * builds (freq 1, docIds only, num_estimated = the sum of the filtered leaves' lengths once settled) — pending as above, or NULL
+ * when the query has no leaf record at all.  No intermediate list per leaf: the range test runs in the union's mark pass.
+ * 4 launches per batch.  Returns 0, or -1 before anything is enqueued (more than 1024 leaves, a NULL leaf or no ranges). */
+int II_NumericFilterBatchDevice(size_t nq, II_NumericList *const *const *leaves, const size_t *n_leaves, const II_NumericRange *ranges,
+                                void *stream, II_ResultSet **out, size_t *built);
 
 /* ---- scoring ------------------------------------------------------------------------------------ */
 typedef enum {

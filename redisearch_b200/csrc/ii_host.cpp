@@ -49,10 +49,36 @@ struct Ctx { // one per calling thread: own stream, events and pinned staging (R
         }
         return h_stage;
     }
+    // pinned staging of the batch filters (II_UnionBatchDevice / II_NumericFilterBatchDevice): a slot is taken again only once its
+    // last upload has executed (cudaEventQuery; a never-recorded event counts as complete), else a new slot is made — never a wait
+    struct UploadSlot {
+        uint8_t *h = nullptr;
+        size_t cap = 0;
+        cudaEvent_t ev = nullptr;
+    };
+    std::vector<UploadSlot> up_ring;
+    UploadSlot *upload_slot(size_t bytes) {
+        for (UploadSlot &u : up_ring)
+            if (u.cap >= bytes && cudaEventQuery(u.ev) == cudaSuccess) return &u;
+        cudaGetLastError(); // cudaErrorNotReady of a slot in flight is no failure
+        UploadSlot u;
+        u.cap = std::max<size_t>(2 * bytes, 64 << 10);
+        if (cudaMallocHost(&u.h, u.cap) != cudaSuccess) return nullptr;
+        if (cudaEventCreateWithFlags(&u.ev, cudaEventDisableTiming) != cudaSuccess) {
+            cudaFreeHost(u.h);
+            return nullptr;
+        }
+        up_ring.push_back(u);
+        return &up_ring.back();
+    }
     bool ok = false;
     ~Ctx() { // worker thread exits; errors after runtime teardown are harmless
         if (!ok) return;
         cudaStreamSynchronize(stream);
+        for (UploadSlot &u : up_ring) {
+            cudaEventDestroy(u.ev);
+            cudaFreeHost(u.h);
+        }
         cudaEventDestroy(e0);
         cudaEventDestroy(e1);
         cudaEventDestroy(e2);
@@ -139,6 +165,7 @@ struct II_PostingList {
     size_t n = 0;
     size_t estimated = 0; // unfiltered unique docs (num_estimated of the leaf iterator)
     uint32_t last_id = 0;
+    uint32_t first_id = 0; // a lower bound on the first docId (0 where the host does not know it): bounds the window of a union batch
     std::shared_ptr<SharedDeviceBlock> owner; // set: d_ids / d_freqs are slices of owner->p
     // term positions (Full codec, kept on request): the encoded block bytes stay on the device and every posting points at
     // its offsets payload inside them
@@ -202,6 +229,7 @@ struct II_ResultSet {
     // II_IntersectBatchDevice: the hit count is known only on the device until settle(); `ready` completes with the AND's kernels
     bool pending = false;
     cudaEvent_t ready = nullptr;
+    bool estimated_on_device = false; // II_NumericFilterBatchDevice: num_estimated is d_len[1] until settle()
     ~II_ResultSet() {
         if (ready) { // allocated on another stream, whose AND may still be writing: the frees below wait for it
             cudaStreamWaitEvent(ctx().stream, ready, 0);
@@ -393,6 +421,7 @@ static size_t from_blocks_batch(size_t n_lists, const II_BlockView *const *block
             }
             pl->n = pl->estimated = e1 - e0;
             pl->last_id = nblocks[l] ? (uint32_t)blocks[l][nblocks[l] - 1].last_doc_id : 0;
+            pl->first_id = nblocks[l] ? (uint32_t)std::min<uint64_t>(blocks[l][0].first_doc_id, pl->last_id) : 0;
             out[l] = pl;
             built++;
         }
@@ -557,6 +586,7 @@ II_PostingList *II_PostingList_FromBlocksWideMask(const II_BlockView *blocks, si
     pl->d_freqs = d_freqs;
     pl->n = kept;
     if (kept) copy_sync(&pl->last_id, d_ids + kept - 1, 4, cudaMemcpyDeviceToHost);
+    if (kept && nblocks) pl->first_id = (uint32_t)std::min<uint64_t>(blocks[0].first_doc_id, pl->last_id);
     return pl;
 }
 
@@ -581,6 +611,7 @@ II_PostingList *II_PostingList_FromArrays(const uint64_t *doc_ids, const uint32_
     }
     pl->n = pl->estimated = n;
     pl->last_id = n ? ids32[n - 1] : 0;
+    pl->first_id = n ? ids32[0] : 0;
     return pl;
 }
 
@@ -701,6 +732,7 @@ struct II_NumericList {
     uint32_t *d_ids = nullptr;
     double *d_values = nullptr;
     size_t n = 0;
+    uint32_t first_id = 0, last_id = 0; // the blocks' docId bounds
     ~II_NumericList() {
         dfree(d_ids);
         dfree(d_values);
@@ -729,6 +761,10 @@ II_NumericList *II_NumericList_FromBlocks(const II_BlockView *blocks, size_t nbl
     const size_t n = entry_off[nblocks], nbytes = byte_off[nblocks];
     auto *nl = new II_NumericList();
     nl->n = n;
+    if (nblocks) {
+        nl->last_id = (uint32_t)blocks[nblocks - 1].last_doc_id;
+        nl->first_id = (uint32_t)std::min<uint64_t>(blocks[0].first_doc_id, nl->last_id);
+    }
     nl->d_ids = dalloc<uint32_t>(n ? n : 1);
     nl->d_values = dalloc<double>(n ? n : 1);
     uint8_t *stg = c.stage(nbytes + 16);
@@ -797,6 +833,7 @@ II_PostingList *II_NumericList_Filter(const II_NumericList *nl, double min, doub
         return nullptr;
     }
     pl->n = pl->estimated = kept;
+    pl->first_id = kept ? std::min(nl->first_id, pl->last_id) : 0;
     pl->result_tag = 16; // numeric results
     return pl;
 }
@@ -1168,7 +1205,17 @@ bool prepare_nested_scores(Ctx &c, II_ResultSet *rs, II_Scorer scorer, const II_
     return true;
 }
 
-bool union_enqueue(Ctx &c, II_PostingList *const *lists, size_t n, int quick_exit, II_ResultSet *rs, bool *trivially_empty) {
+// Everything about an OR of n lists that the host knows before any kernel runs: the set's shape (children, tags, num_estimated,
+// cap), the largest last docId, whether children are nested, whether the hits keep their term positions, and the reference's
+// aggregate child order.  Shared by II_Union and II_UnionBatchDevice, so that both build the same sets.
+struct UnionPlan {
+    uint32_t max_id = 0;
+    size_t total_in = 0;
+    bool any_nested = false, keep_pos = false, flat_order = false;
+    UnionOrder uo{};
+};
+UnionPlan union_plan(II_PostingList *const *lists, size_t n, int quick_exit, II_ResultSet *rs) {
+    UnionPlan p;
     rs->is_union = true;
     rs->n_children = (uint32_t)n;
     rs->has_freqs = !quick_exit;
@@ -1177,39 +1224,26 @@ bool union_enqueue(Ctx &c, II_PostingList *const *lists, size_t n, int quick_exi
     rs->child_off.assign(n, II_ResultSet::ChildOffsets());
     rs->nested.assign(n, nullptr);
     rs->child_tag.assign(n, 4);
-    bool any_nested = false;
-    uint32_t max_id = 0;
-    size_t total_in = 0;
     rs->estimated = 0;
     for (size_t i = 0; i < n; i++) {
-        if (lists[i]->n) max_id = std::max(max_id, lists[i]->last_id);
-        total_in += lists[i]->n;
+        if (lists[i]->n) p.max_id = std::max(p.max_id, lists[i]->last_id);
+        p.total_in += lists[i]->n;
         rs->estimated += lists[i]->estimated; // union_flat.rs:102
         rs->child_tag[i] = lists[i]->result_tag;
         if (lists[i]->nested) {
             rs->nested[i] = lists[i]->nested;
-            any_nested = true;
+            p.any_nested = true;
         }
     }
-    if (any_nested && (n > (size_t)kIIMaxLists || quick_exit)) return false; // nested children need the per-child position rows
-    *trivially_empty = total_in == 0;
-    if (*trivially_empty) return true;
-    const uint32_t nwords = max_id / 32 + 1, nblk = (nwords + 31) / 32;
-    rs->cap = std::min<size_t>(total_in, (size_t)max_id + 1);
-    rs->d_docs = dalloc<uint32_t>(rs->cap);
-    rs->d_freqs = dalloc<uint32_t>(rs->has_freqs ? rs->cap * n : 1);
-    rs->d_scores = dalloc<double>(rs->cap);
-    rs->d_len = dalloc<uint32_t>(4);
-    uint32_t *bitmap = dalloc<uint32_t>(nwords), *blocksum = dalloc<uint32_t>(nblk), *blockoff = dalloc<uint32_t>(nblk);
-    uint32_t *wordoff = dalloc<uint32_t>(nwords);
+    rs->cap = std::min<size_t>(p.total_in, (size_t)p.max_id + 1);
     // the reference's aggregate child order (UnionFlat, full mode, read front to back): children live in an "active" array,
     // an exhausted child is swap-removed by the pass that follows the document it ended on (advance_and_find_min,
     // union_flat.rs:218-258; empty children by initialize_children :263-296), positions visited in ascending order and a
     // swapped-in child examined at once.  (Above min_union_iter_heap = 20 children the reference uses UnionHeap, whose
     // aggregate order follows its heap array: same docIds and children, sums may differ in the last bit.)
-    UnionOrder uo{};
-    const bool flat_order = rs->has_freqs && n <= (size_t)kIIUnionFlatMax; // more children: UnionHeap, whose order follows its heap array
-    if (flat_order) {
+    p.flat_order = rs->has_freqs && n <= (size_t)kIIUnionFlatMax; // more children: UnionHeap, whose order follows its heap array
+    if (p.flat_order && p.total_in) {
+        UnionOrder &uo = p.uo;
         std::vector<uint32_t> active(n);
         for (size_t i = 0; i < n; i++) active[i] = (uint32_t)i;
         size_t num_active = n;
@@ -1233,11 +1267,38 @@ bool union_enqueue(Ctx &c, II_PostingList *const *lists, size_t n, int quick_exi
             for (size_t i = 0; i < num_active; i++) uo.perm[e][i] = (uint8_t)active[i];
             sweep([&](uint32_t ch) { return lists[ch]->last_id == bound; });
         }
-        rs->d_order = dalloc<UnionOrder>(1);
     }
-    bool keep_pos = false;
-    for (size_t i = 0; i < n && n > 1 && n <= (size_t)kIIMaxLists && rs->has_freqs; i++) keep_pos |= lists[i]->d_off_len != nullptr;
-    keep_pos |= any_nested;
+    for (size_t i = 0; i < n && n > 1 && n <= (size_t)kIIMaxLists && rs->has_freqs; i++) p.keep_pos |= lists[i]->d_off_len != nullptr;
+    p.keep_pos |= p.any_nested;
+    if (p.keep_pos)
+        for (size_t j = 0; j < n; j++) {
+            const II_PostingList *L = lists[j];
+            II_ResultSet::ChildOffsets &co = rs->child_off[j];
+            if (!L->d_off_len) continue;
+            co.bytes = L->d_bytes;
+            co.off_pos = L->d_off_pos;
+            co.off_len = L->d_off_len;
+            co.keep_tables = L->owner;
+            co.keep_bytes = L->bytes_owner;
+        }
+    return p;
+}
+
+bool union_enqueue(Ctx &c, II_PostingList *const *lists, size_t n, int quick_exit, II_ResultSet *rs, bool *trivially_empty) {
+    const UnionPlan plan = union_plan(lists, n, quick_exit, rs);
+    const bool any_nested = plan.any_nested, flat_order = plan.flat_order, keep_pos = plan.keep_pos;
+    const UnionOrder &uo = plan.uo;
+    if (any_nested && (n > (size_t)kIIMaxLists || quick_exit)) return false; // nested children need the per-child position rows
+    *trivially_empty = plan.total_in == 0;
+    if (*trivially_empty) return true;
+    const uint32_t nwords = plan.max_id / 32 + 1, nblk = (nwords + 31) / 32;
+    rs->d_docs = dalloc<uint32_t>(rs->cap);
+    rs->d_freqs = dalloc<uint32_t>(rs->has_freqs ? rs->cap * n : 1);
+    rs->d_scores = dalloc<double>(rs->cap);
+    rs->d_len = dalloc<uint32_t>(4);
+    uint32_t *bitmap = dalloc<uint32_t>(nwords), *blocksum = dalloc<uint32_t>(nblk), *blockoff = dalloc<uint32_t>(nblk);
+    uint32_t *wordoff = dalloc<uint32_t>(nwords);
+    if (flat_order) rs->d_order = dalloc<UnionOrder>(1);
     if (keep_pos) rs->d_hit_pos = dalloc<uint32_t>(rs->cap * n);
     bool ok = rs->d_docs && rs->d_freqs && rs->d_scores && rs->d_len && bitmap && blocksum && blockoff && wordoff &&
               (!flat_order || rs->d_order) && (!keep_pos || rs->d_hit_pos);
@@ -1255,19 +1316,7 @@ bool union_enqueue(Ctx &c, II_PostingList *const *lists, size_t n, int quick_exi
             ok = ok && cudaMemcpyAsync(rs->d_order, &uo, sizeof(uo), cudaMemcpyHostToDevice, c.stream) == cudaSuccess;
             rs->h_order.reset(new UnionOrder(uo));
         }
-        if (keep_pos) {
-            ok = ok && cudaMemsetAsync(rs->d_hit_pos, 0xFF, rs->cap * n * 4, c.stream) == cudaSuccess;
-            for (size_t j = 0; j < n; j++) {
-                const II_PostingList *L = lists[j];
-                II_ResultSet::ChildOffsets &co = rs->child_off[j];
-                if (!L->d_off_len) continue;
-                co.bytes = L->d_bytes;
-                co.off_pos = L->d_off_pos;
-                co.off_len = L->d_off_len;
-                co.keep_tables = L->owner;
-                co.keep_bytes = L->bytes_owner;
-            }
-        }
+        if (keep_pos) ok = ok && cudaMemsetAsync(rs->d_hit_pos, 0xFF, rs->cap * n * 4, c.stream) == cudaSuccess;
         ok = ok && ii_launch_union(ids.data(), freqs.data(), lens.data(), (uint32_t)n, nwords, bitmap, blocksum, blockoff, wordoff,
                                    rs->d_len, rs->d_docs, rs->d_freqs, rs->cap, rs->has_freqs, rs->d_hit_pos, c.stream) == cudaSuccess;
         cudaEventRecord(c.e1, c.stream);
@@ -1596,11 +1645,13 @@ void settle(const II_ResultSet *crs) {
     auto *rs = const_cast<II_ResultSet *>(crs);
     if (!rs->pending) return;
     if (!s && cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) return;
-    uint32_t len = 0;
-    if (cudaStreamWaitEvent(s, rs->ready, 0) != cudaSuccess || cudaMemcpyAsync(&len, rs->d_len, 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+    uint32_t len[2] = {0, 0};
+    if (cudaStreamWaitEvent(s, rs->ready, 0) != cudaSuccess ||
+        cudaMemcpyAsync(len, rs->d_len, rs->estimated_on_device ? 8 : 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
         cudaStreamSynchronize(s) != cudaSuccess)
         return;
-    rs->len = len;
+    rs->len = len[0];
+    if (rs->estimated_on_device) rs->estimated = len[1];
     rs->pending = false;
 }
 } // namespace
@@ -1642,6 +1693,198 @@ II_ResultSet *II_Union(II_PostingList *const *lists, size_t n, int quick_exit) {
         return nullptr;
     }
     return rs;
+}
+
+namespace {
+// A batch of ORs (lists) or of numeric range filters (leaves + ranges) with no host wait.  Every set's memory comes from the pool
+// in c.stream order; the tables the kernels read go up in one copy from a pinned slot; ii_launch_union_batch runs the same 4 or
+// 6 launches for any batch; an event per set marks it pending and `stream` waits for the last one.
+int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_NumericList *const *const *leaves, const size_t *counts,
+                        int quick_exit, const II_NumericRange *ranges, void *stream, II_ResultSet **out, size_t *built) {
+    const bool numeric = leaves != nullptr, full = !numeric && !quick_exit;
+    if (built) *built = 0;
+    if (nq && (!out || !counts || !(numeric ? (const void *)leaves : (const void *)lists))) return -1;
+    for (size_t q = 0; q < nq; q++) out[q] = nullptr;
+    for (size_t q = 0; q < nq; q++) { // refused before anything is enqueued
+        if (counts[q] > (size_t)kIIMaxUnionLists || (counts[q] && !(numeric ? (const void *)leaves[q] : (const void *)lists[q]))) return -1;
+        if (numeric && !ranges) return -1;
+        for (size_t i = 0; i < counts[q]; i++)
+            if (numeric ? !leaves[q][i] : (!lists[q][i] || lists[q][i]->nested)) return -1;
+    }
+    Ctx &c = ctx();
+    std::lock_guard<std::mutex> g(c.mu);
+    if (!c.init()) return -1;
+    struct Plan {
+        size_t q;
+        std::unique_ptr<II_ResultSet> rs;
+        uint32_t lo_word, nwords, nblk;
+        uint64_t blk0;
+        bool keep_pos;
+        UnionOrder uo;
+    };
+    std::vector<Plan> plans;
+    uint64_t total_blocks = 0, total_chunks = 0, clear_elems = 0;
+    size_t nlists = 0, n_orders = 0;
+    for (size_t q = 0; q < nq; q++) {
+        const size_t n = counts[q];
+        if (!n) continue;
+        Plan p{q, std::unique_ptr<II_ResultSet>(new II_ResultSet()), 0, 0, 0, 0, false, UnionOrder{}};
+        II_ResultSet *rs = p.rs.get();
+        uint32_t lo = 0xFFFFFFFFu, hi = 0;
+        size_t total_in = 0;
+        for (size_t i = 0; i < n; i++) {
+            const size_t len = numeric ? leaves[q][i]->n : lists[q][i]->n;
+            if (!len) continue;
+            lo = std::min(lo, numeric ? leaves[q][i]->first_id : lists[q][i]->first_id);
+            hi = std::max(hi, numeric ? leaves[q][i]->last_id : lists[q][i]->last_id);
+            total_in += len;
+            total_chunks += (len + kUBChunk - 1) / kUBChunk;
+            nlists++;
+        }
+        if (numeric) { // the shape of II_Union(quick) over II_NumericList_Filter of every leaf
+            rs->is_union = true;
+            rs->n_children = (uint32_t)n;
+            rs->has_freqs = false;
+            rs->child_order.resize(n);
+            for (size_t i = 0; i < n; i++) rs->child_order[i] = (uint32_t)i;
+            rs->child_off.assign(n, II_ResultSet::ChildOffsets());
+            rs->nested.assign(n, nullptr);
+            rs->child_tag.assign(n, 16);
+            rs->cap = std::min<size_t>(total_in, (size_t)hi + 1);
+            rs->estimated_on_device = true;
+        } else {
+            const UnionPlan up = union_plan(lists[q], n, quick_exit, rs);
+            p.keep_pos = up.keep_pos;
+            if (up.flat_order) {
+                p.uo = up.uo;
+                rs->h_order.reset(new UnionOrder(up.uo));
+                n_orders++;
+            }
+        }
+        if (!total_in) continue; // nothing can match: no set
+        p.lo_word = lo / 32;
+        p.nwords = hi / 32 - p.lo_word + 1;
+        p.nblk = (p.nwords + 31) / 32;
+        p.blk0 = total_blocks;
+        total_blocks += p.nblk;
+        if (full) clear_elems = std::max<uint64_t>(clear_elems, (uint64_t)rs->cap * n);
+        plans.push_back(std::move(p));
+    }
+    if (plans.empty()) return 0;
+    if (total_chunks > 0x7FFFFFFFull || plans.size() > 0xFFFFFFFFull) return -1;
+    // per-set memory, then the batch's tables and bitmap scratch (freed below in stream order)
+    bool ok = true;
+    for (Plan &p : plans) {
+        II_ResultSet *rs = p.rs.get();
+        const size_t n = counts[p.q];
+        rs->d_docs = dalloc<uint32_t>(rs->cap);
+        rs->d_freqs = dalloc<uint32_t>(full ? rs->cap * n : 1);
+        rs->d_scores = dalloc<double>(rs->cap);
+        rs->d_len = dalloc<uint32_t>(4);
+        if (rs->h_order) rs->d_order = dalloc<UnionOrder>(1);
+        if (p.keep_pos) rs->d_hit_pos = dalloc<uint32_t>(rs->cap * n);
+        ok = ok && rs->d_docs && rs->d_freqs && rs->d_scores && rs->d_len && (!rs->h_order || rs->d_order) && (!p.keep_pos || rs->d_hit_pos);
+    }
+    const size_t nb = plans.size();
+    const auto align16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    const size_t off_q = align16(nlists * sizeof(UBList)), off_o = off_q + align16(nb * sizeof(UBQuery));
+    const size_t tab_bytes = off_o + n_orders * sizeof(UnionOrder);
+    const size_t est_words = (nb + 31) & ~(size_t)31;
+    const uint64_t total_words = total_blocks * 32;
+    uint8_t *d_tab = ok ? dalloc<uint8_t>(tab_bytes) : nullptr;
+    uint32_t *d_scratch = ok ? dalloc<uint32_t>(est_words + total_words * (full ? 2 : 1) + 2 * total_blocks) : nullptr;
+    Ctx::UploadSlot *slot = ok ? c.upload_slot(tab_bytes) : nullptr;
+    ok = ok && d_tab && d_scratch && slot;
+    uint32_t launches = 0;
+    if (ok) {
+        auto *h_lists = reinterpret_cast<UBList *>(slot->h);
+        auto *h_q = reinterpret_cast<UBQuery *>(slot->h + off_q);
+        auto *h_o = reinterpret_cast<UnionOrder *>(slot->h + off_o);
+        const auto *d_o = reinterpret_cast<const UnionOrder *>(d_tab + off_o);
+        uint32_t li = 0, chunk = 0, oi = 0;
+        for (size_t b = 0; b < nb; b++) {
+            const Plan &p = plans[b];
+            II_ResultSet *rs = p.rs.get();
+            const size_t n = counts[p.q];
+            UBQuery &Q = h_q[b];
+            Q = UBQuery{};
+            Q.docs = rs->d_docs;
+            Q.freqs = full ? rs->d_freqs : nullptr;
+            Q.pos = rs->d_hit_pos;
+            Q.len = rs->d_len;
+            if (rs->h_order) {
+                h_o[oi] = p.uo;
+                Q.order = rs->d_order;
+                Q.order_src = d_o + oi++;
+            }
+            Q.blk0 = p.blk0;
+            Q.nblk = p.nblk;
+            Q.lo_word = p.lo_word;
+            Q.nwords = p.nwords;
+            Q.n_rows = (uint32_t)n;
+            Q.cap = rs->cap;
+            if (numeric) {
+                const II_NumericRange &r = ranges[p.q];
+                Q.mn = r.min;
+                Q.mx = r.max;
+                Q.mni = r.min_inclusive != 0;
+                Q.mxi = r.max_inclusive != 0;
+            }
+            for (size_t i = 0; i < n; i++) {
+                UBList &L = h_lists[li];
+                if (numeric) {
+                    const II_NumericList *nl = leaves[p.q][i];
+                    if (!nl->n) continue;
+                    L = UBList{nl->d_ids, nullptr, nl->d_values, (uint32_t)nl->n, (uint32_t)b, (uint32_t)i, chunk};
+                } else {
+                    const II_PostingList *pl = lists[p.q][i];
+                    if (!pl->n) continue;
+                    L = UBList{pl->d_ids, full ? pl->d_freqs : nullptr, nullptr, (uint32_t)pl->n, (uint32_t)b, (uint32_t)i, chunk};
+                }
+                chunk += (L.len + kUBChunk - 1) / kUBChunk;
+                li++;
+            }
+        }
+        uint32_t *d_est = d_scratch, *d_bitmap = d_scratch + est_words, *d_blocksum = d_bitmap + total_words, *d_blockoff = d_blocksum + total_blocks;
+        uint32_t *d_wordoff = full ? d_blockoff + total_blocks : nullptr;
+        ok = cudaMemcpyAsync(d_tab, slot->h, tab_bytes, cudaMemcpyHostToDevice, c.stream) == cudaSuccess;
+        ok = ok && cudaEventRecord(slot->ev, c.stream) == cudaSuccess;
+        ok = ok && ii_launch_union_batch(reinterpret_cast<const UBList *>(d_tab), (uint32_t)nlists, (uint32_t)total_chunks,
+                                         reinterpret_cast<const UBQuery *>(d_tab + off_q), (uint32_t)nb, total_blocks, clear_elems, d_est,
+                                         d_bitmap, d_blocksum, d_blockoff, d_wordoff, &launches, c.stream) == cudaSuccess;
+        c.stats.kernel_launches += launches;
+    }
+    dfree(d_tab);
+    dfree(d_scratch);
+    for (Plan &p : plans) {
+        II_ResultSet *rs = p.rs.get();
+        ok = ok && cudaEventCreateWithFlags(&rs->ready, cudaEventDisableTiming) == cudaSuccess && cudaEventRecord(rs->ready, c.stream) == cudaSuccess;
+        rs->pending = true;
+    }
+    if (!ok) { // a failed allocation or launch: nothing is handed out (the frees run in c.stream order behind whatever was enqueued)
+        cudaGetLastError();
+        return -1;
+    }
+    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : cudaStreamLegacy;
+    // every set's event completes at the same point of c.stream: waiting for the last one waits for the whole batch
+    if (cudaStreamWaitEvent(st, plans.back().rs->ready, 0) != cudaSuccess) {
+        cudaStreamSynchronize(c.stream);
+        return -1;
+    }
+    for (Plan &p : plans) out[p.q] = p.rs.release();
+    if (built) *built = nb;
+    return 0;
+}
+} // namespace
+
+int II_UnionBatchDevice(size_t nq, II_PostingList *const *const *lists, const size_t *n_lists, int quick_exit, void *stream,
+                        II_ResultSet **out, size_t *built) {
+    return filter_batch_device(nq, lists, nullptr, n_lists, quick_exit, nullptr, stream, out, built);
+}
+
+int II_NumericFilterBatchDevice(size_t nq, II_NumericList *const *const *leaves, const size_t *n_leaves, const II_NumericRange *ranges,
+                                void *stream, II_ResultSet **out, size_t *built) {
+    return filter_batch_device(nq, nullptr, leaves, n_leaves, 1, ranges, stream, out, built);
 }
 
 size_t II_ResultSet_Len(const II_ResultSet *rs) {

@@ -8,6 +8,7 @@
 //   scan_kernel            exclusive prefix sum of per-chunk counts (single CTA)
 //   gather_score_kernel    survivors -> ascending docIds + per-child freqs + score
 //   union: mark / popc / expand / fill kernels over a docId bitmap (order-preserving, O(sum |L|))
+//   ub_*: the same for a whole batch of ORs / numeric range filters, ragged over every list of every query
 //   score_kernel           the reference's scorers, expression tree by expression tree
 //   topn_kernel            (score desc, docId asc) selection
 //
@@ -636,6 +637,189 @@ __global__ void fill_freq_kernel(const uint32_t *__restrict__ ids, const uint32_
         const uint32_t rank = wordoff[w] + __popc(bitmap[w] & ((1u << (id & 31)) - 1u));
         out_freq[rank] = freqs[i];
         if (out_pos) out_pos[rank] = i;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// a batch of unions / numeric range filters: the kernels above, ragged over every list of every query (ii_kernels.h: UBList)
+// ------------------------------------------------------------------------------------------------
+// the list that owns chunk b: the last one whose first chunk is <= b (empty lists own no chunk and are not in the table)
+__device__ __forceinline__ uint32_t ub_list_of(const UBList *__restrict__ lists, uint32_t nlists, uint32_t b) {
+    uint32_t lo = 0, hi = nlists; // answer in [lo, hi)
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (lists[mid].chunk0 <= b) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+// the window bit of docId id, or false when it lies outside (never for lists whose bounds the host tracked)
+__device__ __forceinline__ bool ub_bit(const UBQuery &q, uint32_t id, uint64_t &word, uint32_t &bit) {
+    if (id < q.lo_word * 32u) return false;
+    const uint32_t local = id - q.lo_word * 32u;
+    if ((local >> 5) >= q.nwords) return false;
+    word = q.blk0 * 32 + (local >> 5);
+    bit = local & 31;
+    return true;
+}
+__global__ void __launch_bounds__(256) ub_mark_kernel(const UBList *__restrict__ lists, uint32_t nlists, const UBQuery *__restrict__ qs,
+                                                      uint32_t *__restrict__ bitmap, uint32_t *__restrict__ est) {
+    __shared__ uint32_t s_l, s_kept;
+    if (threadIdx.x == 0) {
+        s_l = ub_list_of(lists, nlists, blockIdx.x);
+        s_kept = 0;
+    }
+    __syncthreads();
+    const UBList L = lists[s_l];
+    const UBQuery &q = qs[L.q];
+    const uint32_t base = (blockIdx.x - L.chunk0) * kUBChunk, end = min(base + kUBChunk, L.len);
+    uint32_t kept = 0;
+    for (uint32_t i = base + threadIdx.x; i < end; i += blockDim.x) {
+        if (L.values) { // a numeric leaf: only records in range mark; the first of its document counts toward num_estimated
+            if (!ii_numeric_in_range(L.values[i], q.mn, q.mx, q.mni, q.mxi)) continue;
+            if (numeric_keep(L.ids, L.values, i, q.mn, q.mx, q.mni, q.mxi)) kept++;
+        }
+        uint64_t w;
+        uint32_t bit;
+        if (ub_bit(q, L.ids[i], w, bit)) atomicOr(&bitmap[w], 1u << bit);
+    }
+    if (!L.values) return;
+    atomicAdd(&s_kept, kept);
+    __syncthreads();
+    if (threadIdx.x == 0 && s_kept) atomicAdd(&est[L.q], s_kept);
+}
+// bits per 32-word block; the windows are whole blocks, so a warp never straddles two queries
+__global__ void ub_popc_kernel(const uint32_t *__restrict__ bitmap, uint64_t total_words, uint32_t *__restrict__ blocksum) {
+    for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; w < total_words; w += (uint64_t)gridDim.x * blockDim.x) {
+        uint32_t c = __popc(bitmap[w]);
+#pragma unroll
+        for (int m = 16; m > 0; m >>= 1) c += __shfl_xor_sync(0xffffffffu, c, m);
+        if ((threadIdx.x & 31) == 0) blocksum[w >> 5] = c;
+    }
+}
+// one CTA per query: exclusive scan of its blocks' counts, the count into len[0] (and len[1] for numeric filters), and the
+// set's epoch table out of the batch table
+constexpr int kUBScanThreads = 1024, kUBScanItems = 8;
+__global__ void __launch_bounds__(kUBScanThreads) ub_scan_kernel(const UBQuery *__restrict__ qs, const uint32_t *__restrict__ blocksum,
+                                                                 uint32_t *__restrict__ blockoff, const uint32_t *__restrict__ est) {
+    __shared__ uint32_t s_warp[32], s_carry;
+    const UBQuery &q = qs[blockIdx.x];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) s_carry = 0;
+    __syncthreads();
+    const uint32_t *in = blocksum + q.blk0;
+    uint32_t *out = blockoff + q.blk0;
+    for (uint32_t t0 = 0; t0 < q.nblk; t0 += kUBScanThreads * kUBScanItems) {
+        const uint32_t i0 = t0 + threadIdx.x * kUBScanItems;
+        uint32_t v[kUBScanItems], sum = 0;
+#pragma unroll
+        for (int k = 0; k < kUBScanItems; k++) {
+            v[k] = i0 + k < q.nblk ? in[i0 + k] : 0;
+            sum += v[k];
+        }
+        uint32_t incl = sum;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += t;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            uint32_t w = s_warp[lane], wi = w;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint32_t t = __shfl_up_sync(0xffffffffu, wi, d);
+                if (lane >= d) wi += t;
+            }
+            s_warp[lane] = wi - w; // exclusive prefix of the warps
+        }
+        __syncthreads();
+        uint32_t o = s_carry + s_warp[warp] + incl - sum;
+#pragma unroll
+        for (int k = 0; k < kUBScanItems; k++) {
+            if (i0 + k < q.nblk) out[i0 + k] = o;
+            o += v[k];
+        }
+        __syncthreads(); // every thread has read s_carry and s_warp
+        if (threadIdx.x == kUBScanThreads - 1) s_carry = o;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        q.len[0] = s_carry;
+        q.len[1] = est[blockIdx.x];
+    }
+    if (q.order) {
+        const uint32_t *src = reinterpret_cast<const uint32_t *>(q.order_src);
+        uint32_t *dst = reinterpret_cast<uint32_t *>(q.order);
+        for (uint32_t w = threadIdx.x; w < sizeof(UnionOrder) / 4; w += blockDim.x) dst[w] = src[w];
+    }
+}
+// ascending docIds of every window: a warp per 32-word block, the query found by binary search over the windows' first blocks
+__device__ __forceinline__ uint32_t ub_query_of(const UBQuery *__restrict__ qs, uint32_t nq, uint64_t blk) {
+    uint32_t lo = 0, hi = nq;
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (qs[mid].blk0 <= blk) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+__global__ void ub_expand_kernel(const UBQuery *__restrict__ qs, uint32_t nq, const uint32_t *__restrict__ bitmap, uint64_t total_words,
+                                 const uint32_t *__restrict__ blockoff, uint32_t *__restrict__ wordoff) {
+    const int lane = threadIdx.x & 31;
+    for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; w < total_words; w += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t blk = w >> 5;
+        const UBQuery &q = qs[ub_query_of(qs, nq, blk)];
+        uint32_t bits = bitmap[w]; // words past the window stay clear
+        const uint32_t c = __popc(bits);
+        uint32_t incl = c;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += t;
+        }
+        uint32_t o = blockoff[blk] + incl - c;
+        if (wordoff) wordoff[w] = o;
+        const uint32_t id0 = (q.lo_word + (uint32_t)(w - q.blk0 * 32)) << 5;
+        while (bits) {
+            const int b = __ffs(bits) - 1;
+            bits &= bits - 1;
+            q.docs[o++] = id0 + b;
+        }
+    }
+}
+// full mode: rows [0, count) of every child zeroed (positions ~0) before the fill; a tile of 256 hits of one row per CTA step
+__global__ void ub_clear_kernel(const UBQuery *__restrict__ qs, uint32_t nq) {
+    for (uint32_t qi = blockIdx.y; qi < nq; qi += gridDim.y) {
+        const UBQuery &q = qs[qi];
+        const uint32_t m = *q.len, tpr = (m + 255) / 256;
+        const uint64_t tiles = (uint64_t)tpr * q.n_rows;
+        for (uint64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
+            const uint64_t r = t / tpr;
+            const uint32_t o = (uint32_t)(t - r * tpr) * 256 + threadIdx.x;
+            if (o >= m) continue;
+            q.freqs[r * q.cap + o] = 0;
+            if (q.pos) q.pos[r * q.cap + o] = 0xFFFFFFFFu;
+        }
+    }
+}
+// full mode: every posting's freq (and position) into its child's row at the rank of its docId (as fill_freq_kernel)
+__global__ void __launch_bounds__(256) ub_fill_kernel(const UBList *__restrict__ lists, uint32_t nlists, const UBQuery *__restrict__ qs,
+                                                      const uint32_t *__restrict__ bitmap, const uint32_t *__restrict__ wordoff) {
+    __shared__ uint32_t s_l;
+    if (threadIdx.x == 0) s_l = ub_list_of(lists, nlists, blockIdx.x);
+    __syncthreads();
+    const UBList L = lists[s_l];
+    const UBQuery &q = qs[L.q];
+    const uint32_t base = (blockIdx.x - L.chunk0) * kUBChunk, end = min(base + kUBChunk, L.len);
+    for (uint32_t i = base + threadIdx.x; i < end; i += blockDim.x) {
+        uint64_t w;
+        uint32_t bit;
+        if (!ub_bit(q, L.ids[i], w, bit)) continue;
+        const uint32_t rank = wordoff[w] + __popc(bitmap[w] & ((1u << bit) - 1u));
+        q.freqs[L.row * q.cap + rank] = L.freqs[i];
+        if (q.pos) q.pos[L.row * q.cap + rank] = i;
     }
 }
 
@@ -1627,6 +1811,29 @@ cudaError_t ii_launch_union(const uint32_t *const *d_ids, const uint32_t *const 
                 fill_freq_kernel<<<grid_for(lens[j], 256, 132 * 8), 256, 0, s>>>(d_ids[j], d_freqs[j], lens[j], d_bitmap, d_wordoff,
                                                                                 d_out_freq + (size_t)j * fstride,
                                                                                 d_out_pos ? d_out_pos + (size_t)j * fstride : nullptr);
+    return cudaGetLastError();
+}
+cudaError_t ii_launch_union_batch(const UBList *d_lists, uint32_t nlists, uint32_t total_chunks, const UBQuery *d_q, uint32_t nq,
+                                  uint64_t total_blocks, uint64_t clear_elems, uint32_t *d_est, uint32_t *d_bitmap, uint32_t *d_blocksum,
+                                  uint32_t *d_blockoff, uint32_t *d_wordoff, uint32_t *launches, cudaStream_t s) {
+    *launches = 0;
+    if (!nq || !nlists || !total_chunks) return cudaSuccess;
+    const uint64_t total_words = total_blocks * 32;
+    cudaError_t e = cudaMemsetAsync(d_est, 0, (size_t)(d_bitmap - d_est + total_words) * 4, s);
+    if (e != cudaSuccess) return e;
+    const uint32_t wgrid = grid_for(total_words, 256, 132 * 16);
+    ub_mark_kernel<<<total_chunks, 256, 0, s>>>(d_lists, nlists, d_q, d_bitmap, d_est);
+    ub_popc_kernel<<<wgrid, 256, 0, s>>>(d_bitmap, total_words, d_blocksum);
+    ub_scan_kernel<<<nq, kUBScanThreads, 0, s>>>(d_q, d_blocksum, d_blockoff, d_est);
+    ub_expand_kernel<<<wgrid, 256, 0, s>>>(d_q, nq, d_bitmap, total_words, d_blockoff, d_wordoff);
+    *launches = 4;
+    if (d_wordoff) {
+        const uint32_t gy = std::min<uint32_t>(nq, 65535);
+        const uint32_t gx = grid_for(clear_elems, 256, std::max<uint32_t>(1, 16384 / gy));
+        ub_clear_kernel<<<dim3(gx, gy), 256, 0, s>>>(d_q, nq);
+        ub_fill_kernel<<<total_chunks, 256, 0, s>>>(d_lists, nlists, d_q, d_bitmap, d_wordoff);
+        *launches = 6;
+    }
     return cudaGetLastError();
 }
 cudaError_t ii_launch_hamming(const uint32_t *d_docs, const uint32_t *d_len, uint32_t cap_len, const uint8_t *d_payloads,

@@ -115,6 +115,43 @@ struct UnionOrder {
     uint8_t perm[kIIMaxLists + 1][kIIMaxLists];
 };
 
+// ---- batches of ORs and numeric range filters (II_UnionBatchDevice, II_NumericFilterBatchDevice) -------------------------
+// Every list of every query of the batch in one ragged launch per step: each query owns a window of a shared bitmap that spans
+// the docIds of its lists, a CTA of the mark / fill passes owns kUBChunk postings of one list (found by binary search over the
+// lists' first chunks), and the scan runs one CTA per query.  Launches: 4 (docIds only) or 6 (per-child freq rows), whatever
+// the batch size and the number of lists.
+constexpr uint32_t kUBChunk = 1024;
+struct UBList {
+    const uint32_t *ids;
+    const uint32_t *freqs; // full mode: the list's freqs (else NULL)
+    const double *values;  // a numeric leaf: its record values, tested against the query's range (NULL: a posting list)
+    uint32_t len;
+    uint32_t q;      // owning query (index into the UBQuery table)
+    uint32_t row;    // the list's child index inside its query: its freq / position row
+    uint32_t chunk0; // first kUBChunk chunk of the list in the batch
+};
+struct UBQuery {
+    uint32_t *docs;  // the set's docIds [cap]
+    uint32_t *freqs; // full mode: [n_rows][cap] (else NULL)
+    uint32_t *pos;   // [n_rows][cap] posting position of the hit inside each child, ~0 = absent (NULL: not kept)
+    uint32_t *len;   // [0] = the count; [1] = in-range records that are the first of their document in their leaf (numeric)
+    UnionOrder *order;           // the set's epoch table (NULL: none) ...
+    const UnionOrder *order_src; // ... copied from the uploaded batch table by the scan
+    uint64_t blk0;     // first 32-word block of the query's window in the batch bitmap
+    uint32_t nblk;     // blocks of the window
+    uint32_t lo_word;  // the window covers docIds lo_word * 32 .. (lo_word + nwords) * 32 - 1
+    uint32_t nwords;
+    uint32_t n_rows;
+    uint64_t cap;      // row stride of freqs / pos
+    double mn, mx;     // numeric range (NumericFilter::value_in_range)
+    int mni, mxi;
+};
+// d_est [nq] and d_bitmap [total_blocks * 32] are contiguous (one memset clears both); d_wordoff NULL = docIds only.
+// clear_elems: the largest n_rows * cap of the batch (sizes the clear of the freq / position rows).  Returns the launches made.
+cudaError_t ii_launch_union_batch(const UBList *d_lists, uint32_t nlists, uint32_t total_chunks, const UBQuery *d_q, uint32_t nq,
+                                  uint64_t total_blocks, uint64_t clear_elems, uint32_t *d_est, uint32_t *d_bitmap, uint32_t *d_blocksum,
+                                  uint32_t *d_blockoff, uint32_t *d_wordoff, uint32_t *launches, cudaStream_t s);
+
 struct ScoreArgs {
     int scorer; // II_Scorer numbering
     int is_union;

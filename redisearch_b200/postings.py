@@ -24,6 +24,10 @@ class II_IndexStats(C.Structure):
     _fields_ = [("numDocs", C.c_size_t), ("numTerms", C.c_size_t), ("avgDocLen", C.c_double)]
 
 
+class II_NumericRange(C.Structure):
+    _fields_ = [("min", C.c_double), ("max", C.c_double), ("min_inclusive", C.c_int), ("max_inclusive", C.c_int)]
+
+
 class II_Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("intersect_device_us", C.c_double), ("score_device_us", C.c_double),
                 ("decode_host_us", C.c_double), ("h2d_us", C.c_double)]
@@ -99,6 +103,8 @@ SIGNATURES = [
     ("II_ResultSet_DeviceLen", _P, [_P]),
     ("II_ResultSet_Capacity", _SZ, [_P]),
     ("II_ResultSet_FreeAfter", None, [_P, _P]),
+    ("II_UnionBatchDevice", C.c_int, [_SZ, _P, _P, C.c_int, _P, _P, C.POINTER(_SZ)]),
+    ("II_NumericFilterBatchDevice", C.c_int, [_SZ, _P, _P, _P, _P, _P, C.POINTER(_SZ)]),
     ("II_IndexWriter_New", _P, [C.c_int]),
     ("II_IndexWriter_NewNumeric", _P, [C.c_int]),
     ("II_IndexWriter_Add", _SZ, [_P, C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint64, _P, C.c_uint32]),
@@ -411,6 +417,50 @@ def intersect_batch_device(batch, stream=None):
         rs = ResultSet(out[i])
         res.append((rs, L.II_ResultSet_DeviceDocIds(rs.h), L.II_ResultSet_DeviceLen(rs.h), L.II_ResultSet_Capacity(rs.h)))
     return res
+
+
+def _pending_sets(rc, out, nq):
+    if rc != 0:
+        raise ValueError("the batch was refused (too many lists, a NULL or nested list)")
+    L, res = lib(), []
+    for i in range(nq):
+        if not out[i]:
+            res.append((None, None, None, 0))
+            continue
+        rs = ResultSet(out[i])
+        res.append((rs, L.II_ResultSet_DeviceDocIds(rs.h), L.II_ResultSet_DeviceLen(rs.h), L.II_ResultSet_Capacity(rs.h)))
+    return res
+
+
+def _handle_table(batch):
+    """(pointer table per query, its keep-alive arrays, counts) of batch[i] = a list of objects with .h"""
+    nq = len(batch)
+    arrays = [(C.c_void_p * len(items))(*[x.h for x in items]) if items else None for items in batch]
+    pp = (C.c_void_p * max(1, nq))(*[C.cast(a, C.c_void_p) if a is not None else None for a in arrays])
+    counts = (C.c_size_t * max(1, nq))(*[len(items) for items in batch])
+    return pp, arrays, counts
+
+
+def union_batch_device(batch, quick_exit=False, stream=None):
+    """II_UnionBatchDevice: batch[i] = the posting lists of query i's OR.  Enqueued without a host wait; `stream` waits for the
+    batch.  Returns [(ResultSet or None, device docId pointer, device count pointer, cap)] per query (a None set has cap 0);
+    raises ValueError when the batch is refused."""
+    nq = len(batch)
+    pp, _keep, counts = _handle_table(batch)
+    out = (C.c_void_p * max(1, nq))()
+    rc = lib().II_UnionBatchDevice(nq, pp, counts, int(quick_exit), _stream_handle(stream), out, None)
+    return _pending_sets(rc, out, nq)
+
+
+def numeric_filter_batch_device(batch, stream=None):
+    """II_NumericFilterBatchDevice: batch[i] = (leaves, lo, hi, lo_inclusive, hi_inclusive), leaves = NumericList objects the
+    range-tree walk picked.  Returns as union_batch_device."""
+    nq = len(batch)
+    pp, _keep, counts = _handle_table([b[0] for b in batch])
+    ranges = (II_NumericRange * max(1, nq))(*[II_NumericRange(float(lo), float(hi), int(li), int(hi_)) for _, lo, hi, li, hi_ in batch])
+    out = (C.c_void_p * max(1, nq))()
+    rc = lib().II_NumericFilterBatchDevice(nq, pp, counts, ranges, _stream_handle(stream), out, None)
+    return _pending_sets(rc, out, nq)
 
 
 def intersect(lists) -> ResultSet:
