@@ -260,6 +260,39 @@ typedef struct {
  * 4 launches per batch.  Returns 0, or -1 before anything is enqueued (more than 1024 leaves, a NULL leaf or no ranges). */
 int II_NumericFilterBatchDevice(size_t nq, II_NumericList *const *const *leaves, const size_t *n_leaves, const II_NumericRange *ranges,
                                 void *stream, II_ResultSet **out, size_t *built);
+/* One child of a filter-mode AND: a posting list, or a set of II_IntersectBatchDevice / II_UnionBatchDevice /
+ * II_NumericFilterBatchDevice / II_IntersectFilterBatchDevice (or any other set), pending or settled.  Both NULL: an empty child
+ * (the NULL those calls hand out for a filter that matches nothing). */
+typedef struct {
+    const II_PostingList *list;
+    const II_ResultSet *set;
+    int mode; /* 0 required, 1 NOT */
+} II_FilterChild;
+/* nq ANDs of lists and sets in FILTER MODE with no host wait — `@brand:nike @category:{shoes|boots}`, `@brand:nike
+ * @price:[50 200]`, `@category:{shoes|boots} @price:[50 200] -@tag:{sale}` ahead of a KNN — without settling the ORs and ranges
+ * first.  out[q] = the ascending docIds and count of the AND of children[q][0 .. n_children[q]), each set counting as the docIds
+ * it holds once settled: what II_IntersectEx gives over the same lists plus II_PostingList_FromDevice of each set's docIds, with
+ * the same modes.  out[q] is NULL when a required child is empty on the host (a list of length 0, a set of capacity 0, an empty
+ * child); an empty NOT child excludes nothing.
+ * Filter mode: a set carries docIds, count, num_estimated and the child order, no per-child freq rows (has no scores): II_Score
+ * returns -1 and II_ResultSet_IntoChild NULL, as for quick unions.  Its shape: n_children = n_children[q]; capacity = the
+ * smallest host bound of a required child (a list's length, a set's II_ResultSet_Capacity); num_estimated = the smallest of the
+ * required children's, a set counting with its own num_estimated and sort weight as II_ResultSet_IntoChild would give them (1
+ * for an OR, 1 / its children for an AND); child order = Intersection::new's stable sort by num_estimated x sort weight, NOT
+ * children last.  Where a required child's estimate is still on the device (a pending numeric set, or a pending set of this call
+ * that has one), the order and the estimate are worked out when the set settles; II_ResultSet_ChildOrder then settles it first.
+ * II_ResultSet_DeviceDocIds / DeviceLen / Capacity are valid in `stream` order; DeviceLen[1] holds the set's num_estimated and
+ * DeviceLen[2 + i] child i's (both saturated at 2^32 - 1).  An output is a valid set child of a later call and a valid KNN
+ * filter (VecSimB200_TopKFilteredBatchDevice).
+ * No host wait: the library's stream waits for each pending child set's own kernels through events, the tables go up from
+ * pinned staging, nothing reads a count back, and `stream` waits for the batch through an event.  3 launches per batch, whatever
+ * nq and the number of children.  The inputs are borrowed: a child set may be freed (II_ResultSet_Free / FreeAfter) right after
+ * the call, from any thread; its memory is released once the call's kernels are done with it.  One set may be a child of calls
+ * on several threads at once.
+ * Returns 0, or -1 before anything is enqueued: NULL arguments, a query with more than 32 children or no required child, a mode
+ * other than 0 or 1, a child with both `list` and `set`.  *built (may be NULL) = the sets created. */
+int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *children, const size_t *n_children, void *stream,
+                                  II_ResultSet **out, size_t *built);
 
 /* ---- scoring ------------------------------------------------------------------------------------ */
 typedef enum {
@@ -310,7 +343,8 @@ int II_ScoreHamming(II_ResultSet *rs, const II_DocTable *docs, const void *qdata
  * (children in aggregate order; 0 = child absent, union only).  scores are 0 before II_Score. */
 int II_ResultSet_Fetch(const II_ResultSet *rs, uint64_t *doc_ids, double *scores, uint32_t *child_freqs);
 size_t II_ResultSet_NumChildren(const II_ResultSet *rs);
-/* child_order[i] = index in the `lists` argument of aggregate child i. */
+/* child_order[i] = index in the `lists` argument of aggregate child i (a set of II_IntersectFilterBatchDevice whose order waits
+ * for estimates on the device is settled first). */
 void II_ResultSet_ChildOrder(const II_ResultSet *rs, uint32_t *child_order);
 /* Best `n` hits by (score desc, docId asc) — RPSorter's cmpByScore, src/result_processor.c:834-850 —
  * selected on device.  Returns the number written. */

@@ -159,6 +159,19 @@ struct SharedDeviceBlock {
     void *p = nullptr;
     ~SharedDeviceBlock() { dfree(p); }
 };
+// an event shared by the sets that must outlive it (destroyed when the last of them goes; a pending event is released once it
+// completes)
+struct SharedEvent {
+    cudaEvent_t ev = nullptr;
+    ~SharedEvent() {
+        if (ev) cudaEventDestroy(ev);
+    }
+};
+// guards II_ResultSet::readers: one set may be a child of II_IntersectFilterBatchDevice calls on several threads at once
+static std::mutex &readers_mu() {
+    static std::mutex m;
+    return m;
+}
 
 struct II_PostingList {
     uint32_t *d_ids = nullptr, *d_freqs = nullptr;
@@ -230,10 +243,20 @@ struct II_ResultSet {
     bool pending = false;
     cudaEvent_t ready = nullptr;
     bool estimated_on_device = false; // II_NumericFilterBatchDevice: num_estimated is d_len[1] until settle()
+    // II_IntersectFilterBatchDevice with a child whose estimate is on the device: the child order waits for settle(), which sorts by
+    // d_len[2 + i] (child i's num_estimated) times order_weight[i] (its sort weight; < 0 = a NOT child, sorted last); child_tag
+    // is in the given order until then
+    std::vector<double> order_weight;
+    // completion events of the II_IntersectFilterBatchDevice calls that read this set as a child: the frees below wait for them
+    std::vector<std::shared_ptr<struct SharedEvent>> readers;
     ~II_ResultSet() {
         if (ready) { // allocated on another stream, whose AND may still be writing: the frees below wait for it
             cudaStreamWaitEvent(ctx().stream, ready, 0);
             cudaEventDestroy(ready);
+        }
+        {
+            std::lock_guard<std::mutex> g(readers_mu());
+            for (const auto &r : readers) cudaStreamWaitEvent(ctx().stream, r->ev, 0);
         }
         dfree(d_docs);
         dfree(d_freqs);
@@ -938,16 +961,18 @@ struct PhraseSpec {
     uint32_t max_slop; // 0xFFFFFFFF: no limit (in-order only)
     bool in_order;
 };
+// sort key of Intersection::new_with_slop_order (intersection.rs:110-120): num_estimated * intersection_sort_weight, as doubles;
+// NOT / OPTIONAL children estimate max_doc_id (not.rs / optional.rs num_estimated): they sort behind every other child
+inline double and_sort_key(bool required, double estimated, double sort_weight) { return required ? estimated * sort_weight : 0x1p62; }
 bool intersect_enqueue(Ctx &c, II_PostingList *const *lists, size_t n, II_ResultSet *rs, bool *trivially_empty, const int *modes = nullptr,
                        const PhraseSpec *phrase = nullptr) {
     auto mode_of = [&](size_t i) { return modes ? modes[i] : 0; };
     if (phrase && n > (size_t)kPhraseMaxLists) return false;
     // Intersection::new: stable sort ascending by num_estimated (leaf weight 1.0), intersection.rs:110-145; NOT / OPTIONAL
-    // children estimate max_doc_id (not.rs / optional.rs num_estimated): they sort behind every term, in their given order
+    // children behind every term, in their given order
     std::vector<uint32_t> order(n);
     for (size_t i = 0; i < n; i++) order[i] = (uint32_t)i;
-    // sort key of Intersection::new_with_slop_order (:110-120): num_estimated * intersection_sort_weight, as doubles
-    auto est = [&](uint32_t a) { return mode_of(a) ? 0x1p62 : (double)lists[a]->estimated * lists[a]->sort_weight; };
+    auto est = [&](uint32_t a) { return and_sort_key(mode_of(a) == 0, (double)lists[a]->estimated, lists[a]->sort_weight); };
     // an in-order intersection keeps the children as given: their order is the order the terms must appear in
     // (intersection.rs new_sorted_by: `if !in_order { children.sort_by(compare) }`)
     if (!(phrase && phrase->in_order)) std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return est(a) < est(b); });
@@ -1645,13 +1670,26 @@ void settle(const II_ResultSet *crs) {
     auto *rs = const_cast<II_ResultSet *>(crs);
     if (!rs->pending) return;
     if (!s && cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) return;
-    uint32_t len[2] = {0, 0};
+    uint32_t len[2 + kIIMaxLists] = {};
+    const size_t words = (rs->estimated_on_device ? 2 : 1) + rs->order_weight.size(); // a deferred child order: estimated on device
     if (cudaStreamWaitEvent(s, rs->ready, 0) != cudaSuccess ||
-        cudaMemcpyAsync(len, rs->d_len, rs->estimated_on_device ? 8 : 4, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-        cudaStreamSynchronize(s) != cudaSuccess)
+        cudaMemcpyAsync(len, rs->d_len, words * 4, cudaMemcpyDeviceToHost, s) != cudaSuccess || cudaStreamSynchronize(s) != cudaSuccess)
         return;
     rs->len = len[0];
     if (rs->estimated_on_device) rs->estimated = len[1];
+    if (!rs->order_weight.empty()) { // Intersection::new's order over the children's estimates, now on the host
+        const std::vector<double> &w = rs->order_weight;
+        std::vector<uint32_t> order(w.size());
+        for (size_t i = 0; i < order.size(); i++) order[i] = (uint32_t)i;
+        std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
+            return and_sort_key(w[a] >= 0, (double)len[2 + a], w[a]) < and_sort_key(w[b] >= 0, (double)len[2 + b], w[b]);
+        });
+        std::vector<uint8_t> tag(order.size());
+        for (size_t j = 0; j < order.size(); j++) tag[j] = rs->child_tag[order[j]];
+        rs->child_order = std::move(order);
+        rs->child_tag = std::move(tag);
+        rs->order_weight.clear();
+    }
     rs->pending = false;
 }
 } // namespace
@@ -1887,12 +1925,207 @@ int II_NumericFilterBatchDevice(size_t nq, II_NumericList *const *const *leaves,
     return filter_batch_device(nq, nullptr, leaves, n_leaves, 1, ranges, stream, out, built);
 }
 
+// ANDs over lists and (pending) sets in filter mode, with no host wait.  The driver of each query is the required child with the
+// smallest host bound; every other child is probed with the AND of intersect_kernel, each set's count read on the device.  Every
+// set's memory comes from the pool in c.stream order, the tables go up in one copy from a pinned slot, ii_launch_filter_and_batch
+// runs the same 3 launches for any batch, an event per set marks it pending and `stream` waits for the last one.  The child sets
+// are borrowed: each keeps the call's completion event, which its destructor waits for.
+int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *children, const size_t *n_children, void *stream,
+                                  II_ResultSet **out, size_t *built) {
+    if (built) *built = 0;
+    if (nq && (!children || !n_children || !out)) return -1;
+    for (size_t q = 0; q < nq; q++) out[q] = nullptr;
+    for (size_t q = 0; q < nq; q++) { // refused before anything is enqueued
+        const size_t n = n_children[q];
+        if (n > (size_t)kIIMaxLists || (n && !children[q])) return -1;
+        size_t required = 0;
+        for (size_t i = 0; i < n; i++) {
+            const II_FilterChild &ch = children[q][i];
+            if ((ch.mode != 0 && ch.mode != 1) || (ch.list && ch.set)) return -1;
+            required += ch.mode == 0;
+        }
+        if (!required) return -1;
+    }
+    const auto bound = [](const II_FilterChild &ch) -> size_t { return ch.list ? ch.list->n : ch.set ? ch.set->cap : 0; };
+    const auto sat = [](size_t v) { return (uint32_t)std::min<size_t>(v, 0xFFFFFFFFu); };
+    struct Plan {
+        size_t q;
+        std::unique_ptr<II_ResultSet> rs;
+        std::vector<uint32_t> probe; // kernel order: the driver, then the others by ascending host bound
+        uint32_t chunk0, nchunks;
+    };
+    std::vector<Plan> plans;
+    std::vector<II_ResultSet *> inputs; // every child set, once
+    uint64_t total_chunks = 0;
+    size_t total_children = 0;
+    for (size_t q = 0; q < nq; q++) {
+        const size_t n = n_children[q];
+        const II_FilterChild *cs = children[q];
+        size_t drv = n;
+        bool empty = false;
+        for (size_t i = 0; i < n; i++) {
+            if (cs[i].set) inputs.push_back(const_cast<II_ResultSet *>(cs[i].set)); // borrowed: only its reader events change
+            if (cs[i].mode != 0) continue;
+            empty |= bound(cs[i]) == 0;
+            if (drv == n || bound(cs[i]) < bound(cs[drv])) drv = i;
+        }
+        if (empty) continue; // a required child empty on the host: no set
+        Plan p{q, std::unique_ptr<II_ResultSet>(new II_ResultSet()), {}, (uint32_t)total_chunks, 0};
+        II_ResultSet *rs = p.rs.get();
+        rs->is_union = false;
+        rs->has_freqs = false;
+        rs->n_children = (uint32_t)n;
+        rs->cap = bound(cs[drv]);
+        rs->child_off.assign(n, II_ResultSet::ChildOffsets());
+        rs->nested.assign(n, nullptr);
+        // the shape Intersection::new gives the children: a set counts as the list view II_ResultSet_IntoChild makes of it
+        std::vector<uint8_t> tag(n);
+        std::vector<double> weight(n);
+        std::vector<size_t> est(n);
+        bool deferred = false;
+        rs->estimated = (size_t)-1;
+        for (size_t i = 0; i < n; i++) {
+            const II_FilterChild &ch = cs[i];
+            const II_ResultSet *s = ch.set;
+            tag[i] = ch.mode == 1 ? 8 : ch.list ? ch.list->result_tag : s->is_union ? 1 : 2;
+            weight[i] = ch.list ? ch.list->sort_weight : s && !s->is_union ? 1.0 / (double)std::max<uint32_t>(1, s->n_children) : 1.0;
+            est[i] = ch.list ? ch.list->estimated : s ? s->estimated : 0;
+            if (ch.mode != 0) continue;
+            deferred |= s && s->pending && s->estimated_on_device;
+            rs->estimated = std::min(rs->estimated, est[i]);
+        }
+        if (deferred) { // the order and the estimate wait for settle()
+            rs->estimated_on_device = true;
+            rs->child_tag = tag;
+            rs->order_weight.resize(n);
+            for (size_t i = 0; i < n; i++) rs->order_weight[i] = cs[i].mode == 0 ? weight[i] : -1.0;
+            rs->child_order.resize(n);
+            for (size_t i = 0; i < n; i++) rs->child_order[i] = (uint32_t)i;
+        } else {
+            std::vector<uint32_t> order(n);
+            for (size_t i = 0; i < n; i++) order[i] = (uint32_t)i;
+            std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
+                return and_sort_key(cs[a].mode == 0, (double)est[a], weight[a]) < and_sort_key(cs[b].mode == 0, (double)est[b], weight[b]);
+            });
+            rs->child_tag.resize(n);
+            for (size_t j = 0; j < n; j++) rs->child_tag[j] = tag[order[j]];
+            rs->child_order = std::move(order);
+        }
+        p.probe.push_back((uint32_t)drv);
+        for (size_t i = 0; i < n; i++)
+            if (i != drv) p.probe.push_back((uint32_t)i);
+        std::stable_sort(p.probe.begin() + 1, p.probe.end(), [&](uint32_t a, uint32_t b) { return bound(cs[a]) < bound(cs[b]); });
+        p.nchunks = (uint32_t)((rs->cap + kIIChunk - 1) / kIIChunk);
+        total_chunks += p.nchunks;
+        total_children += n;
+        plans.push_back(std::move(p));
+    }
+    if (plans.empty()) return 0;
+    if (total_chunks > 0x7FFFFFFFull) return -1;
+    Ctx &c = ctx();
+    std::lock_guard<std::mutex> g(c.mu);
+    if (!c.init()) return -1;
+    // per-set memory, then the batch's tables and scratch in one allocation (freed below in stream order)
+    bool ok = true;
+    for (Plan &p : plans) {
+        II_ResultSet *rs = p.rs.get();
+        rs->d_docs = dalloc<uint32_t>(rs->cap);
+        rs->d_scores = dalloc<double>(rs->cap);
+        rs->d_len = dalloc<uint32_t>(2 + (size_t)rs->n_children);
+        ok = ok && rs->d_docs && rs->d_scores && rs->d_len;
+    }
+    const size_t nb = plans.size();
+    const auto align16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    const size_t off_c = align16(nb * sizeof(IFBQuery)), tab_bytes = off_c + total_children * sizeof(IFBChild);
+    const size_t scratch_bytes = align16(tab_bytes) + ((size_t)total_chunks * kIIChunk + 2 * (size_t)total_chunks) * 4;
+    uint8_t *d_scratch = ok ? dalloc<uint8_t>(scratch_bytes) : nullptr;
+    Ctx::UploadSlot *slot = ok ? c.upload_slot(tab_bytes) : nullptr;
+    ok = ok && d_scratch && slot;
+    if (ok) {
+        auto *h_q = reinterpret_cast<IFBQuery *>(slot->h);
+        auto *h_c = reinterpret_cast<IFBChild *>(slot->h + off_c);
+        uint32_t ci = 0;
+        for (size_t b = 0; b < nb; b++) {
+            const Plan &p = plans[b];
+            II_ResultSet *rs = p.rs.get();
+            h_q[b] = IFBQuery{rs->d_docs, rs->d_len, ci, rs->n_children, p.chunk0, p.nchunks};
+            for (uint32_t slot_i : p.probe) {
+                const II_FilterChild &ch = children[p.q][slot_i];
+                IFBChild &K = h_c[ci++];
+                K = IFBChild{};
+                K.slot = slot_i;
+                K.mode = (uint32_t)ch.mode;
+                if (ch.list) {
+                    K.ids = ch.list->d_ids;
+                    K.len = (uint32_t)ch.list->n;
+                    K.est = sat(ch.list->estimated);
+                } else if (ch.set) {
+                    const II_ResultSet *s = ch.set;
+                    K.ids = s->d_docs;
+                    K.d_len = s->cap ? s->d_len : nullptr; // a set built empty may have no device count
+                    K.len = (uint32_t)s->cap;
+                    K.d_est = K.d_len && s->pending && s->estimated_on_device ? s->d_len + 1 : nullptr;
+                    K.est = sat(s->estimated);
+                }
+            }
+        }
+        // the AND reads each child set once that set's own kernels are done (a settled or host-built set: at once)
+        std::sort(inputs.begin(), inputs.end());
+        inputs.erase(std::unique(inputs.begin(), inputs.end()), inputs.end());
+        for (II_ResultSet *s : inputs)
+            if (s->ready) ok = ok && cudaStreamWaitEvent(c.stream, s->ready, 0) == cudaSuccess;
+        const auto *d_q = reinterpret_cast<const IFBQuery *>(d_scratch);
+        const auto *d_c = reinterpret_cast<const IFBChild *>(d_scratch + off_c);
+        uint32_t *d_surv = reinterpret_cast<uint32_t *>(d_scratch + align16(tab_bytes));
+        uint32_t *d_counts = d_surv + (size_t)total_chunks * kIIChunk, *d_offsets = d_counts + total_chunks;
+        ok = ok && cudaMemcpyAsync(d_scratch, slot->h, tab_bytes, cudaMemcpyHostToDevice, c.stream) == cudaSuccess;
+        ok = ok && cudaEventRecord(slot->ev, c.stream) == cudaSuccess;
+        ok = ok && ii_launch_filter_and_batch(d_c, d_q, (uint32_t)nb, (uint32_t)total_chunks, d_surv, d_counts, d_offsets, c.stream) ==
+                       cudaSuccess;
+        c.stats.kernel_launches += 3;
+        // every input keeps the call's completion event: its memory is not handed out again while the AND may still read it
+        auto done = std::make_shared<SharedEvent>();
+        if (cudaEventCreateWithFlags(&done->ev, cudaEventDisableTiming) == cudaSuccess && cudaEventRecord(done->ev, c.stream) == cudaSuccess) {
+            std::lock_guard<std::mutex> rg(readers_mu());
+            for (II_ResultSet *s : inputs) {
+                auto &r = s->readers;
+                r.erase(std::remove_if(r.begin(), r.end(), [](const std::shared_ptr<SharedEvent> &e) { return cudaEventQuery(e->ev) == cudaSuccess; }),
+                        r.end());
+                r.push_back(done);
+            }
+            cudaGetLastError(); // cudaErrorNotReady of a reader still running is no failure
+        } else {
+            cudaStreamSynchronize(c.stream);
+            ok = false;
+        }
+    }
+    dfree(d_scratch);
+    for (Plan &p : plans) {
+        II_ResultSet *rs = p.rs.get();
+        ok = ok && cudaEventCreateWithFlags(&rs->ready, cudaEventDisableTiming) == cudaSuccess && cudaEventRecord(rs->ready, c.stream) == cudaSuccess;
+        rs->pending = true;
+    }
+    if (!ok) { // nothing is handed out (the frees run in c.stream order behind whatever was enqueued)
+        cudaGetLastError();
+        return -1;
+    }
+    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : cudaStreamLegacy;
+    if (cudaStreamWaitEvent(st, plans.back().rs->ready, 0) != cudaSuccess) {
+        cudaStreamSynchronize(c.stream);
+        return -1;
+    }
+    for (Plan &p : plans) out[p.q] = p.rs.release();
+    if (built) *built = nb;
+    return 0;
+}
+
 size_t II_ResultSet_Len(const II_ResultSet *rs) {
     settle(rs);
     return rs->len;
 }
 size_t II_ResultSet_NumChildren(const II_ResultSet *rs) { return rs->n_children; }
 void II_ResultSet_ChildOrder(const II_ResultSet *rs, uint32_t *child_order) {
+    if (!rs->order_weight.empty()) settle(rs); // the order waits for the children's estimates on the device
     for (uint32_t i = 0; i < rs->n_children; i++) child_order[i] = rs->child_order[i];
 }
 void II_ResultSet_Free(II_ResultSet *rs) { delete rs; }

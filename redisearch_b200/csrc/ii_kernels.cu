@@ -9,6 +9,7 @@
 //   gather_score_kernel    survivors -> ascending docIds + per-child freqs + score
 //   union: mark / popc / expand / fill kernels over a docId bitmap (order-preserving, O(sum |L|))
 //   ub_*: the same for a whole batch of ORs / numeric range filters, ragged over every list of every query
+//   ifb_*: the AND probe of intersect_kernel for a whole batch of filter-mode ANDs, ragged over every query's driver chunks
 //   score_kernel           the reference's scorers, expression tree by expression tree
 //   topn_kernel            (score desc, docId asc) selection
 //
@@ -257,34 +258,33 @@ __device__ __forceinline__ uint32_t warp_lower_bound_u32(const uint32_t *a, uint
     return lo + __popc(__ballot_sync(0xffffffffu, less));
 }
 
-__global__ void __launch_bounds__(kIIThreads) intersect_kernel(const IntersectArgs a) {
-    __shared__ uint32_t sB[kIISmemElems];
-    __shared__ uint32_t s_lo, s_hi;
-    __shared__ uint32_t s_warp[kIIThreads / 32];
-    const uint32_t chunk = blockIdx.x;
-    const uint32_t start = chunk * kIIChunk;
-    const uint32_t end = min(start + (uint32_t)kIIChunk, a.len[0]);
-    const uint32_t *A = a.ids[0];
-    uint32_t doc[kIIItems];
-    bool alive[kIIItems];
-#pragma unroll
-    for (int i = 0; i < kIIItems; i++) {
-        const uint32_t idx = start + threadIdx.x * kIIItems + i; // blocked: a thread owns consecutive entries
-        alive[i] = idx < end;
-        doc[i] = alive[i] ? A[idx] : 0xFFFFFFFFu;
-    }
-    const uint32_t a_lo = A[start], a_hi = A[end - 1];
-    for (uint32_t j = 1; j < a.n; j++) {
-        const uint32_t *B = a.ids[j];
+// One list of a CTA's AND probe: its docIds, exact length, mode (0 required, 1 NOT, 2 OPTIONAL) and the nullable row that
+// receives the position of every driving entry inside it (pos[e] for entry e of the driving list)
+struct ProbeList {
+    const uint32_t *ids;
+    uint32_t len;
+    int mode;
+    uint32_t *pos;
+};
+// The k-way AND of one CTA, shared by intersect_kernel and ifb_probe_kernel: each thread's kIIItems consecutive entries e0 + i
+// of the driving list (doc / alive) against lists 1 .. n-1 (list_of(j) -> ProbeList).  For every list, warps 0 and 1 find the
+// window of docIds [a_lo, a_hi] with a warp-wide lower bound, the window is staged in shared memory when it fits, and each
+// entry's lower bound runs there.  Stops once no entry of the CTA is alive.
+template <typename ListOf>
+__device__ __forceinline__ void and_probe(const uint32_t (&doc)[kIIItems], bool (&alive)[kIIItems], uint32_t e0, uint32_t a_lo, uint32_t a_hi,
+                                          uint32_t n, ListOf list_of, uint32_t *sB, uint32_t &s_lo, uint32_t &s_hi) {
+    for (uint32_t j = 1; j < n; j++) {
+        const ProbeList L = list_of(j);
+        const uint32_t *B = L.ids;
         if (threadIdx.x < 64) { // warp 0 finds the window start, warp 1 its end
             const bool first = threadIdx.x < 32;
-            const uint32_t r = warp_lower_bound_u32(B, 0, a.len[j], first ? a_lo : a_hi + 1u, threadIdx.x & 31); // a_hi < 2^32-1
+            const uint32_t r = warp_lower_bound_u32(B, 0, L.len, first ? a_lo : a_hi + 1u, threadIdx.x & 31); // a_hi < 2^32-1
             if ((threadIdx.x & 31) == 0) *(first ? &s_lo : &s_hi) = r;
         }
         __syncthreads();
         const uint32_t lo = s_lo, hi = s_hi, range = hi - lo;
-        uint32_t *posj = a.tmp_pos + (size_t)j * a.stride;
-        const int mode = a.mode[j];
+        uint32_t *posj = L.pos;
+        const int mode = L.mode;
         const bool staged = range <= (uint32_t)kIISmemElems;
         if (staged) {
             for (uint32_t t = threadIdx.x; t < range; t += kIIThreads) cp_async4(&sB[t], B + lo + t);
@@ -306,11 +306,11 @@ __global__ void __launch_bounds__(kIIThreads) intersect_kernel(const IntersectAr
                 }
                 if (mode == 0) { // required
                     alive[i] = found;
-                    if (found) posj[start + threadIdx.x * kIIItems + i] = p;
+                    if (found && posj) posj[e0 + i] = p;
                 } else if (mode == 1) { // NOT: present = rejected
                     alive[i] = !found;
-                } else { // OPTIONAL: remembered where present
-                    posj[start + threadIdx.x * kIIItems + i] = found ? p : 0xFFFFFFFFu;
+                } else if (posj) { // OPTIONAL: remembered where present
+                    posj[e0 + i] = found ? p : 0xFFFFFFFFu;
                 }
             }
         }
@@ -319,10 +319,10 @@ __global__ void __launch_bounds__(kIIThreads) intersect_kernel(const IntersectAr
         for (int i = 0; i < kIIItems; i++) any |= alive[i];
         if (!__syncthreads_or(any)) break; // also fences sB before the next list reuses it
     }
-    // ordered compaction of the survivors
-    uint32_t cnt = 0;
-#pragma unroll
-    for (int i = 0; i < kIIItems; i++) cnt += alive[i];
+}
+
+// ordered compaction of a CTA's survivors: the rank of this thread's first survivor (it holds cnt of them) and the CTA's total
+__device__ __forceinline__ uint32_t cta_survivor_rank(uint32_t cnt, uint32_t *s_warp, uint32_t &total) {
     uint32_t incl = cnt;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
@@ -332,15 +332,40 @@ __global__ void __launch_bounds__(kIIThreads) intersect_kernel(const IntersectAr
     }
     if (lane == 31) s_warp[warp] = incl;
     __syncthreads();
-    uint32_t warp_base = 0, total = 0;
+    uint32_t warp_base = 0;
+    total = 0;
     for (int w = 0; w < kIIThreads / 32; w++) {
         if (w < warp) warp_base += s_warp[w];
         total += s_warp[w];
     }
-    uint32_t rank = warp_base + incl - cnt;
+    return warp_base + incl - cnt;
+}
+
+__global__ void __launch_bounds__(kIIThreads) intersect_kernel(const IntersectArgs a) {
+    __shared__ uint32_t sB[kIISmemElems];
+    __shared__ uint32_t s_lo, s_hi;
+    __shared__ uint32_t s_warp[kIIThreads / 32];
+    const uint32_t chunk = blockIdx.x;
+    const uint32_t start = chunk * kIIChunk;
+    const uint32_t end = min(start + (uint32_t)kIIChunk, a.len[0]);
+    const uint32_t *A = a.ids[0];
+    const uint32_t e0 = start + threadIdx.x * kIIItems; // blocked: a thread owns consecutive entries
+    uint32_t doc[kIIItems];
+    bool alive[kIIItems];
+#pragma unroll
+    for (int i = 0; i < kIIItems; i++) {
+        alive[i] = e0 + i < end;
+        doc[i] = alive[i] ? A[e0 + i] : 0xFFFFFFFFu;
+    }
+    and_probe(doc, alive, e0, A[start], A[end - 1], a.n,
+              [&](uint32_t j) { return ProbeList{a.ids[j], a.len[j], a.mode[j], a.tmp_pos + (size_t)j * a.stride}; }, sB, s_lo, s_hi);
+    uint32_t cnt = 0, total;
+#pragma unroll
+    for (int i = 0; i < kIIItems; i++) cnt += alive[i];
+    uint32_t rank = cta_survivor_rank(cnt, s_warp, total);
 #pragma unroll
     for (int i = 0; i < kIIItems; i++)
-        if (alive[i]) a.tmp_idx[start + rank++] = start + threadIdx.x * kIIItems + i;
+        if (alive[i]) a.tmp_idx[start + rank++] = e0 + i;
     if (threadIdx.x == 0) a.counts[chunk] = total;
 }
 
@@ -643,12 +668,14 @@ __global__ void fill_freq_kernel(const uint32_t *__restrict__ ids, const uint32_
 // ------------------------------------------------------------------------------------------------
 // a batch of unions / numeric range filters: the kernels above, ragged over every list of every query (ii_kernels.h: UBList)
 // ------------------------------------------------------------------------------------------------
-// the list that owns chunk b: the last one whose first chunk is <= b (empty lists own no chunk and are not in the table)
-__device__ __forceinline__ uint32_t ub_list_of(const UBList *__restrict__ lists, uint32_t nlists, uint32_t b) {
-    uint32_t lo = 0, hi = nlists; // answer in [lo, hi)
+// the table entry (a list here, a query of II_IntersectFilterBatchDevice) that owns chunk b: the last one whose first chunk is
+// <= b (entries that own no chunk, such as empty lists, are not in the table)
+template <typename T>
+__device__ __forceinline__ uint32_t chunk_owner(const T *__restrict__ tab, uint32_t n, uint32_t b) {
+    uint32_t lo = 0, hi = n; // answer in [lo, hi)
     while (hi - lo > 1) {
         const uint32_t mid = (lo + hi) >> 1;
-        if (lists[mid].chunk0 <= b) lo = mid;
+        if (tab[mid].chunk0 <= b) lo = mid;
         else hi = mid;
     }
     return lo;
@@ -666,7 +693,7 @@ __global__ void __launch_bounds__(256) ub_mark_kernel(const UBList *__restrict__
                                                       uint32_t *__restrict__ bitmap, uint32_t *__restrict__ est) {
     __shared__ uint32_t s_l, s_kept;
     if (threadIdx.x == 0) {
-        s_l = ub_list_of(lists, nlists, blockIdx.x);
+        s_l = chunk_owner(lists, nlists, blockIdx.x);
         s_kept = 0;
     }
     __syncthreads();
@@ -700,21 +727,18 @@ __global__ void ub_popc_kernel(const uint32_t *__restrict__ bitmap, uint64_t tot
 // one CTA per query: exclusive scan of its blocks' counts, the count into len[0] (and len[1] for numeric filters), and the
 // set's epoch table out of the batch table
 constexpr int kUBScanThreads = 1024, kUBScanItems = 8;
-__global__ void __launch_bounds__(kUBScanThreads) ub_scan_kernel(const UBQuery *__restrict__ qs, const uint32_t *__restrict__ blocksum,
-                                                                 uint32_t *__restrict__ blockoff, const uint32_t *__restrict__ est) {
-    __shared__ uint32_t s_warp[32], s_carry;
-    const UBQuery &q = qs[blockIdx.x];
+// exclusive scan of in[0, n) into out by one CTA of kUBScanThreads threads; returns the total to every thread
+__device__ uint32_t cta_exclusive_scan(const uint32_t *__restrict__ in, uint32_t *__restrict__ out, uint32_t n, uint32_t *s_warp,
+                                       uint32_t &s_carry) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (threadIdx.x == 0) s_carry = 0;
     __syncthreads();
-    const uint32_t *in = blocksum + q.blk0;
-    uint32_t *out = blockoff + q.blk0;
-    for (uint32_t t0 = 0; t0 < q.nblk; t0 += kUBScanThreads * kUBScanItems) {
+    for (uint32_t t0 = 0; t0 < n; t0 += kUBScanThreads * kUBScanItems) {
         const uint32_t i0 = t0 + threadIdx.x * kUBScanItems;
         uint32_t v[kUBScanItems], sum = 0;
 #pragma unroll
         for (int k = 0; k < kUBScanItems; k++) {
-            v[k] = i0 + k < q.nblk ? in[i0 + k] : 0;
+            v[k] = i0 + k < n ? in[i0 + k] : 0;
             sum += v[k];
         }
         uint32_t incl = sum;
@@ -738,15 +762,22 @@ __global__ void __launch_bounds__(kUBScanThreads) ub_scan_kernel(const UBQuery *
         uint32_t o = s_carry + s_warp[warp] + incl - sum;
 #pragma unroll
         for (int k = 0; k < kUBScanItems; k++) {
-            if (i0 + k < q.nblk) out[i0 + k] = o;
+            if (i0 + k < n) out[i0 + k] = o;
             o += v[k];
         }
         __syncthreads(); // every thread has read s_carry and s_warp
         if (threadIdx.x == kUBScanThreads - 1) s_carry = o;
         __syncthreads();
     }
+    return s_carry;
+}
+__global__ void __launch_bounds__(kUBScanThreads) ub_scan_kernel(const UBQuery *__restrict__ qs, const uint32_t *__restrict__ blocksum,
+                                                                 uint32_t *__restrict__ blockoff, const uint32_t *__restrict__ est) {
+    __shared__ uint32_t s_warp[32], s_carry;
+    const UBQuery &q = qs[blockIdx.x];
+    const uint32_t total = cta_exclusive_scan(blocksum + q.blk0, blockoff + q.blk0, q.nblk, s_warp, s_carry);
     if (threadIdx.x == 0) {
-        q.len[0] = s_carry;
+        q.len[0] = total;
         q.len[1] = est[blockIdx.x];
     }
     if (q.order) {
@@ -808,7 +839,7 @@ __global__ void ub_clear_kernel(const UBQuery *__restrict__ qs, uint32_t nq) {
 __global__ void __launch_bounds__(256) ub_fill_kernel(const UBList *__restrict__ lists, uint32_t nlists, const UBQuery *__restrict__ qs,
                                                       const uint32_t *__restrict__ bitmap, const uint32_t *__restrict__ wordoff) {
     __shared__ uint32_t s_l;
-    if (threadIdx.x == 0) s_l = ub_list_of(lists, nlists, blockIdx.x);
+    if (threadIdx.x == 0) s_l = chunk_owner(lists, nlists, blockIdx.x);
     __syncthreads();
     const UBList L = lists[s_l];
     const UBQuery &q = qs[L.q];
@@ -821,6 +852,85 @@ __global__ void __launch_bounds__(256) ub_fill_kernel(const UBList *__restrict__
         q.freqs[L.row * q.cap + rank] = L.freqs[i];
         if (q.pos) q.pos[L.row * q.cap + rank] = i;
     }
+}
+
+// ------------------------------------------------------------------------------------------------
+// a batch of filter-mode ANDs over lists and sets (ii_kernels.h: IFBChild): the probe of intersect_kernel, ragged over the
+// driver chunks of every query, with each set child's length read on the device
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t ifb_len(const IFBChild &c) { return c.d_len ? min(*c.d_len, c.len) : c.len; }
+
+__global__ void __launch_bounds__(kIIThreads) ifb_probe_kernel(const IFBChild *__restrict__ children, const IFBQuery *__restrict__ qs,
+                                                               uint32_t nq, uint32_t *__restrict__ surv, uint32_t *__restrict__ counts) {
+    __shared__ uint32_t sB[kIISmemElems];
+    __shared__ uint32_t s_lo, s_hi;
+    __shared__ uint32_t s_warp[kIIThreads / 32];
+    __shared__ uint32_t s_q;
+    if (threadIdx.x == 0) s_q = chunk_owner(qs, nq, blockIdx.x);
+    __syncthreads();
+    const IFBQuery &q = qs[s_q];
+    const IFBChild *ch = children + q.child0;
+    const uint32_t start = (blockIdx.x - q.chunk0) * kIIChunk, n0 = ifb_len(ch[0]);
+    if (start >= n0) { // past the driver's count on the device: no entry, and no read of its docIds
+        if (threadIdx.x == 0) counts[blockIdx.x] = 0;
+        return;
+    }
+    const uint32_t end = min(start + (uint32_t)kIIChunk, n0);
+    const uint32_t *A = ch[0].ids;
+    const uint32_t e0 = start + threadIdx.x * kIIItems;
+    uint32_t doc[kIIItems];
+    bool alive[kIIItems];
+#pragma unroll
+    for (int i = 0; i < kIIItems; i++) {
+        alive[i] = e0 + i < end;
+        doc[i] = alive[i] ? A[e0 + i] : 0xFFFFFFFFu;
+    }
+    and_probe(doc, alive, e0, A[start], A[end - 1], q.n,
+              [&](uint32_t j) { return ProbeList{ch[j].ids, ifb_len(ch[j]), (int)ch[j].mode, nullptr}; }, sB, s_lo, s_hi);
+    uint32_t cnt = 0, total;
+#pragma unroll
+    for (int i = 0; i < kIIItems; i++) cnt += alive[i];
+    uint32_t rank = cta_survivor_rank(cnt, s_warp, total);
+    uint32_t *out = surv + (size_t)blockIdx.x * kIIChunk;
+#pragma unroll
+    for (int i = 0; i < kIIItems; i++)
+        if (alive[i]) out[rank++] = doc[i];
+    if (threadIdx.x == 0) counts[blockIdx.x] = total;
+}
+// one CTA per query: exclusive scan of its chunks' counts, the count into len[0], every child's num_estimated into len[2 + slot]
+// and the smallest required one into len[1]
+__global__ void __launch_bounds__(kUBScanThreads) ifb_scan_kernel(const IFBChild *__restrict__ children, const IFBQuery *__restrict__ qs,
+                                                                  const uint32_t *__restrict__ counts, uint32_t *__restrict__ offsets) {
+    __shared__ uint32_t s_warp[32], s_carry;
+    const IFBQuery &q = qs[blockIdx.x];
+    const uint32_t total = cta_exclusive_scan(counts + q.chunk0, offsets + q.chunk0, q.nchunks, s_warp, s_carry);
+    if (threadIdx.x >= 32) return;
+    const uint32_t lane = threadIdx.x;
+    uint32_t est = 0xFFFFFFFFu;
+    if (lane < q.n) { // n <= kIIMaxLists = 32
+        const IFBChild &c = children[q.child0 + lane];
+        const uint32_t e = c.d_est ? *c.d_est : c.est;
+        q.len[2 + c.slot] = e;
+        if (c.mode == 0) est = e;
+    }
+    est = __reduce_min_sync(0xffffffffu, est);
+    if (lane == 0) {
+        q.len[0] = total;
+        q.len[1] = est;
+    }
+}
+// one CTA per driver chunk: its survivors to their place in the query's docIds
+__global__ void __launch_bounds__(kIIThreads) ifb_expand_kernel(const IFBQuery *__restrict__ qs, uint32_t nq, const uint32_t *__restrict__ surv,
+                                                                const uint32_t *__restrict__ counts, const uint32_t *__restrict__ offsets) {
+    __shared__ uint32_t s_q;
+    const uint32_t m = counts[blockIdx.x];
+    if (!m) return; // the whole CTA
+    if (threadIdx.x == 0) s_q = chunk_owner(qs, nq, blockIdx.x);
+    __syncthreads();
+    const IFBQuery &q = qs[s_q];
+    const uint32_t *src = surv + (size_t)blockIdx.x * kIIChunk;
+    uint32_t *dst = q.docs + offsets[blockIdx.x];
+    for (uint32_t i = threadIdx.x; i < m; i += kIIThreads) dst[i] = src[i];
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1834,6 +1944,14 @@ cudaError_t ii_launch_union_batch(const UBList *d_lists, uint32_t nlists, uint32
         ub_fill_kernel<<<total_chunks, 256, 0, s>>>(d_lists, nlists, d_q, d_bitmap, d_wordoff);
         *launches = 6;
     }
+    return cudaGetLastError();
+}
+cudaError_t ii_launch_filter_and_batch(const IFBChild *d_children, const IFBQuery *d_q, uint32_t nq, uint32_t total_chunks,
+                                       uint32_t *d_surv, uint32_t *d_counts, uint32_t *d_offsets, cudaStream_t s) {
+    if (!nq || !total_chunks) return cudaSuccess;
+    ifb_probe_kernel<<<total_chunks, kIIThreads, 0, s>>>(d_children, d_q, nq, d_surv, d_counts);
+    ifb_scan_kernel<<<nq, kUBScanThreads, 0, s>>>(d_children, d_q, d_counts, d_offsets);
+    ifb_expand_kernel<<<total_chunks, kIIThreads, 0, s>>>(d_q, nq, d_surv, d_counts, d_offsets);
     return cudaGetLastError();
 }
 cudaError_t ii_launch_hamming(const uint32_t *d_docs, const uint32_t *d_len, uint32_t cap_len, const uint8_t *d_payloads,

@@ -152,6 +152,31 @@ cudaError_t ii_launch_union_batch(const UBList *d_lists, uint32_t nlists, uint32
                                   uint64_t total_blocks, uint64_t clear_elems, uint32_t *d_est, uint32_t *d_bitmap, uint32_t *d_blocksum,
                                   uint32_t *d_blockoff, uint32_t *d_wordoff, uint32_t *launches, cudaStream_t s);
 
+// ---- batches of filter-mode ANDs over lists and (pending) sets (II_IntersectFilterBatchDevice) ----------------------------
+// A child is a posting list (exact length) or a set whose count is read on the device.  Each query's children sit in the child
+// table in probe order: the driver first, then the others by ascending host bound.
+struct IFBChild {
+    const uint32_t *ids;
+    const uint32_t *d_len; // a set: its count on the device, read as min(*d_len, len) (NULL: a list, len is exact)
+    const uint32_t *d_est; // a set whose num_estimated is still on the device (NULL: `est` holds it)
+    uint32_t len;          // a list: its length; a set: its capacity
+    uint32_t est;          // num_estimated, saturated at 2^32 - 1
+    uint32_t slot;         // the child's index in the order the caller gave (its estimate lands in len[2 + slot])
+    uint32_t mode;         // 0 required, 1 NOT (an empty NOT child: len 0, ids NULL)
+};
+struct IFBQuery {
+    uint32_t *docs;   // the set's docIds [cap]
+    uint32_t *len;    // [0] the count, [1] num_estimated (the smallest required child's), [2 + i] child i's num_estimated
+    uint32_t child0;  // first entry of the query in the child table: the driver
+    uint32_t n;       // children
+    uint32_t chunk0;  // first kIIChunk chunk of the driver in the batch
+    uint32_t nchunks; // chunks of the driver (by its host bound)
+};
+// 3 launches whatever the batch: probe (one CTA per driver chunk, survivors compacted into d_surv[chunk * kIIChunk ...] and
+// counted into d_counts), scan (one CTA per query: offsets, count, estimates), expand (one CTA per chunk: survivors to docs).
+cudaError_t ii_launch_filter_and_batch(const IFBChild *d_children, const IFBQuery *d_q, uint32_t nq, uint32_t total_chunks,
+                                       uint32_t *d_surv, uint32_t *d_counts, uint32_t *d_offsets, cudaStream_t s);
+
 struct ScoreArgs {
     int scorer; // II_Scorer numbering
     int is_union;

@@ -28,6 +28,10 @@ class II_NumericRange(C.Structure):
     _fields_ = [("min", C.c_double), ("max", C.c_double), ("min_inclusive", C.c_int), ("max_inclusive", C.c_int)]
 
 
+class II_FilterChild(C.Structure):
+    _fields_ = [("list", C.c_void_p), ("set", C.c_void_p), ("mode", C.c_int)]
+
+
 class II_Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("intersect_device_us", C.c_double), ("score_device_us", C.c_double),
                 ("decode_host_us", C.c_double), ("h2d_us", C.c_double)]
@@ -105,6 +109,7 @@ SIGNATURES = [
     ("II_ResultSet_FreeAfter", None, [_P, _P]),
     ("II_UnionBatchDevice", C.c_int, [_SZ, _P, _P, C.c_int, _P, _P, C.POINTER(_SZ)]),
     ("II_NumericFilterBatchDevice", C.c_int, [_SZ, _P, _P, _P, _P, _P, C.POINTER(_SZ)]),
+    ("II_IntersectFilterBatchDevice", C.c_int, [_SZ, _P, _P, _P, _P, C.POINTER(_SZ)]),
     ("II_IndexWriter_New", _P, [C.c_int]),
     ("II_IndexWriter_NewNumeric", _P, [C.c_int]),
     ("II_IndexWriter_Add", _SZ, [_P, C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint64, _P, C.c_uint32]),
@@ -460,6 +465,30 @@ def numeric_filter_batch_device(batch, stream=None):
     ranges = (II_NumericRange * max(1, nq))(*[II_NumericRange(float(lo), float(hi), int(li), int(hi_)) for _, lo, hi, li, hi_ in batch])
     out = (C.c_void_p * max(1, nq))()
     rc = lib().II_NumericFilterBatchDevice(nq, pp, counts, ranges, _stream_handle(stream), out, None)
+    return _pending_sets(rc, out, nq)
+
+
+def intersect_filter_batch_device(batch, stream=None):
+    """II_IntersectFilterBatchDevice: batch[q] = [(child, mode)] of query q's filter-mode AND, child = a PostingList, a ResultSet
+    (pending or settled, e.g. from union_batch_device) or None (an empty child), mode 0 = required, 1 = NOT.  The children are
+    borrowed.  Returns as union_batch_device; raises ValueError when the batch is refused or a child is closed or consumed (only
+    None stands for an empty child)."""
+    nq = len(batch)
+    arrays = []
+    for items in batch:
+        a = (II_FilterChild * max(1, len(items)))()
+        for i, (child, mode) in enumerate(items):
+            if child is None:
+                a[i] = II_FilterChild(None, None, mode)
+                continue
+            if not isinstance(child, (PostingList, ResultSet)) or not child.h:
+                raise ValueError(f"child {i} is neither None nor a live PostingList / ResultSet")
+            a[i] = II_FilterChild(child.h, None, mode) if isinstance(child, PostingList) else II_FilterChild(None, child.h, mode)
+        arrays.append(a)
+    pp = (C.c_void_p * max(1, nq))(*[C.cast(a, C.c_void_p) for a in arrays])
+    counts = (C.c_size_t * max(1, nq))(*[len(items) for items in batch])
+    out = (C.c_void_p * max(1, nq))()
+    rc = lib().II_IntersectFilterBatchDevice(nq, pp, counts, _stream_handle(stream), out, None)
     return _pending_sets(rc, out, nq)
 
 
