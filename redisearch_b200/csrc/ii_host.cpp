@@ -2411,16 +2411,25 @@ bool fused_batch(Ctx &c, FusedScratch &fs, const std::vector<size_t> &idx, II_Po
                  II_Scorer scorer, const II_TermParams *const *terms, double agg_weight, const II_IndexStats *stats, const II_DocTable *docs,
                  size_t top_n, uint64_t *doc_ids, double *scores, size_t *counts, size_t *total_hits) {
     constexpr size_t kMaxCand = (size_t)96 << 20; // candidate slots per launch (x 12 B): larger batches are cut into several launches
+    // aggregate child order of every query: stable sort ascending by num_estimated (intersection.rs:110-145).  The kernel drives
+    // with child 0 of that order and scores the children in it, so the driver is not always the list with the fewest entries (a
+    // field-mask filter keeps the unfiltered estimate, II_PostingList_FromBlocks): the scratch, the item count and the
+    // candidate budget all come from the driver's length.
+    std::vector<uint32_t> orders(idx.size() * kFusedMaxLists);
+    std::vector<uint32_t> drive_chunks(idx.size());
+    for (size_t k = 0; k < idx.size(); k++) {
+        const size_t qi = idx[k];
+        uint32_t *order = &orders[k * kFusedMaxLists];
+        for (size_t t = 0; t < n_lists[qi]; t++) order[t] = (uint32_t)t;
+        std::stable_sort(order, order + n_lists[qi], [&](uint32_t a, uint32_t b) { return lists[qi][a]->estimated < lists[qi][b]->estimated; });
+        drive_chunks[k] = (uint32_t)((lists[qi][order[0]]->n + kIIChunk - 1) / kIIChunk);
+    }
     size_t done = 0;
     while (done < idx.size()) {
         // sub-batch [done, stop): as many queries as fit the candidate budget
         size_t stop = done, items = 0;
-        std::vector<uint32_t> order;
         while (stop < idx.size()) {
-            const size_t qi = idx[stop];
-            size_t shortest = SIZE_MAX;
-            for (size_t t = 0; t < n_lists[qi]; t++) shortest = std::min(shortest, lists[qi][t]->n);
-            const size_t ch = (shortest + kIIChunk - 1) / kIIChunk;
+            const size_t ch = drive_chunks[stop];
             if (stop > done && (items + ch) * top_n > kMaxCand) break;
             items += ch;
             stop++;
@@ -2431,13 +2440,9 @@ bool fused_batch(Ctx &c, FusedScratch &fs, const std::vector<size_t> &idx, II_Po
         for (size_t k = 0; k < m; k++) {
             const size_t qi = idx[done + k];
             const size_t n = n_lists[qi];
+            const uint32_t *order = &orders[(done + k) * kFusedMaxLists];
             FusedQuery &fq = fs.h_q[k];
             memset(&fq, 0, sizeof(fq));
-            // aggregate child order: stable sort ascending by num_estimated (intersection.rs:110-145); the kernel drives with
-            // child 0, so put the list with the fewest ACTUAL entries first only when the estimates tie the order anyway
-            order.resize(n);
-            for (size_t t = 0; t < n; t++) order[t] = (uint32_t)t;
-            std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return lists[qi][a]->estimated < lists[qi][b]->estimated; });
             for (size_t t = 0; t < n; t++) {
                 const II_PostingList *pl = lists[qi][order[t]];
                 fq.ids[t] = pl->d_ids;
@@ -2450,9 +2455,12 @@ bool fused_batch(Ctx &c, FusedScratch &fs, const std::vector<size_t> &idx, II_Po
             fq.n = (uint32_t)n;
             max_children = std::max(max_children, fq.n);
             fq.item0 = item0;
-            fq.nchunks = (uint32_t)((fq.len[0] + kIIChunk - 1) / kIIChunk);
+            fq.nchunks = drive_chunks[done + k];
             item0 += fq.nchunks;
         }
+        // the kernels write item0 work items and item0 * top_n candidate slots.  item0 equals the `items` the scratch was sized
+        // for just above; this is a backstop should the two sums ever diverge, not a path taken today
+        if (item0 > fs.item_cap || (size_t)item0 * top_n > fs.cand_cap) return false;
         FusedCommon fc{};
         fc.scorer = (int)scorer;
         fc.agg_weight = agg_weight;

@@ -206,7 +206,8 @@ struct ScoreArgs {
 constexpr int kFusedMaxLists = 8;   // more children: the per-query kernel chain
 constexpr int kFusedMaxTopN = 128;
 // One query of the batch.  Children are in the reference's aggregate order (ascending num_estimated, stable:
-// RS/rqe_iterators/src/intersection.rs:110-145), which for the fused path is also ascending ACTUAL length, so child 0 drives.
+// RS/rqe_iterators/src/intersection.rs:110-145), and child 0 drives.  A field-mask-filtered child keeps its unfiltered
+// estimate, so child 0 is not always the shortest list: the host sizes the batch from child 0 (fused_batch).
 struct FusedQuery {
     const uint32_t *ids[kFusedMaxLists];
     const uint32_t *freqs[kFusedMaxLists];
