@@ -293,6 +293,28 @@ typedef struct {
  * other than 0 or 1, a child with both `list` and `set`.  *built (may be NULL) = the sets created. */
 int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *children, const size_t *n_children, void *stream,
                                   II_ResultSet **out, size_t *built);
+/* nq ORs of lists and sets in FILTER MODE with no host wait — `(@brand:nike @color:red) | (@brand:adidas @color:blue)`,
+ * `@price:[0 50] | @price:[500 +inf]`, `(@category:{shoes} @price:[50 200]) | @brand:nike` ahead of a KNN — without settling the
+ * ANDs and ranges first.  out[q] = the ascending docIds and count of the OR of children[q][0 .. n_children[q]), each set counting
+ * as the docIds it holds once settled: what II_Union(quick_exit = 1) gives over the same lists plus II_PostingList_FromDevice of
+ * each set's docIds.  out[q] is NULL when every child is empty on the host (a list of length 0, a set of capacity 0, both NULL).
+ * Filter mode as for II_IntersectFilterBatchDevice: docIds, count, num_estimated and the child order, no per-child freq rows;
+ * II_Score returns -1 and II_ResultSet_IntoChild NULL, as for quick unions.  Its shape is the one II_Union gives a quick union:
+ * n_children = n_children[q]; the child order is the identity; child tags: a list keeps its own, an OR or numeric set is 1, an
+ * AND set 2, an empty child 4; num_estimated = the sum of the children's (a set counting with its own); capacity = min(the sum of
+ * the children's host bounds (a list's length, a set's II_ResultSet_Capacity), the highest docId the children can hold + 1).
+ * Where a child's estimate is still on the device (a pending numeric set, or a pending filter-mode set that has one) the sum is
+ * formed there and worked out when the set settles.  DeviceLen[1] holds num_estimated, saturated at 2^32 - 1.
+ * II_ResultSet_DeviceDocIds / DeviceLen / Capacity are valid in `stream` order.  An output is a valid set child of a later call
+ * of this function or of II_IntersectFilterBatchDevice, and a valid KNN filter (VecSimB200_TopKFilteredBatchDevice).
+ * No host wait, and the inputs are borrowed, as for II_IntersectFilterBatchDevice.  4 launches per batch (plus one clear and one
+ * upload), whatever nq and the number of children.  Every set carries host-known bounds on its docIds, which size the bitmap
+ * window of each query.
+ * Returns 0, or -1 before anything is enqueued: NULL arguments, a query with more than 1024 children, a mode other than 0 (no
+ * NOT under an OR), a child with both `list` and `set`, a list carrying a nested set (II_ResultSet_IntoChild).  *built (may be
+ * NULL) = the sets created. */
+int II_UnionFilterBatchDevice(size_t nq, const II_FilterChild *const *children, const size_t *n_children, void *stream,
+                              II_ResultSet **out, size_t *built);
 
 /* ---- scoring ------------------------------------------------------------------------------------ */
 typedef enum {

@@ -238,6 +238,9 @@ struct II_ResultSet {
     std::vector<std::shared_ptr<struct NestedSet>> nested;
     std::vector<uint8_t> child_tag; // RSResultData tag per child (aggregate order)
     size_t estimated = 0;           // num_estimated by the reference's rule: min over the children (AND), their sum (OR)
+    // host-known bounds on the docIds the set can hold (lo_id > hi_id: none), filled by every constructor without a device read;
+    // they bound the bitmap window of an OR over sets (II_UnionFilterBatchDevice)
+    uint32_t lo_id = 0, hi_id = 0xFFFFFFFFu;
     std::unique_ptr<UnionOrder> h_order; // host copy of d_order (EXPLAINSCORE walks one hit's children in aggregate order)
     // II_IntersectBatchDevice: the hit count is known only on the device until settle(); `ready` completes with the AND's kernels
     bool pending = false;
@@ -992,7 +995,11 @@ bool intersect_enqueue(Ctx &c, II_PostingList *const *lists, size_t n, II_Result
     for (size_t j = 0; j < n; j++) {
         const II_PostingList *L = lists[order[j]];
         rs->child_tag[j] = mode_of(order[j]) == 1 ? 8 : L->result_tag;
-        if (mode_of(order[j]) == 0) rs->estimated = std::min(rs->estimated, L->estimated); // NOT / OPTIONAL estimate max_doc_id
+        if (mode_of(order[j]) == 0) {
+            rs->estimated = std::min(rs->estimated, L->estimated); // NOT / OPTIONAL estimate max_doc_id
+            rs->lo_id = std::max(rs->lo_id, L->first_id);          // every hit is in each required list
+            rs->hi_id = std::min(rs->hi_id, L->last_id);
+        }
         if (L->nested && mode_of(order[j]) != 1) {
             rs->nested[j] = L->nested;
             any_nested = true;
@@ -1250,8 +1257,12 @@ UnionPlan union_plan(II_PostingList *const *lists, size_t n, int quick_exit, II_
     rs->nested.assign(n, nullptr);
     rs->child_tag.assign(n, 4);
     rs->estimated = 0;
+    rs->lo_id = 0xFFFFFFFFu;
     for (size_t i = 0; i < n; i++) {
-        if (lists[i]->n) p.max_id = std::max(p.max_id, lists[i]->last_id);
+        if (lists[i]->n) {
+            p.max_id = std::max(p.max_id, lists[i]->last_id);
+            rs->lo_id = std::min(rs->lo_id, lists[i]->first_id);
+        }
         p.total_in += lists[i]->n;
         rs->estimated += lists[i]->estimated; // union_flat.rs:102
         rs->child_tag[i] = lists[i]->result_tag;
@@ -1260,6 +1271,7 @@ UnionPlan union_plan(II_PostingList *const *lists, size_t n, int quick_exit, II_
             p.any_nested = true;
         }
     }
+    rs->hi_id = p.max_id; // every hit is in a non-empty child (no child at all: lo_id > hi_id)
     rs->cap = std::min<size_t>(p.total_in, (size_t)p.max_id + 1);
     // the reference's aggregate child order (UnionFlat, full mode, read front to back): children live in an "active" array,
     // an exhausted child is swap-removed by the pass that follows the document it ended on (advance_and_find_min,
@@ -1734,24 +1746,111 @@ II_ResultSet *II_Union(II_PostingList *const *lists, size_t n, int quick_exit) {
 }
 
 namespace {
-// A batch of ORs (lists) or of numeric range filters (leaves + ranges) with no host wait.  Every set's memory comes from the pool
-// in c.stream order; the tables the kernels read go up in one copy from a pinned slot; ii_launch_union_batch runs the same 4 or
-// 6 launches for any batch; an event per set marks it pending and `stream` waits for the last one.
-int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_NumericList *const *const *leaves, const size_t *counts,
-                        int quick_exit, const II_NumericRange *ranges, void *stream, II_ResultSet **out, size_t *built) {
-    const bool numeric = leaves != nullptr, full = !numeric && !quick_exit;
+// A batch call that reads child sets: c.stream waits for each one's own kernels once (a settled or host-built set: at once).
+// inputs is sorted and made unique.
+bool wait_for_inputs(Ctx &c, std::vector<II_ResultSet *> &inputs) {
+    std::sort(inputs.begin(), inputs.end());
+    inputs.erase(std::unique(inputs.begin(), inputs.end()), inputs.end());
+    bool ok = true;
+    for (II_ResultSet *s : inputs)
+        if (s->ready) ok = ok && cudaStreamWaitEvent(c.stream, s->ready, 0) == cudaSuccess;
+    return ok;
+}
+// every input keeps the call's completion event (recorded now on c.stream): its memory is not handed out again while the call's
+// kernels may still read it, whichever thread frees it
+bool borrow_inputs(Ctx &c, const std::vector<II_ResultSet *> &inputs) {
+    auto done = std::make_shared<SharedEvent>();
+    if (cudaEventCreateWithFlags(&done->ev, cudaEventDisableTiming) != cudaSuccess || cudaEventRecord(done->ev, c.stream) != cudaSuccess) {
+        cudaStreamSynchronize(c.stream);
+        return false;
+    }
+    std::lock_guard<std::mutex> rg(readers_mu());
+    for (II_ResultSet *s : inputs) {
+        auto &r = s->readers;
+        r.erase(std::remove_if(r.begin(), r.end(), [](const std::shared_ptr<SharedEvent> &e) { return cudaEventQuery(e->ev) == cudaSuccess; }),
+                r.end());
+        r.push_back(done);
+    }
+    cudaGetLastError(); // cudaErrorNotReady of a reader still running is no failure
+    return true;
+}
+
+// The shape II_Union(quick) gives a filter-mode OR of n children: docIds only, identity child order, every child tagged `tag`
+void filter_union_shape(II_ResultSet *rs, size_t n, uint8_t tag) {
+    rs->is_union = true;
+    rs->n_children = (uint32_t)n;
+    rs->has_freqs = false;
+    rs->child_order.resize(n);
+    for (size_t i = 0; i < n; i++) rs->child_order[i] = (uint32_t)i;
+    rs->child_off.assign(n, II_ResultSet::ChildOffsets());
+    rs->nested.assign(n, nullptr);
+    rs->child_tag.assign(n, tag);
+}
+
+// One child of a batch OR as the kernels see it: a posting list, a numeric leaf or a set.  len: the exact length of a list or a
+// leaf, a set's capacity (its count is read on the device, d_len); [lo, hi]: host-known bounds on its docIds.
+struct OrChild {
+    const uint32_t *ids = nullptr, *freqs = nullptr, *d_len = nullptr, *d_est = nullptr;
+    const double *values = nullptr;
+    size_t len = 0;
+    uint32_t lo = 0, hi = 0;
+};
+
+// A batch of ORs with no host wait, over one of three kinds of children: posting lists (II_UnionBatchDevice), numeric leaves
+// filtered by a range (II_NumericFilterBatchDevice), or filter children, lists and sets (II_UnionFilterBatchDevice).  Every set's
+// memory comes from the pool in c.stream order; the tables the kernels read go up in one copy from a pinned slot;
+// ii_launch_union_batch runs the same 4 or 6 launches for any batch; an event per set marks it pending and `stream` waits for the
+// last one.  Child sets are borrowed as in II_IntersectFilterBatchDevice.
+int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_NumericList *const *const *leaves,
+                        const II_FilterChild *const *children, const size_t *counts, int quick_exit, const II_NumericRange *ranges,
+                        void *stream, II_ResultSet **out, size_t *built) {
+    const bool numeric = leaves != nullptr, sets = children != nullptr, full = !numeric && !sets && !quick_exit;
+    const void *const *tab = numeric ? (const void *const *)leaves : sets ? (const void *const *)children : (const void *const *)lists;
     if (built) *built = 0;
-    if (nq && (!out || !counts || !(numeric ? (const void *)leaves : (const void *)lists))) return -1;
+    if (nq && (!out || !counts || !tab)) return -1;
     for (size_t q = 0; q < nq; q++) out[q] = nullptr;
     for (size_t q = 0; q < nq; q++) { // refused before anything is enqueued
-        if (counts[q] > (size_t)kIIMaxUnionLists || (counts[q] && !(numeric ? (const void *)leaves[q] : (const void *)lists[q]))) return -1;
+        if (counts[q] > (size_t)kIIMaxUnionLists || (counts[q] && !tab[q])) return -1;
         if (numeric && !ranges) return -1;
-        for (size_t i = 0; i < counts[q]; i++)
-            if (numeric ? !leaves[q][i] : (!lists[q][i] || lists[q][i]->nested)) return -1;
+        for (size_t i = 0; i < counts[q]; i++) {
+            if (sets) {
+                const II_FilterChild &ch = children[q][i];
+                if (ch.mode != 0 || (ch.list && ch.set)) return -1;
+            } else if (numeric ? !leaves[q][i] : (!lists[q][i] || lists[q][i]->nested)) {
+                return -1;
+            }
+        }
     }
-    Ctx &c = ctx();
-    std::lock_guard<std::mutex> g(c.mu);
-    if (!c.init()) return -1;
+    for (size_t q = 0; sets && q < nq; q++) // the children are read only once every argument passed the checks above
+        for (size_t i = 0; i < counts[q]; i++)
+            if (children[q][i].list && children[q][i].list->nested) return -1;
+    const auto child = [&](size_t q, size_t i) {
+        OrChild e;
+        const II_PostingList *pl = sets ? children[q][i].list : numeric ? nullptr : lists[q][i];
+        const II_ResultSet *s = sets ? children[q][i].set : nullptr;
+        if (numeric) {
+            const II_NumericList *nl = leaves[q][i];
+            e.ids = nl->d_ids;
+            e.values = nl->d_values;
+            e.len = nl->n;
+            e.lo = nl->first_id;
+            e.hi = nl->last_id;
+        } else if (pl) {
+            e.ids = pl->d_ids;
+            e.freqs = full ? pl->d_freqs : nullptr;
+            e.len = pl->n;
+            e.lo = pl->first_id;
+            e.hi = pl->last_id;
+        } else if (s && s->cap) { // a set built empty may have no device count
+            e.ids = s->d_docs;
+            e.d_len = s->d_len;
+            e.d_est = s->pending && s->estimated_on_device ? s->d_len + 1 : nullptr;
+            e.len = s->cap;
+            e.lo = s->lo_id;
+            e.hi = s->hi_id;
+        }
+        return e;
+    };
     struct Plan {
         size_t q;
         std::unique_ptr<II_ResultSet> rs;
@@ -1759,37 +1858,52 @@ int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_Numer
         uint64_t blk0;
         bool keep_pos;
         UnionOrder uo;
+        uint64_t est_host; // sets: the sum of the estimates known on the host, saturated
+        uint32_t n_est_dev;
     };
     std::vector<Plan> plans;
+    std::vector<II_ResultSet *> inputs; // every child set, once
     uint64_t total_blocks = 0, total_chunks = 0, clear_elems = 0;
-    size_t nlists = 0, n_orders = 0;
+    size_t nlists = 0, n_orders = 0, n_est_dev = 0;
     for (size_t q = 0; q < nq; q++) {
         const size_t n = counts[q];
         if (!n) continue;
-        Plan p{q, std::unique_ptr<II_ResultSet>(new II_ResultSet()), 0, 0, 0, 0, false, UnionOrder{}};
+        Plan p{q, std::unique_ptr<II_ResultSet>(new II_ResultSet()), 0, 0, 0, 0, false, UnionOrder{}, 0, 0};
         II_ResultSet *rs = p.rs.get();
-        uint32_t lo = 0xFFFFFFFFu, hi = 0;
+        uint32_t lo = 0xFFFFFFFFu, hi = 0; // the window: over the children that can hold a docId
         size_t total_in = 0;
         for (size_t i = 0; i < n; i++) {
-            const size_t len = numeric ? leaves[q][i]->n : lists[q][i]->n;
-            if (!len) continue;
-            lo = std::min(lo, numeric ? leaves[q][i]->first_id : lists[q][i]->first_id);
-            hi = std::max(hi, numeric ? leaves[q][i]->last_id : lists[q][i]->last_id);
-            total_in += len;
-            total_chunks += (len + kUBChunk - 1) / kUBChunk;
+            const OrChild e = child(q, i);
+            if (!e.len) continue;
+            if (e.len > 0xFFFFFFFFu) return -1; // not representable in the 32-bit tables
+            if (e.lo <= e.hi) {
+                lo = std::min(lo, e.lo);
+                hi = std::max(hi, e.hi);
+            }
+            total_in += e.len;
+            total_chunks += (e.len + kUBChunk - 1) / kUBChunk;
             nlists++;
         }
         if (numeric) { // the shape of II_Union(quick) over II_NumericList_Filter of every leaf
-            rs->is_union = true;
-            rs->n_children = (uint32_t)n;
-            rs->has_freqs = false;
-            rs->child_order.resize(n);
-            for (size_t i = 0; i < n; i++) rs->child_order[i] = (uint32_t)i;
-            rs->child_off.assign(n, II_ResultSet::ChildOffsets());
-            rs->nested.assign(n, nullptr);
-            rs->child_tag.assign(n, 16);
+            filter_union_shape(rs, n, 16);
             rs->cap = std::min<size_t>(total_in, (size_t)hi + 1);
             rs->estimated_on_device = true;
+        } else if (sets) { // the shape union_plan gives a quick union over the lists plus a list view of each set
+            filter_union_shape(rs, n, 4);
+            size_t est = 0;
+            for (size_t i = 0; i < n; i++) {
+                const II_FilterChild &ch = children[q][i];
+                if (ch.set) inputs.push_back(const_cast<II_ResultSet *>(ch.set)); // borrowed: only its reader events change
+                if (ch.list) rs->child_tag[i] = ch.list->result_tag;
+                if (ch.set) rs->child_tag[i] = ch.set->is_union ? 1 : 2; // an OR or a numeric set 1, an AND 2 (IntoChild's tags)
+                if (child(q, i).d_est) p.n_est_dev++;
+                else est += ch.list ? ch.list->estimated : ch.set ? ch.set->estimated : 0; // union_flat.rs:102
+            }
+            rs->estimated = est;
+            rs->estimated_on_device = p.n_est_dev != 0; // the sum waits for the device: settle() reads it from d_len[1]
+            p.est_host = std::min<uint64_t>(est, 0xFFFFFFFFu);
+            n_est_dev += p.n_est_dev;
+            rs->cap = std::min<size_t>(total_in, (size_t)hi + 1);
         } else {
             const UnionPlan up = union_plan(lists[q], n, quick_exit, rs);
             p.keep_pos = up.keep_pos;
@@ -1799,7 +1913,10 @@ int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_Numer
                 n_orders++;
             }
         }
+        rs->lo_id = lo;
+        rs->hi_id = hi;
         if (!total_in) continue; // nothing can match: no set
+        if (lo > hi) lo = hi = 0; // no child can hold a docId (an AND whose bounds exclude each other): a one-block window
         p.lo_word = lo / 32;
         p.nwords = hi / 32 - p.lo_word + 1;
         p.nblk = (p.nwords + 31) / 32;
@@ -1810,6 +1927,9 @@ int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_Numer
     }
     if (plans.empty()) return 0;
     if (total_chunks > 0x7FFFFFFFull || plans.size() > 0xFFFFFFFFull) return -1;
+    Ctx &c = ctx();
+    std::lock_guard<std::mutex> g(c.mu);
+    if (!c.init()) return -1;
     // per-set memory, then the batch's tables and bitmap scratch (freed below in stream order)
     bool ok = true;
     for (Plan &p : plans) {
@@ -1826,7 +1946,8 @@ int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_Numer
     const size_t nb = plans.size();
     const auto align16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
     const size_t off_q = align16(nlists * sizeof(UBList)), off_o = off_q + align16(nb * sizeof(UBQuery));
-    const size_t tab_bytes = off_o + n_orders * sizeof(UnionOrder);
+    const size_t off_e = align16(off_o + n_orders * sizeof(UnionOrder));
+    const size_t tab_bytes = n_est_dev ? off_e + n_est_dev * sizeof(const uint32_t *) : off_o + n_orders * sizeof(UnionOrder);
     const size_t est_words = (nb + 31) & ~(size_t)31;
     const uint64_t total_words = total_blocks * 32;
     uint8_t *d_tab = ok ? dalloc<uint8_t>(tab_bytes) : nullptr;
@@ -1838,8 +1959,10 @@ int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_Numer
         auto *h_lists = reinterpret_cast<UBList *>(slot->h);
         auto *h_q = reinterpret_cast<UBQuery *>(slot->h + off_q);
         auto *h_o = reinterpret_cast<UnionOrder *>(slot->h + off_o);
+        auto *h_e = reinterpret_cast<const uint32_t **>(slot->h + off_e);
         const auto *d_o = reinterpret_cast<const UnionOrder *>(d_tab + off_o);
-        uint32_t li = 0, chunk = 0, oi = 0;
+        const auto *d_e = reinterpret_cast<const uint32_t *const *>(d_tab + off_e);
+        uint32_t li = 0, chunk = 0, oi = 0, ei = 0;
         for (size_t b = 0; b < nb; b++) {
             const Plan &p = plans[b];
             II_ResultSet *rs = p.rs.get();
@@ -1868,29 +1991,31 @@ int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_Numer
                 Q.mni = r.min_inclusive != 0;
                 Q.mxi = r.max_inclusive != 0;
             }
+            if (sets) {
+                Q.sum_est = 1;
+                Q.est_host = p.est_host;
+                Q.est_dev = d_e + ei;
+                Q.n_est_dev = p.n_est_dev;
+            }
             for (size_t i = 0; i < n; i++) {
-                UBList &L = h_lists[li];
-                if (numeric) {
-                    const II_NumericList *nl = leaves[p.q][i];
-                    if (!nl->n) continue;
-                    L = UBList{nl->d_ids, nullptr, nl->d_values, (uint32_t)nl->n, (uint32_t)b, (uint32_t)i, chunk};
-                } else {
-                    const II_PostingList *pl = lists[p.q][i];
-                    if (!pl->n) continue;
-                    L = UBList{pl->d_ids, full ? pl->d_freqs : nullptr, nullptr, (uint32_t)pl->n, (uint32_t)b, (uint32_t)i, chunk};
-                }
-                chunk += (L.len + kUBChunk - 1) / kUBChunk;
+                const OrChild e = child(p.q, i);
+                if (e.d_est) h_e[ei++] = e.d_est;
+                if (!e.len) continue;
+                h_lists[li] = UBList{e.ids, e.freqs, e.values, e.d_len, (uint32_t)e.len, (uint32_t)b, (uint32_t)i, chunk};
+                chunk += (uint32_t)((e.len + kUBChunk - 1) / kUBChunk);
                 li++;
             }
         }
         uint32_t *d_est = d_scratch, *d_bitmap = d_scratch + est_words, *d_blocksum = d_bitmap + total_words, *d_blockoff = d_blocksum + total_blocks;
         uint32_t *d_wordoff = full ? d_blockoff + total_blocks : nullptr;
-        ok = cudaMemcpyAsync(d_tab, slot->h, tab_bytes, cudaMemcpyHostToDevice, c.stream) == cudaSuccess;
+        ok = wait_for_inputs(c, inputs);
+        ok = ok && cudaMemcpyAsync(d_tab, slot->h, tab_bytes, cudaMemcpyHostToDevice, c.stream) == cudaSuccess;
         ok = ok && cudaEventRecord(slot->ev, c.stream) == cudaSuccess;
         ok = ok && ii_launch_union_batch(reinterpret_cast<const UBList *>(d_tab), (uint32_t)nlists, (uint32_t)total_chunks,
                                          reinterpret_cast<const UBQuery *>(d_tab + off_q), (uint32_t)nb, total_blocks, clear_elems, d_est,
                                          d_bitmap, d_blocksum, d_blockoff, d_wordoff, &launches, c.stream) == cudaSuccess;
         c.stats.kernel_launches += launches;
+        if (!inputs.empty()) ok = borrow_inputs(c, inputs) && ok;
     }
     dfree(d_tab);
     dfree(d_scratch);
@@ -1917,12 +2042,19 @@ int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_Numer
 
 int II_UnionBatchDevice(size_t nq, II_PostingList *const *const *lists, const size_t *n_lists, int quick_exit, void *stream,
                         II_ResultSet **out, size_t *built) {
-    return filter_batch_device(nq, lists, nullptr, n_lists, quick_exit, nullptr, stream, out, built);
+    return filter_batch_device(nq, lists, nullptr, nullptr, n_lists, quick_exit, nullptr, stream, out, built);
 }
 
 int II_NumericFilterBatchDevice(size_t nq, II_NumericList *const *const *leaves, const size_t *n_leaves, const II_NumericRange *ranges,
                                 void *stream, II_ResultSet **out, size_t *built) {
-    return filter_batch_device(nq, nullptr, leaves, n_leaves, 1, ranges, stream, out, built);
+    return filter_batch_device(nq, nullptr, leaves, nullptr, n_leaves, 1, ranges, stream, out, built);
+}
+
+// ORs over lists and (pending) sets in filter mode, with no host wait: the union batch above with each set's count read on the
+// device, and the OR's estimate summed there when a child's is still on the device.
+int II_UnionFilterBatchDevice(size_t nq, const II_FilterChild *const *children, const size_t *n_children, void *stream,
+                              II_ResultSet **out, size_t *built) {
+    return filter_batch_device(nq, nullptr, nullptr, children, n_children, 1, nullptr, stream, out, built);
 }
 
 // ANDs over lists and (pending) sets in filter mode, with no host wait.  The driver of each query is the required child with the
@@ -1993,6 +2125,8 @@ int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *childr
             if (ch.mode != 0) continue;
             deferred |= s && s->pending && s->estimated_on_device;
             rs->estimated = std::min(rs->estimated, est[i]);
+            rs->lo_id = std::max(rs->lo_id, ch.list ? ch.list->first_id : s->lo_id); // every hit is in each required child
+            rs->hi_id = std::min(rs->hi_id, ch.list ? ch.list->last_id : s->hi_id);
         }
         if (deferred) { // the order and the estimate wait for settle()
             rs->estimated_on_device = true;
@@ -2069,11 +2203,8 @@ int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *childr
                 }
             }
         }
-        // the AND reads each child set once that set's own kernels are done (a settled or host-built set: at once)
-        std::sort(inputs.begin(), inputs.end());
-        inputs.erase(std::unique(inputs.begin(), inputs.end()), inputs.end());
-        for (II_ResultSet *s : inputs)
-            if (s->ready) ok = ok && cudaStreamWaitEvent(c.stream, s->ready, 0) == cudaSuccess;
+        // the AND reads each child set once that set's own kernels are done
+        ok = wait_for_inputs(c, inputs);
         const auto *d_q = reinterpret_cast<const IFBQuery *>(d_scratch);
         const auto *d_c = reinterpret_cast<const IFBChild *>(d_scratch + off_c);
         uint32_t *d_surv = reinterpret_cast<uint32_t *>(d_scratch + align16(tab_bytes));
@@ -2083,21 +2214,7 @@ int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *childr
         ok = ok && ii_launch_filter_and_batch(d_c, d_q, (uint32_t)nb, (uint32_t)total_chunks, d_surv, d_counts, d_offsets, c.stream) ==
                        cudaSuccess;
         c.stats.kernel_launches += 3;
-        // every input keeps the call's completion event: its memory is not handed out again while the AND may still read it
-        auto done = std::make_shared<SharedEvent>();
-        if (cudaEventCreateWithFlags(&done->ev, cudaEventDisableTiming) == cudaSuccess && cudaEventRecord(done->ev, c.stream) == cudaSuccess) {
-            std::lock_guard<std::mutex> rg(readers_mu());
-            for (II_ResultSet *s : inputs) {
-                auto &r = s->readers;
-                r.erase(std::remove_if(r.begin(), r.end(), [](const std::shared_ptr<SharedEvent> &e) { return cudaEventQuery(e->ev) == cudaSuccess; }),
-                        r.end());
-                r.push_back(done);
-            }
-            cudaGetLastError(); // cudaErrorNotReady of a reader still running is no failure
-        } else {
-            cudaStreamSynchronize(c.stream);
-            ok = false;
-        }
+        if (!borrow_inputs(c, inputs)) ok = false;
     }
     dfree(d_scratch);
     for (Plan &p : plans) {

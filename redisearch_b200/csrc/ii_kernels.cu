@@ -699,7 +699,9 @@ __global__ void __launch_bounds__(256) ub_mark_kernel(const UBList *__restrict__
     __syncthreads();
     const UBList L = lists[s_l];
     const UBQuery &q = qs[L.q];
-    const uint32_t base = (blockIdx.x - L.chunk0) * kUBChunk, end = min(base + kUBChunk, L.len);
+    const uint32_t base = (blockIdx.x - L.chunk0) * kUBChunk, len = L.d_len ? min(*L.d_len, L.len) : L.len;
+    if (base >= len) return; // a set's chunk past its count on the device: no read of its docIds (never a numeric leaf)
+    const uint32_t end = min(base + kUBChunk, len);
     uint32_t kept = 0;
     for (uint32_t i = base + threadIdx.x; i < end; i += blockDim.x) {
         if (L.values) { // a numeric leaf: only records in range mark; the first of its document counts toward num_estimated
@@ -724,8 +726,8 @@ __global__ void ub_popc_kernel(const uint32_t *__restrict__ bitmap, uint64_t tot
         if ((threadIdx.x & 31) == 0) blocksum[w >> 5] = c;
     }
 }
-// one CTA per query: exclusive scan of its blocks' counts, the count into len[0] (and len[1] for numeric filters), and the
-// set's epoch table out of the batch table
+// one CTA per query: exclusive scan of its blocks' counts, the count into len[0] (and len[1] for numeric filters and ORs over
+// sets), and the set's epoch table out of the batch table
 constexpr int kUBScanThreads = 1024, kUBScanItems = 8;
 // exclusive scan of in[0, n) into out by one CTA of kUBScanThreads threads; returns the total to every thread
 __device__ uint32_t cta_exclusive_scan(const uint32_t *__restrict__ in, uint32_t *__restrict__ out, uint32_t n, uint32_t *s_warp,
@@ -778,7 +780,14 @@ __global__ void __launch_bounds__(kUBScanThreads) ub_scan_kernel(const UBQuery *
     const uint32_t total = cta_exclusive_scan(blocksum + q.blk0, blockoff + q.blk0, q.nblk, s_warp, s_carry);
     if (threadIdx.x == 0) {
         q.len[0] = total;
-        q.len[1] = est[blockIdx.x];
+        if (!q.sum_est) q.len[1] = est[blockIdx.x];
+    }
+    if (q.sum_est && threadIdx.x < 32) { // an OR over sets: the estimates still on the device (at most 1024) summed by one warp
+        unsigned long long sum = 0;
+        for (uint32_t i = threadIdx.x; i < q.n_est_dev; i += 32) sum += *q.est_dev[i];
+#pragma unroll
+        for (int m = 16; m > 0; m >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, m);
+        if (threadIdx.x == 0) q.len[1] = (uint32_t)min(sum + q.est_host, 0xFFFFFFFFull);
     }
     if (q.order) {
         const uint32_t *src = reinterpret_cast<const uint32_t *>(q.order_src);

@@ -115,17 +115,19 @@ struct UnionOrder {
     uint8_t perm[kIIMaxLists + 1][kIIMaxLists];
 };
 
-// ---- batches of ORs and numeric range filters (II_UnionBatchDevice, II_NumericFilterBatchDevice) -------------------------
+// ---- batches of ORs and numeric range filters (II_UnionBatchDevice, II_NumericFilterBatchDevice, II_UnionFilterBatchDevice) --
 // Every list of every query of the batch in one ragged launch per step: each query owns a window of a shared bitmap that spans
 // the docIds of its lists, a CTA of the mark / fill passes owns kUBChunk postings of one list (found by binary search over the
 // lists' first chunks), and the scan runs one CTA per query.  Launches: 4 (docIds only) or 6 (per-child freq rows), whatever
-// the batch size and the number of lists.
+// the batch size and the number of lists.  A set child's chunks are counted from its capacity; those past its count on the device
+// return at once.
 constexpr uint32_t kUBChunk = 1024;
 struct UBList {
     const uint32_t *ids;
     const uint32_t *freqs; // full mode: the list's freqs (else NULL)
     const double *values;  // a numeric leaf: its record values, tested against the query's range (NULL: a posting list)
-    uint32_t len;
+    const uint32_t *d_len; // a set: its count on the device, read as min(*d_len, len) (NULL: a list or a leaf, len is exact)
+    uint32_t len;          // a list's or a leaf's length, a set's capacity
     uint32_t q;      // owning query (index into the UBQuery table)
     uint32_t row;    // the list's child index inside its query: its freq / position row
     uint32_t chunk0; // first kUBChunk chunk of the list in the batch
@@ -145,6 +147,12 @@ struct UBQuery {
     uint64_t cap;      // row stride of freqs / pos
     double mn, mx;     // numeric range (NumericFilter::value_in_range)
     int mni, mxi;
+    // an OR over sets (sum_est = 1): len[1] = min(est_host + the sum of *est_dev[0 .. n_est_dev), 2^32 - 1), the children's
+    // num_estimated with those still on the device read there; sum_est = 0: len[1] = the mark pass's count (numeric) or 0
+    const uint32_t *const *est_dev;
+    uint64_t est_host;
+    uint32_t n_est_dev;
+    uint32_t sum_est;
 };
 // d_est [nq] and d_bitmap [total_blocks * 32] are contiguous (one memset clears both); d_wordoff NULL = docIds only.
 // clear_elems: the largest n_rows * cap of the batch (sizes the clear of the freq / position rows).  Returns the launches made.

@@ -110,6 +110,7 @@ SIGNATURES = [
     ("II_UnionBatchDevice", C.c_int, [_SZ, _P, _P, C.c_int, _P, _P, C.POINTER(_SZ)]),
     ("II_NumericFilterBatchDevice", C.c_int, [_SZ, _P, _P, _P, _P, _P, C.POINTER(_SZ)]),
     ("II_IntersectFilterBatchDevice", C.c_int, [_SZ, _P, _P, _P, _P, C.POINTER(_SZ)]),
+    ("II_UnionFilterBatchDevice", C.c_int, [_SZ, _P, _P, _P, _P, C.POINTER(_SZ)]),
     ("II_IndexWriter_New", _P, [C.c_int]),
     ("II_IndexWriter_NewNumeric", _P, [C.c_int]),
     ("II_IndexWriter_Add", _SZ, [_P, C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint64, _P, C.c_uint32]),
@@ -468,11 +469,9 @@ def numeric_filter_batch_device(batch, stream=None):
     return _pending_sets(rc, out, nq)
 
 
-def intersect_filter_batch_device(batch, stream=None):
-    """II_IntersectFilterBatchDevice: batch[q] = [(child, mode)] of query q's filter-mode AND, child = a PostingList, a ResultSet
-    (pending or settled, e.g. from union_batch_device) or None (an empty child), mode 0 = required, 1 = NOT.  The children are
-    borrowed.  Returns as union_batch_device; raises ValueError when the batch is refused or a child is closed or consumed (only
-    None stands for an empty child)."""
+def _filter_child_table(batch):
+    """(pointer table per query, its keep-alive arrays, counts) of batch[q] = [(child, mode)], child = a PostingList, a ResultSet
+    or None; a closed or consumed child raises ValueError"""
     nq = len(batch)
     arrays = []
     for items in batch:
@@ -487,8 +486,30 @@ def intersect_filter_batch_device(batch, stream=None):
         arrays.append(a)
     pp = (C.c_void_p * max(1, nq))(*[C.cast(a, C.c_void_p) for a in arrays])
     counts = (C.c_size_t * max(1, nq))(*[len(items) for items in batch])
+    return pp, arrays, counts
+
+
+def intersect_filter_batch_device(batch, stream=None):
+    """II_IntersectFilterBatchDevice: batch[q] = [(child, mode)] of query q's filter-mode AND, child = a PostingList, a ResultSet
+    (pending or settled, e.g. from union_batch_device) or None (an empty child), mode 0 = required, 1 = NOT.  The children are
+    borrowed.  Returns as union_batch_device; raises ValueError when the batch is refused or a child is closed or consumed (only
+    None stands for an empty child)."""
+    nq = len(batch)
+    pp, _keep, counts = _filter_child_table(batch)
     out = (C.c_void_p * max(1, nq))()
     rc = lib().II_IntersectFilterBatchDevice(nq, pp, counts, _stream_handle(stream), out, None)
+    return _pending_sets(rc, out, nq)
+
+
+def union_filter_batch_device(batch, stream=None):
+    """II_UnionFilterBatchDevice: batch[q] = the children of query q's filter-mode OR, each a PostingList, a ResultSet (pending
+    or settled, e.g. from intersect_filter_batch_device or numeric_filter_batch_device) or None (an empty child).  The children
+    are borrowed.  Returns as union_batch_device; raises ValueError when the batch is refused or a child is closed or consumed
+    (only None stands for an empty child)."""
+    nq = len(batch)
+    pp, _keep, counts = _filter_child_table([[(c, 0) for c in items] for items in batch])
+    out = (C.c_void_p * max(1, nq))()
+    rc = lib().II_UnionFilterBatchDevice(nq, pp, counts, _stream_handle(stream), out, None)
     return _pending_sets(rc, out, nq)
 
 
