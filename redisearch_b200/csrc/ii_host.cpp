@@ -2683,6 +2683,8 @@ int II_SearchTopNBatch(size_t nq, II_PostingList *const *const *lists, const siz
     // synchronised when it is needed again
     PendingSearch pend[kBatchSlots];
     size_t owner[kBatchSlots] = {0};
+    uint64_t slot_launches0[kBatchSlots];
+    for (size_t sl = 0; sl < kBatchSlots; sl++) slot_launches0[sl] = pool.slot[sl].stats.kernel_launches;
     auto finish = [&](size_t sl) {
         CtxScope scope(&pool.slot[sl]);
         const size_t qi = owner[sl];
@@ -2705,6 +2707,8 @@ int II_SearchTopNBatch(size_t nq, II_PostingList *const *const *lists, const siz
     }
     for (size_t sl = 0; sl < kBatchSlots; sl++)
         if (pend[sl].active) finish(sl);
+    // the chains' launches, like the fused ones, go to the calling thread's counters
+    for (size_t sl = 0; sl < kBatchSlots; sl++) ctx().stats.kernel_launches += pool.slot[sl].stats.kernel_launches - slot_launches0[sl];
     return rc;
 }
 
