@@ -1,6 +1,7 @@
 // Host side of libii_b200.so: posting-list objects, block decoding, the iterator algebra entry
 // points, scoring, ranking and the QueryIterator facade.  Contract: include/ii_b200.h.
 #include "../../include/ii_b200.h"
+#include "batch_scratch.h"
 #include "ii_explain.h"
 #include "ii_kernels.h"
 #include "ii_codec.h"
@@ -49,8 +50,9 @@ struct Ctx { // one per calling thread: own stream, events and pinned staging (R
         }
         return h_stage;
     }
-    // pinned staging of the batch filters (II_UnionBatchDevice / II_NumericFilterBatchDevice): a slot is taken again only once its
-    // last upload has executed (cudaEventQuery; a never-recorded event counts as complete), else a new slot is made — never a wait
+    // pinned staging of the tables the device filter batches upload (filter_batch_device, II_IntersectFilterBatchDevice): a slot is
+    // taken again only once its last upload has executed (cudaEventQuery; a never-recorded event counts as complete), else a new
+    // slot is made — never a wait
     struct UploadSlot {
         uint8_t *h = nullptr;
         size_t cap = 0;
@@ -167,7 +169,7 @@ struct SharedEvent {
         if (ev) cudaEventDestroy(ev);
     }
 };
-// guards II_ResultSet::readers: one set may be a child of II_IntersectFilterBatchDevice calls on several threads at once
+// guards II_ResultSet::readers: one set may be an input of device filter batch calls on several threads at once
 static std::mutex &readers_mu() {
     static std::mutex m;
     return m;
@@ -242,15 +244,16 @@ struct II_ResultSet {
     // they bound the bitmap window of an OR over sets (II_UnionFilterBatchDevice)
     uint32_t lo_id = 0, hi_id = 0xFFFFFFFFu;
     std::unique_ptr<UnionOrder> h_order; // host copy of d_order (EXPLAINSCORE walks one hit's children in aggregate order)
-    // II_IntersectBatchDevice: the hit count is known only on the device until settle(); `ready` completes with the AND's kernels
+    // a set of a device batch (II_IntersectBatchDevice, the filter batches): the hit count is known only on the device until
+    // settle(); `ready` completes with the kernels that build the set
     bool pending = false;
     cudaEvent_t ready = nullptr;
-    bool estimated_on_device = false; // II_NumericFilterBatchDevice: num_estimated is d_len[1] until settle()
+    bool estimated_on_device = false; // a filter batch set whose num_estimated is summed on the device: d_len[1] until settle()
     // II_IntersectFilterBatchDevice with a child whose estimate is on the device: the child order waits for settle(), which sorts by
     // d_len[2 + i] (child i's num_estimated) times order_weight[i] (its sort weight; < 0 = a NOT child, sorted last); child_tag
     // is in the given order until then
     std::vector<double> order_weight;
-    // completion events of the II_IntersectFilterBatchDevice calls that read this set as a child: the frees below wait for them
+    // completion events of the device filter batch calls that read this set as a child: the frees below wait for them
     std::vector<std::shared_ptr<struct SharedEvent>> readers;
     ~II_ResultSet() {
         if (ready) { // allocated on another stream, whose AND may still be writing: the frees below wait for it
@@ -957,44 +960,70 @@ int II_DocTable_SetPayloads(II_DocTable *dt, const uint8_t *payloads, const uint
 // ------------------------------------------------------------------------------------------------
 namespace {
 
-// Enqueue the kernels of an intersection on ctx().stream.  On return rs->d_len holds (will hold, in
-// stream order) the number of hits; rs->len is NOT set.  *trivially_empty = an input list is empty.
-// modes (nullable): per list 0 = required, 1 = NOT, 2 = OPTIONAL (IntersectArgs::mode); at least one list is required
+// The shape every aggregate starts from: n children in the given order, each tagged `tag` (RSResultData), none nested, no term
+// positions
+void init_children(II_ResultSet *rs, size_t n, uint8_t tag) {
+    rs->n_children = (uint32_t)n;
+    rs->child_order.resize(n);
+    for (size_t i = 0; i < n; i++) rs->child_order[i] = (uint32_t)i;
+    rs->child_off.assign(n, II_ResultSet::ChildOffsets());
+    rs->nested.assign(n, nullptr);
+    rs->child_tag.assign(n, tag);
+}
+
+// sort key of Intersection::new_with_slop_order (intersection.rs:110-120): num_estimated * intersection_sort_weight, as doubles;
+// NOT / OPTIONAL children estimate max_doc_id (not.rs / optional.rs num_estimated): they sort behind every other child
+inline double and_sort_key(bool required, double estimated, double sort_weight) { return required ? estimated * sort_weight : 0x1p62; }
+struct AndKey {
+    bool required;
+    double estimated, sort_weight;
+};
+// Intersection::new's aggregate child order (intersection.rs:110-145): a stable sort of the n children ascending by and_sort_key of
+// key(i), so NOT / OPTIONAL children come last in their given order.  rs->child_order becomes that order, and rs->child_tag, given
+// in the children's given order, is permuted into it.
+extern "C++" template <class Key> void and_order(II_ResultSet *rs, size_t n, Key &&key) {
+    std::vector<double> k(n);
+    for (size_t i = 0; i < n; i++) {
+        const AndKey a = key(i);
+        k[i] = and_sort_key(a.required, a.estimated, a.sort_weight);
+    }
+    std::vector<uint32_t> order(n);
+    for (size_t i = 0; i < n; i++) order[i] = (uint32_t)i;
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return k[a] < k[b]; });
+    std::vector<uint8_t> tag(n);
+    for (size_t j = 0; j < n; j++) tag[j] = rs->child_tag[order[j]];
+    rs->child_order = std::move(order);
+    rs->child_tag = std::move(tag);
+}
+
 struct PhraseSpec {
     uint32_t max_slop; // 0xFFFFFFFF: no limit (in-order only)
     bool in_order;
 };
-// sort key of Intersection::new_with_slop_order (intersection.rs:110-120): num_estimated * intersection_sort_weight, as doubles;
-// NOT / OPTIONAL children estimate max_doc_id (not.rs / optional.rs num_estimated): they sort behind every other child
-inline double and_sort_key(bool required, double estimated, double sort_weight) { return required ? estimated * sort_weight : 0x1p62; }
+// Enqueue the kernels of an intersection on ctx().stream.  On return rs->d_len holds (will hold, in
+// stream order) the number of hits; rs->len is NOT set.  *trivially_empty = an input list is empty.
+// modes (nullable): per list 0 = required, 1 = NOT, 2 = OPTIONAL (IntersectArgs::mode); at least one list is required
 bool intersect_enqueue(Ctx &c, II_PostingList *const *lists, size_t n, II_ResultSet *rs, bool *trivially_empty, const int *modes = nullptr,
                        const PhraseSpec *phrase = nullptr) {
     auto mode_of = [&](size_t i) { return modes ? modes[i] : 0; };
     if (phrase && n > (size_t)kPhraseMaxLists) return false;
-    // Intersection::new: stable sort ascending by num_estimated (leaf weight 1.0), intersection.rs:110-145; NOT / OPTIONAL
-    // children behind every term, in their given order
-    std::vector<uint32_t> order(n);
-    for (size_t i = 0; i < n; i++) order[i] = (uint32_t)i;
-    auto est = [&](uint32_t a) { return and_sort_key(mode_of(a) == 0, (double)lists[a]->estimated, lists[a]->sort_weight); };
+    init_children(rs, n, 4);
+    for (size_t i = 0; i < n; i++) rs->child_tag[i] = mode_of(i) == 1 ? 8 : lists[i]->result_tag;
     // an in-order intersection keeps the children as given: their order is the order the terms must appear in
     // (intersection.rs new_sorted_by: `if !in_order { children.sort_by(compare) }`)
-    if (!(phrase && phrase->in_order)) std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return est(a) < est(b); });
+    if (!(phrase && phrase->in_order))
+        and_order(rs, n, [&](size_t i) { return AndKey{mode_of(i) == 0, (double)lists[i]->estimated, lists[i]->sort_weight}; });
+    const std::vector<uint32_t> &order = rs->child_order;
     // the kernel is driven by the REQUIRED list with the fewest actual entries (a field-mask filter may make
     // that differ from the estimate order); the aggregate child order stays the reference's
     size_t drv = n;
     for (size_t i = 0; i < n; i++)
         if (mode_of(order[i]) == 0 && (drv == n || lists[order[i]]->n < lists[order[drv]]->n)) drv = i;
     if (drv == n) return false;
-    rs->n_children = (uint32_t)n;
-    rs->child_order.assign(order.begin(), order.end());
-    rs->child_off.assign(n, II_ResultSet::ChildOffsets());
-    rs->nested.assign(n, nullptr);
-    rs->child_tag.assign(n, 4);
     bool any_nested = false;
     rs->estimated = (size_t)-1;
     for (size_t j = 0; j < n; j++) {
         const II_PostingList *L = lists[order[j]];
-        rs->child_tag[j] = mode_of(order[j]) == 1 ? 8 : L->result_tag;
         if (mode_of(order[j]) == 0) {
             rs->estimated = std::min(rs->estimated, L->estimated); // NOT / OPTIONAL estimate max_doc_id
             rs->lo_id = std::max(rs->lo_id, L->first_id);          // every hit is in each required list
@@ -1215,7 +1244,47 @@ bool ensure_slop(Ctx &c, II_ResultSet *rs, const uint32_t *d_len, uint32_t cap_l
 }
 
 ScoreArgs make_score_args(II_ResultSet *rs, II_Scorer scorer, const II_TermParams *terms, double agg_weight,
-                          const II_IndexStats *stats, const II_DocTable *docs, double min_score, uint64_t tanh_factor);
+                          const II_IndexStats *stats, const II_DocTable *docs, double min_score, uint64_t tanh_factor) {
+    ScoreArgs sa{};
+    sa.scorer = (int)scorer;
+    sa.is_union = rs->is_union;
+    sa.n_children = rs->n_children;
+    if (rs->n_children <= (uint32_t)kIIMaxLists) {
+        for (uint32_t i = 0; i < rs->n_children; i++) {
+            const II_TermParams &t = terms[rs->child_order[i]];
+            sa.weight[i] = t.weight;
+            sa.idf[i] = t.idf;
+            sa.bm25_idf[i] = t.bm25_idf;
+        }
+    } else { // a wide union: the tables do not fit the kernel arguments (pageable source: staged before the copy call returns)
+        const uint32_t n = rs->n_children;
+        std::vector<double> ext(3 * (size_t)n);
+        for (uint32_t i = 0; i < n; i++) {
+            const II_TermParams &t = terms[rs->child_order[i]];
+            ext[i] = t.weight;
+            ext[n + i] = t.idf;
+            ext[2 * (size_t)n + i] = t.bm25_idf;
+        }
+        if (!rs->d_ext) rs->d_ext = dalloc<double>(ext.size());
+        if (rs->d_ext) cudaMemcpyAsync(rs->d_ext, ext.data(), ext.size() * 8, cudaMemcpyHostToDevice, ctx().stream);
+        sa.ext = rs->d_ext;
+        sa.n_children = rs->d_ext ? n : 0; // no table, no children: the launch scores nothing rather than reading past the inline arrays
+    }
+    sa.agg_weight = agg_weight;
+    sa.avg_doc_len = stats ? stats->avgDocLen : 0.0;
+    sa.min_score = min_score;
+    sa.tanh_factor = tanh_factor ? tanh_factor : 1;
+    sa.doc_len = docs ? docs->d_len : nullptr;
+    sa.doc_score = docs ? docs->d_score : nullptr;
+    sa.max_freq = docs ? docs->d_maxf : nullptr;
+    sa.slop = rs->d_slop; // NULL: no term positions on the device, the kernel uses `children - 1`
+    sa.order = rs->d_order;
+    for (uint32_t i = 0; i < rs->n_children && i < rs->nested.size() && i < (uint32_t)kIIMaxLists; i++)
+        if (rs->nested[i]) sa.sub[i] = rs->nested[i]->d_sub;
+    sa.pos = rs->d_hit_pos;
+    sa.pstride = rs->cap;
+    return sa;
+}
 
 // The recursive value of every hit of every nested child of `rs` for `scorer` (ScoreArgs::sub), innermost first.
 bool prepare_nested_scores(Ctx &c, II_ResultSet *rs, II_Scorer scorer, const II_IndexStats *stats, const II_DocTable *docs) {
@@ -1249,13 +1318,8 @@ struct UnionPlan {
 UnionPlan union_plan(II_PostingList *const *lists, size_t n, int quick_exit, II_ResultSet *rs) {
     UnionPlan p;
     rs->is_union = true;
-    rs->n_children = (uint32_t)n;
     rs->has_freqs = !quick_exit;
-    rs->child_order.resize(n);
-    for (size_t i = 0; i < n; i++) rs->child_order[i] = (uint32_t)i;
-    rs->child_off.assign(n, II_ResultSet::ChildOffsets());
-    rs->nested.assign(n, nullptr);
-    rs->child_tag.assign(n, 4);
+    init_children(rs, n, 4);
     rs->estimated = 0;
     rs->lo_id = 0xFFFFFFFFu;
     for (size_t i = 0; i < n; i++) {
@@ -1373,47 +1437,21 @@ void finish_len(Ctx &c, II_ResultSet *rs) {
     if (cudaEventElapsedTime(&ms, c.e0, c.e1) == cudaSuccess) c.stats.intersect_device_us = ms * 1000.0;
 }
 
-ScoreArgs make_score_args(II_ResultSet *rs, II_Scorer scorer, const II_TermParams *terms, double agg_weight,
-                          const II_IndexStats *stats, const II_DocTable *docs, double min_score, uint64_t tanh_factor) {
-    ScoreArgs sa{};
-    sa.scorer = (int)scorer;
-    sa.is_union = rs->is_union;
-    sa.n_children = rs->n_children;
-    if (rs->n_children <= (uint32_t)kIIMaxLists) {
-        for (uint32_t i = 0; i < rs->n_children; i++) {
-            const II_TermParams &t = terms[rs->child_order[i]];
-            sa.weight[i] = t.weight;
-            sa.idf[i] = t.idf;
-            sa.bm25_idf[i] = t.bm25_idf;
-        }
-    } else { // a wide union: the tables do not fit the kernel arguments (pageable source: staged before the copy call returns)
-        const uint32_t n = rs->n_children;
-        std::vector<double> ext(3 * (size_t)n);
-        for (uint32_t i = 0; i < n; i++) {
-            const II_TermParams &t = terms[rs->child_order[i]];
-            ext[i] = t.weight;
-            ext[n + i] = t.idf;
-            ext[2 * (size_t)n + i] = t.bm25_idf;
-        }
-        if (!rs->d_ext) rs->d_ext = dalloc<double>(ext.size());
-        if (rs->d_ext) cudaMemcpyAsync(rs->d_ext, ext.data(), ext.size() * 8, cudaMemcpyHostToDevice, ctx().stream);
-        sa.ext = rs->d_ext;
-        sa.n_children = rs->d_ext ? n : 0; // no table, no children: the launch scores nothing rather than reading past the inline arrays
+// One set built synchronously on the calling thread's context: `enqueue(c, rs, &trivially_empty)` (intersect_enqueue or
+// union_enqueue) queues its kernels, then the count is read back.  NULL where the enqueue or the read-back failed.
+extern "C++" template <class Enqueue> II_ResultSet *build_sync(Enqueue &&enqueue) {
+    Ctx &c = ctx();
+    std::lock_guard<std::mutex> g(c.mu);
+    if (!c.init()) return nullptr;
+    std::unique_ptr<II_ResultSet> rs(new II_ResultSet());
+    bool empty = false;
+    bool ok = enqueue(c, rs.get(), &empty);
+    if (ok && !empty) {
+        ok = cudaMemcpyAsync(c.h_total, rs->d_len, 4, cudaMemcpyDeviceToHost, c.stream) == cudaSuccess;
+        ok = ok && cudaStreamSynchronize(c.stream) == cudaSuccess;
+        if (ok) finish_len(c, rs.get());
     }
-    sa.agg_weight = agg_weight;
-    sa.avg_doc_len = stats ? stats->avgDocLen : 0.0;
-    sa.min_score = min_score;
-    sa.tanh_factor = tanh_factor ? tanh_factor : 1;
-    sa.doc_len = docs ? docs->d_len : nullptr;
-    sa.doc_score = docs ? docs->d_score : nullptr;
-    sa.max_freq = docs ? docs->d_maxf : nullptr;
-    sa.slop = rs->d_slop; // NULL: no term positions on the device, the kernel uses `children - 1`
-    sa.order = rs->d_order;
-    for (uint32_t i = 0; i < rs->n_children && i < rs->nested.size() && i < (uint32_t)kIIMaxLists; i++)
-        if (rs->nested[i]) sa.sub[i] = rs->nested[i]->d_sub;
-    sa.pos = rs->d_hit_pos;
-    sa.pstride = rs->cap;
-    return sa;
+    return ok ? rs.release() : nullptr;
 }
 
 // merge the per-warp top-N lists the device selected (<= lists*k survivors)
@@ -1509,46 +1547,13 @@ size_t search_finish(Ctx &c, PendingSearch &p, uint64_t *doc_ids, double *scores
 
 } // namespace
 
-II_ResultSet *II_Intersect(II_PostingList *const *lists, size_t n) {
-    if (n == 0 || n > (size_t)kIIMaxLists) return nullptr;
-    Ctx &c = ctx();
-    std::lock_guard<std::mutex> g(c.mu);
-    if (!c.init()) return nullptr;
-    auto *rs = new II_ResultSet();
-    bool empty = false;
-    bool ok = intersect_enqueue(c, lists, n, rs, &empty);
-    if (ok && !empty) {
-        ok = cudaMemcpyAsync(c.h_total, rs->d_len, 4, cudaMemcpyDeviceToHost, c.stream) == cudaSuccess;
-        ok = ok && cudaStreamSynchronize(c.stream) == cudaSuccess;
-        if (ok) finish_len(c, rs);
-    }
-    if (!ok) {
-        delete rs;
-        return nullptr;
-    }
-    return rs;
-}
+II_ResultSet *II_Intersect(II_PostingList *const *lists, size_t n) { return II_IntersectEx(lists, nullptr, n); }
 
 // AND with NOT / OPTIONAL children: modes[i] 0 = required, 1 = NOT (docIds of lists[i] are excluded), 2 = OPTIONAL (never
 // rejects; its freq is kept where present).  The excluded / absent children yield virtual results (freq 0, score 0).
 II_ResultSet *II_IntersectEx(II_PostingList *const *lists, const int *modes, size_t n) {
     if (n == 0 || n > (size_t)kIIMaxLists) return nullptr;
-    Ctx &c = ctx();
-    std::lock_guard<std::mutex> g(c.mu);
-    if (!c.init()) return nullptr;
-    auto *rs = new II_ResultSet();
-    bool empty = false;
-    bool ok = intersect_enqueue(c, lists, n, rs, &empty, modes);
-    if (ok && !empty) {
-        ok = cudaMemcpyAsync(c.h_total, rs->d_len, 4, cudaMemcpyDeviceToHost, c.stream) == cudaSuccess;
-        ok = ok && cudaStreamSynchronize(c.stream) == cudaSuccess;
-        if (ok) finish_len(c, rs);
-    }
-    if (!ok) {
-        delete rs;
-        return nullptr;
-    }
-    return rs;
+    return build_sync([&](Ctx &c, II_ResultSet *rs, bool *empty) { return intersect_enqueue(c, lists, n, rs, empty, modes); });
 }
 
 // AND with the reference's proximity constraints (intersection.rs:201-242 -> index_result proximity.rs): max_slop < 0 = no
@@ -1558,24 +1563,10 @@ II_ResultSet *II_IntersectPhrase(II_PostingList *const *lists, const int *modes,
     if (n == 0 || n > (size_t)kPhraseMaxLists) return nullptr;
     for (size_t i = 0; i < n; i++)
         if ((!modes || modes[i] != 1) && !lists[i]->d_off_len) return nullptr;
-    Ctx &c = ctx();
-    std::lock_guard<std::mutex> g(c.mu);
-    if (!c.init()) return nullptr;
-    auto *rs = new II_ResultSet();
-    bool empty = false;
     const PhraseSpec ph{max_slop < 0 ? 0xFFFFFFFFu : (uint32_t)max_slop, in_order != 0};
     const bool constrained = max_slop >= 0 || in_order;
-    bool ok = intersect_enqueue(c, lists, n, rs, &empty, modes, constrained ? &ph : nullptr);
-    if (ok && !empty) {
-        ok = cudaMemcpyAsync(c.h_total, rs->d_len, 4, cudaMemcpyDeviceToHost, c.stream) == cudaSuccess;
-        ok = ok && cudaStreamSynchronize(c.stream) == cudaSuccess;
-        if (ok) finish_len(c, rs);
-    }
-    if (!ok) {
-        delete rs;
-        return nullptr;
-    }
-    return rs;
+    return build_sync(
+        [&](Ctx &c, II_ResultSet *rs, bool *empty) { return intersect_enqueue(c, lists, n, rs, empty, modes, constrained ? &ph : nullptr); });
 }
 
 // nq independent ANDs in one call (the filters of a batch of hybrid queries): every intersection is enqueued on its own stream
@@ -1691,15 +1682,7 @@ void settle(const II_ResultSet *crs) {
     if (rs->estimated_on_device) rs->estimated = len[1];
     if (!rs->order_weight.empty()) { // Intersection::new's order over the children's estimates, now on the host
         const std::vector<double> &w = rs->order_weight;
-        std::vector<uint32_t> order(w.size());
-        for (size_t i = 0; i < order.size(); i++) order[i] = (uint32_t)i;
-        std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
-            return and_sort_key(w[a] >= 0, (double)len[2 + a], w[a]) < and_sort_key(w[b] >= 0, (double)len[2 + b], w[b]);
-        });
-        std::vector<uint8_t> tag(order.size());
-        for (size_t j = 0; j < order.size(); j++) tag[j] = rs->child_tag[order[j]];
-        rs->child_order = std::move(order);
-        rs->child_tag = std::move(tag);
+        and_order(rs, w.size(), [&](size_t i) { return AndKey{w[i] >= 0, (double)len[2 + i], w[i]}; });
         rs->order_weight.clear();
     }
     rs->pending = false;
@@ -1727,22 +1710,7 @@ void II_ResultSet_FreeAfter(II_ResultSet *rs, void *stream) {
 
 II_ResultSet *II_Union(II_PostingList *const *lists, size_t n, int quick_exit) {
     if (n == 0 || n > (size_t)kIIMaxUnionLists) return nullptr;
-    Ctx &c = ctx();
-    std::lock_guard<std::mutex> g(c.mu);
-    if (!c.init()) return nullptr;
-    auto *rs = new II_ResultSet();
-    bool empty = false;
-    bool ok = union_enqueue(c, lists, n, quick_exit, rs, &empty);
-    if (ok && !empty) {
-        ok = cudaMemcpyAsync(c.h_total, rs->d_len, 4, cudaMemcpyDeviceToHost, c.stream) == cudaSuccess;
-        ok = ok && cudaStreamSynchronize(c.stream) == cudaSuccess;
-        if (ok) finish_len(c, rs);
-    }
-    if (!ok) {
-        delete rs;
-        return nullptr;
-    }
-    return rs;
+    return build_sync([&](Ctx &c, II_ResultSet *rs, bool *empty) { return union_enqueue(c, lists, n, quick_exit, rs, empty); });
 }
 
 namespace {
@@ -1775,16 +1743,52 @@ bool borrow_inputs(Ctx &c, const std::vector<II_ResultSet *> &inputs) {
     return true;
 }
 
+// The part of a batch plan that publish_pending hands out: the set built for query q
+struct PendingPlan {
+    size_t q;
+    std::unique_ptr<II_ResultSet> rs;
+};
+// The end of a batch call that hands out pending sets, once their memory, the device buffer `d_buf` and the pinned `slot` are
+// allocated and the tables filled in the slot (ok: all of that succeeded).  The first tab_bytes of the slot go up to d_buf in one
+// copy, `launch` runs once every input set's own kernels are done, and the inputs are borrowed: each keeps the call's completion
+// event, which its destructor waits for.  d_buf is freed in stream order, an event per set marks it pending, `stream` waits for
+// the last one and out[q] / *built receive the sets.  On failure nothing is handed out and the result is -1.
+extern "C++" template <class Plan, class Launch>
+int publish_pending(Ctx &c, bool ok, Ctx::UploadSlot *slot, uint8_t *d_buf, size_t tab_bytes, std::vector<II_ResultSet *> &inputs,
+                    Launch &&launch, std::vector<Plan> &plans, void *stream, II_ResultSet **out, size_t *built) {
+    if (ok) {
+        ok = wait_for_inputs(c, inputs);
+        ok = ok && cudaMemcpyAsync(d_buf, slot->h, tab_bytes, cudaMemcpyHostToDevice, c.stream) == cudaSuccess;
+        ok = ok && cudaEventRecord(slot->ev, c.stream) == cudaSuccess;
+        ok = ok && launch();
+        if (!inputs.empty()) ok = borrow_inputs(c, inputs) && ok;
+    }
+    dfree(d_buf);
+    for (Plan &p : plans) {
+        II_ResultSet *rs = p.rs.get();
+        ok = ok && cudaEventCreateWithFlags(&rs->ready, cudaEventDisableTiming) == cudaSuccess && cudaEventRecord(rs->ready, c.stream) == cudaSuccess;
+        rs->pending = true;
+    }
+    if (!ok) { // a failed allocation or launch: nothing is handed out (the frees run in c.stream order behind whatever was enqueued)
+        cudaGetLastError();
+        return -1;
+    }
+    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : cudaStreamLegacy;
+    // every set's event completes at the same point of c.stream: waiting for the last one waits for the whole batch
+    if (cudaStreamWaitEvent(st, plans.back().rs->ready, 0) != cudaSuccess) {
+        cudaStreamSynchronize(c.stream);
+        return -1;
+    }
+    for (Plan &p : plans) out[p.q] = p.rs.release();
+    if (built) *built = plans.size();
+    return 0;
+}
+
 // The shape II_Union(quick) gives a filter-mode OR of n children: docIds only, identity child order, every child tagged `tag`
 void filter_union_shape(II_ResultSet *rs, size_t n, uint8_t tag) {
     rs->is_union = true;
-    rs->n_children = (uint32_t)n;
     rs->has_freqs = false;
-    rs->child_order.resize(n);
-    for (size_t i = 0; i < n; i++) rs->child_order[i] = (uint32_t)i;
-    rs->child_off.assign(n, II_ResultSet::ChildOffsets());
-    rs->nested.assign(n, nullptr);
-    rs->child_tag.assign(n, tag);
+    init_children(rs, n, tag);
 }
 
 // One child of a batch OR as the kernels see it: a posting list, a numeric leaf or a set.  len: the exact length of a list or a
@@ -1798,9 +1802,8 @@ struct OrChild {
 
 // A batch of ORs with no host wait, over one of three kinds of children: posting lists (II_UnionBatchDevice), numeric leaves
 // filtered by a range (II_NumericFilterBatchDevice), or filter children, lists and sets (II_UnionFilterBatchDevice).  Every set's
-// memory comes from the pool in c.stream order; the tables the kernels read go up in one copy from a pinned slot;
-// ii_launch_union_batch runs the same 4 or 6 launches for any batch; an event per set marks it pending and `stream` waits for the
-// last one.  Child sets are borrowed as in II_IntersectFilterBatchDevice.
+// memory comes from the pool in c.stream order and ii_launch_union_batch runs the same 4 or 6 launches for any batch; the upload,
+// the borrowed child sets and the pending sets are publish_pending's.
 int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_NumericList *const *const *leaves,
                         const II_FilterChild *const *children, const size_t *counts, int quick_exit, const II_NumericRange *ranges,
                         void *stream, II_ResultSet **out, size_t *built) {
@@ -1851,9 +1854,7 @@ int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_Numer
         }
         return e;
     };
-    struct Plan {
-        size_t q;
-        std::unique_ptr<II_ResultSet> rs;
+    struct Plan : PendingPlan {
         uint32_t lo_word, nwords, nblk;
         uint64_t blk0;
         bool keep_pos;
@@ -1868,7 +1869,7 @@ int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_Numer
     for (size_t q = 0; q < nq; q++) {
         const size_t n = counts[q];
         if (!n) continue;
-        Plan p{q, std::unique_ptr<II_ResultSet>(new II_ResultSet()), 0, 0, 0, 0, false, UnionOrder{}, 0, 0};
+        Plan p{{q, std::unique_ptr<II_ResultSet>(new II_ResultSet())}, 0, 0, 0, 0, false, UnionOrder{}, 0, 0};
         II_ResultSet *rs = p.rs.get();
         uint32_t lo = 0xFFFFFFFFu, hi = 0; // the window: over the children that can hold a docId
         size_t total_in = 0;
@@ -1930,7 +1931,7 @@ int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_Numer
     Ctx &c = ctx();
     std::lock_guard<std::mutex> g(c.mu);
     if (!c.init()) return -1;
-    // per-set memory, then the batch's tables and bitmap scratch (freed below in stream order)
+    // per-set memory, then the batch's tables and bitmap scratch in one buffer (freed by publish_pending in stream order)
     bool ok = true;
     for (Plan &p : plans) {
         II_ResultSet *rs = p.rs.get();
@@ -1944,39 +1945,58 @@ int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_Numer
         ok = ok && rs->d_docs && rs->d_freqs && rs->d_scores && rs->d_len && (!rs->h_order || rs->d_order) && (!p.keep_pos || rs->d_hit_pos);
     }
     const size_t nb = plans.size();
-    const auto align16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
-    const size_t off_q = align16(nlists * sizeof(UBList)), off_o = off_q + align16(nb * sizeof(UBQuery));
-    const size_t off_e = align16(off_o + n_orders * sizeof(UnionOrder));
-    const size_t tab_bytes = n_est_dev ? off_e + n_est_dev * sizeof(const uint32_t *) : off_o + n_orders * sizeof(UnionOrder);
-    const size_t est_words = (nb + 31) & ~(size_t)31;
     const uint64_t total_words = total_blocks * 32;
-    uint8_t *d_tab = ok ? dalloc<uint8_t>(tab_bytes) : nullptr;
-    uint32_t *d_scratch = ok ? dalloc<uint32_t>(est_words + total_words * (full ? 2 : 1) + 2 * total_blocks) : nullptr;
-    Ctx::UploadSlot *slot = ok ? c.upload_slot(tab_bytes) : nullptr;
-    ok = ok && d_tab && d_scratch && slot;
-    uint32_t launches = 0;
+    struct Layout {
+        UBList *lists;
+        UBQuery *q;
+        UnionOrder *orders;
+        const uint32_t **est_dev;
+        size_t tab_bytes; // the tables above: what the pinned slot holds and the upload copies
+        uint32_t *est, *bitmap, *blocksum, *blockoff, *wordoff;
+        size_t bytes;
+    };
+    const auto layout = [&](void *base, bool tables_only) {
+        BatchScratch s(base);
+        Layout L{};
+        L.lists = s.take<UBList>(nlists);
+        L.q = s.take<UBQuery>(nb);
+        L.orders = s.take<UnionOrder>(n_orders);
+        L.est_dev = s.take<const uint32_t *>(n_est_dev);
+        L.tab_bytes = s.bytes();
+        if (tables_only) return L;
+        // ii_launch_union_batch clears [est, bitmap + total_words) with one memset: the estimate words must come from this
+        // buffer, right before the bitmap
+        L.est = s.take<uint32_t>(nb);
+        L.bitmap = s.take<uint32_t>(total_words);
+        L.blocksum = s.take<uint32_t>(total_blocks);
+        L.blockoff = s.take<uint32_t>(total_blocks);
+        L.wordoff = s.take<uint32_t>(full ? total_words : 0);
+        L.bytes = s.bytes();
+        return L;
+    };
+    const Layout size = layout(nullptr, false);
+    uint8_t *d_buf = ok ? dalloc<uint8_t>(size.bytes) : nullptr;
+    Ctx::UploadSlot *slot = ok ? c.upload_slot(size.tab_bytes) : nullptr;
+    ok = ok && d_buf && slot;
+    Layout h{}, d{};
     if (ok) {
-        auto *h_lists = reinterpret_cast<UBList *>(slot->h);
-        auto *h_q = reinterpret_cast<UBQuery *>(slot->h + off_q);
-        auto *h_o = reinterpret_cast<UnionOrder *>(slot->h + off_o);
-        auto *h_e = reinterpret_cast<const uint32_t **>(slot->h + off_e);
-        const auto *d_o = reinterpret_cast<const UnionOrder *>(d_tab + off_o);
-        const auto *d_e = reinterpret_cast<const uint32_t *const *>(d_tab + off_e);
+        h = layout(slot->h, true);
+        d = layout(d_buf, false);
         uint32_t li = 0, chunk = 0, oi = 0, ei = 0;
         for (size_t b = 0; b < nb; b++) {
             const Plan &p = plans[b];
             II_ResultSet *rs = p.rs.get();
             const size_t n = counts[p.q];
-            UBQuery &Q = h_q[b];
+            UBQuery &Q = h.q[b];
             Q = UBQuery{};
             Q.docs = rs->d_docs;
             Q.freqs = full ? rs->d_freqs : nullptr;
             Q.pos = rs->d_hit_pos;
             Q.len = rs->d_len;
             if (rs->h_order) {
-                h_o[oi] = p.uo;
+                h.orders[oi] = p.uo;
                 Q.order = rs->d_order;
-                Q.order_src = d_o + oi++;
+                Q.order_src = d.orders + oi++;
             }
             Q.blk0 = p.blk0;
             Q.nblk = p.nblk;
@@ -1994,49 +2014,27 @@ int filter_batch_device(size_t nq, II_PostingList *const *const *lists, II_Numer
             if (sets) {
                 Q.sum_est = 1;
                 Q.est_host = p.est_host;
-                Q.est_dev = d_e + ei;
+                Q.est_dev = d.est_dev + ei;
                 Q.n_est_dev = p.n_est_dev;
             }
             for (size_t i = 0; i < n; i++) {
                 const OrChild e = child(p.q, i);
-                if (e.d_est) h_e[ei++] = e.d_est;
+                if (e.d_est) h.est_dev[ei++] = e.d_est;
                 if (!e.len) continue;
-                h_lists[li] = UBList{e.ids, e.freqs, e.values, e.d_len, (uint32_t)e.len, (uint32_t)b, (uint32_t)i, chunk};
+                h.lists[li] = UBList{e.ids, e.freqs, e.values, e.d_len, (uint32_t)e.len, (uint32_t)b, (uint32_t)i, chunk};
                 chunk += (uint32_t)((e.len + kUBChunk - 1) / kUBChunk);
                 li++;
             }
         }
-        uint32_t *d_est = d_scratch, *d_bitmap = d_scratch + est_words, *d_blocksum = d_bitmap + total_words, *d_blockoff = d_blocksum + total_blocks;
-        uint32_t *d_wordoff = full ? d_blockoff + total_blocks : nullptr;
-        ok = wait_for_inputs(c, inputs);
-        ok = ok && cudaMemcpyAsync(d_tab, slot->h, tab_bytes, cudaMemcpyHostToDevice, c.stream) == cudaSuccess;
-        ok = ok && cudaEventRecord(slot->ev, c.stream) == cudaSuccess;
-        ok = ok && ii_launch_union_batch(reinterpret_cast<const UBList *>(d_tab), (uint32_t)nlists, (uint32_t)total_chunks,
-                                         reinterpret_cast<const UBQuery *>(d_tab + off_q), (uint32_t)nb, total_blocks, clear_elems, d_est,
-                                         d_bitmap, d_blocksum, d_blockoff, d_wordoff, &launches, c.stream) == cudaSuccess;
+    }
+    const auto launch = [&] {
+        uint32_t launches = 0;
+        const bool r = ii_launch_union_batch(d.lists, (uint32_t)nlists, (uint32_t)total_chunks, d.q, (uint32_t)nb, total_blocks, clear_elems,
+                                             d.est, d.bitmap, d.blocksum, d.blockoff, d.wordoff, &launches, c.stream) == cudaSuccess;
         c.stats.kernel_launches += launches;
-        if (!inputs.empty()) ok = borrow_inputs(c, inputs) && ok;
-    }
-    dfree(d_tab);
-    dfree(d_scratch);
-    for (Plan &p : plans) {
-        II_ResultSet *rs = p.rs.get();
-        ok = ok && cudaEventCreateWithFlags(&rs->ready, cudaEventDisableTiming) == cudaSuccess && cudaEventRecord(rs->ready, c.stream) == cudaSuccess;
-        rs->pending = true;
-    }
-    if (!ok) { // a failed allocation or launch: nothing is handed out (the frees run in c.stream order behind whatever was enqueued)
-        cudaGetLastError();
-        return -1;
-    }
-    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : cudaStreamLegacy;
-    // every set's event completes at the same point of c.stream: waiting for the last one waits for the whole batch
-    if (cudaStreamWaitEvent(st, plans.back().rs->ready, 0) != cudaSuccess) {
-        cudaStreamSynchronize(c.stream);
-        return -1;
-    }
-    for (Plan &p : plans) out[p.q] = p.rs.release();
-    if (built) *built = nb;
-    return 0;
+        return r;
+    };
+    return publish_pending(c, ok, slot, d_buf, size.tab_bytes, inputs, launch, plans, stream, out, built);
 }
 } // namespace
 
@@ -2059,9 +2057,8 @@ int II_UnionFilterBatchDevice(size_t nq, const II_FilterChild *const *children, 
 
 // ANDs over lists and (pending) sets in filter mode, with no host wait.  The driver of each query is the required child with the
 // smallest host bound; every other child is probed with the AND of intersect_kernel, each set's count read on the device.  Every
-// set's memory comes from the pool in c.stream order, the tables go up in one copy from a pinned slot, ii_launch_filter_and_batch
-// runs the same 3 launches for any batch, an event per set marks it pending and `stream` waits for the last one.  The child sets
-// are borrowed: each keeps the call's completion event, which its destructor waits for.
+// set's memory comes from the pool in c.stream order and ii_launch_filter_and_batch runs the same 3 launches for any batch; the
+// upload, the borrowed child sets and the pending sets are publish_pending's.
 int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *children, const size_t *n_children, void *stream,
                                   II_ResultSet **out, size_t *built) {
     if (built) *built = 0;
@@ -2080,9 +2077,7 @@ int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *childr
     }
     const auto bound = [](const II_FilterChild &ch) -> size_t { return ch.list ? ch.list->n : ch.set ? ch.set->cap : 0; };
     const auto sat = [](size_t v) { return (uint32_t)std::min<size_t>(v, 0xFFFFFFFFu); };
-    struct Plan {
-        size_t q;
-        std::unique_ptr<II_ResultSet> rs;
+    struct Plan : PendingPlan {
         std::vector<uint32_t> probe; // kernel order: the driver, then the others by ascending host bound
         uint32_t chunk0, nchunks;
     };
@@ -2102,16 +2097,13 @@ int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *childr
             if (drv == n || bound(cs[i]) < bound(cs[drv])) drv = i;
         }
         if (empty) continue; // a required child empty on the host: no set
-        Plan p{q, std::unique_ptr<II_ResultSet>(new II_ResultSet()), {}, (uint32_t)total_chunks, 0};
+        Plan p{{q, std::unique_ptr<II_ResultSet>(new II_ResultSet())}, {}, (uint32_t)total_chunks, 0};
         II_ResultSet *rs = p.rs.get();
         rs->is_union = false;
         rs->has_freqs = false;
-        rs->n_children = (uint32_t)n;
         rs->cap = bound(cs[drv]);
-        rs->child_off.assign(n, II_ResultSet::ChildOffsets());
-        rs->nested.assign(n, nullptr);
         // the shape Intersection::new gives the children: a set counts as the list view II_ResultSet_IntoChild makes of it
-        std::vector<uint8_t> tag(n);
+        init_children(rs, n, 4);
         std::vector<double> weight(n);
         std::vector<size_t> est(n);
         bool deferred = false;
@@ -2119,7 +2111,7 @@ int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *childr
         for (size_t i = 0; i < n; i++) {
             const II_FilterChild &ch = cs[i];
             const II_ResultSet *s = ch.set;
-            tag[i] = ch.mode == 1 ? 8 : ch.list ? ch.list->result_tag : s->is_union ? 1 : 2;
+            rs->child_tag[i] = ch.mode == 1 ? 8 : ch.list ? ch.list->result_tag : s->is_union ? 1 : 2;
             weight[i] = ch.list ? ch.list->sort_weight : s && !s->is_union ? 1.0 / (double)std::max<uint32_t>(1, s->n_children) : 1.0;
             est[i] = ch.list ? ch.list->estimated : s ? s->estimated : 0;
             if (ch.mode != 0) continue;
@@ -2130,20 +2122,10 @@ int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *childr
         }
         if (deferred) { // the order and the estimate wait for settle()
             rs->estimated_on_device = true;
-            rs->child_tag = tag;
             rs->order_weight.resize(n);
             for (size_t i = 0; i < n; i++) rs->order_weight[i] = cs[i].mode == 0 ? weight[i] : -1.0;
-            rs->child_order.resize(n);
-            for (size_t i = 0; i < n; i++) rs->child_order[i] = (uint32_t)i;
         } else {
-            std::vector<uint32_t> order(n);
-            for (size_t i = 0; i < n; i++) order[i] = (uint32_t)i;
-            std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
-                return and_sort_key(cs[a].mode == 0, (double)est[a], weight[a]) < and_sort_key(cs[b].mode == 0, (double)est[b], weight[b]);
-            });
-            rs->child_tag.resize(n);
-            for (size_t j = 0; j < n; j++) rs->child_tag[j] = tag[order[j]];
-            rs->child_order = std::move(order);
+            and_order(rs, n, [&](size_t i) { return AndKey{cs[i].mode == 0, (double)est[i], weight[i]}; });
         }
         p.probe.push_back((uint32_t)drv);
         for (size_t i = 0; i < n; i++)
@@ -2159,7 +2141,7 @@ int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *childr
     Ctx &c = ctx();
     std::lock_guard<std::mutex> g(c.mu);
     if (!c.init()) return -1;
-    // per-set memory, then the batch's tables and scratch in one allocation (freed below in stream order)
+    // per-set memory, then the batch's tables and scratch in one buffer (freed by publish_pending in stream order)
     bool ok = true;
     for (Plan &p : plans) {
         II_ResultSet *rs = p.rs.get();
@@ -2169,23 +2151,42 @@ int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *childr
         ok = ok && rs->d_docs && rs->d_scores && rs->d_len;
     }
     const size_t nb = plans.size();
-    const auto align16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
-    const size_t off_c = align16(nb * sizeof(IFBQuery)), tab_bytes = off_c + total_children * sizeof(IFBChild);
-    const size_t scratch_bytes = align16(tab_bytes) + ((size_t)total_chunks * kIIChunk + 2 * (size_t)total_chunks) * 4;
-    uint8_t *d_scratch = ok ? dalloc<uint8_t>(scratch_bytes) : nullptr;
-    Ctx::UploadSlot *slot = ok ? c.upload_slot(tab_bytes) : nullptr;
-    ok = ok && d_scratch && slot;
+    struct Layout {
+        IFBQuery *q;
+        IFBChild *children;
+        size_t tab_bytes; // the tables above: what the pinned slot holds and the upload copies
+        uint32_t *surv, *counts, *offsets;
+        size_t bytes;
+    };
+    const auto layout = [&](void *base, bool tables_only) {
+        BatchScratch s(base);
+        Layout L{};
+        L.q = s.take<IFBQuery>(nb);
+        L.children = s.take<IFBChild>(total_children);
+        L.tab_bytes = s.bytes();
+        if (tables_only) return L;
+        L.surv = s.take<uint32_t>((size_t)total_chunks * kIIChunk);
+        L.counts = s.take<uint32_t>(total_chunks);
+        L.offsets = s.take<uint32_t>(total_chunks);
+        L.bytes = s.bytes();
+        return L;
+    };
+    const Layout size = layout(nullptr, false);
+    uint8_t *d_buf = ok ? dalloc<uint8_t>(size.bytes) : nullptr;
+    Ctx::UploadSlot *slot = ok ? c.upload_slot(size.tab_bytes) : nullptr;
+    ok = ok && d_buf && slot;
+    Layout d{};
     if (ok) {
-        auto *h_q = reinterpret_cast<IFBQuery *>(slot->h);
-        auto *h_c = reinterpret_cast<IFBChild *>(slot->h + off_c);
+        const Layout h = layout(slot->h, true);
+        d = layout(d_buf, false);
         uint32_t ci = 0;
         for (size_t b = 0; b < nb; b++) {
             const Plan &p = plans[b];
             II_ResultSet *rs = p.rs.get();
-            h_q[b] = IFBQuery{rs->d_docs, rs->d_len, ci, rs->n_children, p.chunk0, p.nchunks};
+            h.q[b] = IFBQuery{rs->d_docs, rs->d_len, ci, rs->n_children, p.chunk0, p.nchunks};
             for (uint32_t slot_i : p.probe) {
                 const II_FilterChild &ch = children[p.q][slot_i];
-                IFBChild &K = h_c[ci++];
+                IFBChild &K = h.children[ci++];
                 K = IFBChild{};
                 K.slot = slot_i;
                 K.mode = (uint32_t)ch.mode;
@@ -2203,37 +2204,13 @@ int II_IntersectFilterBatchDevice(size_t nq, const II_FilterChild *const *childr
                 }
             }
         }
-        // the AND reads each child set once that set's own kernels are done
-        ok = wait_for_inputs(c, inputs);
-        const auto *d_q = reinterpret_cast<const IFBQuery *>(d_scratch);
-        const auto *d_c = reinterpret_cast<const IFBChild *>(d_scratch + off_c);
-        uint32_t *d_surv = reinterpret_cast<uint32_t *>(d_scratch + align16(tab_bytes));
-        uint32_t *d_counts = d_surv + (size_t)total_chunks * kIIChunk, *d_offsets = d_counts + total_chunks;
-        ok = ok && cudaMemcpyAsync(d_scratch, slot->h, tab_bytes, cudaMemcpyHostToDevice, c.stream) == cudaSuccess;
-        ok = ok && cudaEventRecord(slot->ev, c.stream) == cudaSuccess;
-        ok = ok && ii_launch_filter_and_batch(d_c, d_q, (uint32_t)nb, (uint32_t)total_chunks, d_surv, d_counts, d_offsets, c.stream) ==
-                       cudaSuccess;
+    }
+    const auto launch = [&] {
         c.stats.kernel_launches += 3;
-        if (!borrow_inputs(c, inputs)) ok = false;
-    }
-    dfree(d_scratch);
-    for (Plan &p : plans) {
-        II_ResultSet *rs = p.rs.get();
-        ok = ok && cudaEventCreateWithFlags(&rs->ready, cudaEventDisableTiming) == cudaSuccess && cudaEventRecord(rs->ready, c.stream) == cudaSuccess;
-        rs->pending = true;
-    }
-    if (!ok) { // nothing is handed out (the frees run in c.stream order behind whatever was enqueued)
-        cudaGetLastError();
-        return -1;
-    }
-    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : cudaStreamLegacy;
-    if (cudaStreamWaitEvent(st, plans.back().rs->ready, 0) != cudaSuccess) {
-        cudaStreamSynchronize(c.stream);
-        return -1;
-    }
-    for (Plan &p : plans) out[p.q] = p.rs.release();
-    if (built) *built = nb;
-    return 0;
+        return ii_launch_filter_and_batch(d.children, d.q, (uint32_t)nb, (uint32_t)total_chunks, d.surv, d.counts, d.offsets, c.stream) ==
+               cudaSuccess;
+    };
+    return publish_pending(c, ok, slot, d_buf, size.tab_bytes, inputs, launch, plans, stream, out, built);
 }
 
 size_t II_ResultSet_Len(const II_ResultSet *rs) {
@@ -2888,57 +2865,75 @@ void II_TermCache_Release(II_TermCache *c, size_t n, II_PostingList *const *list
 // QueryIterator facade (src/iterators/iterator_api.h:46-151 contract)
 // ------------------------------------------------------------------------------------------------
 namespace {
-struct ResultIter {
-    II_QueryIterator base; // MUST be first: RediSearch sees a QueryIterator*
+// What an iterator over a finished result set walks on the host: its docIds, scores and per-hit freq (the sum of the children's),
+// and the result it yields.  load() downloads a set; read / skip_to / rewind follow the QueryIterator contract on `b`.
+struct HostCursor {
     II_IndexResult res;
     std::vector<uint64_t> ids;
-    std::vector<double> scores;
-    std::vector<uint32_t> freq_sum;
+    std::vector<double> scores; // zeros unless loaded with the set's scores
+    std::vector<uint32_t> freq_sum; // empty: every hit yields freq 1
     size_t pos = 0; // index of the NEXT entry to yield
+    bool load(const II_ResultSet *rs, bool with_scores) {
+        const size_t m = rs->len;
+        ids.resize(m);
+        scores.assign(m, 0.0);
+        if (II_ResultSet_Fetch(rs, ids.data(), with_scores ? scores.data() : nullptr, nullptr) != 0) return false;
+        if (rs->has_freqs && m) {
+            std::vector<uint32_t> fr((size_t)rs->n_children * m);
+            if (II_ResultSet_Fetch(rs, nullptr, nullptr, fr.data()) != 0) return false;
+            freq_sum.assign(m, 0);
+            for (uint32_t ch = 0; ch < rs->n_children; ch++)
+                for (size_t i = 0; i < m; i++) freq_sum[i] += fr[(size_t)ch * m + i];
+        }
+        return true;
+    }
+    static IteratorStatus eof(II_QueryIterator *b) {
+        b->atEOF = true;
+        b->current = nullptr;
+        return ITERATOR_EOF;
+    }
+    void publish(II_QueryIterator *b, size_t i) {
+        res.docId = ids[i];
+        res.freq = freq_sum.empty() ? 1u : freq_sum[i];
+        res.data.metric = scores[i];
+        b->lastDocId = ids[i];
+        b->current = &res;
+    }
+    IteratorStatus read(II_QueryIterator *b) {
+        if (pos >= ids.size()) return eof(b);
+        publish(b, pos++);
+        return ITERATOR_OK;
+    }
+    IteratorStatus skip_to(II_QueryIterator *b, t_docId doc) {
+        auto lb = std::lower_bound(ids.begin() + pos, ids.end(), doc);
+        if (lb == ids.end()) {
+            pos = ids.size();
+            return eof(b);
+        }
+        const size_t i = (size_t)(lb - ids.begin());
+        publish(b, i);
+        pos = i + 1;
+        return *lb == doc ? ITERATOR_OK : ITERATOR_NOTFOUND;
+    }
+    void rewind(II_QueryIterator *b) {
+        pos = 0;
+        b->atEOF = false;
+        b->lastDocId = 0;
+        b->current = nullptr;
+    }
+};
+
+struct ResultIter {
+    II_QueryIterator base; // MUST be first: RediSearch sees a QueryIterator*
+    HostCursor cur;
 };
 inline ResultIter *RI(II_QueryIterator *b) { return reinterpret_cast<ResultIter *>(b); }
 
-void ri_publish(ResultIter *it, size_t i) {
-    it->res.docId = it->ids[i];
-    it->res.freq = it->freq_sum.empty() ? 1u : it->freq_sum[i];
-    it->res.data.metric = it->scores[i];
-    it->base.lastDocId = it->ids[i];
-    it->base.current = &it->res;
-}
-size_t ri_num_estimated(const II_QueryIterator *b) { return reinterpret_cast<const ResultIter *>(b)->ids.size(); }
-IteratorStatus ri_read(II_QueryIterator *b) {
-    ResultIter *it = RI(b);
-    if (it->pos >= it->ids.size()) {
-        b->atEOF = true;
-        b->current = nullptr;
-        return ITERATOR_EOF;
-    }
-    ri_publish(it, it->pos++);
-    return ITERATOR_OK;
-}
-IteratorStatus ri_skip_to(II_QueryIterator *b, t_docId doc) {
-    ResultIter *it = RI(b);
-    auto first = it->ids.begin() + it->pos;
-    auto lb = std::lower_bound(first, it->ids.end(), doc);
-    if (lb == it->ids.end()) {
-        it->pos = it->ids.size();
-        b->atEOF = true;
-        b->current = nullptr;
-        return ITERATOR_EOF;
-    }
-    const size_t i = (size_t)(lb - it->ids.begin());
-    ri_publish(it, i);
-    it->pos = i + 1;
-    return *lb == doc ? ITERATOR_OK : ITERATOR_NOTFOUND;
-}
+size_t ri_num_estimated(const II_QueryIterator *b) { return reinterpret_cast<const ResultIter *>(b)->cur.ids.size(); }
+IteratorStatus ri_read(II_QueryIterator *b) { return RI(b)->cur.read(b); }
+IteratorStatus ri_skip_to(II_QueryIterator *b, t_docId doc) { return RI(b)->cur.skip_to(b, doc); }
 ValidateStatus ri_revalidate(II_QueryIterator *, struct IndexSpec *) { return VALIDATE_OK; } // a snapshot never moves
-void ri_rewind(II_QueryIterator *b) {
-    ResultIter *it = RI(b);
-    it->pos = 0;
-    b->atEOF = false;
-    b->lastDocId = 0;
-    b->current = nullptr;
-}
+void ri_rewind(II_QueryIterator *b) { RI(b)->cur.rewind(b); }
 void ri_free(II_QueryIterator *b) { delete RI(b); }
 } // namespace
 
@@ -2947,18 +2942,8 @@ II_QueryIterator *II_NewResultIterator(II_ResultSet *rs, double weight) {
     if (!rs) return nullptr;
     auto *it = new ResultIter();
     memset(&it->base, 0, sizeof(it->base));
-    memset(&it->res, 0, sizeof(it->res));
-    const size_t m = rs->len;
-    it->ids.resize(m);
-    it->scores.assign(m, 0.0);
-    bool ok = II_ResultSet_Fetch(rs, it->ids.data(), it->scores.data(), nullptr) == 0;
-    if (ok && rs->has_freqs && m) {
-        std::vector<uint32_t> fr((size_t)rs->n_children * m);
-        ok = II_ResultSet_Fetch(rs, nullptr, nullptr, fr.data()) == 0;
-        it->freq_sum.assign(m, 0);
-        for (uint32_t ch = 0; ch < rs->n_children; ch++)
-            for (size_t i = 0; i < m; i++) it->freq_sum[i] += fr[(size_t)ch * m + i];
-    }
+    memset(&it->cur.res, 0, sizeof(it->cur.res));
+    const bool ok = it->cur.load(rs, true);
     it->base.type = rs->is_union ? II_IteratorType_Union : II_IteratorType_Intersect;
     it->base.NumEstimated = ri_num_estimated;
     it->base.Read = ri_read;
@@ -2966,9 +2951,9 @@ II_QueryIterator *II_NewResultIterator(II_ResultSet *rs, double weight) {
     it->base.Revalidate = ri_revalidate;
     it->base.Free = ri_free;
     it->base.Rewind = ri_rewind;
-    it->res.data.tag = II_ResultData_Metric;
-    it->res.weight = weight;
-    it->res.fieldMask = ~(unsigned __int128)0; // RS_FIELDMASK_ALL
+    it->cur.res.data.tag = II_ResultData_Metric;
+    it->cur.res.weight = weight;
+    it->cur.res.fieldMask = ~(unsigned __int128)0; // RS_FIELDMASK_ALL
     II_ResultSet_Free(rs);
     if (!ok) {
         delete it;
@@ -3017,13 +3002,8 @@ struct NodeIter {
     double agg_weight = 1.0;
     int scored_with = -1; // II_Scorer the host score array holds
     const II_DocTable *docs = nullptr;
-    // host cursor
-    bool host_ready = false;
-    std::vector<uint64_t> ids;
-    std::vector<double> scores;
-    std::vector<uint32_t> freq_sum;
-    size_t pos = 0;
-    II_IndexResult res;
+    bool host_ready = false; // cur holds rs
+    HostCursor cur;
     ~NodeIter() {
         if (host_term && host_term_free) host_term_free(host_term);
         if (pl) {
@@ -3069,27 +3049,9 @@ bool node_host(NodeIter *it) {
         it->host_ready = true;
         return true;
     }
-    if (!node_materialise(it) || !it->rs) return false;
-    const size_t m = it->rs->len;
-    it->ids.resize(m);
-    it->scores.assign(m, 0.0);
-    if (II_ResultSet_Fetch(it->rs, it->ids.data(), nullptr, nullptr) != 0) return false;
-    if (it->rs->has_freqs && m) {
-        std::vector<uint32_t> fr((size_t)it->rs->n_children * m);
-        if (II_ResultSet_Fetch(it->rs, nullptr, nullptr, fr.data()) != 0) return false;
-        it->freq_sum.assign(m, 0);
-        for (uint32_t ch = 0; ch < it->rs->n_children; ch++)
-            for (size_t i = 0; i < m; i++) it->freq_sum[i] += fr[(size_t)ch * m + i];
-    }
+    if (!node_materialise(it) || !it->rs || !it->cur.load(it->rs, false)) return false;
     it->host_ready = true;
     return true;
-}
-void node_publish(NodeIter *it, size_t i) {
-    it->res.docId = it->ids[i];
-    it->res.freq = it->freq_sum.empty() ? 1u : it->freq_sum[i];
-    it->res.data.metric = it->scores[i];
-    it->base.lastDocId = it->ids[i];
-    it->base.current = &it->res;
 }
 size_t node_num_estimated(const II_QueryIterator *b) {
     const NodeIter *it = reinterpret_cast<const NodeIter *>(b);
@@ -3100,41 +3062,14 @@ size_t node_num_estimated(const II_QueryIterator *b) {
 }
 IteratorStatus node_read(II_QueryIterator *b) {
     NodeIter *it = NI(b);
-    if (!node_host(it) || it->pos >= it->ids.size()) {
-        b->atEOF = true;
-        b->current = nullptr;
-        return ITERATOR_EOF;
-    }
-    node_publish(it, it->pos++);
-    return ITERATOR_OK;
+    return node_host(it) ? it->cur.read(b) : HostCursor::eof(b);
 }
 IteratorStatus node_skip_to(II_QueryIterator *b, t_docId doc) {
     NodeIter *it = NI(b);
-    if (!node_host(it)) {
-        b->atEOF = true;
-        b->current = nullptr;
-        return ITERATOR_EOF;
-    }
-    auto lb = std::lower_bound(it->ids.begin() + it->pos, it->ids.end(), doc);
-    if (lb == it->ids.end()) {
-        it->pos = it->ids.size();
-        b->atEOF = true;
-        b->current = nullptr;
-        return ITERATOR_EOF;
-    }
-    const size_t i = (size_t)(lb - it->ids.begin());
-    node_publish(it, i);
-    it->pos = i + 1;
-    return *lb == doc ? ITERATOR_OK : ITERATOR_NOTFOUND;
+    return node_host(it) ? it->cur.skip_to(b, doc) : HostCursor::eof(b);
 }
 ValidateStatus node_revalidate(II_QueryIterator *, struct IndexSpec *) { return VALIDATE_OK; } // a snapshot never moves
-void node_rewind(II_QueryIterator *b) {
-    NodeIter *it = NI(b);
-    it->pos = 0;
-    b->atEOF = false;
-    b->lastDocId = 0;
-    b->current = nullptr;
-}
+void node_rewind(II_QueryIterator *b) { NI(b)->cur.rewind(b); }
 void node_free(II_QueryIterator *b) { delete NI(b); }
 
 // ---- wildcard (rqe_iterators/src/wildcard.rs:83-180): a counter over 1..top_id yielding one virtual result
@@ -3152,8 +3087,8 @@ IteratorStatus wc_read(II_QueryIterator *b) {
     NodeIter *it = NI(b);
     if (wc_exhausted(it)) return ITERATOR_EOF;
     b->lastDocId += 1;
-    it->res.docId = b->lastDocId;
-    b->current = &it->res;
+    it->cur.res.docId = b->lastDocId;
+    b->current = &it->cur.res;
     return ITERATOR_OK;
 }
 IteratorStatus wc_skip_to(II_QueryIterator *b, t_docId doc) {
@@ -3166,8 +3101,8 @@ IteratorStatus wc_skip_to(II_QueryIterator *b, t_docId doc) {
         return ITERATOR_EOF;
     }
     b->lastDocId = doc;
-    it->res.docId = doc;
-    b->current = &it->res;
+    it->cur.res.docId = doc;
+    b->current = &it->cur.res;
     return ITERATOR_OK;
 }
 void wc_rewind(II_QueryIterator *b) {
@@ -3181,7 +3116,7 @@ void wc_rewind(II_QueryIterator *b) {
 NodeIter *new_node(NodeKind kind, uint32_t type, double weight) {
     auto *it = new NodeIter();
     memset(&it->base, 0, sizeof(it->base));
-    memset(&it->res, 0, sizeof(it->res));
+    memset(&it->cur.res, 0, sizeof(it->cur.res));
     it->kind = kind;
     it->base.type = type;
     it->base.NumEstimated = node_num_estimated;
@@ -3190,13 +3125,13 @@ NodeIter *new_node(NodeKind kind, uint32_t type, double weight) {
     it->base.Revalidate = node_revalidate;
     it->base.Free = node_free;
     it->base.Rewind = node_rewind;
-    it->res.data.tag = II_ResultData_Metric;
-    it->res.weight = weight;
-    it->res.fieldMask = ~(unsigned __int128)0; // RS_FIELDMASK_ALL
+    it->cur.res.data.tag = II_ResultData_Metric;
+    it->cur.res.weight = weight;
+    it->cur.res.fieldMask = ~(unsigned __int128)0; // RS_FIELDMASK_ALL
     // back-pointer for the scoring functions: bytes the Metric variant of the reference's result union does not use
-    memcpy(it->res.data._rest, &kNodeMagic, 8);
+    memcpy(it->cur.res.data._rest, &kNodeMagic, 8);
     NodeIter *self = it;
-    memcpy(it->res.data._rest + 8, &self, 8);
+    memcpy(it->cur.res.data._rest + 8, &self, 8);
     it->docs = g_default_docs;
     if (kind == NODE_EMPTY) it->base.atEOF = false;
     return it;
@@ -3241,7 +3176,7 @@ bool child_view(II_QueryIterator *c, ChildView &v, bool need_offsets) {
         if (n->kind == NODE_WILDCARD) { // every document, as a virtual result with freq 1: a leaf with idf = 1 scores the same
             v.pl = posting_list_all_docs(n->max_doc_id);
             v.temp = true;
-            v.term = II_TermParams{n->res.weight, 1.0, 1.0};
+            v.term = II_TermParams{n->cur.res.weight, 1.0, 1.0};
             return v.pl != nullptr;
         }
         if (n->kind == NODE_RESULT && n->rs) {
@@ -3259,9 +3194,9 @@ bool child_view(II_QueryIterator *c, ChildView &v, bool need_offsets) {
             if (need_offsets) return false;
             // a quick union (no per-child freqs: never scored): its docIds as a flat list
             if (!node_host(n)) return false;
-            std::vector<uint32_t> fr(n->ids.size(), 1u);
-            for (size_t i = 0; i < fr.size() && i < n->freq_sum.size(); i++) fr[i] = n->freq_sum[i];
-            v.pl = II_PostingList_FromArrays(n->ids.data(), fr.data(), n->ids.size());
+            std::vector<uint32_t> fr(n->cur.ids.size(), 1u);
+            for (size_t i = 0; i < fr.size() && i < n->cur.freq_sum.size(); i++) fr[i] = n->cur.freq_sum[i];
+            v.pl = II_PostingList_FromArrays(n->cur.ids.data(), fr.data(), n->cur.ids.size());
             v.temp = true;
             v.term = II_TermParams{n->agg_weight, 1.0, 1.0};
             if (v.pl) v.pl->result_tag = n->rs->is_union ? 1 : 2;
@@ -3307,9 +3242,9 @@ II_QueryIterator *II_NewWildcardIterator(t_docId top_id, double weight) {
     n->base.Read = wc_read;
     n->base.SkipTo = wc_skip_to;
     n->base.Rewind = wc_rewind;
-    n->res.data.tag = II_ResultData_Virtual;
-    memset(n->res.data._rest, 0, sizeof(n->res.data._rest)); // a virtual result carries no payload (and no scorer back-pointer)
-    n->res.freq = 1;
+    n->cur.res.data.tag = II_ResultData_Virtual;
+    memset(n->cur.res.data._rest, 0, sizeof(n->cur.res.data._rest)); // a virtual result carries no payload (and no scorer back-pointer)
+    n->cur.res.freq = 1;
     return &n->base;
 }
 // the reference's own name and signature (RS/headers/iterators_ffi.h:647)
@@ -3541,7 +3476,7 @@ II_QueryIterator *II_NewNotIterator(II_QueryIterator *child, t_docId max_doc_id,
     n->mode = LEAF_NOT;
     n->max_doc_id = max_doc_id;
     n->base.type = 8; // IteratorType_Not
-    n->res.weight = weight;
+    n->cur.res.weight = weight;
     n->term.weight = 0.0; // a NOT child contributes a virtual result: nothing to the score (default.c:289-297)
     return child;
 }
@@ -3552,7 +3487,7 @@ II_QueryIterator *II_NewOptionalIterator(II_QueryIterator *child, t_docId max_do
     n->mode = LEAF_OPTIONAL;
     n->max_doc_id = max_doc_id;
     n->base.type = 10; // IteratorType_Optional
-    n->res.weight = weight;
+    n->cur.res.weight = weight;
     n->term.weight = weight; // optional.rs:260: the weight is applied to real hits only; misses are virtual (score 0)
     return child;
 }
@@ -3831,12 +3766,12 @@ double b200_scorer(const ScoringFunctionArgsC *args, const void *res_v, const vo
         } else if (II_Score(it->rs, (II_Scorer)kScorer, it->terms.data(), it->agg_weight, &st, it->docs, min_score,
                             args->tanhFactor ? args->tanhFactor : 4) != 0)
             return 0.0;
-        if (II_ResultSet_Fetch(it->rs, nullptr, it->scores.data(), nullptr) != 0) return 0.0;
+        if (II_ResultSet_Fetch(it->rs, nullptr, it->cur.scores.data(), nullptr) != 0) return 0.0;
         it->scored_with = kScorer;
     }
     // `res` is the iterator's current result: pos points one past it
-    const size_t i = it->pos ? it->pos - 1 : 0;
-    const double score = i < it->scores.size() ? it->scores[i] : 0.0;
+    const size_t i = it->cur.pos ? it->cur.pos - 1 : 0;
+    const double score = i < it->cur.scores.size() ? it->cur.scores[i] : 0.0;
     if (args->scrExp) {
         // EXPLAINSCORE (src/result_processor.c:582-584 hands the node to the reply, src/score_explain.c:19-21 prints `str`
         // unconditionally): the hit's result tree is read back from the device and explained with the reference's own strings
@@ -3847,10 +3782,10 @@ double b200_scorer(const ScoringFunctionArgsC *args, const void *res_v, const vo
         if (kScorer == II_SCORER_HAMMING) {
             iiexplain::explain_hamming(score, args->qdatalen, ex);
             itemised = true;
-        } else if (i < it->ids.size()) {
+        } else if (i < it->cur.ids.size()) {
             Ctx &c = ctx();
             std::lock_guard<std::mutex> g(c.mu);
-            const uint32_t doc = (uint32_t)it->ids[i];
+            const uint32_t doc = (uint32_t)it->cur.ids[i];
             iiexplain::TreeNode tree;
             iiexplain::DocParams dp;
             dp.avg_doc_len = args->indexStats.avgDocLen;
