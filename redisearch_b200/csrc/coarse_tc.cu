@@ -141,6 +141,10 @@ __device__ __forceinline__ void bulk_load_1d_mc(void *dst, const void *src, uint
         "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"(mask)
         : "memory");
 }
+// pull `bytes` of global memory into L2 ahead of a later bulk copy (no completion to wait for)
+__device__ __forceinline__ void bulk_prefetch_l2(const void *src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
+}
 // address of `local_smem_addr` in the shared memory of CTA `rank` of the cluster
 __device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, uint32_t rank) {
     uint32_t r;
@@ -797,6 +801,12 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         // the shadow copy is stored tile by tile in the swizzled shared-memory image (to_f16_tiled_kernel):
                         // the K blocks of a stage are one contiguous run in HBM
                         const uint8_t *src = shadow + ((size_t)tile * num_kb + kb0) * kQBlockBytes;
+                        // fixed-bound pass: the same slice of the CTA's next tile into L2, so that its bulk copy waits on L2
+                        // rather than HBM.  Only two of the ring's stages can load ahead of the MMAs, which is too little
+                        // to cover HBM latency (DESIGN.md §4.2); one tile ahead is 5.8 MB of L2 at 10M x 768, four thrash it
+                        if constexpr (kFixed) {
+                            if (i + 1 < my_tiles) bulk_prefetch_l2(src + (size_t)gx * num_kb * kQBlockBytes + crank * slice, slice);
+                        }
                         if (csize > 1) {
                             bulk_load_1d_mc(sB + (size_t)s * kQStageBytes + crank * slice, src + crank * slice, slice, &full[s], cmask);
                         } else {
