@@ -572,6 +572,28 @@ int VecSimB200_TopKFilteredBatch(VecSimIndex *index, const void *const *queryBlo
 int VecSimB200_TopKFilteredBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, size_t k, const uint32_t *const *d_doc_ids,
                                        const uint32_t *const *d_counts, const size_t *caps, int64_t *d_out_labels, float *d_out_scores,
                                        uint32_t *d_out_counts, void *stream);
+/* The same batch, each query answered by one of two device routes (the device counterpart of hybrid_reader.c's mode choice,
+ * DESIGN.md §4.10).  HYBRID_ADHOC_BF: the ragged gather of VecSimB200_TopKFilteredBatchDevice.  HYBRID_BATCHES: the fp32
+ * tensor-core route of VecSimB200_TopKQueryBatchDevice (sample pass, fixed-bound main pass, exact rescoring and proof) with the
+ * filter applied to the rows, its open queries finished by the gather.  Every row equals, bit for bit, the row
+ * VecSimB200_TopKFilteredBatchDevice returns for the same query and filter (labels, distances, counts, exact ties at the k-th
+ * place resolved by docId); only the route and its cost differ.  Filter lists must be STRICTLY ascending, as every II_* set is.
+ * Arguments, outputs, stream and return codes are those of VecSimB200_TopKFilteredBatchDevice; in addition -1 for a
+ * queryParams->searchMode other than EMPTY_MODE (0), HYBRID_ADHOC_BF and HYBRID_BATCHES.  batchSize is not read.
+ * queryParams NULL or searchMode 0: each query's route is chosen on the host from its cap, n, dim, k and the queries that would
+ * share the dense pass (DESIGN.md §4.10); HYBRID_ADHOC_BF forces the gather, HYBRID_BATCHES the dense route for every query
+ * where the batch is eligible: a single-value FLOAT32 index in coarse mode 1 with the fixed bound on (VECSIM_B200_FIXED), dim % 8
+ * == 0 in 32..1024, >= 65536 rows within the fp16 range, and 16 dense queries or more unless the fp16 shadow is already built.
+ * Elsewhere every query takes the gather.  out_modes (nullable host [nq]): the route of each query, written before the call
+ * returns.  After a synchronise, VecSimB200_LastCoarseFlags gives per query 1 / 2 = proven by the first / second tier, 0 =
+ * answered by the gather (every ad-hoc query); VecSimB200_LastBatchPath is 1 when any query took the dense route, and the
+ * index's last search mode HYBRID_BATCHES then, else HYBRID_ADHOC_BF.
+ * Host waits: those of VecSimB200_TopKFilteredBatchDevice, and the first build of the fp16 shadow (or its refresh after
+ * mutations).  Launches do not depend on nq: 2 + 2 ceil(k / 128) with no dense query; with dense queries 10 + 2 ceil(k / 128),
+ * +1 for L2 / inner product and +4 for the second tier (on unless VECSIM_B200_TIER2=0). */
+int VecSimB200_HybridTopKBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, size_t k, const uint32_t *const *d_doc_ids,
+                                     const uint32_t *const *d_counts, const size_t *caps, VecSimQueryParams *queryParams, int64_t *d_out_labels,
+                                     float *d_out_scores, uint32_t *d_out_counts, int *out_modes, void *stream);
 /* Batched fp32 queries (cosine, and in mode 1 also L2 and raw inner product; nq >= 16, k <= 16, dim % 8 == 0,
  * >= 65536 rows) take a wgmma coarse
  * pass + exact rescoring from the fp32 rows + a per-query completeness proof, with the exact scan as

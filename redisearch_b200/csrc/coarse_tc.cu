@@ -713,14 +713,19 @@ __device__ __forceinline__ uint32_t select_keep(uint64_t *lists, int q, uint32_t
 //   tile_stride > 1: only every tile_stride-th row tile is visited (the sample pass)
 //   kVar     operand type: 16-bit operands 1 = bfloat16 (else IEEE half); 8-bit 1 = int8 (else uint8).  A template parameter so
 //            that the MMA sequence of a stage is one straight run of wgmma instructions (no branch between them)
-template <bool kDirect, int kEpl, int kOp, int kMode, int kVar = 0>
+//   kFilt    hybrid batches (DESIGN.md §4.10): only rows whose bit is set in the query's row-space bitmap count.  Query q's
+//            bitmap is filt + filt_words * (filt_q ? filt_q[q] : q).  The sample pass takes each chunk's maximum over its
+//            filtered rows; the adaptive lists and the fixed bound admit only filtered rows (the fixed bound tests the bit on
+//            its rare survivor path, after the key test).  fp32 route only.
+template <bool kDirect, int kEpl, int kOp, int kMode, int kVar = 0, bool kFilt = false>
 __global__ void __launch_bounds__(coarse_threads(kMode), 1)
 coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t *__restrict__ shadow, size_t row_pitch,
                     const uint8_t *__restrict__ q16, size_t q16_pitch, const float *__restrict__ row_norm2,
                     const float *__restrict__ q_norm2, uint32_t n_rows, uint32_t nq, uint32_t dim, uint32_t row_bytes,
                     uint32_t num_kb, uint32_t tiles_total, uint32_t keep, uint32_t nstages, uint32_t csize,
                     uint64_t *__restrict__ list_scratch, uint64_t *__restrict__ cand_out, const uint32_t *__restrict__ nq_dev,
-                    uint32_t tile_stride, const float *__restrict__ thr_fixed, uint32_t *__restrict__ overflow) {
+                    uint32_t tile_stride, const float *__restrict__ thr_fixed, uint32_t *__restrict__ overflow,
+                    const uint32_t *__restrict__ filt, uint32_t filt_words, const uint32_t *__restrict__ filt_q) {
     constexpr bool kFixed = kMode == 1, kSample = kMode == 2;
     constexpr bool kInt = kOp == 1 || kOp == 2 || kOp == 4;
     constexpr int kCons = coarse_consumers(kMode), kConsThreads = 128 * kCons;
@@ -729,6 +734,9 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
     const uint32_t bx = blockIdx.x, by = blockIdx.y, gx = gridDim.x;
     static_assert(kMode == 0 || (!kDirect && (kOp == 0 || kOp == 3)) || (kDirect && kOp == 0),
                   "fixed bound / sample pass: the fp32 route and 16-bit corpora (inner product / cosine)");
+    static_assert(!kFilt || (!kDirect && (kOp == 0 || kOp == 3)), "row filters: the fp32 route");
+    // kFilt: the row-space bitmap of the query at position `pos` of this batch
+    auto filt_row = [&](uint32_t pos) { return filt + (size_t)filt_words * (filt_q ? filt_q[pos] : pos); };
     constexpr int kSliceSets = (int)kCoarseSampleSlices / (kQN / 32); // tiles i, i + kSliceSets, ... share a slice set
     constexpr int kQListCap = kEpl * 32;
     if (nq_dev) { // second tier: the number of live queries is only known on the device; nothing to do = every CTA leaves
@@ -1046,7 +1054,11 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         else
                             d = __fsub_rn(__fadd_rn(fnq[i2], __ldg(row_norm2 + row)), __fmul_rn(2.0f, raw));
                         const uint32_t key = orderable_key(d);
-                        if (key < fthr[i2]) {
+                        bool admit = key < fthr[i2];
+                        if constexpr (kFilt) { // a row below the bound enters the list only if the query's filter holds it
+                            if (admit) admit = (__ldg(filt_row(q_base + 16 * ew + (lane >> 2) + 8 * i2) + (row >> 5)) >> (row & 31)) & 1u;
+                        }
+                        if (admit) {
                             const int qs = 16 * ew + (lane >> 2) + 8 * i2;
                             const uint32_t slot = atomicAdd(&qcount[qs], 1u);
                             if (slot < (uint32_t)kQListCap) lists[slot * kQListStride + qs] = ((uint64_t)key << 32) | row;
@@ -1086,11 +1098,21 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
 #pragma unroll
             for (int h = 0; h < kQN / 32; h++) {
                 const uint32_t row0 = tile * kQN + h * 32;
+                // kFilt: the filter's word for the 32 rows of this chunk (no bit is set past the last row)
+                uint32_t fw = 0xFFFFFFFFu;
+                if constexpr (kFilt) fw = (live && row0 < n_rows) ? __ldg(filt_row(q) + (row0 >> 5)) : 0u;
                 if constexpr (kSample) {
                     // largest dot (cosine / inner product) or largest dot - |row|^2 / 2 (squared L2) of the chunk
                     float mx = -__int_as_float(0x7f800000);
                     const bool tail = row0 + 32 > n_rows; // rows past the end (zero fill / stale shadow bytes) must not count
-                    if constexpr (kOp == 0) {
+                    if constexpr (kFilt) { // the maximum over the chunk's filtered rows only
+#pragma unroll
+                        for (int j = 0; j < 32; j++) {
+                            float u = __uint_as_float(v[h][j]);
+                            if constexpr (kOp != 0) u = fmaf(__shfl_sync(0xFFFFFFFFu, nrm[h], j), -0.5f, u);
+                            if ((fw >> j) & 1u) mx = fmaxf(mx, u);
+                        }
+                    } else if constexpr (kOp == 0) {
                         if (!tail) {
                             float m8[8];
 #pragma unroll
@@ -1135,6 +1157,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                     if (p) pass |= 1u << j;
                 }
                 if (row0 + 32 > n_rows) pass &= (n_rows > row0) ? ((1u << (n_rows - row0)) - 1u) : 0u; // TMA zero fill past the end
+                if constexpr (kFilt) pass &= fw;
                 while (pass) {
                     const int j = __ffs(pass) - 1;
                     pass &= pass - 1;
@@ -1365,14 +1388,16 @@ __global__ void __launch_bounds__(256) threshold_kernel(const uint64_t *__restri
 // thr_T == NULL: adaptive lists (a full list's worst kept approximate distance bounds what its row range dropped).
 // thr_T != NULL: lists of the fixed-bound pass — every list holds ALL rows of its range with approx < thr_T[pos] unless
 //                overflow[pos] is set; what was dropped has approx >= thr_T[pos].
-template <int MT, uint32_t kSurv>
+// kLab (hybrid batches, DESIGN.md §4.10): the exact composites carry the row's label row_label[row] instead of the row, so the
+//      answer is the k smallest (distance, docId) — the order of the ragged gather over an ascending filter
+template <int MT, uint32_t kSurv, bool kLab = false>
 __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t pitch, uint32_t dim, const uint8_t *queries,
                                                      size_t qpitch, uint32_t nq, uint32_t lists_per_query, uint32_t keep, uint32_t k,
                                                      const uint64_t *__restrict__ cand, float eps, const float *__restrict__ q_norm2,
                                                      float max_norm, uint32_t *__restrict__ ok, uint32_t ok_value, uint64_t *__restrict__ out,
                                                      const uint32_t *__restrict__ q_index, const uint32_t *__restrict__ nq_dev,
                                                      const float *__restrict__ thr_T, const uint32_t *__restrict__ overflow,
-                                                     uint32_t smem_cap) {
+                                                     uint32_t smem_cap, const uint64_t *__restrict__ row_label) {
     using Tile = DistTile<DT_F32, MT, 1, 1>;
     __shared__ uint64_t surv[kSurv];
     __shared__ uint32_t hist[256];
@@ -1437,7 +1462,7 @@ __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t
         float d[1];
         Tile::run(rowb, qb, dim, lane, d);
         __syncwarp();
-        if (lane == 0) surv[i] = make_composite(d[0], row);
+        if (lane == 0) surv[i] = make_composite(d[0], kLab ? (uint32_t)row_label[row] : row);
     }
     const uint32_t n_sort = max(32u, next_pow2(n_surv));
     __syncthreads();
@@ -1655,13 +1680,21 @@ static const void *wgmma_kernel_fn_v(CoarseKind kind, uint32_t epl, int epi, int
     return nullptr;
 }
 // variant: 16-bit corpora 1 = bf16, 8-bit corpora 1 = int8 (the fp32 route's shadow is always fp16); epi: CoarseOperands::epilogue
-static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, int epi, int mode = 0, uint32_t variant = 0) {
+// filt: the kFilt instantiations (fp32 route; every adaptive-list pass with a filter keeps lists of up to 128)
+static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, int epi, int mode = 0, uint32_t variant = 0, bool filt = false) {
     const bool l2 = epi != 0;
     if (kind == CoarseDirect16 || kind == CoarseDirect8)
         return variant ? wgmma_kernel_fn_v<1>(kind, epl, epi, mode) : wgmma_kernel_fn_v<0>(kind, epl, epi, mode);
     // fp32 route (shadow rows): the flag selects the squared-L2 epilogue; epl 8 = lists of up to 128 (second tier);
     // mode 1 = fixed admission bound (lists of 96, no compaction), mode 2 = the sample pass (slice minima only)
     // (epl 8: lists of 256, k > kCoarseMaxK)
+    if (filt) { // hybrid batches: the same passes with the row filter
+        if (mode == 1 && epl == 8) return l2 ? (const void *)coarse_wgmma_kernel<false, 8, 3, 1, 0, true> : (const void *)coarse_wgmma_kernel<false, 8, 0, 1, 0, true>;
+        if (mode == 1) return l2 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 1, 0, true> : (const void *)coarse_wgmma_kernel<false, 3, 0, 1, 0, true>;
+        if (mode == 2) return l2 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 2, 0, true> : (const void *)coarse_wgmma_kernel<false, 3, 0, 2, 0, true>;
+        if (epl != 8) return nullptr;
+        return l2 ? (const void *)coarse_wgmma_kernel<false, 8, 3, 0, 0, true> : (const void *)coarse_wgmma_kernel<false, 8, 0, 0, 0, true>;
+    }
     if (mode == 1 && epl == 8) return l2 ? (const void *)coarse_wgmma_kernel<false, 8, 3, 1> : (const void *)coarse_wgmma_kernel<false, 8, 0, 1>;
     if (mode == 1) return l2 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 1> : (const void *)coarse_wgmma_kernel<false, 3, 0, 1>;
     if (mode == 2) return l2 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 2> : (const void *)coarse_wgmma_kernel<false, 3, 0, 2>;
@@ -1800,12 +1833,15 @@ static cudaError_t launch_coarse_t(const void *rows, size_t pitch, uint32_t n_ro
 }
 
 cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim, uint32_t nq, const CoarsePlan &p, uint64_t *d_cand,
-                          uint64_t *d_scratch, cudaStream_t s, const uint32_t *d_nq_dev, const float *d_thr_fixed, uint32_t *d_overflow) {
+                          uint64_t *d_scratch, cudaStream_t s, const uint32_t *d_nq_dev, const float *d_thr_fixed, uint32_t *d_overflow,
+                          const uint32_t *d_filt, uint32_t filt_words, const uint32_t *d_filt_q) {
+    if (d_filt && p.kind != CoarseF16) return cudaErrorInvalidValue;
     if (p.kind == CoarseF16 || p.kind == CoarseDirect16 || p.kind == CoarseDirect8) {
         if (p.mode == 1 && (!d_thr_fixed || !d_overflow)) return cudaErrorInvalidValue;
         // operand variant: 16-bit 1 = bf16 (else fp16); 8-bit 1 = int8 (else uint8); the fp16 shadow of the fp32 route: 0
         const uint32_t ev = (p.kind == CoarseDirect16 || p.kind == CoarseDirect8) && o.elem_variant ? 1u : 0u;
-        const void *kfn = wgmma_kernel_fn(p.kind, p.epl, o.epilogue, p.mode, ev);
+        const void *kfn = wgmma_kernel_fn(p.kind, p.epl, o.epilogue, p.mode, ev, d_filt != nullptr);
+        if (!kfn) return cudaErrorInvalidValue;
         cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes);
         if (e != cudaSuccess) {
             fprintf(stderr, "vecsim_b200: coarse pass: %zu bytes of shared memory refused: %s\n", p.smem_bytes, cudaGetErrorString(e));
@@ -1836,7 +1872,8 @@ cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim
         uint32_t a_nrows = n_rows, a_nq = nq, a_dim = dim, a_rb = row_bytes, a_kb = p.num_kb, a_tiles = p.tiles, a_keep = p.keep,
                  a_st = p.stages, a_cs = p.csize, a_stride = p.tile_stride;
         void *args[] = {&mr,   &rows,    &rp,     &qs,   &qp,   &rn2,  &qn2,      &a_nrows, &a_nq,     &a_dim,       &a_rb, &a_kb,
-                        &a_tiles, &a_keep, &a_st, &a_cs, &d_scratch, &d_cand, &d_nq_dev, &a_stride, &d_thr_fixed, &d_overflow};
+                        &a_tiles, &a_keep, &a_st, &a_cs, &d_scratch, &d_cand, &d_nq_dev, &a_stride, &d_thr_fixed, &d_overflow,
+                        &d_filt, &filt_words, &d_filt_q};
         const cudaError_t le = cudaLaunchKernelExC(&cfg, kfn, args);
         if (le != cudaSuccess)
             fprintf(stderr, "vecsim_b200: coarse pass launch failed (kind %d mode %d csize %u grid %u x %u smem %zu): %s\n", (int)p.kind,
@@ -1980,7 +2017,7 @@ cudaError_t launch_to_f16(const void *src, size_t spitch, uint32_t dim, uint32_t
 cudaError_t launch_refine(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t lists_per_query, uint32_t keep,
                           uint32_t k, const uint64_t *d_cand, float eps, const float *d_q_norm2, float max_norm, uint32_t *d_ok,
                           uint64_t *d_out, const uint32_t *d_q_index, const uint32_t *d_nq_dev, cudaStream_t s, const float *d_thr_T,
-                          const uint32_t *d_overflow) {
+                          const uint32_t *d_overflow, const uint64_t *d_row_label) {
     if (nq == 0) return cudaSuccess;
     const uint32_t okv = d_q_index ? 2u : 1u;
     const uint8_t *rows = static_cast<const uint8_t *>(c.rows), *qs = static_cast<const uint8_t *>(d_queries);
@@ -1991,7 +2028,9 @@ cudaError_t launch_refine(const CorpusView &c, const void *d_queries, size_t qpi
     const uint32_t max_cap = wide ? 8192 : 2560;
     const uint32_t smem_cap = std::min<uint32_t>(lists_per_query * keep, max_cap);
     const size_t smem = (size_t)smem_cap * 8;
-    const auto kern = c.metric == MT_L2 ? (wide ? refine_kernel<MT_L2, kRefineMaxSurvWide> : refine_kernel<MT_L2, kRefineMaxSurv>)
+    const auto kern = d_row_label ? (c.metric == MT_L2 ? (wide ? refine_kernel<MT_L2, kRefineMaxSurvWide, true> : refine_kernel<MT_L2, kRefineMaxSurv, true>)
+                                                      : (wide ? refine_kernel<MT_IP, kRefineMaxSurvWide, true> : refine_kernel<MT_IP, kRefineMaxSurv, true>))
+                    : c.metric == MT_L2 ? (wide ? refine_kernel<MT_L2, kRefineMaxSurvWide> : refine_kernel<MT_L2, kRefineMaxSurv>)
                                         : (wide ? refine_kernel<MT_IP, kRefineMaxSurvWide> : refine_kernel<MT_IP, kRefineMaxSurv>);
     // the 48 KB a launch gets without opting in cover static + dynamic shared memory (the wide survivor buffer alone is 32 KB).
     // Opt in to the largest packing this instantiation can ask for, the same value every time: concurrent launches of the same
@@ -2004,7 +2043,7 @@ cudaError_t launch_refine(const CorpusView &c, const void *d_queries, size_t qpi
         if (e != cudaSuccess) return e;
     }
     kern<<<nq, 256, smem, s>>>(rows, c.pitch, c.dim, qs, qpitch, nq, lists_per_query, keep, k, d_cand, eps, d_q_norm2, max_norm, d_ok, okv,
-                               d_out, d_q_index, d_nq_dev, d_thr_T, d_overflow, smem_cap);
+                               d_out, d_q_index, d_nq_dev, d_thr_T, d_overflow, smem_cap, d_row_label);
     return cudaGetLastError();
 }
 

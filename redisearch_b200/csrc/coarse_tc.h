@@ -56,10 +56,13 @@ bool coarse_supported(const CorpusView &c, uint32_t nq, uint32_t k, CoarseKind k
 // keep_override != 0 (CoarseF16 only): candidates per list instead of the default for k
 CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32_t k, uint32_t keep_override = 0, uint32_t tile_stride = 1,
                        int mode = 0);
-// d_nq_dev (nullable): the number of live queries is read from device memory (min with nq); 0 = the kernel exits at once
+// d_nq_dev (nullable): the number of live queries is read from device memory (min with nq); 0 = the kernel exits at once.
+// d_filt (nullable, CoarseF16 only): row filters of a hybrid batch, one bitmap of filt_words u32 per query (bit r = row r); query
+// i of the pass uses bitmap d_filt_q[i] (d_filt_q NULL: bitmap i).  Only filtered rows enter the lists and the sample minima
 cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim, uint32_t nq, const CoarsePlan &p, uint64_t *d_cand,
                           uint64_t *d_scratch, cudaStream_t s, const uint32_t *d_nq_dev = nullptr, const float *d_thr_fixed = nullptr,
-                          uint32_t *d_overflow = nullptr);
+                          uint32_t *d_overflow = nullptr, const uint32_t *d_filt = nullptr, uint32_t filt_words = 0,
+                          const uint32_t *d_filt_q = nullptr);
 // bound of the fixed pass from the sample pass's candidate lists: d_thr[q] = k-th smallest approximate distance + 2 eps;
 // clears d_overflow[q]
 cudaError_t launch_threshold(const uint64_t *d_cand, uint32_t nq, uint32_t lists_per_query, uint32_t keep, uint32_t k, float eps,
@@ -75,11 +78,12 @@ cudaError_t launch_to_f16(const void *src, size_t spitch, uint32_t dim, uint32_t
 // (d_out[q][k], ascending, kEmptySlot padded) and the completeness proof (d_ok[q]).  d_q_norm2 == NULL: unit vectors,
 // |approx - exact| <= eps; otherwise the bound scales with max_norm (over all rows) and |q| (refine_kernel).  Second tier:
 // d_q_index[i] = query of the original batch whose lists sit at position i (d_q_norm2 is indexed by position), *d_nq_dev
-// live positions.
+// live positions.  d_row_label (nullable): the answer's composites carry row_label[row] (a docId) in place of the row, and ties
+// resolve by it.
 cudaError_t launch_refine(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t lists_per_query, uint32_t keep,
                           uint32_t k, const uint64_t *d_cand, float eps, const float *d_q_norm2, float max_norm, uint32_t *d_ok,
                           uint64_t *d_out, const uint32_t *d_q_index, const uint32_t *d_nq_dev, cudaStream_t s,
-                          const float *d_thr_T = nullptr, const uint32_t *d_overflow = nullptr);
+                          const float *d_thr_T = nullptr, const uint32_t *d_overflow = nullptr, const uint64_t *d_row_label = nullptr);
 // direct 16-bit route: d_ok[q] = d_overflow[q] ? 0 : 1
 cudaError_t launch_flags_from_overflow(const uint32_t *d_overflow, uint32_t nq, uint32_t *d_ok, cudaStream_t s);
 // second tier of the direct route: row i of src ([.][k] composites) -> row d_idx[i] of dst, d_ok[d_idx[i]] = 2, for i < *d_count

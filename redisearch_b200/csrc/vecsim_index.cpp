@@ -1900,6 +1900,26 @@ int FlatIndex::topk_filtered_batch(const void *const *queries, size_t nq, size_t
     return rc;
 }
 
+// dev_mu_ held: a staging slot of at least `elems` words whose previous upload has executed (a never-recorded event counts as
+// complete), else a new one; NULL on an allocation failure
+FlatIndex::TableSlot *FlatIndex::table_slot(size_t elems) {
+    for (TableSlot &t : table_ring_)
+        if (t.cap >= elems && cudaEventQuery(t.ev) == cudaSuccess) {
+            cudaGetLastError();
+            return &t;
+        }
+    cudaGetLastError(); // cudaErrorNotReady of a slot in flight is no failure
+    TableSlot t;
+    t.cap = std::max<size_t>(2 * elems, 1024);
+    if (cudaMallocHost(&t.h, t.cap * 8) != cudaSuccess) return nullptr;
+    if (cudaEventCreateWithFlags(&t.ev, cudaEventDisableTiming) != cudaSuccess) {
+        cudaFreeHost(t.h);
+        return nullptr;
+    }
+    table_ring_.push_back(t);
+    return &table_ring_.back();
+}
+
 // The same batch with device pointers end to end (DESIGN.md §4.6): no filter length comes back to the host.  One ragged gather over
 // the flat space of the caps, 2 ceil(k / 128) segmented selects, one unpack: 2 + 2 ceil(k / 128) launches whatever nq.  Selection is
 // by (distance, position in the filter) as in topk_filtered, so every row equals its answer.
@@ -1938,25 +1958,8 @@ int FlatIndex::topk_filtered_batch_device(const void *d_q, size_t nq, size_t k, 
     };
     if (!c->need_cand(layout(nullptr))) return -1;
     layout(c->d_cand);
-    // a staging slot whose previous upload has executed (a never-recorded event counts as complete), else a new one
-    TableSlot *slot = nullptr;
-    for (TableSlot &t : table_ring_)
-        if (t.cap >= tab_elems && cudaEventQuery(t.ev) == cudaSuccess) {
-            slot = &t;
-            break;
-        }
-    cudaGetLastError(); // cudaErrorNotReady of a slot in flight is no failure
-    if (!slot) {
-        TableSlot t;
-        t.cap = std::max<size_t>(2 * tab_elems, 1024);
-        if (cudaMallocHost(&t.h, t.cap * 8) != cudaSuccess) return -1;
-        if (cudaEventCreateWithFlags(&t.ev, cudaEventDisableTiming) != cudaSuccess) {
-            cudaFreeHost(t.h);
-            return -1;
-        }
-        table_ring_.push_back(t);
-        slot = &table_ring_.back();
-    }
+    TableSlot *slot = table_slot(tab_elems);
+    if (!slot) return -1;
     uint64_t *h = slot->h, off = 0, blk = 0;
     for (size_t i = 0; i < nq; i++) {
         h[i] = (uint64_t)(uintptr_t)d_doc_ids[i];
@@ -1977,6 +1980,211 @@ int FlatIndex::topk_filtered_batch_device(const void *d_q, size_t nq, size_t k, 
                                     multi_ ? d_label_rows_ : nullptr, scores, st, &lc) == cudaSuccess;
     ok = ok && launch_topk_ragged(b, scores, (uint32_t)k, parts, cand, out, st, &lc) == cudaSuccess;
     ok = ok && launch_unpack_ragged(b, out, (uint32_t)k, d_labels, d_scores, d_counts_out, st, &lc) == cudaSuccess;
+    launches_total_ += lc.launches;
+    return ok ? 0 : -1;
+}
+
+// Mode choice of a hybrid batch (DESIGN.md §4.10), from what the host already knows.  A query can take the dense route when its cap
+// lets the sample pass meet enough filtered rows: at a filtered fraction f = cap / n the sample must visit tiles_per_k * k / f row
+// tiles, and that must stay within a quarter of the corpus, so cap >= 4 * tiles_per_k * k * 128 (rows per tile).  Those queries
+// take it together when the bytes their gathers would read exceed what the dense route reads: the shadow once (+ the sample
+// pass), the bitmaps and their lists.
+static constexpr double kHybridSampleShare = 0.25;
+static double hybrid_tiles_per_k(uint32_t ke) { return ke > kCoarseMaxK ? 1 / 32.0 : 2.0; }
+static size_t hybrid_cap_floor(uint32_t ke) { return (size_t)std::ceil(hybrid_tiles_per_k(ke) * ke * 128 / kHybridSampleShare); }
+
+int FlatIndex::hybrid_topk_batch_device(const void *d_q, size_t nq, size_t k, const uint32_t *const *d_doc_ids,
+                                        const uint32_t *const *d_counts, const size_t *caps, VecSimQueryParams *qp, int64_t *d_labels,
+                                        float *d_scores, uint32_t *d_counts_out, int *out_modes, cudaStream_t s) {
+    const int policy = qp ? (int)qp->searchMode : (int)EMPTY_MODE;
+    if (policy != EMPTY_MODE && policy != HYBRID_ADHOC_BF && policy != HYBRID_BATCHES) return -1;
+    if (out_modes)
+        for (size_t i = 0; i < nq; i++) out_modes[i] = HYBRID_ADHOC_BF;
+    last_mode_ = HYBRID_ADHOC_BF;
+    if (nq == 0 || k == 0) return 0;
+    if (k > (size_t)kMaxWideK || nq > 0x7FFFFFFFull) return -1;
+    size_t total = 0, max_cap = 0;
+    uint64_t blocks = 0;
+    for (size_t i = 0; i < nq; i++) {
+        if (caps[i] > 0xFFFFFFF0ull) return -2;
+        total += caps[i];
+        max_cap = std::max(max_cap, caps[i]);
+        blocks += ragged_blocks(caps[i]);
+    }
+    if (!flush()) return -1;
+    if (!sync_label_table()) return -2;
+    const size_t n = count_;
+    const uint32_t nq32 = (uint32_t)nq, ke = (uint32_t)std::min<size_t>(k, std::max<size_t>(n, 1));
+    cudaStream_t st = s ? s : cudaStreamLegacy; // NULL = the legacy default stream, as everywhere in CUDA
+    const CorpusView v = view();
+    const bool unit = unit_rows();
+    // the dense route: the fp32 two-pass route of §4.5 over the fp16 shadow (L2 / raw inner product: its norm-scaled bound)
+    const bool eligible = policy != HYBRID_ADHOC_BF && !multi_ && dtype_ == DT_F32 && coarse_mode() == 1 && coarse_fixed_enabled() &&
+                          !coarse_disabled_ && n >= 65536 && coarse_supported(v, 16, ke, CoarseF16);
+    std::vector<uint32_t> dense_q;
+    if (eligible) {
+        const size_t floor_cap = policy == HYBRID_BATCHES ? 0 : hybrid_cap_floor(ke);
+        double gather_bytes = 0, list_bytes = 0;
+        for (size_t i = 0; i < nq; i++)
+            if (caps[i] >= floor_cap) {
+                dense_q.push_back((uint32_t)i);
+                gather_bytes += (double)caps[i] * (double)(stored_bytes_ + 8);
+                list_bytes += (double)caps[i] * 8;
+            }
+        if (policy != HYBRID_BATCHES && !dense_q.empty()) {
+            const double shadow = (double)n * dim_ * 2 * (1 + kHybridSampleShare), bitmaps = (double)dense_q.size() * ((n + 31) / 32) * 4 * 2;
+            if (!(gather_bytes > shadow + bitmaps + list_bytes)) dense_q.clear();
+        }
+        // a subset below the batch route's own 16 queries does not pay for a first shadow build
+        if (dense_q.size() < 16 && !d_shadow_) dense_q.clear();
+        if (!dense_q.empty() && !ensure_shadow(st)) dense_q.clear();
+        if (!dense_q.empty() && !unit && !(shadow_max_abs_ <= 60000.0f)) {
+            dense_q.clear();
+            disable_coarse(); // values outside the fp16 range (or NaN): exact scans from now on, as batch_scan_rows
+        }
+        if (!dense_q.empty() && !sync_labels_to_device()) return -1;
+    }
+    const uint32_t nd = (uint32_t)dense_q.size();
+    if (out_modes)
+        for (uint32_t p : dense_q) out_modes[p] = HYBRID_BATCHES;
+    last_mode_ = nd ? HYBRID_BATCHES : HYBRID_ADHOC_BF;
+    const uint32_t chunk = (uint32_t)std::min<size_t>(k, kMaxFusedK);
+    const uint32_t parts = plan_ragged_select_parts(max_cap, nq32);
+    std::lock_guard<std::mutex> dg(dev_mu_);
+    if (!dev_ctx_) dev_ctx_ = checkout();
+    QueryCtx *c = dev_ctx_.get();
+    if (!c) return -1;
+    // dense-route plans (positions 0 .. nd - 1 = the dense queries in batch order)
+    const bool wide = ke > kCoarseMaxK, tier2 = coarse_tier2_enabled();
+    CoarsePlan cp{}, cps{}, cp2{};
+    const uint32_t words = (uint32_t)((n + 31) / 32);
+    if (nd) {
+        cp = plan_coarse(v, nd, CoarseF16, ke, 0, 1, 1);
+        // the sample must hold a few times k FILTERED rows: at the smallest filtered fraction among the dense queries it visits
+        // tiles_per_k / f times the tiles of the unfiltered route (caps bound the counts from above: a low count only costs time)
+        double fmin = 1.0;
+        for (uint32_t q : dense_q) fmin = std::min(fmin, std::max((double)caps[q] / (double)n, 1e-9));
+        const double tpk = hybrid_tiles_per_k(ke) / fmin;
+        cps = wide ? plan_coarse(v, nd, CoarseF16, ke, kCoarseKeepWide, sample_stride(cp, ke, 128.0, tpk), 0)
+                   : plan_coarse(v, nd, CoarseF16, ke, 0, sample_stride(cp, ke, 24.0, tpk), 2);
+        if (tier2) cp2 = plan_coarse(v, nd, CoarseF16, ke, kCoarseKeepWide);
+    }
+    const size_t qpitch = query_pitch(), q16_pitch = (dim_ * 2 + 15) & ~(size_t)15;
+    // pinned table: [docId pointers nq][count pointers nq][score offsets nq + 1][first chunks nq + 1], then u32 words:
+    // [dense queries nd][dense count 1][dense position of each query nq]
+    const size_t tab_elems = 4 * nq + 2 + (nd + 1 + nq + 1) / 2;
+    uint64_t *tab, *cand, *out, *cand_m, *cand_s, *cand_t2, *out_d, *list_scratch;
+    float *scores, *d_qn2, *d_qn2_t2, *d_thr;
+    uint8_t *q32, *q16, *q16_t2;
+    uint32_t *bm, *d_ok_d, *d_idx, *d_n2, *d_ovf, *d_flags, *d_live;
+    const uint32_t **d_live_ptr;
+    const auto layout = [&](void *base) {
+        BatchScratch sc(base);
+        tab = sc.take<uint64_t>(tab_elems);
+        scores = sc.take<float>(total);
+        cand = sc.take<uint64_t>((size_t)nq * parts * 8 * chunk); // 8 lists (one per warp) per select CTA
+        out = sc.take<uint64_t>(nq * k);
+        d_flags = sc.take<uint32_t>(nq);
+        d_live = sc.take<uint32_t>(nd ? nq : 0);
+        d_live_ptr = sc.take<const uint32_t *>(nd ? nq : 0);
+        bm = sc.take<uint32_t>((size_t)nd * words);
+        q32 = sc.take<uint8_t>((size_t)nd * qpitch);
+        q16 = sc.take<uint8_t>((size_t)nd * q16_pitch);
+        q16_t2 = sc.take<uint8_t>(tier2 ? (size_t)nd * q16_pitch : 0);
+        cand_m = sc.take<uint64_t>((size_t)nd * cp.grid_x * cp.keep);
+        cand_s = sc.take<uint64_t>((size_t)nd * cps.grid_x * cps.keep);
+        cand_t2 = sc.take<uint64_t>(tier2 ? (size_t)nd * cp2.grid_x * cp2.keep : 0);
+        list_scratch = sc.take<uint64_t>(std::max(std::max(cp.scratch_elems, cps.scratch_elems), cp2.scratch_elems));
+        out_d = sc.take<uint64_t>((size_t)nd * ke);
+        d_qn2 = sc.take<float>(unit ? 0 : nd);
+        d_qn2_t2 = sc.take<float>(unit || !tier2 ? 0 : nd);
+        d_ok_d = sc.take<uint32_t>(nd);
+        d_idx = sc.take<uint32_t>(nd);
+        d_n2 = sc.take<uint32_t>(nd ? 1 : 0);
+        d_thr = sc.take<float>(nd);
+        d_ovf = sc.take<uint32_t>(nd);
+        return sc.words();
+    };
+    if (!c->need_cand(layout(nullptr))) return -1;
+    layout(c->d_cand);
+    TableSlot *slot = table_slot(tab_elems);
+    if (!slot) return -1;
+    uint64_t *h = slot->h, off = 0, blk = 0;
+    for (size_t i = 0; i < nq; i++) {
+        h[i] = (uint64_t)(uintptr_t)d_doc_ids[i];
+        h[nq + i] = d_counts ? (uint64_t)(uintptr_t)d_counts[i] : 0;
+        h[2 * nq + i] = off;
+        h[3 * nq + 1 + i] = blk;
+        off += caps[i];
+        blk += ragged_blocks(caps[i]);
+    }
+    h[3 * nq] = off;
+    h[4 * nq + 1] = blk;
+    uint32_t *h32 = reinterpret_cast<uint32_t *>(h + 4 * nq + 2);
+    for (uint32_t p = 0; p < nd; p++) h32[p] = dense_q[p];
+    h32[nd] = nd;
+    for (size_t i = 0; i < nq; i++) h32[nd + 1 + i] = 0xFFFFFFFFu;
+    for (uint32_t p = 0; p < nd; p++) h32[nd + 1 + dense_q[p]] = p;
+    const uint32_t *d_dense_q = reinterpret_cast<const uint32_t *>(tab + 4 * nq + 2), *d_nd = d_dense_q + nd, *d_pos = d_nd + 1;
+    bool ok = cudaMemcpyAsync(tab, h, tab_elems * 8, cudaMemcpyHostToDevice, st) == cudaSuccess;
+    ok = ok && cudaEventRecord(slot->ev, st) == cudaSuccess;
+    const RaggedBatch b{reinterpret_cast<const uint32_t *const *>(tab), reinterpret_cast<const uint32_t *const *>(tab + nq), tab + 2 * nq, nq32};
+    LaunchCounters lc;
+    DenseRows dr;
+    RaggedBatch bg = b; // the gather's batch: every query, or (dense route) the open ones
+    if (nd) {
+        // 1. row-space filter bitmaps of the dense queries; their queries packed to the front (fp32 for the rescoring, fp16 for the GEMM)
+        ok = ok && cudaMemsetAsync(bm, 0, (size_t)nd * words * 4, st) == cudaSuccess;
+        ok = ok && launch_filter_bitmaps(b, d_dense_q, nd, max_cap, d_label_to_id_, (uint32_t)l2i_size_, bm, words, st, &lc) == cudaSuccess;
+        ok = ok && launch_gather_queries(d_q, qpitch, nullptr, d_dense_q, d_nd, nd, q32, nullptr, st) == cudaSuccess;
+        ok = ok && launch_to_f16(q32, qpitch, (uint32_t)dim_, 0, nd, q16, q16_pitch, st) == cudaSuccess;
+        if (!unit) ok = ok && launch_row_stats(q32, qpitch, (uint32_t)dim_, 0, nd, d_qn2, nullptr, st) == cudaSuccess;
+        lc.launches += unit ? 2 : 3;
+        const CoarseOperands ops{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
+        const float eps = coarse_eps(CoarseF16);
+        const int l2 = mkind_ == MT_L2 ? 1 : 0;
+        // 2. sample pass over the filtered rows and the bound; 3. main pass; 4. exact rescoring + proof, selected by (distance, docId)
+        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nd, cps, cand_s, list_scratch, st, nullptr, nullptr, nullptr, bm, words) == cudaSuccess;
+        ok = ok && launch_threshold(cand_s, nd, cps.grid_x, cps.keep, ke, eps, d_qn2, shadow_max_norm_, (uint32_t)dim_, l2, d_thr, d_ovf, st) ==
+                       cudaSuccess;
+        cudaEventRecord(c->ev_start, st);
+        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nd, cp, cand_m, list_scratch, st, nullptr, d_thr, d_ovf, bm, words) == cudaSuccess;
+        cudaEventRecord(c->ev_stop, st);
+        ok = ok && launch_refine(v, q32, qpitch, nd, cp.grid_x, cp.keep, ke, cand_m, eps, d_qn2, shadow_max_norm_, d_ok_d, out_d, nullptr, nullptr, st,
+                                 d_thr, d_ovf, d_id_to_label_) == cudaSuccess;
+        lc.launches += 4;
+        // 5. second tier for the queries whose lists overflowed: adaptive lists of 128 over the filtered rows
+        if (tier2) {
+            ok = ok && launch_compact_unproven(d_ok_d, nd, d_idx, d_n2, st) == cudaSuccess;
+            ok = ok && launch_gather_queries(q16, q16_pitch, d_qn2, d_idx, d_n2, nd, q16_t2, d_qn2_t2, st) == cudaSuccess;
+            CoarseOperands ops2 = ops;
+            ops2.queries = q16_t2;
+            ops2.q_norm2 = d_qn2_t2;
+            ok = ok && launch_coarse(ops2, v.n_rows, v.dim, nd, cp2, cand_t2, list_scratch, st, d_n2, nullptr, nullptr, bm, words, d_idx) ==
+                           cudaSuccess;
+            ok = ok && launch_refine(v, q32, qpitch, nd, cp2.grid_x, cp2.keep, ke, cand_t2, eps, d_qn2_t2, shadow_max_norm_, d_ok_d, out_d, d_idx,
+                                     d_n2, st, nullptr, nullptr, d_id_to_label_) == cudaSuccess;
+            lc.launches += 4;
+        }
+        // 6. the gather answers the ad-hoc queries and the dense ones still open; a proven query's count is 0
+        ok = ok && launch_hybrid_open(b, d_pos, d_ok_d, d_flags, d_live, d_live_ptr, st, &lc) == cudaSuccess;
+        bg.counts = d_live_ptr;
+        dr = DenseRows{out_d, d_pos, d_flags};
+    } else {
+        ok = ok && cudaMemsetAsync(d_flags, 0, nq * 4, st) == cudaSuccess;
+    }
+    // with dense queries in the batch most chunks of the caps are empty: a grid of a few CTAs per SM strides over them
+    const uint64_t max_grid = nd ? (uint64_t)device_sm_count() * 16 : 0;
+    ok = ok && launch_gather_ragged(v, d_q, qpitch, bg, tab + 3 * nq + 1, blocks, d_label_to_id_, (uint32_t)l2i_size_,
+                                    multi_ ? d_label_rows_ : nullptr, scores, st, &lc, max_grid) == cudaSuccess;
+    ok = ok && launch_topk_ragged(bg, scores, (uint32_t)k, parts, cand, out, st, &lc) == cudaSuccess;
+    // 7. one unpack: gather rows map positions to docIds, proven dense rows carry them
+    ok = ok && launch_unpack_ragged(b, out, (uint32_t)k, d_labels, d_scores, d_counts_out, st, &lc, dr) == cudaSuccess;
+    c->d_last_ok = d_flags;
+    c->last_ok_n = nq32;
+    last_batch_coarse_ = true;
+    last_batch_path_ = nd ? 1 : 0;
+    if (nd) coarse_batches_++;
     launches_total_ += lc.launches;
     return ok ? 0 : -1;
 }

@@ -158,6 +158,10 @@ class FlatIndex {
     // the same, device pointers end to end and stream-ordered: VecSimB200_TopKFilteredBatchDevice
     int topk_filtered_batch_device(const void *d_q, size_t nq, size_t k, const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts,
                                    const size_t *caps, int64_t *d_labels, float *d_scores, uint32_t *d_counts_out, cudaStream_t s);
+    // the same rows, each query on the ragged gather or on the filtered tensor-core route: VecSimB200_HybridTopKBatchDevice
+    int hybrid_topk_batch_device(const void *d_q, size_t nq, size_t k, const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts,
+                                 const size_t *caps, VecSimQueryParams *qp, int64_t *d_labels, float *d_scores, uint32_t *d_counts_out,
+                                 int *out_modes, cudaStream_t s);
 
     VecSimIndexBasicInfo basic_info() const;
     VecSimIndexStatsInfo stats_info() const;
@@ -304,6 +308,7 @@ class FlatIndex {
         cudaEvent_t ev = nullptr;
     };
     std::vector<TableSlot> table_ring_;
+    TableSlot *table_slot(size_t elems);
     bool dev_timing_pending_ = false;
     uint64_t dev_timing_bytes_ = 0;
     void collect_dev_timing_locked();

@@ -631,68 +631,74 @@ struct GatherRaggedArgs {
     uint32_t q_smem_pitch;
     RaggedBatch b;
     const uint64_t *blk; // [nq + 1] first CTA of each query (prefix of ragged_blocks over the caps)
+    uint64_t n_blocks;   // blk[nq]: chunks of kRaggedPerBlock entries; a grid of fewer CTAs strides over them
     const uint32_t *table; // single-value: docId -> row (0xFFFFFFFF absent); multi-value: CSR offsets [table_size + 1]
     uint32_t table_size;
     const uint32_t *label_rows; // multi-value: rows of each label in insertion order
     float *scores;
 };
 
-// One CTA = kRaggedPerBlock consecutive entries of ONE query (its blob stays in shared memory), one warp per entry, with the
-// arithmetic of gather_kernel (single-value) / gather_min_kernel's fold (multi-value).  A CTA past its query's device count
-// leaves after reading the count.
+// One chunk = kRaggedPerBlock consecutive entries of ONE query (its blob stays in shared memory), one warp per entry, with the
+// arithmetic of gather_kernel (single-value) / gather_min_kernel's fold (multi-value).  A chunk past its query's device count ends
+// after reading the count.  CTA i takes chunks i, i + gridDim.x, ... (one each when the grid covers them all).
 template <int DT, int MT, bool MULTI>
 __global__ void __launch_bounds__(kScanThreads) gather_ragged_kernel(const GatherRaggedArgs a) {
     extern __shared__ __align__(16) uint8_t smem[];
     using Tile = DistTile<DT, MT, 1, 1>;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint64_t bid = blockIdx.x;
-    uint32_t lo = 0, hi = a.b.nq; // blk[lo] <= bid < blk[hi]: lo is this CTA's query
-    while (hi - lo > 1) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (a.blk[mid] <= bid) lo = mid;
-        else hi = mid;
-    }
-    const uint32_t q = lo;
-    const uint32_t e0 = (uint32_t)(bid - a.blk[q]) * kRaggedPerBlock;
-    const uint32_t n = ragged_count(a.b, q);
-    if (e0 >= n) return;
-    const uint32_t e1 = min(n, e0 + kRaggedPerBlock);
-    const uint8_t *query = a.queries + (size_t)q * a.qpitch;
-    for (uint32_t i = threadIdx.x; i < (a.q_smem_pitch >> 4); i += blockDim.x)
-        reinterpret_cast<uint4 *>(smem)[i] = reinterpret_cast<const uint4 *>(query)[i];
-    __syncthreads();
-    const uint8_t *qb[1] = {smem};
-    const uint32_t *ids = a.b.doc_ids[q];
-    float *out = a.scores + a.b.off[q];
-    for (uint32_t w = e0 + warp; w < e1; w += kScanWarps) {
-        const uint32_t l = ids[w];
-        if (MULTI) {
-            uint32_t r = 0, e = 0;
-            if (l < a.table_size) {
-                r = a.table[l];
-                e = a.table[l + 1];
-            }
-            float dist = r < e ? __uint_as_float(0x7F800000u) : __uint_as_float(0x7FC00000u);
-            uint32_t id = r < e ? a.label_rows[r] : 0u;
+    for (uint64_t bid = blockIdx.x; bid < a.n_blocks; bid += gridDim.x) {
+        uint32_t lo = 0, hi = a.b.nq; // blk[lo] <= bid < blk[hi]: lo is this chunk's query
+        while (hi - lo > 1) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (a.blk[mid] <= bid) lo = mid;
+            else hi = mid;
+        }
+        const uint32_t q = lo;
+        const uint32_t e0 = (uint32_t)(bid - a.blk[q]) * kRaggedPerBlock;
+        const uint32_t n = ragged_count(a.b, q);
+        if (e0 >= n) { // the query's later chunks are past its count too: on to this CTA's first chunk of the next query
+            bid += (a.blk[q + 1] - bid - 1) / gridDim.x * gridDim.x;
+            continue;
+        }
+        const uint32_t e1 = min(n, e0 + kRaggedPerBlock);
+        __syncthreads(); // the previous chunk's reads of the query blob are done
+        const uint8_t *query = a.queries + (size_t)q * a.qpitch;
+        for (uint32_t i = threadIdx.x; i < (a.q_smem_pitch >> 4); i += blockDim.x)
+            reinterpret_cast<uint4 *>(smem)[i] = reinterpret_cast<const uint4 *>(query)[i];
+        __syncthreads();
+        const uint8_t *qb[1] = {smem};
+        const uint32_t *ids = a.b.doc_ids[q];
+        float *out = a.scores + a.b.off[q];
+        for (uint32_t w = e0 + warp; w < e1; w += kScanWarps) {
+            const uint32_t l = ids[w];
+            if (MULTI) {
+                uint32_t r = 0, e = 0;
+                if (l < a.table_size) {
+                    r = a.table[l];
+                    e = a.table[l + 1];
+                }
+                float dist = r < e ? __uint_as_float(0x7F800000u) : __uint_as_float(0x7FC00000u);
+                uint32_t id = r < e ? a.label_rows[r] : 0u;
 #pragma unroll 1
-            for (; r < e; r++) {
+                for (; r < e; r++) {
+                    const uint8_t *rowb[1] = {a.rows + (size_t)id * a.pitch};
+                    if (r + 1 < e) id = a.label_rows[r + 1];
+                    float d[1];
+                    Tile::run(rowb, qb, a.dim, lane, d);
+                    if (lane == 0) dist = (dist < d[0]) ? dist : d[0];
+                }
+                if (lane == 0) out[w] = dist;
+            } else {
+                const uint32_t id = l < a.table_size ? a.table[l] : 0xFFFFFFFFu;
+                if (id == 0xFFFFFFFFu) {
+                    if (lane == 0) out[w] = __uint_as_float(0x7FC00000u);
+                    continue;
+                }
                 const uint8_t *rowb[1] = {a.rows + (size_t)id * a.pitch};
-                if (r + 1 < e) id = a.label_rows[r + 1];
                 float d[1];
                 Tile::run(rowb, qb, a.dim, lane, d);
-                if (lane == 0) dist = (dist < d[0]) ? dist : d[0];
+                if (lane == 0) out[w] = d[0];
             }
-            if (lane == 0) out[w] = dist;
-        } else {
-            const uint32_t id = l < a.table_size ? a.table[l] : 0xFFFFFFFFu;
-            if (id == 0xFFFFFFFFu) {
-                if (lane == 0) out[w] = __uint_as_float(0x7FC00000u);
-                continue;
-            }
-            const uint8_t *rowb[1] = {a.rows + (size_t)id * a.pitch};
-            float d[1];
-            Tile::run(rowb, qb, a.dim, lane, d);
-            if (lane == 0) out[w] = d[0];
         }
     }
 }
@@ -715,25 +721,57 @@ __global__ void __launch_bounds__(kScanThreads) final_select_ragged_kernel(const
 
 // [nq][k] composites (position in the filter, ascending) -> docId labels and distances; NaN distances and empty slots -> -1 / NaN.
 // They sort after every real entry, so a row's real entries are a prefix: counts[q] = its length.
+// Hybrid batches (d.ok != NULL): a query with d.ok[q] != 0 takes row d.pos[q] of d.comp instead, whose composites carry docIds.
 __global__ void unpack_ragged_kernel(const RaggedBatch b, const uint64_t *__restrict__ comp, uint32_t k, int64_t *__restrict__ labels,
-                                     float *__restrict__ scores, uint32_t *__restrict__ counts) {
+                                     float *__restrict__ scores, uint32_t *__restrict__ counts, const DenseRows d) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)b.nq * k) return;
     const uint32_t q = (uint32_t)(i / k), j = (uint32_t)(i - (size_t)q * k);
-    const uint64_t c = comp[i];
+    const bool dense = d.ok && d.ok[q] != 0;
+    const uint64_t *row = dense ? d.comp + (size_t)d.pos[q] * k : comp + (size_t)q * k;
+    const uint64_t c = row[j];
     const bool real = c < ((uint64_t)kNaNKey << 32);
     if (real) {
-        labels[i] = (int64_t)b.doc_ids[q][(uint32_t)c];
+        labels[i] = dense ? (int64_t)(uint32_t)c : (int64_t)b.doc_ids[q][(uint32_t)c];
         scores[i] = key_to_float((uint32_t)(c >> 32));
     } else {
         labels[i] = -1;
         scores[i] = __uint_as_float(0x7FC00000u);
     }
     if (counts) {
-        const bool next_real = j + 1 < k && comp[i + 1] < ((uint64_t)kNaNKey << 32);
+        const bool next_real = j + 1 < k && row[j + 1] < ((uint64_t)kNaNKey << 32);
         if (real && !next_real) counts[q] = j + 1;
         if (j == 0 && !real) counts[q] = 0;
     }
+}
+
+// Row-space filter bitmaps of the dense queries of a hybrid batch (DESIGN.md §4.10): query p of the dense subset (dense_q[p] of the
+// batch) sets bit `row` of bm[p] for every live entry docId -> table[docId] of its list; absent and deleted docIds set nothing.
+// `parts` CTAs per dense query stride over its live entries.  bm must be zero.
+__global__ void __launch_bounds__(256) filter_bitmap_kernel(const RaggedBatch b, const uint32_t *__restrict__ dense_q, uint32_t parts,
+                                                            const uint32_t *__restrict__ table, uint32_t table_size, uint32_t *__restrict__ bm,
+                                                            uint32_t words) {
+    const uint32_t p = blockIdx.x / parts, part = blockIdx.x - p * parts, q = dense_q[p];
+    const uint32_t n = ragged_count(b, q);
+    const uint32_t *ids = b.doc_ids[q];
+    uint32_t *mine = bm + (size_t)p * words;
+    for (uint32_t e = part * blockDim.x + threadIdx.x; e < n; e += parts * blockDim.x) {
+        const uint32_t l = ids[e];
+        const uint32_t row = l < table_size ? table[l] : 0xFFFFFFFFu;
+        if (row != 0xFFFFFFFFu) atomicOr(mine + (row >> 5), 1u << (row & 31));
+    }
+}
+
+// Which queries of a hybrid batch the gather still answers: ok[q] = dense_ok[pos[q]] for a dense query (pos[q] != ~0), else 0;
+// live[q] = 0 for a proven query, else its live filter length, and live_ptr[q] = &live[q] (the counts of the gather's RaggedBatch)
+__global__ void hybrid_open_kernel(const RaggedBatch b, const uint32_t *__restrict__ pos, const uint32_t *__restrict__ dense_ok,
+                                   uint32_t *__restrict__ ok, uint32_t *__restrict__ live, const uint32_t **__restrict__ live_ptr) {
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= b.nq) return;
+    const uint32_t f = pos[q] != 0xFFFFFFFFu ? dense_ok[pos[q]] : 0u;
+    ok[q] = f;
+    live[q] = f ? 0u : ragged_count(b, q);
+    live_ptr[q] = live + q;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1175,19 +1213,20 @@ cudaError_t launch_gather_min_distances(const CorpusView &c, const void *d_query
 }
 
 template <int DT, int MT, bool MULTI>
-static cudaError_t launch_gather_ragged_inst(const GatherRaggedArgs &a, uint64_t n_blocks, cudaStream_t s) {
+static cudaError_t launch_gather_ragged_inst(const GatherRaggedArgs &a, uint64_t grid, cudaStream_t s) {
     auto kern = gather_ragged_kernel<DT, MT, MULTI>;
     cudaError_t e = ensure_smem(kern, a.q_smem_pitch);
     if (e != cudaSuccess) return e;
-    kern<<<(uint32_t)n_blocks, kScanThreads, a.q_smem_pitch, s>>>(a);
+    kern<<<(uint32_t)grid, kScanThreads, a.q_smem_pitch, s>>>(a);
     return cudaGetLastError();
 }
 
 cudaError_t launch_gather_ragged(const CorpusView &c, const void *d_queries, size_t qpitch, const RaggedBatch &b, const uint64_t *d_blk,
                                  uint64_t n_blocks, const uint32_t *d_table, uint32_t table_size, const uint32_t *d_label_rows, float *d_scores,
-                                 cudaStream_t s, LaunchCounters *ctr) {
+                                 cudaStream_t s, LaunchCounters *ctr, uint64_t max_grid) {
     if (n_blocks == 0 || b.nq == 0) return cudaSuccess;
-    if (n_blocks > 0x7FFFFFFFull) return cudaErrorInvalidValue;
+    const uint64_t grid = max_grid ? std::min(n_blocks, max_grid) : n_blocks;
+    if (grid > 0x7FFFFFFFull) return cudaErrorInvalidValue;
     GatherRaggedArgs a{};
     a.rows = static_cast<const uint8_t *>(c.rows);
     a.pitch = c.pitch;
@@ -1197,13 +1236,14 @@ cudaError_t launch_gather_ragged(const CorpusView &c, const void *d_queries, siz
     a.q_smem_pitch = round16(query_blob_bytes(c));
     a.b = b;
     a.blk = d_blk;
+    a.n_blocks = n_blocks;
     a.table = d_table;
     a.table_size = table_size;
     a.label_rows = d_label_rows;
     a.scores = d_scores;
     cudaError_t e = cudaErrorInvalidValue;
 #define CALL_GATHER_RAGGED(DT, MT)                                                                       \
-    e = d_label_rows ? launch_gather_ragged_inst<DT, MT, true>(a, n_blocks, s) : launch_gather_ragged_inst<DT, MT, false>(a, n_blocks, s)
+    e = d_label_rows ? launch_gather_ragged_inst<DT, MT, true>(a, grid, s) : launch_gather_ragged_inst<DT, MT, false>(a, grid, s)
     RSB_DISPATCH_DM(c.dtype, c.metric, CALL_GATHER_RAGGED)
 #undef CALL_GATHER_RAGGED
     if (ctr) ctr->launches++;
@@ -1236,11 +1276,31 @@ cudaError_t launch_topk_ragged(const RaggedBatch &b, const float *d_scores, uint
 }
 
 cudaError_t launch_unpack_ragged(const RaggedBatch &b, const uint64_t *d_comp, uint32_t k, int64_t *d_labels, float *d_scores,
-                                 uint32_t *d_counts, cudaStream_t s, LaunchCounters *ctr) {
+                                 uint32_t *d_counts, cudaStream_t s, LaunchCounters *ctr, const DenseRows &dense) {
     const size_t total = (size_t)b.nq * k;
     if (total == 0) return cudaSuccess;
     if ((total + 255) / 256 > 0x7FFFFFFFull) return cudaErrorInvalidValue;
-    unpack_ragged_kernel<<<(uint32_t)((total + 255) / 256), 256, 0, s>>>(b, d_comp, k, d_labels, d_scores, d_counts);
+    unpack_ragged_kernel<<<(uint32_t)((total + 255) / 256), 256, 0, s>>>(b, d_comp, k, d_labels, d_scores, d_counts, dense);
+    if (ctr) ctr->launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_filter_bitmaps(const RaggedBatch &b, const uint32_t *d_dense_q, uint32_t n_dense, size_t max_cap, const uint32_t *d_table,
+                                  uint32_t table_size, uint32_t *d_bm, uint32_t words, cudaStream_t s, LaunchCounters *ctr) {
+    if (n_dense == 0) return cudaSuccess;
+    // about four CTAs per SM over the dense queries, never more per query than its largest list can feed
+    const uint32_t parts = (uint32_t)std::max<size_t>(1, std::min<size_t>((max_cap + 255) / 256,
+                                                                           std::max(1u, (uint32_t)device_sm_count() * 4u / n_dense)));
+    if ((uint64_t)n_dense * parts > 0x7FFFFFFFull) return cudaErrorInvalidValue;
+    filter_bitmap_kernel<<<n_dense * parts, 256, 0, s>>>(b, d_dense_q, parts, d_table, table_size, d_bm, words);
+    if (ctr) ctr->launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_hybrid_open(const RaggedBatch &b, const uint32_t *d_pos, const uint32_t *d_dense_ok, uint32_t *d_ok, uint32_t *d_live,
+                               const uint32_t **d_live_ptr, cudaStream_t s, LaunchCounters *ctr) {
+    if (b.nq == 0) return cudaSuccess;
+    hybrid_open_kernel<<<(b.nq + 255) / 256, 256, 0, s>>>(b, d_pos, d_dense_ok, d_ok, d_live, d_live_ptr);
     if (ctr) ctr->launches++;
     return cudaGetLastError();
 }

@@ -116,19 +116,35 @@ constexpr uint32_t kRaggedPerBlock = 128; // filter entries per gather CTA
 inline uint64_t ragged_blocks(size_t cap) { return (cap + kRaggedPerBlock - 1) / kRaggedPerBlock; }
 // distances of every live entry: one launch of n_blocks CTAs, d_blk [nq + 1] = prefix of ragged_blocks over the caps.  Single-value
 // index (d_label_rows NULL): d_table maps docId -> row as launch_map_labels; multi-value: CSR offsets over d_label_rows and the fold
-// of launch_gather_min_distances.  d_queries: nq stored-form blobs qpitch bytes apart.
+// of launch_gather_min_distances.  d_queries: nq stored-form blobs qpitch bytes apart.  max_grid != 0: at most that many CTAs stride
+// over the n_blocks chunks (a batch whose counts are mostly 0 does not pay a CTA per chunk of its caps)
 cudaError_t launch_gather_ragged(const CorpusView &c, const void *d_queries, size_t qpitch, const RaggedBatch &b, const uint64_t *d_blk,
                                  uint64_t n_blocks, const uint32_t *d_table, uint32_t table_size, const uint32_t *d_label_rows, float *d_scores,
-                                 cudaStream_t s, LaunchCounters *ctr);
+                                 cudaStream_t s, LaunchCounters *ctr, uint64_t max_grid = 0);
 // CTAs per query of the segmented select (their lists: parts * 8 per query and chunk)
 uint32_t plan_ragged_select_parts(size_t max_cap, uint32_t nq);
 // d_out [nq][k] = each query's k smallest (score, position) composites over its live scores, ascending, kEmptySlot-padded;
 // k <= kMaxWideK in cursor chunks of kMaxFusedK: 2 ceil(k / 128) launches.  d_cand: nq * parts * 8 * min(k, 128) elements.
 cudaError_t launch_topk_ragged(const RaggedBatch &b, const float *d_scores, uint32_t k, uint32_t parts, uint64_t *d_cand, uint64_t *d_out,
                                cudaStream_t s, LaunchCounters *ctr);
+// Answer rows of a hybrid batch's tensor-core route (DESIGN.md §4.10): query q with ok[q] != 0 takes row pos[q] of comp [.][k],
+// composites (distance, docId).  ok NULL: none
+struct DenseRows {
+    const uint64_t *comp = nullptr;
+    const uint32_t *pos = nullptr;
+    const uint32_t *ok = nullptr;
+};
 // d_out -> int64 docIds (-1) and float distances (NaN) for empty or NaN entries; d_counts (nullable) [nq] real entries per query
 cudaError_t launch_unpack_ragged(const RaggedBatch &b, const uint64_t *d_comp, uint32_t k, int64_t *d_labels, float *d_scores,
-                                 uint32_t *d_counts, cudaStream_t s, LaunchCounters *ctr);
+                                 uint32_t *d_counts, cudaStream_t s, LaunchCounters *ctr, const DenseRows &dense = DenseRows{});
+// hybrid batches: bit `row` of d_bm[p] (words u32 per bitmap, zeroed) for every live entry of the list of query d_dense_q[p] whose
+// docId maps to a row through d_table; one launch.  max_cap: the largest cap among those queries
+cudaError_t launch_filter_bitmaps(const RaggedBatch &b, const uint32_t *d_dense_q, uint32_t n_dense, size_t max_cap, const uint32_t *d_table,
+                                  uint32_t table_size, uint32_t *d_bm, uint32_t words, cudaStream_t s, LaunchCounters *ctr);
+// hybrid batches: d_ok[q] = d_dense_ok[d_pos[q]] (0 for d_pos[q] == ~0: an ad-hoc query); d_live[q] = 0 for a proven query, else
+// its live filter length; d_live_ptr[q] = d_live + q, the count table of the gather that answers the open queries
+cudaError_t launch_hybrid_open(const RaggedBatch &b, const uint32_t *d_pos, const uint32_t *d_dense_ok, uint32_t *d_ok, uint32_t *d_live,
+                               const uint32_t **d_live_ptr, cudaStream_t s, LaunchCounters *ctr);
 
 // filter-set plumbing of the fused hybrid query: docId -> row id through a dense table; selected positions -> docIds
 cudaError_t launch_map_labels(const uint32_t *d_labels, uint32_t n, const uint32_t *d_table, uint32_t table_size, uint32_t *d_ids,

@@ -122,6 +122,7 @@ SIGNATURES = [
     ("VecSimIndex_DebugInfo", VecSimIndexDebugInfo, [_P]),
     ("VecSimB200_TopKFilteredBatch", C.c_int, [_P, _P, _SZ, _SZ, _P, _P, _P, _P, _P]),
     ("VecSimB200_TopKFilteredBatchDevice", C.c_int, [_P, _P, _SZ, _SZ, _P, _P, _P, _P, _P, _P, _P]),
+    ("VecSimB200_HybridTopKBatchDevice", C.c_int, [_P, _P, _SZ, _SZ, _P, _P, _P, C.POINTER(VecSimQueryParams), _P, _P, _P, _P, _P]),
     ("VecSimIndex_DebugInfoIterator", _P, [_P]),
     ("VecSimDebugInfoIterator_NumberOfFields", _SZ, [_P]),
     ("VecSimDebugInfoIterator_HasNextField", C.c_bool, [_P]),
@@ -318,6 +319,33 @@ class VecSimIndex:
         rc = self.L.VecSimB200_TopKFilteredBatchDevice(self.h, C.c_void_p(qp), nq, k, ids, cnt, cap_arr, C.c_void_p(out_labels.data_ptr()),
                                                        C.c_void_p(out_scores.data_ptr()), C.c_void_p(out_counts.data_ptr()), sh)
         return out_labels, out_scores, out_counts, rc
+
+    def hybrid_topk_batch_device(self, d_queries, k, doc_ids, caps, counts=None, params=None, out_labels=None, out_scores=None,
+                                 out_counts=None, stream=None):
+        """VecSimB200_HybridTopKBatchDevice: topk_filtered_batch_device's arguments and rows, each query on the ragged gather or
+        the filtered tensor-core route.  params: a VecSimQueryParams whose searchMode picks the policy (None = automatic).
+        Returns (labels, scores, counts, modes, rc); modes[i] = HYBRID_ADHOC_BF or HYBRID_BATCHES, the route query i took."""
+        import torch
+
+        nq = len(caps)
+        dev = torch.device("cuda")
+        if out_labels is None:
+            out_labels = torch.empty((nq, k), dtype=torch.int64, device=dev)
+        if out_scores is None:
+            out_scores = torch.empty((nq, k), dtype=torch.float32, device=dev)
+        if out_counts is None:
+            out_counts = torch.empty(nq, dtype=torch.int32, device=dev)
+        n = max(1, nq)
+        ids = (C.c_void_p * n)(*[int(p) if p else None for p in doc_ids])
+        cnt = (C.c_void_p * n)(*[int(p) if p else None for p in counts]) if counts is not None else None
+        cap_arr = (C.c_size_t * n)(*[int(c) for c in caps])
+        modes = np.zeros(n, dtype=np.int32)
+        qp = d_queries.data_ptr() if hasattr(d_queries, "data_ptr") else int(d_queries)
+        sh = None if stream is None else C.c_void_p(int(getattr(stream, "cuda_stream", stream)) or None)
+        rc = self.L.VecSimB200_HybridTopKBatchDevice(self.h, C.c_void_p(qp), nq, k, ids, cnt, cap_arr,
+                                                     C.byref(params) if params is not None else None, C.c_void_p(out_labels.data_ptr()),
+                                                     C.c_void_p(out_scores.data_ptr()), C.c_void_p(out_counts.data_ptr()), _ptr(modes), sh)
+        return out_labels, out_scores, out_counts, modes[:nq], rc
 
     def query_pitch(self) -> int:
         """bytes between the stored-form query blobs of a device batch"""
