@@ -209,6 +209,30 @@ __device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t adesc, u
           "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
+// the same with A from registers: this thread's fragment of the 64 x 16 A tile, (row r, halves c, c + 1) per register,
+// a = {(r0, c0), (r0 + 8, c0), (r0, c0 + 8), (r0 + 8, c0 + 8)} with r0 = 16 (warp % 4) + lane / 4, c0 = 2 (lane % 4)
+__device__ __forceinline__ void wgmma_f16_n128_ra(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %69, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d));
+}
 __device__ __forceinline__ void wgmma_bf16_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
     asm volatile(
         "{\n"
@@ -717,7 +741,11 @@ __device__ __forceinline__ uint32_t select_keep(uint64_t *lists, int q, uint32_t
 //            bitmap is filt + filt_words * (filt_q ? filt_q[q] : q).  The sample pass takes each chunk's maximum over its
 //            filtered rows; the adaptive lists and the fixed bound admit only filtered rows (the fixed bound tests the bit on
 //            its rare survivor path, after the key test).  fp32 route only.
-template <bool kDirect, int kEpl, int kOp, int kMode, int kVar = 0, bool kFilt = false>
+//   kRegKb   the fixed-bound pass over the fp16 shadow: the first kRegKb K blocks of the CTA's queries are held in registers
+//            (the wgmma A fragment, 16 per K block and thread, loaded once per consumer warpgroup) instead of shared memory,
+//            which frees kRegKb x 8 KB for the ring (DESIGN.md §4.2).  The first kRegKb / kQKbPerStage stages of a tile take
+//            A from those registers; the MMA sequence in K is unchanged, so every distance is the same.  0 = all in sQ.
+template <bool kDirect, int kEpl, int kOp, int kMode, int kVar = 0, bool kFilt = false, int kRegKb = 0>
 __global__ void __launch_bounds__(coarse_threads(kMode), 1)
 coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t *__restrict__ shadow, size_t row_pitch,
                     const uint8_t *__restrict__ q16, size_t q16_pitch, const float *__restrict__ row_norm2,
@@ -735,6 +763,8 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
     static_assert(kMode == 0 || (!kDirect && (kOp == 0 || kOp == 3)) || (kDirect && kOp == 0),
                   "fixed bound / sample pass: the fp32 route and 16-bit corpora (inner product / cosine)");
     static_assert(!kFilt || (!kDirect && (kOp == 0 || kOp == 3)), "row filters: the fp32 route");
+    static_assert(kRegKb == 0 || (!kDirect && kFixed && kRegKb % kQKbPerStage == 0),
+                  "register-held queries: the fixed-bound pass over the fp16 shadow, whole stages");
     // kFilt: the row-space bitmap of the query at position `pos` of this batch
     auto filt_row = [&](uint32_t pos) { return filt + (size_t)filt_words * (filt_q ? filt_q[pos] : pos); };
     constexpr int kSliceSets = (int)kCoarseSampleSlices / (kQN / 32); // tiles i, i + kSliceSets, ... share a slice set
@@ -749,8 +779,8 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
     // so their accesses compile to STS / LDS rather than generic stores and loads
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t *sB = smem;                                                   // nstages x kQKbPerStage x [128 rows x 128B]
-    uint8_t *sQ = sB + (size_t)nstages * kQStageBytes;                    // num_kb x [64 queries x 128B], swizzled
-    uint32_t *sacc = reinterpret_cast<uint32_t *>(sQ + (size_t)num_kb * kQABlockBytes); // [kQM][kQAccStride]; not kFixed
+    uint8_t *sQ = sB + (size_t)nstages * kQStageBytes;                    // K blocks kRegKb .. num_kb - 1 x [64 queries x 128B], swizzled
+    uint32_t *sacc = reinterpret_cast<uint32_t *>(sQ + (size_t)(num_kb - kRegKb) * kQABlockBytes); // [kQM][kQAccStride]; not kFixed
     uint64_t *bars = reinterpret_cast<uint64_t *>(sacc + (kFixed ? 0 : kQM * kQAccStride));
     uint64_t *full = bars, *empty = bars + kQMaxStages;
     uint32_t *qcount = reinterpret_cast<uint32_t *>(bars + 2 * kQMaxStages); // kFixed: [kQM] appends per query
@@ -838,9 +868,9 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         // ===== queries -> shared memory (zero padded to num_kb * 128 bytes and to 64 queries) =====
         if (cw == 0 && et < kQM) {
             const uint4 *src = reinterpret_cast<const uint4 *>(q16 + (size_t)q * q16_pitch);
-            for (uint32_t kb = 0; kb < num_kb; kb++) {
+            for (uint32_t kb = kRegKb; kb < num_kb; kb++) {
                 // row `et` of a K-major 128B-swizzled operand tile: chunk u at et*128 + ((u ^ (et & 7)) * 16)
-                uint8_t *row = sQ + (size_t)kb * kQABlockBytes + et * 128;
+                uint8_t *row = sQ + (size_t)(kb - kRegKb) * kQABlockBytes + et * 128;
 #pragma unroll
                 for (int u = 0; u < 8; u++) {
                     uint4 x = make_uint4(0, 0, 0, 0);
@@ -849,6 +879,24 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                 }
             }
             if constexpr (kFixed) qcount[et] = 0;
+        }
+        // kRegKb: this thread's A fragments of K blocks 0 .. kRegKb - 1 (k16 step t = 4 kb + kk), straight from q16 in every
+        // consumer warpgroup, zero padded as sQ is (query slots >= nq, bytes past the row).  The wgmma.fence in front of
+        // each stage's MMAs orders these register writes before the first MMA that reads them.
+        uint32_t qa[kRegKb ? 4 * kRegKb : 1][4];
+        if constexpr (kRegKb > 0) {
+#pragma unroll
+            for (int i2 = 0; i2 < 2; i2++) {
+                const uint32_t fq = q_base + 16 * ew + (lane >> 2) + 8 * i2;
+                const uint8_t *src = q16 + (size_t)fq * q16_pitch;
+#pragma unroll
+                for (int t = 0; t < 4 * kRegKb; t++)
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        const uint32_t off = 32 * t + 4 * (lane & 3) + 16 * h; // halves 16 t + 2 (lane % 4) + 8 h, + 1
+                        qa[t][i2 + 2 * h] = (fq < nq && off < row_bytes) ? __ldg(reinterpret_cast<const uint32_t *>(src + off)) : 0u;
+                    }
+            }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy writes of sQ -> tensor-core reads
         named_sync<1, kConsThreads>();
@@ -971,18 +1019,15 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
             // ===== D[64 queries x 128 rows] (+)= Q[smem] * rows[smem]^T =====
             Acc acc[64];
             uint32_t prev = 0;
-            for (uint32_t kb0 = 0; kb0 < num_kb; kb0 += kQKbPerStage) {
+            // one ring stage (K blocks kb0, kb0 + 1): wait for it, issue(bd) its MMAs against the stage's B descriptor, hand
+            // the tile on after its last stage, release the stage before
+            auto stage = [&](uint32_t kb0, auto issue) {
                 const long long t_wait = ca.now();
                 mbar_wait_spin(&full[s], ph);
                 const long long t_issue = ca.now();
                 ca.add(kCaWait, t_wait);
                 wg_fence(); // the accumulator registers are handed to the MMA pipe for this stage's run
-                const uint64_t bd = bdesc_first + (uint64_t)s * kStageStep, ad = adesc_first + (uint64_t)kb0 * kABlockStep;
-                // x = 4 j + kk: K block j of the stage, 32-byte step kk inside its swizzled rows
-#pragma unroll
-                for (int x = 0; x < 4 * kQKbPerStage; x++)
-                    wgmma_n128<kInt, kVar>(acc, ad + (x >> 2) * kABlockStep + 2 * (x & 3), bd + (x >> 2) * kBlockStep + 2 * (x & 3),
-                                           (kb0 | (uint32_t)x) != 0);
+                issue(bdesc_first + (uint64_t)s * kStageStep);
                 wg_commit();
                 if constexpr (kCons > 1) { // the tile's last MMAs are issued: the other warpgroup may start the next tile
                     if (kb0 + kQKbPerStage >= num_kb && i + 1 < my_tiles) {
@@ -999,7 +1044,25 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                 if (kb0 != 0) release(prev);
                 prev = s;
                 if (++s == nstages) s = 0, ph ^= 1;
+            };
+            // x = 4 j + kk: K block j of the stage, 32-byte step kk inside its swizzled rows
+            if constexpr (kRegKb > 0) { // K blocks 0 .. kRegKb - 1: A from registers, unrolled so that the indices are static
+#pragma unroll
+                for (int rs = 0; rs < kRegKb / kQKbPerStage; rs++)
+                    stage(rs * kQKbPerStage, [&](uint64_t bd) {
+#pragma unroll
+                        for (int x = 0; x < 4 * kQKbPerStage; x++)
+                            wgmma_f16_n128_ra(acc, qa[4 * kQKbPerStage * rs + x], bd + (x >> 2) * kBlockStep + 2 * (x & 3), (rs | x) != 0);
+                    });
             }
+            for (uint32_t kb0 = kRegKb; kb0 < num_kb; kb0 += kQKbPerStage)
+                stage(kb0, [&](uint64_t bd) {
+                    const uint64_t ad = adesc_first + (uint64_t)(kb0 - kRegKb) * kABlockStep;
+#pragma unroll
+                    for (int x = 0; x < 4 * kQKbPerStage; x++)
+                        wgmma_n128<kInt, kVar>(acc, ad + (x >> 2) * kABlockStep + 2 * (x & 3), bd + (x >> 2) * kBlockStep + 2 * (x & 3),
+                                               (kb0 | (uint32_t)x) != 0);
+                });
             const long long t_epilogue = ca.now();
             wg_wait<0>();
             release(prev);
@@ -1679,12 +1742,23 @@ static const void *wgmma_kernel_fn_v(CoarseKind kind, uint32_t epl, int epi, int
     }
     return nullptr;
 }
+// K blocks of the resident queries that the fixed-bound pass over the fp16 shadow can hold in registers (16 registers per
+// thread each), besides 0: 4 for cosine / inner product with lists of 96 (160 of the launch's 168 registers, no spills).
+// The filtered (112 registers without them), squared-L2 (136) and 256-entry-list passes have no room for 64 more and hold none
+static constexpr uint32_t kFixedRegKb = 4;
+static uint32_t fixed_reg_kb(uint32_t epl, bool l2, bool filt) { return (epl == 3 && !l2 && !filt) ? kFixedRegKb : 0u; }
 // variant: 16-bit corpora 1 = bf16, 8-bit corpora 1 = int8 (the fp32 route's shadow is always fp16); epi: CoarseOperands::epilogue
 // filt: the kFilt instantiations (fp32 route; every adaptive-list pass with a filter keeps lists of up to 128)
-static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, int epi, int mode = 0, uint32_t variant = 0, bool filt = false) {
+// reg_kb: the fixed-bound pass with that many K blocks of the queries in registers (fixed_reg_kb), else 0
+static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, int epi, int mode = 0, uint32_t variant = 0, bool filt = false,
+                                   uint32_t reg_kb = 0) {
     const bool l2 = epi != 0;
     if (kind == CoarseDirect16 || kind == CoarseDirect8)
         return variant ? wgmma_kernel_fn_v<1>(kind, epl, epi, mode) : wgmma_kernel_fn_v<0>(kind, epl, epi, mode);
+    if (reg_kb) {
+        if (mode != 1 || reg_kb != fixed_reg_kb(epl, l2, filt)) return nullptr;
+        return (const void *)coarse_wgmma_kernel<false, 3, 0, 1, 0, false, kFixedRegKb>;
+    }
     // fp32 route (shadow rows): the flag selects the squared-L2 epilogue; epl 8 = lists of up to 128 (second tier);
     // mode 1 = fixed admission bound (lists of 96, no compaction), mode 2 = the sample pass (slice minima only)
     // (epl 8: lists of 256, k > kCoarseMaxK)
@@ -1701,10 +1775,14 @@ static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, int epi, int m
     if (l2) return epl == 3 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 0> : (const void *)coarse_wgmma_kernel<false, 8, 3, 0>;
     return epl == 3 ? (const void *)coarse_wgmma_kernel<false, 3, 0, 0> : (const void *)coarse_wgmma_kernel<false, 8, 0, 0>;
 }
-// shared memory of coarse_wgmma_kernel besides the ring: the resident queries, the accumulator transpose (the
-// fixed-bound pass, mode 1, tests the accumulators in registers and keeps a counter per query instead), the barriers
-static size_t wgmma_fixed_smem(uint32_t num_kb, int mode = 0) {
-    return 1024 + (size_t)num_kb * kQABlockBytes + (mode == 1 ? kQM * 4 : kQAccBytes) + 2 * kQMaxStages * 8 + 64;
+// shared memory of coarse_wgmma_kernel besides the ring: the resident queries (less the reg_kb K blocks held in registers), the
+// accumulator transpose (the fixed-bound pass, mode 1, tests the accumulators in registers and keeps a counter per query
+// instead), the barriers
+static size_t wgmma_fixed_smem(uint32_t num_kb, int mode = 0, uint32_t reg_kb = 0) {
+    return 1024 + (size_t)(num_kb - reg_kb) * kQABlockBytes + (mode == 1 ? kQM * 4 : kQAccBytes) + 2 * kQMaxStages * 8 + 64;
+}
+static uint32_t wgmma_stages(uint32_t num_kb, int mode, uint32_t reg_kb) {
+    return (uint32_t)std::min<size_t>(kQMaxStages, (kSmemLimit - wgmma_fixed_smem(num_kb, mode, reg_kb)) / kQStageBytes);
 }
 // the 16/8-bit kernel needs at least two ring stages next to the resident queries (1024 fp16 dimensions fit)
 static bool wgmma_fits_bytes(uint32_t row_bytes) { return wgmma_fixed_smem(coarse_kb(row_bytes)) + 2 * (size_t)kQStageBytes <= kSmemLimit; }
@@ -1743,7 +1821,7 @@ bool coarse_supported(const CorpusView &c, uint32_t nq, uint32_t k, CoarseKind k
 }
 
 CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32_t k, uint32_t keep_override, uint32_t tile_stride,
-                       int mode) {
+                       int mode, bool filt) {
     CoarsePlan p{};
     p.kind = kind;
     p.tile_stride = std::max(1u, tile_stride);
@@ -1764,8 +1842,22 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
         if (p.mode == 1 && kind == CoarseDirect16) p.keep = kCoarseFixedCapDirect, p.epl = 8;
         if (p.mode == 2) p.keep = kCoarseSampleSlices, p.epl = 3; // the slice minima
         p.threads = (uint32_t)coarse_threads(p.mode);
-        p.stages = (uint32_t)std::min<size_t>(kQMaxStages, (kSmemLimit - wgmma_fixed_smem(p.num_kb, p.mode)) / kQStageBytes);
-        p.smem_bytes = wgmma_fixed_smem(p.num_kb, p.mode) + (size_t)p.stages * kQStageBytes;
+        const int epi = kind == CoarseF16 ? (c.metric == MT_L2 ? 1 : 0) : c.metric == MT_COS ? 1 : (kind == CoarseDirect8 && c.metric == MT_L2) ? 2 : 0;
+        // the fixed-bound pass over the shadow holds the leading K blocks of its queries in registers where that frees shared
+        // memory for one more ring stage and leaves at least one stage of queries in shared memory
+        static int rcap = -1; // VECSIM_B200_REGKB caps the register-held K blocks (0 = none)
+        if (rcap < 0) {
+            const char *e = getenv("VECSIM_B200_REGKB");
+            rcap = e ? std::max(0, atoi(e)) : (int)kFixedRegKb;
+        }
+        p.reg_kb = 0;
+        if (kind == CoarseF16 && p.mode == 1) {
+            const uint32_t rk = fixed_reg_kb(p.epl, epi != 0, filt);
+            if (rk && (int)rk <= rcap && p.num_kb >= rk + kQKbPerStage && wgmma_stages(p.num_kb, p.mode, rk) > wgmma_stages(p.num_kb, p.mode, 0))
+                p.reg_kb = rk;
+        }
+        p.stages = wgmma_stages(p.num_kb, p.mode, p.reg_kb);
+        p.smem_bytes = wgmma_fixed_smem(p.num_kb, p.mode, p.reg_kb) + (size_t)p.stages * kQStageBytes;
         // the query groups of a row range form a thread-block cluster (multicast of the row tiles)
         p.csize = 1;
         static int ccap = -1; // VECSIM_B200_CLUSTER caps the cluster size (1 = no clusters)
@@ -1778,8 +1870,7 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
                 p.csize = cs;
                 break;
             }
-        const int epi = kind == CoarseF16 ? (c.metric == MT_L2 ? 1 : 0) : c.metric == MT_COS ? 1 : (kind == CoarseDirect8 && c.metric == MT_L2) ? 2 : 0;
-        const void *kfn = wgmma_kernel_fn(kind, p.epl, epi, p.mode, (c.dtype == DT_BF16 || c.dtype == DT_I8) ? 1u : 0u);
+        const void *kfn = wgmma_kernel_fn(kind, p.epl, epi, p.mode, (c.dtype == DT_BF16 || c.dtype == DT_I8) ? 1u : 0u, filt, p.reg_kb);
         if (p.csize > 1) {
             cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes);
             cudaLaunchConfig_t cfg{};
@@ -1840,7 +1931,7 @@ cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim
         if (p.mode == 1 && (!d_thr_fixed || !d_overflow)) return cudaErrorInvalidValue;
         // operand variant: 16-bit 1 = bf16 (else fp16); 8-bit 1 = int8 (else uint8); the fp16 shadow of the fp32 route: 0
         const uint32_t ev = (p.kind == CoarseDirect16 || p.kind == CoarseDirect8) && o.elem_variant ? 1u : 0u;
-        const void *kfn = wgmma_kernel_fn(p.kind, p.epl, o.epilogue, p.mode, ev, d_filt != nullptr);
+        const void *kfn = wgmma_kernel_fn(p.kind, p.epl, o.epilogue, p.mode, ev, d_filt != nullptr, p.reg_kb);
         if (!kfn) return cudaErrorInvalidValue;
         cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes);
         if (e != cudaSuccess) {

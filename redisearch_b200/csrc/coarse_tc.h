@@ -35,6 +35,7 @@ struct CoarsePlan {
     uint32_t tile_stride; // 1 = every row tile; n = every n-th (the sample pass)
     int mode;        // CoarseF16: 0 adaptive top-`keep` lists, 1 fixed admission bound per query (main pass), 2 sample pass (slice minima)
     uint32_t csize;  // thread-block cluster size along y (query groups sharing multicast row tiles); 1 = none
+    uint32_t reg_kb; // CoarseF16 mode 1: leading K blocks of the resident queries held in registers (0 = all in shared memory)
     size_t cand_elems; // uint64 per (query, list, keep)
     size_t scratch_elems; // uint64 of per-CTA candidate-list scratch (CoarseF16), 0 otherwise
     size_t smem_bytes;
@@ -53,9 +54,10 @@ struct CoarseOperands {
     const float *q_norm2;   //                 |q|^2 per query;                CoarseDirect8 / L2: exact int32 |q|^2 per query
 };
 bool coarse_supported(const CorpusView &c, uint32_t nq, uint32_t k, CoarseKind kind);
-// keep_override != 0 (CoarseF16 only): candidates per list instead of the default for k
+// keep_override != 0 (CoarseF16 only): candidates per list instead of the default for k.  filt: the pass is launched with row
+// filters (launch_coarse's d_filt)
 CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32_t k, uint32_t keep_override = 0, uint32_t tile_stride = 1,
-                       int mode = 0);
+                       int mode = 0, bool filt = false);
 // d_nq_dev (nullable): the number of live queries is read from device memory (min with nq); 0 = the kernel exits at once.
 // d_filt (nullable, CoarseF16 only): row filters of a hybrid batch, one bitmap of filt_words u32 per query (bit r = row r); query
 // i of the pass uses bitmap d_filt_q[i] (d_filt_q NULL: bitmap i).  Only filtered rows enter the lists and the sample minima

@@ -2059,7 +2059,7 @@ int FlatIndex::hybrid_topk_batch_device(const void *d_q, size_t nq, size_t k, co
     CoarsePlan cp{}, cps{}, cp2{};
     const uint32_t words = (uint32_t)((n + 31) / 32);
     if (nd) {
-        cp = plan_coarse(v, nd, CoarseF16, ke, 0, 1, 1);
+        cp = plan_coarse(v, nd, CoarseF16, ke, 0, 1, 1, true);
         // the sample must hold a few times k FILTERED rows: at the smallest filtered fraction among the dense queries it visits
         // tiles_per_k / f times the tiles of the unfiltered route (caps bound the counts from above: a low count only costs time)
         double fmin = 1.0;
