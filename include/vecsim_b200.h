@@ -459,6 +459,27 @@ int VecSimB200_TopKQueryBatchDevice(VecSimIndex *index, const void *d_queries, s
 int VecSimB200_RangeQueryBatch(VecSimIndex *index, const void *queryBlobs, size_t qstride, size_t nq,
                                const double *radii, VecSimQueryParams *queryParams,
                                VecSimQueryReply_Order order, VecSimQueryReply **replies, uint32_t *out_flags);
+/* nq range queries with DEVICE pointers end to end (DESIGN.md §4.11).  d_queries: stored-form blobs as for
+ * VecSimB200_TopKQueryBatchDevice; d_radii: one float per query, in DistType.  Query i's answer is every row with
+ * score <= d_radii[i] (a float compare: -0.0 == +0.0, a NaN score never passes, a NaN radius keeps nothing).  A negative
+ * radius is answered as given (inner-product distances can be negative), where VecSimB200_RangeQueryBatch refuses it.
+ * d_out_counts[i] = the true number of hits, even past cap.  count <= cap: entries [0, count) of row i of d_out_labels /
+ * d_out_scores ([nq][cap], int64 / float) hold them, BY_SCORE ordered by (score, label), BY_ID by label, as
+ * VecSimIndex_RangeQuery orders its reply; the rest of the row is label -1, score NaN.  count > cap: the whole row is -1 / NaN
+ * (re-issue the query with a larger cap, or use VecSimB200_RangeQueryBatch).
+ * Routes: single-value fp32 batches the fp32 route of VecSimB200_RangeQueryBatch serves take it; int8 / uint8 batches of
+ * >= 16 queries (dim % 16 == 0, 32..2048, >= 65536 rows, coarse mode 1 or 2, VECSIM_B200_FIXED not 0) take a fixed-radius
+ * pass on the integer tensor cores, whose distances are the reference's; every other query, and every query a route cannot
+ * complete, takes the exact scan on the device.  The call only enqueues on `stream` (NULL = the legacy default stream); the
+ * host waits only for the first build of the fp16 shadow / the int32 |row|^2 table of 8-bit L2 indexes or their refresh
+ * after mutations.  After a synchronise, VecSimB200_LastCoarseFlags gives 1 per query a tensor-core route answered and 0 per
+ * query the exact scan answered; VecSimB200_LastBatchPath is 1 (fp32 route), 2 (8-bit route) or 0 (exact scan only).  The
+ * scratch is that of VecSimB200_TopKQueryBatchDevice.
+ * Returns 0 (0 with nothing enqueued for nq == 0); -1 for a multi-value index, cap == 0 or cap > 4096, an order other than
+ * BY_ID / BY_SCORE, or a CUDA failure. */
+int VecSimB200_RangeQueryBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, const float *d_radii, size_t cap,
+                                     VecSimQueryReply_Order order, int64_t *d_out_labels, float *d_out_scores,
+                                     uint32_t *d_out_counts, void *stream);
 /* Bulk ingest of n host blobs (stride bytes apart) with labels[i] (NULL -> label0+i).  Equivalent
  * to n VecSimIndex_AddVector calls on fresh labels, with one H2D transfer per staging buffer. */
 int VecSimB200_AddVectors(VecSimIndex *index, const void *blobs, size_t stride, size_t n,

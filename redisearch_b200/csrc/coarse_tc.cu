@@ -710,6 +710,19 @@ __device__ __forceinline__ uint32_t select_keep(uint64_t *lists, int q, uint32_t
     return prefix;
 }
 
+// Fixed-radius pass over 8-bit corpora: the largest integer x with (float)x <= r, the pre-test bound of the integer distances
+// (1 - dot for inner product, the int32 e of L2).  int -> float rounding is monotone, so {x : (float)x <= r} is the set of
+// integers up to that x and `x <= range_int_bound(r)` is exactly `(float)x <= r` for |x| < 2^30 (8-bit distances stay below
+// 2^29).  floor(r) is in the set (below 2^24 it is exact; above, r is itself an integer); the loop adds the integers above r
+// that round down to it (at most half an ulp of r, 64 at 2^30).  NaN: nothing passes; beyond +-2^30: everything / nothing.
+__device__ __forceinline__ int range_int_bound(float r) {
+    if (!(r == r) || r < -1073741824.0f) return INT_MIN;
+    if (r >= 1073741824.0f) return INT_MAX;
+    int x = (int)floorf(r);
+    while (__int2float_rn(x + 1) <= r) x++;
+    return x;
+}
+
 // kDirect = false: fp32 corpus, rows come from the tiled fp16 shadow (bulk copies), output = sorted candidate lists for
 //                  the exact rescoring + proof.
 // kDirect = true : fp16 / bf16 corpus, rows come straight from the row-major corpus through a 128B-swizzle tensor
@@ -728,7 +741,9 @@ __device__ __forceinline__ uint32_t select_keep(uint64_t *lists, int q, uint32_t
 //            65025 * dim <= 1.4e8 at the widest 8-bit dim (2048): no int32 overflow.
 //   kFixed   the admission threshold of every query is FIXED for the whole pass (thr_fixed[q], a distance, from the sample
 //            pass): every row with approximate distance < thr_fixed[q] is kept — no running threshold, no list compaction;
-//            a list that runs full sets overflow[q] (the query goes to the next tier).  fp32 route only (kOp 0 / 3).
+//            a list that runs full sets overflow[q] (the query goes to the next tier).  fp32 route (kOp 0 / 3) and 16-bit
+//            corpora.  8-bit corpora (kOp 1 / 2 / 4): thr_fixed[q] is the radius of a range query and a row is kept iff its
+//            exact float distance d satisfies d <= thr_fixed[q] (range_int_bound for the pre-tests, DESIGN.md §4.11).
 //   kSample  the sample pass: no lists at all — every thread keeps the smallest approximate distance it has seen in each of
 //            8 interleaved slices of its row range (chunk of the tile x tile parity) and publishes those 8 values as
 //            keep = 8 composites per (query, row range).  The k-th smallest of a query's lists x 8 minima is an upper
@@ -760,8 +775,8 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
     using Acc = typename std::conditional<kInt, uint32_t, float>::type;
     // bx = row range, by = query group
     const uint32_t bx = blockIdx.x, by = blockIdx.y, gx = gridDim.x;
-    static_assert(kMode == 0 || (!kDirect && (kOp == 0 || kOp == 3)) || (kDirect && kOp == 0),
-                  "fixed bound / sample pass: the fp32 route and 16-bit corpora (inner product / cosine)");
+    static_assert(kMode == 0 || (!kDirect && (kOp == 0 || kOp == 3)) || (kDirect && kOp == 0) || (kDirect && kFixed && kInt && kEpl == 8),
+                  "fixed bound / sample pass: the fp32 route and 16-bit corpora (inner product / cosine); fixed radius: 8-bit corpora");
     static_assert(!kFilt || (!kDirect && (kOp == 0 || kOp == 3)), "row filters: the fp32 route");
     static_assert(kRegKb == 0 || (!kDirect && kFixed && kRegKb % kQKbPerStage == 0),
                   "register-held queries: the fixed-bound pass over the fp16 shadow, whole stages");
@@ -932,7 +947,26 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         // fq[i2] = 16 ew + lane / 4 + 8 i2 (i2 = 0, 1) against 32 rows of each tile
         uint32_t fthr[2];
         float fthr_dot[2], fnq[2];
-        if constexpr (kFixed) {
+        // 8-bit fixed radius: the radius, the integer bound of the inner-product / L2 pre-test, |q|^2 (L2)
+        float frad[2];
+        int fix[2], fnqi[2];
+        if constexpr (kFixed && kInt) {
+#pragma unroll
+            for (int i2 = 0; i2 < 2; i2++) {
+                const uint32_t fq = q_base + 16 * ew + (lane >> 2) + 8 * i2;
+                const bool flive = fq < nq;
+                frad[i2] = flive ? thr_fixed[fq] : __int_as_float(0x7fffffff); // slots without a query: a NaN radius keeps nothing
+                fix[i2] = range_int_bound(frad[i2]);
+                fnqi[i2] = (kOp == 4 && flive) ? reinterpret_cast<const int *>(q_norm2)[fq] : 0;
+                // cosine: d = 1 - fl(D / fl(nr nq)) with D = fl(dot).  d <= r implies D >= nr nq (t - 1.3e-7 (1 + |r|)), t = 1 - r
+                // (relative rounding 2^-24 of the subtraction, the division, D and the norm product, |D / P| <= 1 + 4 ulp by
+                // Cauchy-Schwarz on rows that carry their own norm).  The pre-test D >= fl(nr fthr_dot) with fthr_dot =
+                // fl(nq fl(t - 1e-6 (1 + |r|))) rounds three more times (< 2.4e-7 (1 + |r|) nr nq) and so never drops such a row.
+                fnq[i2] = (kOp == 2 && flive) ? *reinterpret_cast<const float *>(q16 + (size_t)fq * q16_pitch + dim) : 0.0f;
+                fthr_dot[i2] = fnq[i2] * ((1.0f - frad[i2]) - 1e-6f * (1.0f + fabsf(frad[i2])));
+            }
+        }
+        if constexpr (kFixed && !kInt) {
 #pragma unroll
             for (int i2 = 0; i2 < 2; i2++) {
                 const uint32_t fq = q_base + 16 * ew + (lane >> 2) + 8 * i2;
@@ -1068,7 +1102,78 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
             release(prev);
             wg_fence_operands(acc);
             // accumulator fragment: acc[4j + 2 i2 + c] = (query 16 ew + lane / 4 + 8 i2, row 8 j + 2 (lane % 4) + c)
-            if constexpr (kFixed) {
+            if constexpr (kFixed && kInt) {
+                // 8-bit fixed radius: a conservative pre-test on the integer dot products (exact for inner product and L2,
+                // range_int_bound), then the epilogue's own float distance and the range test d <= r on the rare survivors.
+                // Every entry of a list is a hit with its final distance; a list that runs full sets the overflow flag.
+                uint32_t pass2[2] = {0u, 0u}; // bit 2 j + c: acc[4 j + 2 i2 + c]
+                if constexpr (kOp == 1) { // 1 - dot <= X  <=>  dot >= 1 - X: one compare against the largest dot decides most rows
+#pragma unroll
+                    for (int i2 = 0; i2 < 2; i2++) {
+                        int mx = (int)acc[2 * i2];
+#pragma unroll
+                        for (int x = 1; x < 32; x++) mx = max(mx, (int)acc[4 * (x >> 1) + 2 * i2 + (x & 1)]);
+                        if (1 - mx <= fix[i2]) {
+#pragma unroll
+                            for (int x = 0; x < 32; x++)
+                                if (1 - (int)acc[4 * (x >> 1) + 2 * i2 + (x & 1)] <= fix[i2]) pass2[i2] |= 1u << x;
+                        }
+                    }
+                } else { // per row: |row|^2 (L2) or the row norm (cosine) from the lane that loaded it
+#pragma unroll
+                    for (int j = 0; j < kQN / 8; j++)
+#pragma unroll
+                        for (int c = 0; c < 2; c++) {
+                            const int src = 8 * (j & 3) + 2 * (lane & 3) + c; // row 8 j + 2 (lane % 4) + c of the tile
+                            if constexpr (kOp == 4) {
+                                const int rn = __shfl_sync(0xFFFFFFFFu, inrm[j >> 2], src);
+#pragma unroll
+                                for (int i2 = 0; i2 < 2; i2++)
+                                    if (rn + fnqi[i2] - 2 * (int)acc[4 * j + 2 * i2 + c] <= fix[i2]) pass2[i2] |= 1u << (2 * j + c);
+                            } else {
+                                const float nr = __shfl_sync(0xFFFFFFFFu, nrm[j >> 2], src);
+#pragma unroll
+                                for (int i2 = 0; i2 < 2; i2++)
+                                    if (__int2float_rn((int)acc[4 * j + 2 * i2 + c]) >= nr * fthr_dot[i2]) pass2[i2] |= 1u << (2 * j + c);
+                            }
+                        }
+                }
+#pragma unroll
+                for (int i2 = 0; i2 < 2; i2++) {
+                    uint32_t pass = pass2[i2];
+                    if (pass && tile * kQN + kQN > n_rows) { // rows past the end (TMA zero fill)
+#pragma unroll
+                        for (int x = 0; x < 32; x++)
+                            if (rbase + 8 * (x >> 1) + (x & 1) >= n_rows) pass &= ~(1u << x);
+                    }
+                    while (pass) {
+                        const int b = __ffs(pass) - 1;
+                        pass &= pass - 1;
+                        uint32_t raw = 0;
+#pragma unroll
+                        for (int x = 0; x < 32; x++)
+                            if (x == b) raw = acc[4 * (x >> 1) + 2 * i2 + (x & 1)];
+                        const uint32_t row = rbase + 8 * (b >> 1) + (b & 1);
+                        float d; // the expressions of the adaptive-list epilogue below
+                        if constexpr (kOp == 1) {
+                            d = (float)(1 - (int)raw);
+                        } else if constexpr (kOp == 2) {
+                            const float nr = __ldg(reinterpret_cast<const float *>(shadow + (size_t)row * row_pitch + dim));
+                            d = __fsub_rn(1.0f, __fdiv_rn((float)(int)raw, __fmul_rn(nr, fnq[i2])));
+                        } else {
+                            d = __int2float_rn(__ldg(irn2 + row) + fnqi[i2] - 2 * (int)raw);
+                        }
+                        if (d <= frad[i2]) { // the reference's inclusive range test: NaN never passes, -0 == +0
+                            const int qs = 16 * ew + (lane >> 2) + 8 * i2;
+                            const uint32_t slot = atomicAdd(&qcount[qs], 1u);
+                            if (slot < (uint32_t)kQListCap) lists[slot * kQListStride + qs] = ((uint64_t)orderable_key(d) << 32) | row;
+                        }
+                    }
+                }
+                ca.add(kCaEpilogue, t_epilogue);
+                continue;
+            }
+            if constexpr (kFixed && !kInt) {
                 // With a fixed bound only ~k * (rows / sample rows) rows of the whole corpus pass: for each of its two
                 // queries the thread takes the max of its 32 values and ONE compare decides the common case.  The rare
                 // survivors take the exact distance and key comparison and append to the query's list, unordered, at a
@@ -1603,7 +1708,7 @@ __global__ void __launch_bounds__(256) range_refine_kernel(const uint8_t *rows, 
                                                            const float *__restrict__ q_norm2, const float *__restrict__ thr,
                                                            const uint32_t *__restrict__ overflow, uint64_t *__restrict__ out,
                                                            uint32_t *__restrict__ total, uint32_t *__restrict__ ok, uint32_t *__restrict__ cnt,
-                                                           uint32_t *__restrict__ off) {
+                                                           uint32_t *__restrict__ off, uint32_t cap) {
     using Tile = DistTile<DT_F32, MT, 1, 1>;
     __shared__ uint64_t s_cand[kRangeWindow];
     __shared__ uint32_t s_n, s_kept, s_base;
@@ -1612,7 +1717,8 @@ __global__ void __launch_bounds__(256) range_refine_kernel(const uint8_t *rows, 
     bool proven = overflow[q] == 0 && isfinite(thr[q]);
     if (q_norm2 && !(q_norm2[q] == q_norm2[q])) proven = false;
     if (!proven) { // the same for every thread of the CTA
-        if (threadIdx.x == 0) ok[q] = 0, cnt[q] = 0, off[q] = 0;
+        if (threadIdx.x == 0) ok[q] = 0, cnt[q] = 0;
+        if (threadIdx.x == 0 && !cap) off[q] = 0;
         return;
     }
     const float r = radius[q];
@@ -1644,6 +1750,11 @@ __global__ void __launch_bounds__(256) range_refine_kernel(const uint8_t *rows, 
         __syncthreads();
     }
     const uint32_t kept = s_kept;
+    if (cap) { // device range batches: the hits into the query's own cap slots, the true count even past cap
+        if (threadIdx.x == 0) ok[q] = 1, cnt[q] = kept;
+        for (uint32_t i = threadIdx.x; i < min(kept, cap); i += blockDim.x) out[(size_t)q * cap + i] = mine[i];
+        return;
+    }
     if (threadIdx.x == 0) {
         s_base = atomicAdd(total, kept);
         ok[q] = 1;
@@ -1652,6 +1763,31 @@ __global__ void __launch_bounds__(256) range_refine_kernel(const uint8_t *rows, 
     }
     __syncthreads();
     for (uint32_t i = threadIdx.x; i < kept; i += blockDim.x) out[s_base + i] = mine[i];
+}
+
+// Fixed-radius pass over 8-bit corpora, one CTA per query: every real entry of its `slots` list entries is a hit with its final
+// distance, so they are only packed into out[q][0, cap) (unordered) and counted, the count kept past cap.  ok[q] = 1 unless a
+// list overflowed; an overflowed query writes cnt[q] = 0 and nothing else.
+__global__ void __launch_bounds__(256) range_pack_kernel(const uint64_t *__restrict__ cand, uint32_t slots, const uint32_t *__restrict__ overflow,
+                                                         uint32_t cap, uint64_t *__restrict__ out, uint32_t *__restrict__ cnt,
+                                                         uint32_t *__restrict__ ok) {
+    __shared__ uint32_t s_n;
+    const uint32_t q = blockIdx.x;
+    if (overflow[q]) {
+        if (threadIdx.x == 0) ok[q] = 0, cnt[q] = 0;
+        return;
+    }
+    if (threadIdx.x == 0) s_n = 0;
+    __syncthreads();
+    const uint64_t *mine = cand + (size_t)q * slots;
+    for (uint32_t i = threadIdx.x; i < slots; i += blockDim.x) {
+        const uint64_t c = mine[i];
+        if (c == kEmptySlot) continue;
+        const uint32_t pos = atomicAdd(&s_n, 1u);
+        if (pos < cap) out[(size_t)q * cap + pos] = c;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) ok[q] = 1, cnt[q] = s_n;
 }
 
 // indices of the queries the first tier left unproven, densely packed: idx[0, *count)
@@ -1736,6 +1872,10 @@ static const void *wgmma_kernel_fn_v(CoarseKind kind, uint32_t epl, int epi, int
         return epl == 3 ? (const void *)coarse_wgmma_kernel<true, 3, 0, 0, V> : (const void *)coarse_wgmma_kernel<true, 8, 0, 0, V>;
     }
     if (kind == CoarseDirect8) {
+        if (mode == 1) { // fixed radius (range batches), lists of 256
+            if (epi == 2) return (const void *)coarse_wgmma_kernel<true, 8, 4, 1, V>;
+            return epi == 1 ? (const void *)coarse_wgmma_kernel<true, 8, 2, 1, V> : (const void *)coarse_wgmma_kernel<true, 8, 1, 1, V>;
+        }
         if (epi == 2) return epl == 3 ? (const void *)coarse_wgmma_kernel<true, 3, 4, 0, V> : (const void *)coarse_wgmma_kernel<true, 8, 4, 0, V>;
         if (epi == 1) return epl == 3 ? (const void *)coarse_wgmma_kernel<true, 3, 2, 0, V> : (const void *)coarse_wgmma_kernel<true, 8, 2, 0, V>;
         return epl == 3 ? (const void *)coarse_wgmma_kernel<true, 3, 1, 0, V> : (const void *)coarse_wgmma_kernel<true, 8, 1, 0, V>;
@@ -1825,7 +1965,8 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
     CoarsePlan p{};
     p.kind = kind;
     p.tile_stride = std::max(1u, tile_stride);
-    p.mode = (kind == CoarseF16 || (kind == CoarseDirect16 && c.metric == MT_IP)) ? mode : 0;
+    // 8-bit corpora: the fixed-radius pass of range batches (mode 1) only
+    p.mode = (kind == CoarseF16 || (kind == CoarseDirect16 && c.metric == MT_IP)) ? mode : (kind == CoarseDirect8 && mode == 1) ? 1 : 0;
     if (kind == CoarseF16 || kind == CoarseDirect16 || kind == CoarseDirect8) {
         p.num_kb = coarse_kb(kind == CoarseDirect8 ? c.dim : c.dim * 2);
         p.tiles = ((c.n_rows + kQN - 1) / kQN + p.tile_stride - 1) / p.tile_stride; // row tiles this pass visits
@@ -1839,7 +1980,7 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
         p.epl = p.keep <= 32 ? 3 : 8;
         if (p.mode == 1 && kind == CoarseF16) // every row below the bound, up to the list capacity
             p.keep = k > kCoarseMaxK ? kCoarseFixedCapWide : kCoarseFixedCap, p.epl = k > kCoarseMaxK ? 8 : 3;
-        if (p.mode == 1 && kind == CoarseDirect16) p.keep = kCoarseFixedCapDirect, p.epl = 8;
+        if (p.mode == 1 && (kind == CoarseDirect16 || kind == CoarseDirect8)) p.keep = kCoarseFixedCapDirect, p.epl = 8;
         if (p.mode == 2) p.keep = kCoarseSampleSlices, p.epl = 3; // the slice minima
         p.threads = (uint32_t)coarse_threads(p.mode);
         const int epi = kind == CoarseF16 ? (c.metric == MT_L2 ? 1 : 0) : c.metric == MT_COS ? 1 : (kind == CoarseDirect8 && c.metric == MT_L2) ? 2 : 0;
@@ -2182,15 +2323,21 @@ cudaError_t launch_range_bound(const float *d_radius, uint32_t nq, float eps, co
 }
 cudaError_t launch_range_refine(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t slots, uint64_t *d_cand,
                                 const float *d_radius, const float *d_q_norm2, const float *d_thr, const uint32_t *d_overflow, uint64_t *d_out,
-                                uint32_t *d_total, uint32_t *d_ok, uint32_t *d_cnt, uint32_t *d_off, cudaStream_t s) {
+                                uint32_t *d_total, uint32_t *d_ok, uint32_t *d_cnt, uint32_t *d_off, cudaStream_t s, uint32_t cap) {
     if (nq == 0) return cudaSuccess;
     const uint8_t *rows = static_cast<const uint8_t *>(c.rows), *qs = static_cast<const uint8_t *>(d_queries);
     if (c.metric == MT_L2)
         range_refine_kernel<MT_L2><<<nq, 256, 0, s>>>(rows, c.pitch, c.dim, qs, qpitch, slots, d_cand, d_radius, d_q_norm2, d_thr, d_overflow,
-                                                      d_out, d_total, d_ok, d_cnt, d_off);
+                                                      d_out, d_total, d_ok, d_cnt, d_off, cap);
     else
         range_refine_kernel<MT_IP><<<nq, 256, 0, s>>>(rows, c.pitch, c.dim, qs, qpitch, slots, d_cand, d_radius, d_q_norm2, d_thr, d_overflow,
-                                                      d_out, d_total, d_ok, d_cnt, d_off);
+                                                      d_out, d_total, d_ok, d_cnt, d_off, cap);
+    return cudaGetLastError();
+}
+cudaError_t launch_range_pack(const uint64_t *d_cand, uint32_t nq, uint32_t slots, const uint32_t *d_overflow, uint32_t cap, uint64_t *d_out,
+                              uint32_t *d_cnt, uint32_t *d_ok, cudaStream_t s) {
+    if (nq == 0) return cudaSuccess;
+    range_pack_kernel<<<nq, 256, 0, s>>>(d_cand, slots, d_overflow, cap, d_out, d_cnt, d_ok);
     return cudaGetLastError();
 }
 cudaError_t launch_gather_queries(const void *d_src, size_t pitch, const float *d_src_n2, const uint32_t *d_idx, const uint32_t *d_count,

@@ -103,10 +103,16 @@ cudaError_t launch_range_bound(const float *d_radius, uint32_t nq, float eps, co
 // range batches, one CTA per query over its `slots` list entries of the main pass (d_cand, overwritten): exact rescoring and
 // the inclusive test d <= d_radius[q].  Query q's hits go to d_out[d_off[q], d_off[q] + d_cnt[q]) (composites, unordered;
 // d_out holds nq * slots); d_ok[q] = 1 if the answer is proven complete, else 0 with d_cnt[q] = 0.  d_q_norm2 == NULL: unit
-// rows.
+// rows.  cap != 0 (device range batches): query q's hits go to d_out[q * cap, q * cap + min(d_cnt[q], cap)) instead, d_cnt[q] the
+// true count; d_total and d_off are not used.
 cudaError_t launch_range_refine(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t slots, uint64_t *d_cand,
                                 const float *d_radius, const float *d_q_norm2, const float *d_thr, const uint32_t *d_overflow, uint64_t *d_out,
-                                uint32_t *d_total, uint32_t *d_ok, uint32_t *d_cnt, uint32_t *d_off, cudaStream_t s);
+                                uint32_t *d_total, uint32_t *d_ok, uint32_t *d_cnt, uint32_t *d_off, cudaStream_t s, uint32_t cap = 0);
+// fixed-radius pass over 8-bit corpora (launch_coarse on a CoarseDirect8 plan of mode 1, d_thr_fixed = the radii): the real
+// entries of query q's `slots` list entries -> d_out[q * cap, ...) unordered, d_cnt[q] = their number (past cap too), d_ok[q] = 1;
+// a query whose lists overflowed: d_ok[q] = 0, d_cnt[q] = 0
+cudaError_t launch_range_pack(const uint64_t *d_cand, uint32_t nq, uint32_t slots, const uint32_t *d_overflow, uint32_t cap, uint64_t *d_out,
+                              uint32_t *d_cnt, uint32_t *d_ok, cudaStream_t s);
 // |row|^2 of fp32 rows [first, first+n) into d_norm2[first..], NaN for a row whose fp16 form is not finite (a component
 // with |x| >= 65520, or NaN: refine_kernel never proves such a query); d_stats (nullable) = {max |row|^2, max |x|} as float bits
 cudaError_t launch_row_stats(const void *rows, size_t pitch, uint32_t dim, uint32_t first, uint32_t n, float *d_norm2, uint32_t *d_stats,

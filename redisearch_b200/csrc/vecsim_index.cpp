@@ -1504,6 +1504,119 @@ int FlatIndex::range_batch(const void *qs, size_t qstride, size_t nq, const doub
     return rc;
 }
 
+// Device range batches (DESIGN.md §4.11): one route per batch, then the exact scan on the device for the queries it left open
+// (or for the whole batch), then one CTA per query orders its hits and maps rows to labels.  Hits are gathered as composites in
+// d_labels itself ([nq][cap] uint64) with the true count in d_counts.  Nothing waits on the host except ensure_shadow.
+int FlatIndex::range_batch_device(const void *d_q, size_t nq, const float *d_radii, size_t cap, VecSimQueryReply_Order order, int64_t *d_labels,
+                                  float *d_scores, uint32_t *d_counts, cudaStream_t s) {
+    if (multi_ || cap == 0 || cap > kRangeDeviceMaxCap || (order != BY_ID && order != BY_SCORE) || nq > 0xFFFFFFFFu) return -1;
+    last_mode_ = RANGE_QUERY;
+    if (nq == 0) return 0;
+    if (!flush() || !sync_labels_to_device()) return -1;
+    const size_t n = count_;
+    std::lock_guard<std::mutex> dg(dev_mu_);
+    if (!dev_ctx_) dev_ctx_ = checkout();
+    QueryCtx *c = dev_ctx_.get();
+    if (!c) return -1;
+    collect_dev_timing_locked();
+    cudaStream_t st = s ? s : cudaStreamLegacy;
+    const uint32_t nq32 = (uint32_t)nq, cap32 = (uint32_t)cap;
+    const size_t qpitch = query_pitch();
+    const CorpusView v = view();
+    const int cmode = coarse_mode();
+    const bool is8 = dtype_ == DT_I8 || dtype_ == DT_U8;
+    // 1: the fp32 route of range_batch (same eligibility); 2: the fixed-radius pass over 8-bit rows; 0: the exact scan only
+    int path = 0;
+    if (n > 0 && is8 && cmode != 0 && nq >= 16 && coarse_fixed_enabled() && coarse_supported(v, nq32, 1, CoarseDirect8) &&
+        (!int_l2() || ensure_shadow(st))) {
+        path = 2;
+    } else if (n > 0 && cmode == 1 && dtype_ == DT_F32 && !coarse_disabled_ && coarse_fixed_enabled() && coarse_supported(v, nq32, 1, CoarseF16) &&
+               (nq >= 16 || single_query_takes_coarse(1)) && ensure_shadow(st)) {
+        path = 1;
+        if (!unit_rows() && !(shadow_max_abs_ <= 60000.0f)) { // values outside the fp16 range: exact scans from now on
+            disable_coarse();
+            path = 0;
+        }
+    }
+    const bool unit = unit_rows();
+    const CoarsePlan cp = path == 1 ? plan_coarse(v, nq32, CoarseF16, 1, 0, 1, 1) : path == 2 ? plan_coarse(v, nq32, CoarseDirect8, 1, 0, 1, 1)
+                                                                                             : CoarsePlan{};
+    const size_t slots = (size_t)cp.grid_x * cp.keep, q16_pitch = (dim_ * 2 + 15) & ~(size_t)15;
+    const WidePlan wp = n > 0 ? plan_topk_wide(v.n_rows, nq32) : WidePlan{};
+    uint64_t *cand, *list_scratch;
+    uint8_t *q16;
+    float *d_qn2, *d_thr;
+    uint32_t *d_ok, *d_idx, *d_n2, *d_ovf, *d_total;
+    const auto layout = [&](void *base) {
+        BatchScratch sc(base);
+        cand = sc.take<uint64_t>(path ? nq * slots : 0);
+        list_scratch = sc.take<uint64_t>(path ? cp.scratch_elems : 0);
+        q16 = sc.take<uint8_t>(path == 1 ? nq * q16_pitch : 0);
+        d_qn2 = sc.take<float>((path == 1 && !unit) || (path == 2 && int_l2()) ? nq : 0); // |q|^2 (fp32), or int32 for 8-bit L2
+        d_thr = sc.take<float>(path == 1 ? nq : 0);
+        d_ovf = sc.take<uint32_t>(path ? nq : 0);
+        d_total = sc.take<uint32_t>(1);
+        d_ok = sc.take<uint32_t>(nq);  // reported flags
+        d_idx = sc.take<uint32_t>(nq); // the open queries
+        d_n2 = sc.take<uint32_t>(1);   // and their count
+        return sc.words();
+    };
+    if (!c->need_cand(layout(nullptr)) || (n > 0 && !c->need_scores(wp.score_elems))) return -1;
+    layout(c->d_cand);
+    LaunchCounters lc;
+    uint64_t *comp = reinterpret_cast<uint64_t *>(d_labels);
+    bool ok = cudaMemsetAsync(d_counts, 0, nq * 4, st) == cudaSuccess && cudaMemsetAsync(d_ok, 0, nq * 4, st) == cudaSuccess;
+    // the timed span (VecSimB200_GetStats): the route's main pass, or the exact scan of a batch no route serves
+    if (path == 1) {
+        ok = ok && launch_to_f16(d_q, qpitch, (uint32_t)dim_, 0, nq32, q16, q16_pitch, st) == cudaSuccess;
+        if (!unit) ok = ok && launch_row_stats(d_q, qpitch, (uint32_t)dim_, 0, nq32, d_qn2, nullptr, st) == cudaSuccess;
+        ok = ok && launch_range_bound(d_radii, nq32, kCoarseEpsF16, d_qn2, shadow_max_norm_, (uint32_t)dim_, mkind_ == MT_L2 ? 1 : 0, d_thr, d_ovf,
+                                      d_total, st) == cudaSuccess;
+        const CoarseOperands ops{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
+        cudaEventRecord(c->ev_start, st);
+        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_thr, d_ovf) == cudaSuccess;
+        cudaEventRecord(c->ev_stop, st);
+        ok = ok && launch_range_refine(v, d_q, qpitch, nq32, (uint32_t)slots, cand, d_radii, d_qn2, d_thr, d_ovf, comp, d_total, d_ok, d_counts,
+                                       nullptr, st, cap32) == cudaSuccess;
+        lc.launches += unit ? 4 : 5;
+    } else if (path == 2) {
+        CoarseOperands ops{v.rows, v.pitch, d_q, qpitch, dtype_ == DT_I8 ? 1 : 0, mkind_ == MT_COS ? 1 : int_l2() ? 2 : 0, nullptr, nullptr};
+        ok = ok && cudaMemsetAsync(d_ovf, 0, nq * 4, st) == cudaSuccess;
+        if (int_l2()) {
+            ok = ok && launch_int_norm2(d_q, qpitch, v.dim, 0, nq32, dtype_ == DT_I8, reinterpret_cast<int32_t *>(d_qn2), st) == cudaSuccess;
+            ops.row_norm2 = reinterpret_cast<const float *>(d_norm2_); // int32 values (CoarseOperands)
+            ops.q_norm2 = d_qn2;
+            lc.launches++;
+        }
+        cudaEventRecord(c->ev_start, st);
+        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_radii, d_ovf) == cudaSuccess;
+        cudaEventRecord(c->ev_stop, st);
+        ok = ok && launch_range_pack(cand, nq32, (uint32_t)slots, d_ovf, cap32, comp, d_counts, d_ok, st) == cudaSuccess;
+        lc.launches += 2;
+    }
+    if (n > 0) {
+        // the exact scan: the queries a route left open (compacted on the device; none open = every launch exits at once), or all
+        if (path) {
+            ok = ok && launch_compact_unproven(d_ok, nq32, d_idx, d_n2, st) == cudaSuccess;
+            lc.launches++;
+        }
+        if (!path) cudaEventRecord(c->ev_start, st);
+        ok = ok && launch_range_wide(v, d_q, qpitch, nq32, path ? d_idx : nullptr, path ? d_n2 : nullptr, wp, c->d_scores, d_radii, cap32, comp,
+                                     d_counts, c->d_abort, st, &lc) == cudaSuccess;
+        if (!path) cudaEventRecord(c->ev_stop, st);
+    }
+    ok = ok && launch_range_finish(d_labels, d_scores, d_counts, nq32, cap32, d_id_to_label_, order == BY_ID, st, &lc) == cudaSuccess;
+    c->d_last_ok = d_ok;
+    c->last_ok_n = nq32;
+    last_batch_coarse_ = true; // LastCoarseFlags: 1 = a tensor-core route answered the query, 0 = the exact scan
+    last_batch_path_ = path;
+    if (path) coarse_batches_++;
+    dev_timing_pending_ = ok && n > 0;
+    dev_timing_bytes_ = (uint64_t)n * stored_bytes_;
+    launches_total_ += lc.launches;
+    return ok ? 0 : -1;
+}
+
 double FlatIndex::distance_from(size_t label, const void *blob) {
     const double nan = std::numeric_limits<double>::quiet_NaN();
     std::vector<idType> ids;

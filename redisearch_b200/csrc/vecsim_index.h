@@ -142,6 +142,9 @@ class FlatIndex {
     // answered there, 0 for one answered by range().  Arguments are validated by the caller.
     int range_batch(const void *qs, size_t qstride, size_t nq, const double *radii, VecSimQueryParams *qp, VecSimQueryReply_Order order,
                     VecSimQueryReply **replies, uint32_t *out_flags);
+    // the same with device pointers end to end, stream-ordered: VecSimB200_RangeQueryBatchDevice (DESIGN.md §4.11)
+    int range_batch_device(const void *d_q, size_t nq, const float *d_radii, size_t cap, VecSimQueryReply_Order order, int64_t *d_labels,
+                           float *d_scores, uint32_t *d_counts, cudaStream_t s);
     double distance_from(size_t label, const void *stored_form_blob);
     bool prefer_adhoc(size_t subset, size_t k, bool initial);
 

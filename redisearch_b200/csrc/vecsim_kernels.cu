@@ -546,6 +546,76 @@ __global__ void range_compact_kernel(const float *__restrict__ scores, uint32_t 
     }
 }
 
+// exact range answers of a batch (DESIGN.md §4.11): slot blockIdx.y of the group, scores <= its query's radius into the query's
+// cap slots (unordered), counted past cap
+__global__ void __launch_bounds__(256) range_compact_wide_kernel(const float *__restrict__ scores, uint32_t n, const WideGroup g,
+                                                                 const float *__restrict__ radii, uint32_t cap, uint64_t *__restrict__ out,
+                                                                 uint32_t *__restrict__ counts) {
+    const uint32_t y = blockIdx.y;
+    if (y >= wide_live(g)) return;
+    const uint32_t q = wide_query(g, y);
+    const float r = radii[q];
+    const float *mine = scores + (size_t)y * n;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const float s = mine[i];
+        if (s <= r) { // brute_force.h:315 (NaN never passes)
+            const uint32_t pos = atomicAdd(counts + q, 1u);
+            if (pos < cap) out[(size_t)q * cap + pos] = make_composite(s, i);
+        }
+    }
+}
+
+// One CTA per query: its count and the composites (score key, row) in out[q][0, count) -> labels / scores in the reply order
+// (finish_reply: BY_SCORE by (score, label), BY_ID by label), padded with -1 / NaN; a count past cap pads the whole row.  comp
+// and labels are the same buffer: every composite is read before the first label is written.  Bitonic sort in shared memory
+// over next_pow2(count) <= 4096 (key, label) pairs.
+__global__ void __launch_bounds__(512) range_finish_kernel(int64_t *__restrict__ labels, float *__restrict__ scores,
+                                                           const uint32_t *__restrict__ counts, uint32_t cap,
+                                                           const uint64_t *__restrict__ id_to_label, int by_id) {
+    extern __shared__ uint64_t s_lab[];
+    const uint32_t q = blockIdx.x, cnt = counts[q];
+    int64_t *L = labels + (size_t)q * cap;
+    float *S = scores + (size_t)q * cap;
+    const float nan = __int_as_float(0x7fffffff);
+    if (cnt > cap || cnt == 0) {
+        for (uint32_t i = threadIdx.x; i < cap; i += blockDim.x) L[i] = -1, S[i] = nan;
+        return;
+    }
+    uint32_t n2 = 1;
+    while (n2 < cnt) n2 <<= 1;
+    uint32_t *s_key = reinterpret_cast<uint32_t *>(s_lab + n2);
+    for (uint32_t i = threadIdx.x; i < n2; i += blockDim.x) {
+        if (i < cnt) {
+            const uint64_t c = (uint64_t)L[i];
+            s_key[i] = (uint32_t)(c >> 32);
+            s_lab[i] = id_to_label[(uint32_t)c];
+        } else { // padding sorts last in either order
+            s_key[i] = 0xFFFFFFFFu;
+            s_lab[i] = ~0ull;
+        }
+    }
+    __syncthreads();
+    for (uint32_t k = 2; k <= n2; k <<= 1)
+        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+            for (uint32_t i = threadIdx.x; i < n2; i += blockDim.x) {
+                const uint32_t p = i ^ j;
+                if (p <= i) continue;
+                const uint32_t ka = s_key[i], kb = s_key[p];
+                const uint64_t la = s_lab[i], lb = s_lab[p];
+                const bool b_first = by_id ? (lb < la || (lb == la && kb < ka)) : (kb < ka || (kb == ka && lb < la));
+                if (b_first == ((i & k) == 0)) {
+                    s_key[i] = kb, s_key[p] = ka;
+                    s_lab[i] = lb, s_lab[p] = la;
+                }
+            }
+            __syncthreads();
+        }
+    for (uint32_t i = threadIdx.x; i < cap; i += blockDim.x) {
+        L[i] = i < cnt ? (int64_t)s_lab[i] : -1;
+        S[i] = i < cnt ? key_to_float(s_key[i]) : nan;
+    }
+}
+
 // ------------------------------------------------------------------------------------------------
 // ad-hoc gather: one warp per listed row
 // ------------------------------------------------------------------------------------------------
@@ -1118,6 +1188,50 @@ cudaError_t launch_topk_wide(const CorpusView &c, const void *d_queries, size_t 
         }
     }
     return cudaSuccess;
+}
+
+cudaError_t launch_range_wide(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, const uint32_t *d_pos,
+                              const uint32_t *d_count, const WidePlan &p, float *d_scores, const float *d_radii, uint32_t cap, uint64_t *d_out,
+                              uint32_t *d_counts, const uint32_t *d_abort, cudaStream_t s, LaunchCounters *ctr) {
+    if (cap == 0 || p.group == 0 || c.n_rows == 0) return cudaErrorInvalidValue;
+    WideScanArgs a{};
+    a.rows = static_cast<const uint8_t *>(c.rows);
+    a.pitch = c.pitch;
+    a.n_rows = c.n_rows;
+    a.dim = c.dim;
+    a.queries = static_cast<const uint8_t *>(d_queries);
+    a.qpitch = qpitch;
+    a.scores = d_scores;
+    a.abort = d_abort;
+    a.poll_mask = 15u;
+    for (uint32_t base = 0; base < nq; base += p.group) {
+        const WideGroup g{d_pos, d_count, nq, base};
+        a.g = g;
+        a.slots = std::min(p.group, nq - base);
+        const uint32_t groups8 = (a.slots + 7) / 8;
+        a.wq = groups8 >= 8 ? 8 : groups8 >= 4 ? 4 : groups8 >= 2 ? 2 : 1;
+        cudaError_t e = cudaErrorInvalidValue;
+#define CALL_SCORES_WIDE(DT, MT) e = launch_scores_wide_inst<DT, MT>(a, s)
+        RSB_DISPATCH_DM(c.dtype, c.metric, CALL_SCORES_WIDE)
+#undef CALL_SCORES_WIDE
+        if (e != cudaSuccess) return e;
+        const uint32_t gx = std::max(1u, std::min((c.n_rows + 255u) / 256u, (uint32_t)device_sm_count() * 8u / a.slots));
+        range_compact_wide_kernel<<<dim3(gx, a.slots), 256, 0, s>>>(d_scores, c.n_rows, g, d_radii, cap, d_out, d_counts);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        if (ctr) ctr->launches += 2;
+    }
+    return cudaSuccess;
+}
+
+cudaError_t launch_range_finish(int64_t *d_labels, float *d_scores, const uint32_t *d_counts, uint32_t nq, uint32_t cap,
+                                const uint64_t *d_id_to_label, bool by_id, cudaStream_t s, LaunchCounters *ctr) {
+    if (nq == 0) return cudaSuccess;
+    if (cap == 0 || cap > kRangeDeviceMaxCap) return cudaErrorInvalidValue;
+    uint32_t n2 = 1;
+    while (n2 < cap) n2 <<= 1;
+    range_finish_kernel<<<nq, 512, (size_t)n2 * 12, s>>>(d_labels, d_scores, d_counts, cap, d_id_to_label, by_id ? 1 : 0);
+    if (ctr) ctr->launches++;
+    return cudaGetLastError();
 }
 
 cudaError_t launch_range_compact(const float *d_scores, uint32_t n, float radius, uint64_t *d_out, uint32_t *d_count,

@@ -89,6 +89,19 @@ WidePlan plan_topk_wide(uint32_t n_rows, uint32_t nq);
 cudaError_t launch_topk_wide(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t k, const uint32_t *d_pos,
                              const uint32_t *d_count, const WidePlan &p, float *d_scores, uint64_t *d_cand, uint64_t *d_out,
                              const uint32_t *d_abort, cudaStream_t s, LaunchCounters *ctr);
+// ---- device range batches (DESIGN.md §4.11) --------------------------------------------------------
+constexpr uint32_t kRangeDeviceMaxCap = 4096; // largest per-query result capacity (range_finish_kernel sorts in shared memory)
+// The exact range answer of the queries at batch positions p < *d_count (nq without d_count) — query d_pos[p] (p without
+// d_pos) — by the scores of launch_topk_wide's grouping (the single-query range() bits): composites of the rows with
+// score <= d_radii[q] into d_out[q * cap, ...) unordered, atomically counted in d_counts[q] (zeroed by the caller), past cap
+// too.  2 launches per group; a launch whose positions are all answered exits at once.
+cudaError_t launch_range_wide(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, const uint32_t *d_pos,
+                              const uint32_t *d_count, const WidePlan &p, float *d_scores, const float *d_radii, uint32_t cap, uint64_t *d_out,
+                              uint32_t *d_counts, const uint32_t *d_abort, cudaStream_t s, LaunchCounters *ctr);
+// Row q of d_labels [nq][cap] holds d_counts[q] composites (as uint64): they become labels (int64) and scores in reply order,
+// BY_SCORE (score, label) or BY_ID (label), padded with -1 / NaN; a count past cap pads the whole row.  One launch.
+cudaError_t launch_range_finish(int64_t *d_labels, float *d_scores, const uint32_t *d_counts, uint32_t nq, uint32_t cap,
+                                const uint64_t *d_id_to_label, bool by_id, cudaStream_t s, LaunchCounters *ctr);
 // Append composite(score,id) of every score <= radius to d_out (capacity n), count in *d_count.
 cudaError_t launch_range_compact(const float *d_scores, uint32_t n, float radius, uint64_t *d_out,
                                  uint32_t *d_count, cudaStream_t s, LaunchCounters *ctr);

@@ -139,6 +139,7 @@ SIGNATURES = [
     ("VecSim_GetSharedMemory", _SZ, []),
     ("VecSimB200_TopKQueryBatch", C.c_int, [_P, _P, _SZ, _SZ, _SZ, C.POINTER(VecSimQueryParams), _P, _P]),
     ("VecSimB200_TopKQueryBatchDevice", C.c_int, [_P, _P, _SZ, _SZ, _P, _P, _P]),
+    ("VecSimB200_RangeQueryBatchDevice", C.c_int, [_P, _P, _SZ, _P, _SZ, C.c_int, _P, _P, _P, _P]),
     ("VecSimB200_RangeQueryBatch", C.c_int, [_P, _P, _SZ, _SZ, _P, C.POINTER(VecSimQueryParams), C.c_int, _P, _P]),
     ("VecSimB200_AddVectors", C.c_int, [_P, _P, _SZ, _SZ, _P, _SZ]),
     ("VecSimB200_AddVectorsDevice", C.c_int, [_P, _P, _SZ, _SZ]),
@@ -346,6 +347,27 @@ class VecSimIndex:
                                                      C.byref(params) if params is not None else None, C.c_void_p(out_labels.data_ptr()),
                                                      C.c_void_p(out_scores.data_ptr()), C.c_void_p(out_counts.data_ptr()), _ptr(modes), sh)
         return out_labels, out_scores, out_counts, modes[:nq], rc
+
+    def range_batch_device(self, d_queries, d_radii, cap, order=BY_SCORE, out_labels=None, out_scores=None, out_counts=None, stream=None):
+        """VecSimB200_RangeQueryBatchDevice, enqueued on `stream` (a torch.cuda.Stream, a raw cudaStream_t or None = the legacy
+        default stream) without waiting.  d_queries: a [nq, query_pitch] CUDA tensor of stored-form blobs; d_radii: a [nq] float32
+        CUDA tensor.  Outputs are torch CUDA tensors ([nq, cap] int64 / float32, [nq] int32 holding the u32 counts), allocated when
+        not given.  Returns (labels, scores, counts, rc)."""
+        import torch
+
+        nq = int(d_queries.shape[0])
+        dev = torch.device("cuda")
+        if out_labels is None:
+            out_labels = torch.empty((nq, max(cap, 0)), dtype=torch.int64, device=dev)
+        if out_scores is None:
+            out_scores = torch.empty((nq, max(cap, 0)), dtype=torch.float32, device=dev)
+        if out_counts is None:
+            out_counts = torch.empty(nq, dtype=torch.int32, device=dev)
+        sh = None if stream is None else C.c_void_p(int(getattr(stream, "cuda_stream", stream)) or None)
+        rc = self.L.VecSimB200_RangeQueryBatchDevice(self.h, C.c_void_p(d_queries.data_ptr()), nq, C.c_void_p(d_radii.data_ptr()), cap, order,
+                                                     C.c_void_p(out_labels.data_ptr()), C.c_void_p(out_scores.data_ptr()),
+                                                     C.c_void_p(out_counts.data_ptr()), sh)
+        return out_labels, out_scores, out_counts, rc
 
     def query_pitch(self) -> int:
         """bytes between the stored-form query blobs of a device batch"""
