@@ -480,6 +480,19 @@ int VecSimB200_RangeQueryBatch(VecSimIndex *index, const void *queryBlobs, size_
 int VecSimB200_RangeQueryBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, const float *d_radii, size_t cap,
                                      VecSimQueryReply_Order order, int64_t *d_out_labels, float *d_out_scores,
                                      uint32_t *d_out_counts, void *stream);
+/* nq range queries, device pointers end to end, answered per LABEL as VecSimIndex_RangeQuery answers them on any FLAT index
+ * (DESIGN.md §4.12).  Arguments, outputs, cap rule, orders, stream and host waits as VecSimB200_RangeQueryBatchDevice.
+ * Multi-value index: a label is in query i's answer iff one of its rows has score <= d_radii[i] (float compare; a NaN score
+ * never passes); its score is the smallest such row score; d_out_counts[i] is the true number of such LABELS.  The first call
+ * after a mutation also waits for the rebuild of the label tables.  After a synchronise, VecSimB200_LastCoarseFlags gives 1 per
+ * query a route answered, 3 per query a route proved whose hit rows were too many to fold (more than 4096; the exact scan
+ * answered it) and 0 per query the exact scan answered.  Single-value index: exactly VecSimB200_RangeQueryBatchDevice.
+ * Returns 0; -1 as VecSimB200_RangeQueryBatchDevice (except for multi-value indexes); -2, before anything is enqueued, for a
+ * multi-value index whose labels are too sparse for the dense table (the rule of VecSimB200_TopKFiltered: a label >= 2^32 - 1
+ * or beyond 4 x rows + 2^24). */
+int VecSimB200_LabelRangeQueryBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, const float *d_radii, size_t cap,
+                                          VecSimQueryReply_Order order, int64_t *d_out_labels, float *d_out_scores,
+                                          uint32_t *d_out_counts, void *stream);
 /* Bulk ingest of n host blobs (stride bytes apart) with labels[i] (NULL -> label0+i).  Equivalent
  * to n VecSimIndex_AddVector calls on fresh labels, with one H2D transfer per staging buffer. */
 int VecSimB200_AddVectors(VecSimIndex *index, const void *blobs, size_t stride, size_t n,

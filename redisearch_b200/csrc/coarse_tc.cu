@@ -1790,6 +1790,73 @@ __global__ void __launch_bounds__(256) range_pack_kernel(const uint64_t *__restr
     if (threadIdx.x == 0) ok[q] = 1, cnt[q] = s_n;
 }
 
+// Device range batches on multi-value indexes (DESIGN.md §4.12), one CTA per query a route proved: its hit rows (the proven
+// answer at row level, so every answered label and its best passing row are among them) are mapped to labels, sorted by
+// (label, score key, row) in shared memory and the first entry of each label goes to out[q][0, cap) (unordered), counted past
+// cap.  front != NULL (fp32 route): the hits are cand[q * slots, + front[q]) of a query with ok[q] != 0; front == NULL (8-bit
+// route): the real entries of cand[q * slots, + slots) of a query with overflow[q] == 0.  A proven query with more than
+// kRangeFoldMaxHits hits is left open (ok[q] = 0, flags[q] = 3); ok[q] / flags[q] = 1 for a folded query, 0 / 0 for an open one.
+// cnt[q] is written for folded queries only.
+__global__ void __launch_bounds__(512) range_label_fold_kernel(const uint64_t *__restrict__ cand, uint32_t slots, const uint32_t *__restrict__ front,
+                                                               const uint32_t *__restrict__ overflow, const uint64_t *__restrict__ id_to_label,
+                                                               uint32_t cap, uint64_t *__restrict__ out, uint32_t *__restrict__ cnt,
+                                                               uint32_t *__restrict__ ok, uint32_t *__restrict__ flags) {
+    extern __shared__ uint64_t s_hi[]; // (label << 32 | score key) [kRangeFoldMaxHits], then the rows [kRangeFoldMaxHits]
+    uint32_t *s_row = reinterpret_cast<uint32_t *>(s_hi + kRangeFoldMaxHits);
+    __shared__ uint32_t s_n, s_labels;
+    const uint32_t q = blockIdx.x;
+    const bool proven = front ? ok[q] != 0 : overflow[q] == 0;
+    if (!proven) {
+        if (threadIdx.x == 0) ok[q] = 0, flags[q] = 0;
+        return;
+    }
+    const uint64_t *mine = cand + (size_t)q * slots;
+    if (threadIdx.x == 0) s_n = 0, s_labels = 0;
+    __syncthreads();
+    const uint32_t span = front ? front[q] : slots;
+    for (uint32_t i = threadIdx.x; i < span; i += blockDim.x) {
+        const uint64_t c = mine[i];
+        if (c == kEmptySlot) continue;
+        const uint32_t pos = atomicAdd(&s_n, 1u);
+        if (pos < kRangeFoldMaxHits) {
+            s_hi[pos] = (id_to_label[(uint32_t)c] << 32) | (c >> 32); // labels < 2^32 - 1 (the dense label table's rule)
+            s_row[pos] = (uint32_t)c;
+        }
+    }
+    __syncthreads();
+    const uint32_t n = s_n;
+    if (n > kRangeFoldMaxHits) {
+        if (threadIdx.x == 0) ok[q] = 0, flags[q] = 3;
+        return;
+    }
+    uint32_t n2 = 1;
+    while (n2 < n) n2 <<= 1;
+    for (uint32_t i = n + threadIdx.x; i < n2; i += blockDim.x) s_hi[i] = ~0ull, s_row[i] = ~0u; // padding sorts last
+    __syncthreads();
+    for (uint32_t k = 2; k <= n2; k <<= 1)
+        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+            for (uint32_t i = threadIdx.x; i < n2; i += blockDim.x) {
+                const uint32_t p = i ^ j;
+                if (p <= i) continue;
+                const uint64_t ha = s_hi[i], hb = s_hi[p];
+                const uint32_t ra = s_row[i], rb = s_row[p];
+                const bool b_first = hb < ha || (hb == ha && rb < ra);
+                if (b_first == ((i & k) == 0)) {
+                    s_hi[i] = hb, s_hi[p] = ha;
+                    s_row[i] = rb, s_row[p] = ra;
+                }
+            }
+            __syncthreads();
+        }
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+        if (i > 0 && (s_hi[i] >> 32) == (s_hi[i - 1] >> 32)) continue; // not the label's best row
+        const uint32_t pos = atomicAdd(&s_labels, 1u);
+        if (pos < cap) out[(size_t)q * cap + pos] = (s_hi[i] << 32) | s_row[i];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) ok[q] = 1, flags[q] = 1, cnt[q] = s_labels;
+}
+
 // indices of the queries the first tier left unproven, densely packed: idx[0, *count)
 __global__ void compact_unproven_kernel(const uint32_t *__restrict__ ok, uint32_t nq, uint32_t *__restrict__ idx,
                                         uint32_t *__restrict__ count) {
@@ -2338,6 +2405,16 @@ cudaError_t launch_range_pack(const uint64_t *d_cand, uint32_t nq, uint32_t slot
                               uint32_t *d_cnt, uint32_t *d_ok, cudaStream_t s) {
     if (nq == 0) return cudaSuccess;
     range_pack_kernel<<<nq, 256, 0, s>>>(d_cand, slots, d_overflow, cap, d_out, d_cnt, d_ok);
+    return cudaGetLastError();
+}
+cudaError_t launch_range_label_fold(const uint64_t *d_cand, uint32_t nq, uint32_t slots, const uint32_t *d_front, const uint32_t *d_overflow,
+                                    const uint64_t *d_id_to_label, uint32_t cap, uint64_t *d_out, uint32_t *d_cnt, uint32_t *d_ok,
+                                    uint32_t *d_flags, cudaStream_t s) {
+    if (nq == 0) return cudaSuccess;
+    constexpr size_t smem = (size_t)kRangeFoldMaxHits * 12;
+    cudaError_t e = cudaFuncSetAttribute(range_label_fold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    range_label_fold_kernel<<<nq, 512, smem, s>>>(d_cand, slots, d_front, d_overflow, d_id_to_label, cap, d_out, d_cnt, d_ok, d_flags);
     return cudaGetLastError();
 }
 cudaError_t launch_gather_queries(const void *d_src, size_t pitch, const float *d_src_n2, const uint32_t *d_idx, const uint32_t *d_count,

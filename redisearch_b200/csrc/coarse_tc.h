@@ -15,6 +15,7 @@ constexpr uint32_t kCoarseFixedCapWide = 256; // list capacity of the fp32 main 
 constexpr uint32_t kCoarseSampleSlices = 32; // minima the sample pass publishes per (query, row range)
 constexpr uint32_t kCoarseFixedCapDirect = 256; // list capacity of the fixed-bound pass on 16-bit corpora (k up to 128)
 constexpr uint32_t kCoarseFixedCap = 96;   // list capacity of the fixed-bound main pass (rows below the bound per row range)
+constexpr uint32_t kRangeFoldMaxHits = 4096; // most hit rows range_label_fold_kernel sorts per query (48 KB of shared memory)
 // |approx - exact| bounds for unit vectors (Cauchy-Schwarz over the dot product: sum |a_i b_i| <= 1):
 //  TF32: each operand truncated to 11 significant bits -> 2 * 2^-10 relative per product, + accumulation slack;
 //  F16 : each operand rounded to nearest, 11 significant bits -> 2 * 2^-11 = 9.8e-4 per product; elements below
@@ -113,6 +114,16 @@ cudaError_t launch_range_refine(const CorpusView &c, const void *d_queries, size
 // a query whose lists overflowed: d_ok[q] = 0, d_cnt[q] = 0
 cudaError_t launch_range_pack(const uint64_t *d_cand, uint32_t nq, uint32_t slots, const uint32_t *d_overflow, uint32_t cap, uint64_t *d_out,
                               uint32_t *d_cnt, uint32_t *d_ok, cudaStream_t s);
+// device range batches on multi-value indexes (DESIGN.md §4.12): the label fold of the queries a route proved.  d_front != NULL (fp32
+// route, after launch_range_refine with d_out = d_cand and cap = slots): query q's hit rows are d_cand[q * slots, + d_front[q]), proven
+// iff d_ok[q] != 0; d_front == NULL (8-bit route, in place of launch_range_pack): its hits are the real entries of its `slots` list
+// entries, proven iff d_overflow[q] == 0.  A proven query with at most kRangeFoldMaxHits hits gets one composite (score key, row)
+// per label, the label's smallest (score, row), in d_out[q * cap, ...) unordered, d_cnt[q] = the number of labels (past cap too),
+// d_ok[q] = d_flags[q] = 1.  With more hits: d_ok[q] = 0, d_flags[q] = 3; an unproven query: d_ok[q] = d_flags[q] = 0.  d_cnt[q]
+// is left as it was (zero) for both.
+cudaError_t launch_range_label_fold(const uint64_t *d_cand, uint32_t nq, uint32_t slots, const uint32_t *d_front, const uint32_t *d_overflow,
+                                    const uint64_t *d_id_to_label, uint32_t cap, uint64_t *d_out, uint32_t *d_cnt, uint32_t *d_ok,
+                                    uint32_t *d_flags, cudaStream_t s);
 // |row|^2 of fp32 rows [first, first+n) into d_norm2[first..], NaN for a row whose fp16 form is not finite (a component
 // with |x| >= 65520, or NaN: refine_kernel never proves such a query); d_stats (nullable) = {max |row|^2, max |x|} as float bits
 cudaError_t launch_row_stats(const void *rows, size_t pitch, uint32_t dim, uint32_t first, uint32_t n, float *d_norm2, uint32_t *d_stats,

@@ -264,6 +264,12 @@ int VecSimB200_RangeQueryBatchDevice(VecSimIndex *index, const void *d_queries, 
     return IX(index)->range_batch_device(d_queries, nq, d_radii, cap, order, d_out_labels, d_out_scores, d_out_counts,
                                          static_cast<cudaStream_t>(stream));
 }
+int VecSimB200_LabelRangeQueryBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, const float *d_radii, size_t cap,
+                                          VecSimQueryReply_Order order, int64_t *d_out_labels, float *d_out_scores, uint32_t *d_out_counts,
+                                          void *stream) {
+    return IX(index)->label_range_batch_device(d_queries, nq, d_radii, cap, order, d_out_labels, d_out_scores, d_out_counts,
+                                               static_cast<cudaStream_t>(stream));
+}
 int VecSimB200_AddVectors(VecSimIndex *index, const void *blobs, size_t stride, size_t n, const size_t *labels,
                           size_t label0) {
     return IX(index)->add_bulk(blobs, stride, n, labels, label0);

@@ -1504,15 +1504,30 @@ int FlatIndex::range_batch(const void *qs, size_t qstride, size_t nq, const doub
     return rc;
 }
 
-// Device range batches (DESIGN.md §4.11): one route per batch, then the exact scan on the device for the queries it left open
-// (or for the whole batch), then one CTA per query orders its hits and maps rows to labels.  Hits are gathered as composites in
-// d_labels itself ([nq][cap] uint64) with the true count in d_counts.  Nothing waits on the host except ensure_shadow.
 int FlatIndex::range_batch_device(const void *d_q, size_t nq, const float *d_radii, size_t cap, VecSimQueryReply_Order order, int64_t *d_labels,
                                   float *d_scores, uint32_t *d_counts, cudaStream_t s) {
-    if (multi_ || cap == 0 || cap > kRangeDeviceMaxCap || (order != BY_ID && order != BY_SCORE) || nq > 0xFFFFFFFFu) return -1;
+    if (multi_) return -1;
+    return range_device(d_q, nq, d_radii, cap, order, d_labels, d_scores, d_counts, s);
+}
+
+int FlatIndex::label_range_batch_device(const void *d_q, size_t nq, const float *d_radii, size_t cap, VecSimQueryReply_Order order,
+                                        int64_t *d_labels, float *d_scores, uint32_t *d_counts, cudaStream_t s) {
+    if (!multi_) return range_batch_device(d_q, nq, d_radii, cap, order, d_labels, d_scores, d_counts, s);
+    return range_device(d_q, nq, d_radii, cap, order, d_labels, d_scores, d_counts, s);
+}
+
+// Device range batches (DESIGN.md §4.11): one route per batch, then the exact scan on the device for the queries it left open
+// (or for the whole batch), then one CTA per query orders its hits and maps rows to labels.  Hits are gathered as composites in
+// d_labels itself ([nq][cap] uint64) with the true count in d_counts.  Nothing waits on the host except ensure_shadow (and, on a
+// multi-value index, the label tables' rebuild after a mutation).  Multi-value index (§4.12): a route's proven row answer is folded
+// to one entry per label (launch_range_label_fold) and the exact scan folds label-major over the CSR label table.
+int FlatIndex::range_device(const void *d_q, size_t nq, const float *d_radii, size_t cap, VecSimQueryReply_Order order, int64_t *d_labels,
+                            float *d_scores, uint32_t *d_counts, cudaStream_t s) {
+    if (cap == 0 || cap > kRangeDeviceMaxCap || (order != BY_ID && order != BY_SCORE) || nq > 0xFFFFFFFFu) return -1;
     last_mode_ = RANGE_QUERY;
     if (nq == 0) return 0;
     if (!flush() || !sync_labels_to_device()) return -1;
+    if (multi_ && !sync_label_table()) return -2; // sparse labels: no CSR table for the exact fold
     const size_t n = count_;
     std::lock_guard<std::mutex> dg(dev_mu_);
     if (!dev_ctx_) dev_ctx_ = checkout();
@@ -1546,7 +1561,8 @@ int FlatIndex::range_batch_device(const void *d_q, size_t nq, const float *d_rad
     uint64_t *cand, *list_scratch;
     uint8_t *q16;
     float *d_qn2, *d_thr;
-    uint32_t *d_ok, *d_idx, *d_n2, *d_ovf, *d_total;
+    uint32_t *d_ok, *d_idx, *d_n2, *d_ovf, *d_total, *d_flags, *d_front;
+    const bool fold = multi_ && path; // a route's rows -> labels
     const auto layout = [&](void *base) {
         BatchScratch sc(base);
         cand = sc.take<uint64_t>(path ? nq * slots : 0);
@@ -1559,6 +1575,8 @@ int FlatIndex::range_batch_device(const void *d_q, size_t nq, const float *d_rad
         d_ok = sc.take<uint32_t>(nq);  // reported flags
         d_idx = sc.take<uint32_t>(nq); // the open queries
         d_n2 = sc.take<uint32_t>(1);   // and their count
+        d_flags = sc.take<uint32_t>(fold ? nq : 0);          // multi-value: the reported flags (d_ok: 1 = folded, 0 = open)
+        d_front = sc.take<uint32_t>(fold && path == 1 ? nq : 0); // multi-value fp32 route: the hit rows at the front of each list segment
         return sc.words();
     };
     if (!c->need_cand(layout(nullptr)) || (n > 0 && !c->need_scores(wp.score_elems))) return -1;
@@ -1576,8 +1594,16 @@ int FlatIndex::range_batch_device(const void *d_q, size_t nq, const float *d_rad
         cudaEventRecord(c->ev_start, st);
         ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_thr, d_ovf) == cudaSuccess;
         cudaEventRecord(c->ev_stop, st);
-        ok = ok && launch_range_refine(v, d_q, qpitch, nq32, (uint32_t)slots, cand, d_radii, d_qn2, d_thr, d_ovf, comp, d_total, d_ok, d_counts,
-                                       nullptr, st, cap32) == cudaSuccess;
+        if (fold) { // the kept rows stay at the front of each list segment (cap = slots onto cand itself: a copy onto itself)
+            ok = ok && launch_range_refine(v, d_q, qpitch, nq32, (uint32_t)slots, cand, d_radii, d_qn2, d_thr, d_ovf, cand, d_total, d_ok,
+                                           d_front, nullptr, st, (uint32_t)slots) == cudaSuccess;
+            ok = ok && launch_range_label_fold(cand, nq32, (uint32_t)slots, d_front, nullptr, d_id_to_label_, cap32, comp, d_counts, d_ok, d_flags,
+                                               st) == cudaSuccess;
+            lc.launches++;
+        } else {
+            ok = ok && launch_range_refine(v, d_q, qpitch, nq32, (uint32_t)slots, cand, d_radii, d_qn2, d_thr, d_ovf, comp, d_total, d_ok,
+                                           d_counts, nullptr, st, cap32) == cudaSuccess;
+        }
         lc.launches += unit ? 4 : 5;
     } else if (path == 2) {
         CoarseOperands ops{v.rows, v.pitch, d_q, qpitch, dtype_ == DT_I8 ? 1 : 0, mkind_ == MT_COS ? 1 : int_l2() ? 2 : 0, nullptr, nullptr};
@@ -1591,7 +1617,11 @@ int FlatIndex::range_batch_device(const void *d_q, size_t nq, const float *d_rad
         cudaEventRecord(c->ev_start, st);
         ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_radii, d_ovf) == cudaSuccess;
         cudaEventRecord(c->ev_stop, st);
-        ok = ok && launch_range_pack(cand, nq32, (uint32_t)slots, d_ovf, cap32, comp, d_counts, d_ok, st) == cudaSuccess;
+        if (fold)
+            ok = ok && launch_range_label_fold(cand, nq32, (uint32_t)slots, nullptr, d_ovf, d_id_to_label_, cap32, comp, d_counts, d_ok, d_flags,
+                                               st) == cudaSuccess;
+        else
+            ok = ok && launch_range_pack(cand, nq32, (uint32_t)slots, d_ovf, cap32, comp, d_counts, d_ok, st) == cudaSuccess;
         lc.launches += 2;
     }
     if (n > 0) {
@@ -1602,13 +1632,14 @@ int FlatIndex::range_batch_device(const void *d_q, size_t nq, const float *d_rad
         }
         if (!path) cudaEventRecord(c->ev_start, st);
         ok = ok && launch_range_wide(v, d_q, qpitch, nq32, path ? d_idx : nullptr, path ? d_n2 : nullptr, wp, c->d_scores, d_radii, cap32, comp,
-                                     d_counts, c->d_abort, st, &lc) == cudaSuccess;
+                                     d_counts, c->d_abort, st, &lc, multi_ ? d_label_to_id_ : nullptr, multi_ ? d_label_rows_ : nullptr,
+                                     multi_ ? (uint32_t)l2i_size_ : 0) == cudaSuccess;
         if (!path) cudaEventRecord(c->ev_stop, st);
     }
     ok = ok && launch_range_finish(d_labels, d_scores, d_counts, nq32, cap32, d_id_to_label_, order == BY_ID, st, &lc) == cudaSuccess;
-    c->d_last_ok = d_ok;
+    c->d_last_ok = fold ? d_flags : d_ok;
     c->last_ok_n = nq32;
-    last_batch_coarse_ = true; // LastCoarseFlags: 1 = a tensor-core route answered the query, 0 = the exact scan
+    last_batch_coarse_ = true; // LastCoarseFlags: 1 = a tensor-core route answered the query, 0 = the exact scan, 3 = too many hit rows to fold
     last_batch_path_ = path;
     if (path) coarse_batches_++;
     dev_timing_pending_ = ok && n > 0;

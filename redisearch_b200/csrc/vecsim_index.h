@@ -145,6 +145,9 @@ class FlatIndex {
     // the same with device pointers end to end, stream-ordered: VecSimB200_RangeQueryBatchDevice (DESIGN.md §4.11)
     int range_batch_device(const void *d_q, size_t nq, const float *d_radii, size_t cap, VecSimQueryReply_Order order, int64_t *d_labels,
                            float *d_scores, uint32_t *d_counts, cudaStream_t s);
+    // the same answered per label on any index: VecSimB200_LabelRangeQueryBatchDevice (DESIGN.md §4.12)
+    int label_range_batch_device(const void *d_q, size_t nq, const float *d_radii, size_t cap, VecSimQueryReply_Order order, int64_t *d_labels,
+                                 float *d_scores, uint32_t *d_counts, cudaStream_t s);
     double distance_from(size_t label, const void *stored_form_blob);
     bool prefer_adhoc(size_t subset, size_t k, bool initial);
 
@@ -288,6 +291,9 @@ class FlatIndex {
     size_t label_rows_cap_ = 0;
     bool l2i_dirty_ = true;
     bool sync_label_table();
+    // the body of range_batch_device / label_range_batch_device: per row on a single-value index, per label on a multi-value one
+    int range_device(const void *d_q, size_t nq, const float *d_radii, size_t cap, VecSimQueryReply_Order order, int64_t *d_labels,
+                     float *d_scores, uint32_t *d_counts, cudaStream_t s);
 
     mutable std::mutex mu_;      // guards mutation + staging
     std::mutex pool_mu_;

@@ -565,6 +565,35 @@ __global__ void __launch_bounds__(256) range_compact_wide_kernel(const float *__
     }
 }
 
+// exact range answers of a batch on a multi-value index (DESIGN.md §4.12), label-major over the CSR label table: slot blockIdx.y
+// of the group, one thread per label, the smallest composite (score key, row) among the label's rows with score <= the radius;
+// a label with such a row is appended to the query's cap slots (unordered) and counted past cap
+__global__ void __launch_bounds__(256) range_label_wide_kernel(const float *__restrict__ scores, uint32_t n, const WideGroup g,
+                                                               const float *__restrict__ radii, const uint32_t *__restrict__ label_off,
+                                                               const uint32_t *__restrict__ label_rows, uint32_t n_labels, uint32_t cap,
+                                                               uint64_t *__restrict__ out, uint32_t *__restrict__ counts) {
+    const uint32_t y = blockIdx.y;
+    if (y >= wide_live(g)) return;
+    const uint32_t q = wide_query(g, y);
+    const float r = radii[q];
+    const float *mine = scores + (size_t)y * n;
+    for (uint32_t l = blockIdx.x * blockDim.x + threadIdx.x; l < n_labels; l += gridDim.x * blockDim.x) {
+        uint64_t best = ~0ull;
+        for (uint32_t j = label_off[l], e = label_off[l + 1]; j < e; j++) {
+            const uint32_t row = label_rows[j];
+            const float s = mine[row];
+            if (s <= r) { // brute_force.h:315 (NaN never passes)
+                const uint64_t c = make_composite(s, row);
+                best = c < best ? c : best;
+            }
+        }
+        if (best != ~0ull) {
+            const uint32_t pos = atomicAdd(counts + q, 1u);
+            if (pos < cap) out[(size_t)q * cap + pos] = best;
+        }
+    }
+}
+
 // One CTA per query: its count and the composites (score key, row) in out[q][0, count) -> labels / scores in the reply order
 // (finish_reply: BY_SCORE by (score, label), BY_ID by label), padded with -1 / NaN; a count past cap pads the whole row.  comp
 // and labels are the same buffer: every composite is read before the first label is written.  Bitonic sort in shared memory
@@ -1192,7 +1221,8 @@ cudaError_t launch_topk_wide(const CorpusView &c, const void *d_queries, size_t 
 
 cudaError_t launch_range_wide(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, const uint32_t *d_pos,
                               const uint32_t *d_count, const WidePlan &p, float *d_scores, const float *d_radii, uint32_t cap, uint64_t *d_out,
-                              uint32_t *d_counts, const uint32_t *d_abort, cudaStream_t s, LaunchCounters *ctr) {
+                              uint32_t *d_counts, const uint32_t *d_abort, cudaStream_t s, LaunchCounters *ctr, const uint32_t *label_off,
+                              const uint32_t *label_rows, uint32_t n_labels) {
     if (cap == 0 || p.group == 0 || c.n_rows == 0) return cudaErrorInvalidValue;
     WideScanArgs a{};
     a.rows = static_cast<const uint8_t *>(c.rows);
@@ -1215,8 +1245,13 @@ cudaError_t launch_range_wide(const CorpusView &c, const void *d_queries, size_t
         RSB_DISPATCH_DM(c.dtype, c.metric, CALL_SCORES_WIDE)
 #undef CALL_SCORES_WIDE
         if (e != cudaSuccess) return e;
-        const uint32_t gx = std::max(1u, std::min((c.n_rows + 255u) / 256u, (uint32_t)device_sm_count() * 8u / a.slots));
-        range_compact_wide_kernel<<<dim3(gx, a.slots), 256, 0, s>>>(d_scores, c.n_rows, g, d_radii, cap, d_out, d_counts);
+        const uint32_t items = label_off ? n_labels : c.n_rows;
+        const uint32_t gx = std::max(1u, std::min((items + 255u) / 256u, (uint32_t)device_sm_count() * 8u / a.slots));
+        if (label_off)
+            range_label_wide_kernel<<<dim3(gx, a.slots), 256, 0, s>>>(d_scores, c.n_rows, g, d_radii, label_off, label_rows, n_labels, cap,
+                                                                      d_out, d_counts);
+        else
+            range_compact_wide_kernel<<<dim3(gx, a.slots), 256, 0, s>>>(d_scores, c.n_rows, g, d_radii, cap, d_out, d_counts);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
         if (ctr) ctr->launches += 2;
     }

@@ -94,10 +94,13 @@ constexpr uint32_t kRangeDeviceMaxCap = 4096; // largest per-query result capaci
 // The exact range answer of the queries at batch positions p < *d_count (nq without d_count) — query d_pos[p] (p without
 // d_pos) — by the scores of launch_topk_wide's grouping (the single-query range() bits): composites of the rows with
 // score <= d_radii[q] into d_out[q * cap, ...) unordered, atomically counted in d_counts[q] (zeroed by the caller), past cap
-// too.  2 launches per group; a launch whose positions are all answered exits at once.
+// too.  2 launches per group; a launch whose positions are all answered exits at once.  label_off != NULL (multi-value index,
+// DESIGN.md §4.12): the answer is per label instead — label_off [n_labels + 1] / label_rows the CSR label -> rows table, and each
+// label with a passing row contributes one composite, its smallest (score key, row), counted per label.
 cudaError_t launch_range_wide(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, const uint32_t *d_pos,
                               const uint32_t *d_count, const WidePlan &p, float *d_scores, const float *d_radii, uint32_t cap, uint64_t *d_out,
-                              uint32_t *d_counts, const uint32_t *d_abort, cudaStream_t s, LaunchCounters *ctr);
+                              uint32_t *d_counts, const uint32_t *d_abort, cudaStream_t s, LaunchCounters *ctr, const uint32_t *label_off = nullptr,
+                              const uint32_t *label_rows = nullptr, uint32_t n_labels = 0);
 // Row q of d_labels [nq][cap] holds d_counts[q] composites (as uint64): they become labels (int64) and scores in reply order,
 // BY_SCORE (score, label) or BY_ID (label), padded with -1 / NaN; a count past cap pads the whole row.  One launch.
 cudaError_t launch_range_finish(int64_t *d_labels, float *d_scores, const uint32_t *d_counts, uint32_t nq, uint32_t cap,

@@ -140,6 +140,7 @@ SIGNATURES = [
     ("VecSimB200_TopKQueryBatch", C.c_int, [_P, _P, _SZ, _SZ, _SZ, C.POINTER(VecSimQueryParams), _P, _P]),
     ("VecSimB200_TopKQueryBatchDevice", C.c_int, [_P, _P, _SZ, _SZ, _P, _P, _P]),
     ("VecSimB200_RangeQueryBatchDevice", C.c_int, [_P, _P, _SZ, _P, _SZ, C.c_int, _P, _P, _P, _P]),
+    ("VecSimB200_LabelRangeQueryBatchDevice", C.c_int, [_P, _P, _SZ, _P, _SZ, C.c_int, _P, _P, _P, _P]),
     ("VecSimB200_RangeQueryBatch", C.c_int, [_P, _P, _SZ, _SZ, _P, C.POINTER(VecSimQueryParams), C.c_int, _P, _P]),
     ("VecSimB200_AddVectors", C.c_int, [_P, _P, _SZ, _SZ, _P, _SZ]),
     ("VecSimB200_AddVectorsDevice", C.c_int, [_P, _P, _SZ, _SZ]),
@@ -353,6 +354,17 @@ class VecSimIndex:
         default stream) without waiting.  d_queries: a [nq, query_pitch] CUDA tensor of stored-form blobs; d_radii: a [nq] float32
         CUDA tensor.  Outputs are torch CUDA tensors ([nq, cap] int64 / float32, [nq] int32 holding the u32 counts), allocated when
         not given.  Returns (labels, scores, counts, rc)."""
+        return self._range_device(self.L.VecSimB200_RangeQueryBatchDevice, d_queries, d_radii, cap, order, out_labels, out_scores,
+                                  out_counts, stream)
+
+    def label_range_batch_device(self, d_queries, d_radii, cap, order=BY_SCORE, out_labels=None, out_scores=None, out_counts=None,
+                                 stream=None):
+        """VecSimB200_LabelRangeQueryBatchDevice: range_batch_device answered per label, on multi-value indexes too (one entry per
+        label at its best passing row, counts in labels).  Returns (labels, scores, counts, rc); rc -2 = labels too sparse."""
+        return self._range_device(self.L.VecSimB200_LabelRangeQueryBatchDevice, d_queries, d_radii, cap, order, out_labels, out_scores,
+                                  out_counts, stream)
+
+    def _range_device(self, fn, d_queries, d_radii, cap, order, out_labels, out_scores, out_counts, stream):
         import torch
 
         nq = int(d_queries.shape[0])
@@ -364,9 +376,8 @@ class VecSimIndex:
         if out_counts is None:
             out_counts = torch.empty(nq, dtype=torch.int32, device=dev)
         sh = None if stream is None else C.c_void_p(int(getattr(stream, "cuda_stream", stream)) or None)
-        rc = self.L.VecSimB200_RangeQueryBatchDevice(self.h, C.c_void_p(d_queries.data_ptr()), nq, C.c_void_p(d_radii.data_ptr()), cap, order,
-                                                     C.c_void_p(out_labels.data_ptr()), C.c_void_p(out_scores.data_ptr()),
-                                                     C.c_void_p(out_counts.data_ptr()), sh)
+        rc = fn(self.h, C.c_void_p(d_queries.data_ptr()), nq, C.c_void_p(d_radii.data_ptr()), cap, order, C.c_void_p(out_labels.data_ptr()),
+                C.c_void_p(out_scores.data_ptr()), C.c_void_p(out_counts.data_ptr()), sh)
         return out_labels, out_scores, out_counts, rc
 
     def query_pitch(self) -> int:
