@@ -628,6 +628,32 @@ int VecSimB200_TopKFilteredBatchDevice(VecSimIndex *index, const void *d_queries
 int VecSimB200_HybridTopKBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, size_t k, const uint32_t *const *d_doc_ids,
                                      const uint32_t *const *d_counts, const size_t *caps, VecSimQueryParams *queryParams, int64_t *d_out_labels,
                                      float *d_out_scores, uint32_t *d_out_counts, int *out_modes, void *stream);
+/* nq filtered range queries ("@tag:{...} @v:[VECTOR_RANGE $r $B]"), device pointers end to end (DESIGN.md §4.13).  d_queries,
+ * d_radii, cap (1..4096), order, the outputs and stream as in VecSimB200_LabelRangeQueryBatchDevice; d_doc_ids, d_counts and caps as
+ * in VecSimB200_HybridTopKBatchDevice (host arrays of device pointers, counts read in stream order, caps host upper bounds).  Filter
+ * lists must be STRICTLY ascending.
+ * Query i's answer is exactly VecSimB200_LabelRangeQueryBatchDevice's answer for (query i, d_radii[i]) restricted to the docIds of
+ * filter i: the same labels, score bits, order and cap rule, with d_out_counts[i] the true number of such labels.  A docId is in it
+ * iff it is live and one of its rows scores <= d_radii[i] (a float compare: a NaN score never passes, a NaN radius keeps nothing, a
+ * negative radius is answered as given); its score is the smallest passing row score.  Absent and deleted docIds contribute nothing.
+ * Routes: every query can take the range form of the ragged gather of VecSimB200_TopKFilteredBatchDevice.  A single-value batch
+ * that VecSimB200_RangeQueryBatchDevice would send to its fp32 or 8-bit tensor-core route can instead take that route as a whole
+ * with the filters applied to the rows; the queries it leaves open go to the gather.  queryParams NULL or searchMode 0: the
+ * batch goes dense when the bytes its gathers would read exceed what the dense route reads (DESIGN.md §4.13); HYBRID_ADHOC_BF
+ * forces the gather, HYBRID_BATCHES the dense route where the batch is eligible.  fp16 / bf16 and multi-value indexes always take
+ * the gather.  out_modes (nullable host [nq]): each query's route, written before the call returns.  After a synchronise,
+ * VecSimB200_LastCoarseFlags gives 1 per query a dense route answered and 0 per query the gather answered; VecSimB200_LastBatchPath
+ * is 1 (fp32 route), 2 (8-bit route) or 0 (gather only).  The index's last search mode is RANGE_QUERY.
+ * Host waits: those of VecSimB200_TopKFilteredBatchDevice and VecSimB200_RangeQueryBatchDevice (flush, docId table rebuild, first
+ * fp16 shadow or int32 |row|^2 table).  Launches do not depend on nq: 2 on the gather alone; 8 on the fp32 route (+1 for L2 / inner
+ * product), 6 on the 8-bit route (+1 for L2).
+ * Returns 0 (with nothing enqueued for nq == 0); -1 for cap == 0 or cap > 4096, an order other than BY_ID / BY_SCORE, a searchMode
+ * other than 0 / HYBRID_ADHOC_BF / HYBRID_BATCHES, or a CUDA failure; -2, before anything is enqueued, for labels too sparse for
+ * the dense docId table or a cap beyond the 32-bit id range (the rules of VecSimB200_TopKFilteredBatchDevice). */
+int VecSimB200_HybridRangeQueryBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, const float *d_radii, size_t cap,
+                                           VecSimQueryReply_Order order, const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts,
+                                           const size_t *caps, VecSimQueryParams *queryParams, int64_t *d_out_labels, float *d_out_scores,
+                                           uint32_t *d_out_counts, int *out_modes, void *stream);
 /* Batched fp32 queries (cosine, and in mode 1 also L2 and raw inner product; nq >= 16, k <= 16, dim % 8 == 0,
  * >= 65536 rows) take a wgmma coarse
  * pass + exact rescoring from the fp32 rows + a per-query completeness proof, with the exact scan as

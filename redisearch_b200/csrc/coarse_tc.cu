@@ -755,7 +755,8 @@ __device__ __forceinline__ int range_int_bound(float r) {
 //   kFilt    hybrid batches (DESIGN.md §4.10): only rows whose bit is set in the query's row-space bitmap count.  Query q's
 //            bitmap is filt + filt_words * (filt_q ? filt_q[q] : q).  The sample pass takes each chunk's maximum over its
 //            filtered rows; the adaptive lists and the fixed bound admit only filtered rows (the fixed bound tests the bit on
-//            its rare survivor path, after the key test).  fp32 route only.
+//            its rare survivor path, after the key test).  fp32 route, and the 8-bit fixed-radius pass (DESIGN.md §4.13), which
+//            tests the bit after both the integer pre-test and the float range test.
 //   kRegKb   the fixed-bound pass over the fp16 shadow: the first kRegKb K blocks of the CTA's queries are held in registers
 //            (the wgmma A fragment, 16 per K block and thread, loaded once per consumer warpgroup) instead of shared memory,
 //            which frees kRegKb x 8 KB for the ring (DESIGN.md §4.2).  The first kRegKb / kQKbPerStage stages of a tile take
@@ -777,7 +778,8 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
     const uint32_t bx = blockIdx.x, by = blockIdx.y, gx = gridDim.x;
     static_assert(kMode == 0 || (!kDirect && (kOp == 0 || kOp == 3)) || (kDirect && kOp == 0) || (kDirect && kFixed && kInt && kEpl == 8),
                   "fixed bound / sample pass: the fp32 route and 16-bit corpora (inner product / cosine); fixed radius: 8-bit corpora");
-    static_assert(!kFilt || (!kDirect && (kOp == 0 || kOp == 3)), "row filters: the fp32 route");
+    static_assert(!kFilt || (!kDirect && (kOp == 0 || kOp == 3)) || (kDirect && kFixed && kInt && kEpl == 8),
+                  "row filters: the fp32 route and the 8-bit fixed-radius pass");
     static_assert(kRegKb == 0 || (!kDirect && kFixed && kRegKb % kQKbPerStage == 0),
                   "register-held queries: the fixed-bound pass over the fp16 shadow, whole stages");
     // kFilt: the row-space bitmap of the query at position `pos` of this batch
@@ -1163,7 +1165,11 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         } else {
                             d = __int2float_rn(__ldg(irn2 + row) + fnqi[i2] - 2 * (int)raw);
                         }
-                        if (d <= frad[i2]) { // the reference's inclusive range test: NaN never passes, -0 == +0
+                        bool hit = d <= frad[i2]; // the reference's inclusive range test: NaN never passes, -0 == +0
+                        if constexpr (kFilt) { // a hit counts only if the query's filter holds the row
+                            if (hit) hit = (__ldg(filt_row(q_base + 16 * ew + (lane >> 2) + 8 * i2) + (row >> 5)) >> (row & 31)) & 1u;
+                        }
+                        if (hit) {
                             const int qs = 16 * ew + (lane >> 2) + 8 * i2;
                             const uint32_t slot = atomicAdd(&qcount[qs], 1u);
                             if (slot < (uint32_t)kQListCap) lists[slot * kQListStride + qs] = ((uint64_t)orderable_key(d) << 32) | row;
@@ -1932,7 +1938,12 @@ static bool make_map(CUtensorMap *m, CUtensorMapDataType dt, const void *base, u
 static constexpr size_t kSmemLimit = 232448; // 227 KB opt-in maximum of dynamic shared memory per CTA on sm_90
 
 template <int V>
-static const void *wgmma_kernel_fn_v(CoarseKind kind, uint32_t epl, int epi, int mode) {
+static const void *wgmma_kernel_fn_v(CoarseKind kind, uint32_t epl, int epi, int mode, bool filt) {
+    if (filt) { // filtered range batches (DESIGN.md §4.13): the 8-bit fixed-radius pass only
+        if (kind != CoarseDirect8 || mode != 1) return nullptr;
+        if (epi == 2) return (const void *)coarse_wgmma_kernel<true, 8, 4, 1, V, true>;
+        return epi == 1 ? (const void *)coarse_wgmma_kernel<true, 8, 2, 1, V, true> : (const void *)coarse_wgmma_kernel<true, 8, 1, 1, V, true>;
+    }
     if (kind == CoarseDirect16) {
         if (mode == 1) return (const void *)coarse_wgmma_kernel<true, 8, 0, 1, V>; // fixed bound, lists of 256
         if (mode == 2) return (const void *)coarse_wgmma_kernel<true, 3, 0, 2, V>; // sample pass
@@ -1955,13 +1966,14 @@ static const void *wgmma_kernel_fn_v(CoarseKind kind, uint32_t epl, int epi, int
 static constexpr uint32_t kFixedRegKb = 4;
 static uint32_t fixed_reg_kb(uint32_t epl, bool l2, bool filt) { return (epl == 3 && !l2 && !filt) ? kFixedRegKb : 0u; }
 // variant: 16-bit corpora 1 = bf16, 8-bit corpora 1 = int8 (the fp32 route's shadow is always fp16); epi: CoarseOperands::epilogue
-// filt: the kFilt instantiations (fp32 route; every adaptive-list pass with a filter keeps lists of up to 128)
+// filt: the kFilt instantiations (fp32 route, where every adaptive-list pass with a filter keeps lists of up to 128; the 8-bit
+// fixed-radius pass)
 // reg_kb: the fixed-bound pass with that many K blocks of the queries in registers (fixed_reg_kb), else 0
 static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, int epi, int mode = 0, uint32_t variant = 0, bool filt = false,
                                    uint32_t reg_kb = 0) {
     const bool l2 = epi != 0;
     if (kind == CoarseDirect16 || kind == CoarseDirect8)
-        return variant ? wgmma_kernel_fn_v<1>(kind, epl, epi, mode) : wgmma_kernel_fn_v<0>(kind, epl, epi, mode);
+        return variant ? wgmma_kernel_fn_v<1>(kind, epl, epi, mode, filt) : wgmma_kernel_fn_v<0>(kind, epl, epi, mode, filt);
     if (reg_kb) {
         if (mode != 1 || reg_kb != fixed_reg_kb(epl, l2, filt)) return nullptr;
         return (const void *)coarse_wgmma_kernel<false, 3, 0, 1, 0, false, kFixedRegKb>;
@@ -2134,7 +2146,7 @@ static cudaError_t launch_coarse_t(const void *rows, size_t pitch, uint32_t n_ro
 cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim, uint32_t nq, const CoarsePlan &p, uint64_t *d_cand,
                           uint64_t *d_scratch, cudaStream_t s, const uint32_t *d_nq_dev, const float *d_thr_fixed, uint32_t *d_overflow,
                           const uint32_t *d_filt, uint32_t filt_words, const uint32_t *d_filt_q) {
-    if (d_filt && p.kind != CoarseF16) return cudaErrorInvalidValue;
+    if (d_filt && p.kind != CoarseF16 && !(p.kind == CoarseDirect8 && p.mode == 1)) return cudaErrorInvalidValue;
     if (p.kind == CoarseF16 || p.kind == CoarseDirect16 || p.kind == CoarseDirect8) {
         if (p.mode == 1 && (!d_thr_fixed || !d_overflow)) return cudaErrorInvalidValue;
         // operand variant: 16-bit 1 = bf16 (else fp16); 8-bit 1 = int8 (else uint8); the fp16 shadow of the fp32 route: 0

@@ -60,8 +60,9 @@ bool coarse_supported(const CorpusView &c, uint32_t nq, uint32_t k, CoarseKind k
 CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32_t k, uint32_t keep_override = 0, uint32_t tile_stride = 1,
                        int mode = 0, bool filt = false);
 // d_nq_dev (nullable): the number of live queries is read from device memory (min with nq); 0 = the kernel exits at once.
-// d_filt (nullable, CoarseF16 only): row filters of a hybrid batch, one bitmap of filt_words u32 per query (bit r = row r); query
-// i of the pass uses bitmap d_filt_q[i] (d_filt_q NULL: bitmap i).  Only filtered rows enter the lists and the sample minima
+// d_filt (nullable; CoarseF16, and CoarseDirect8 of mode 1): row filters of a hybrid batch, one bitmap of filt_words u32 per query
+// (bit r = row r); query i of the pass uses bitmap d_filt_q[i] (d_filt_q NULL: bitmap i).  Only filtered rows enter the lists and
+// the sample minima
 cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim, uint32_t nq, const CoarsePlan &p, uint64_t *d_cand,
                           uint64_t *d_scratch, cudaStream_t s, const uint32_t *d_nq_dev = nullptr, const float *d_thr_fixed = nullptr,
                           uint32_t *d_overflow = nullptr, const uint32_t *d_filt = nullptr, uint32_t filt_words = 0,

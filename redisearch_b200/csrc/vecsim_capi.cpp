@@ -318,6 +318,13 @@ int VecSimB200_HybridTopKBatchDevice(VecSimIndex *index, const void *d_queries, 
     return IX(index)->hybrid_topk_batch_device(d_queries, nq, k, d_doc_ids, d_counts, caps, queryParams, d_out_labels, d_out_scores, d_out_counts,
                                                out_modes, static_cast<cudaStream_t>(stream));
 }
+int VecSimB200_HybridRangeQueryBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, const float *d_radii, size_t cap,
+                                           VecSimQueryReply_Order order, const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts,
+                                           const size_t *caps, VecSimQueryParams *queryParams, int64_t *d_out_labels, float *d_out_scores,
+                                           uint32_t *d_out_counts, int *out_modes, void *stream) {
+    return IX(index)->hybrid_range_batch_device(d_queries, nq, d_radii, cap, order, d_doc_ids, d_counts, caps, queryParams, d_out_labels,
+                                                d_out_scores, d_out_counts, out_modes, static_cast<cudaStream_t>(stream));
+}
 int VecSimB200_LastBatchPath(VecSimIndex *index) { return IX(index)->last_batch_path(); }
 void VecSimB200_SetCoarseMode(int mode) { rsb200::set_coarse_mode(mode); }
 int VecSimB200_LastCoarseFlags(VecSimIndex *index, uint32_t *out_ok, size_t nq) { return IX(index)->last_coarse_flags(out_ok, nq); }

@@ -2333,6 +2333,182 @@ int FlatIndex::hybrid_topk_batch_device(const void *d_q, size_t nq, size_t k, co
     return ok ? 0 : -1;
 }
 
+// Mode choice of a filtered range batch (DESIGN.md §4.13), from what the host already knows.  There is no sample pass, so no cap
+// floor: the batch takes a dense route as a whole when the bytes its gathers would read exceed what the dense route reads, the
+// rows of its main pass (`pass_bytes`), two passes over one row bitmap per query, and the lists.
+static constexpr size_t kHybridRangeMinDense = 16; // queries below which a dense route does not pay for its first shadow / table
+static bool hybrid_range_dense_pays(size_t cap_sum, size_t stored_bytes, double pass_bytes, size_t nq, size_t n) {
+    const double gather = (double)cap_sum * (double)(stored_bytes + 8), bitmaps = (double)nq * ((n + 31) / 32) * 4 * 2;
+    return gather > pass_bytes + bitmaps + 8.0 * (double)cap_sum;
+}
+
+// Filtered range batches (DESIGN.md §4.13): range_device's answer for each query restricted to its filter.  Either every query takes
+// the range form of the ragged gather, or the whole batch takes one of range_device's routes with the filter bitmaps applied to the
+// rows of its main pass; the gather then answers the queries that route left open.  Hits are gathered as (score key, row)
+// composites in d_labels itself and ordered by range_finish, as in range_device.  Launches: 2 on the gather alone; the fp32 route
+// 8 (+1 for L2 / inner product), the 8-bit route 6 (+1 for L2).
+int FlatIndex::hybrid_range_batch_device(const void *d_q, size_t nq, const float *d_radii, size_t cap, VecSimQueryReply_Order order,
+                                         const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts, const size_t *caps,
+                                         VecSimQueryParams *qp, int64_t *d_labels, float *d_scores, uint32_t *d_counts_out, int *out_modes,
+                                         cudaStream_t s) {
+    const int policy = qp ? (int)qp->searchMode : (int)EMPTY_MODE;
+    if (policy != EMPTY_MODE && policy != HYBRID_ADHOC_BF && policy != HYBRID_BATCHES) return -1;
+    if (cap == 0 || cap > kRangeDeviceMaxCap || (order != BY_ID && order != BY_SCORE) || nq > 0x7FFFFFFFull) return -1;
+    if (out_modes)
+        for (size_t i = 0; i < nq; i++) out_modes[i] = HYBRID_ADHOC_BF;
+    last_mode_ = RANGE_QUERY;
+    if (nq == 0) return 0;
+    size_t total = 0, max_cap = 0;
+    uint64_t blocks = 0;
+    for (size_t i = 0; i < nq; i++) {
+        if (caps[i] > 0xFFFFFFF0ull) return -2;
+        total += caps[i];
+        max_cap = std::max(max_cap, caps[i]);
+        blocks += ragged_blocks(caps[i]);
+    }
+    if (!flush()) return -1;
+    if (!sync_label_table()) return -2;
+    if (!sync_labels_to_device()) return -1;
+    const size_t n = count_;
+    const uint32_t nq32 = (uint32_t)nq, cap32 = (uint32_t)cap;
+    cudaStream_t st = s ? s : cudaStreamLegacy; // NULL = the legacy default stream, as everywhere in CUDA
+    const CorpusView v = view();
+    const int cmode = coarse_mode();
+    // 1: range_device's fp32 route, 2: its 8-bit fixed-radius route (each with range_device's eligibility), 0: the gather only
+    int path = 0;
+    if (policy != HYBRID_ADHOC_BF && !multi_ && n > 0 && coarse_fixed_enabled()) {
+        const bool r8 = (dtype_ == DT_I8 || dtype_ == DT_U8) && cmode != 0 && nq >= kHybridRangeMinDense &&
+                        coarse_supported(v, nq32, 1, CoarseDirect8);
+        const bool r32 = dtype_ == DT_F32 && cmode == 1 && !coarse_disabled_ && coarse_supported(v, nq32, 1, CoarseF16) &&
+                         (nq >= kHybridRangeMinDense || single_query_takes_coarse(1));
+        const double pass_bytes = (double)n * dim_ * (r8 ? 1 : 2); // the 8-bit rows, or the fp16 shadow
+        if ((r8 || r32) && (policy == HYBRID_BATCHES || hybrid_range_dense_pays(total, stored_bytes_, pass_bytes, nq, n))) {
+            if (r8 && (!int_l2() || ensure_shadow(st))) {
+                path = 2;
+            } else if (r32 && ensure_shadow(st)) {
+                path = 1;
+                if (!unit_rows() && !(shadow_max_abs_ <= 60000.0f)) { // values outside the fp16 range: exact scans from now on
+                    disable_coarse();
+                    path = 0;
+                }
+            }
+        }
+    }
+    if (out_modes && path)
+        for (size_t i = 0; i < nq; i++) out_modes[i] = HYBRID_BATCHES;
+    std::lock_guard<std::mutex> dg(dev_mu_);
+    if (!dev_ctx_) dev_ctx_ = checkout();
+    QueryCtx *c = dev_ctx_.get();
+    if (!c) return -1;
+    collect_dev_timing_locked();
+    const bool unit = unit_rows();
+    const CoarsePlan cp = path == 1   ? plan_coarse(v, nq32, CoarseF16, 1, 0, 1, 1, true)
+                          : path == 2 ? plan_coarse(v, nq32, CoarseDirect8, 1, 0, 1, 1, true)
+                                      : CoarsePlan{};
+    const size_t slots = (size_t)cp.grid_x * cp.keep, qpitch = query_pitch(), q16_pitch = (dim_ * 2 + 15) & ~(size_t)15;
+    const uint32_t words = path ? (uint32_t)((n + 31) / 32) : 0;
+    // pinned table: [docId pointers nq][count pointers nq][score offsets nq + 1][first chunks nq + 1], then u32 [nq] = 0, 1, ..:
+    // a dense route runs over the whole batch, so its positions are the queries themselves
+    const size_t tab_elems = 4 * nq + 2 + (nq + 1) / 2;
+    uint64_t *tab, *cand, *list_scratch;
+    uint8_t *q16;
+    float *d_qn2, *d_thr;
+    uint32_t *d_ovf, *d_total, *d_ok, *d_flags, *d_live, *bm;
+    const uint32_t **d_live_ptr;
+    const auto layout = [&](void *base) {
+        BatchScratch sc(base);
+        tab = sc.take<uint64_t>(tab_elems);
+        cand = sc.take<uint64_t>(path ? nq * slots : 0);
+        list_scratch = sc.take<uint64_t>(path ? cp.scratch_elems : 0);
+        q16 = sc.take<uint8_t>(path == 1 ? nq * q16_pitch : 0);
+        d_qn2 = sc.take<float>((path == 1 && !unit) || (path == 2 && int_l2()) ? nq : 0); // |q|^2 (fp32), or int32 for 8-bit L2
+        d_thr = sc.take<float>(path == 1 ? nq : 0);
+        d_ovf = sc.take<uint32_t>(path ? nq : 0);
+        d_total = sc.take<uint32_t>(1);
+        d_ok = sc.take<uint32_t>(path ? nq : 0); // the route proved the query
+        d_flags = sc.take<uint32_t>(nq);         // LastCoarseFlags
+        d_live = sc.take<uint32_t>(path ? nq : 0);
+        d_live_ptr = sc.take<const uint32_t *>(path ? nq : 0);
+        bm = sc.take<uint32_t>((size_t)(path ? nq : 0) * words);
+        return sc.words();
+    };
+    if (!c->need_cand(layout(nullptr))) return -1;
+    layout(c->d_cand);
+    TableSlot *slot = table_slot(tab_elems);
+    if (!slot) return -1;
+    uint64_t *h = slot->h, off = 0, blk = 0;
+    for (size_t i = 0; i < nq; i++) {
+        h[i] = (uint64_t)(uintptr_t)d_doc_ids[i];
+        h[nq + i] = d_counts ? (uint64_t)(uintptr_t)d_counts[i] : 0;
+        h[2 * nq + i] = off;
+        h[3 * nq + 1 + i] = blk;
+        off += caps[i];
+        blk += ragged_blocks(caps[i]);
+    }
+    h[3 * nq] = off;
+    h[4 * nq + 1] = blk;
+    uint32_t *h32 = reinterpret_cast<uint32_t *>(h + 4 * nq + 2);
+    for (uint32_t i = 0; i < nq32; i++) h32[i] = i;
+    const uint32_t *d_iota = reinterpret_cast<const uint32_t *>(tab + 4 * nq + 2);
+    bool ok = cudaMemcpyAsync(tab, h, tab_elems * 8, cudaMemcpyHostToDevice, st) == cudaSuccess;
+    ok = ok && cudaEventRecord(slot->ev, st) == cudaSuccess;
+    ok = ok && cudaMemsetAsync(d_counts_out, 0, nq * 4, st) == cudaSuccess;
+    const RaggedBatch b{reinterpret_cast<const uint32_t *const *>(tab), reinterpret_cast<const uint32_t *const *>(tab + nq), tab + 2 * nq, nq32};
+    RaggedBatch bg = b; // the gather's batch: every query, or (dense route) the open ones
+    LaunchCounters lc;
+    uint64_t *comp = reinterpret_cast<uint64_t *>(d_labels);
+    if (path) {
+        // 1. row-space filter bitmaps; 2. range_device's route over the whole batch with them; 3. the open queries to the gather
+        ok = ok && cudaMemsetAsync(bm, 0, (size_t)nq * words * 4, st) == cudaSuccess;
+        ok = ok && launch_filter_bitmaps(b, d_iota, nq32, max_cap, d_label_to_id_, (uint32_t)l2i_size_, bm, words, st, &lc) == cudaSuccess;
+        if (path == 1) {
+            ok = ok && launch_to_f16(d_q, qpitch, (uint32_t)dim_, 0, nq32, q16, q16_pitch, st) == cudaSuccess;
+            if (!unit) ok = ok && launch_row_stats(d_q, qpitch, (uint32_t)dim_, 0, nq32, d_qn2, nullptr, st) == cudaSuccess;
+            ok = ok && launch_range_bound(d_radii, nq32, kCoarseEpsF16, d_qn2, shadow_max_norm_, (uint32_t)dim_, mkind_ == MT_L2 ? 1 : 0, d_thr, d_ovf,
+                                          d_total, st) == cudaSuccess;
+            const CoarseOperands ops{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
+            cudaEventRecord(c->ev_start, st);
+            ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_thr, d_ovf, bm, words) == cudaSuccess;
+            cudaEventRecord(c->ev_stop, st);
+            ok = ok && launch_range_refine(v, d_q, qpitch, nq32, (uint32_t)slots, cand, d_radii, d_qn2, d_thr, d_ovf, comp, d_total, d_ok,
+                                           d_counts_out, nullptr, st, cap32) == cudaSuccess;
+            lc.launches += unit ? 4 : 5;
+        } else {
+            CoarseOperands ops{v.rows, v.pitch, d_q, qpitch, dtype_ == DT_I8 ? 1 : 0, mkind_ == MT_COS ? 1 : int_l2() ? 2 : 0, nullptr, nullptr};
+            ok = ok && cudaMemsetAsync(d_ovf, 0, nq * 4, st) == cudaSuccess;
+            if (int_l2()) {
+                ok = ok && launch_int_norm2(d_q, qpitch, v.dim, 0, nq32, dtype_ == DT_I8, reinterpret_cast<int32_t *>(d_qn2), st) == cudaSuccess;
+                ops.row_norm2 = reinterpret_cast<const float *>(d_norm2_); // int32 values (CoarseOperands)
+                ops.q_norm2 = d_qn2;
+                lc.launches++;
+            }
+            cudaEventRecord(c->ev_start, st);
+            ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_radii, d_ovf, bm, words) == cudaSuccess;
+            cudaEventRecord(c->ev_stop, st);
+            ok = ok && launch_range_pack(cand, nq32, (uint32_t)slots, d_ovf, cap32, comp, d_counts_out, d_ok, st) == cudaSuccess;
+            lc.launches += 2;
+        }
+        ok = ok && launch_hybrid_open(b, d_iota, d_ok, d_flags, d_live, d_live_ptr, st, &lc) == cudaSuccess;
+        bg.counts = d_live_ptr;
+    } else {
+        ok = ok && cudaMemsetAsync(d_flags, 0, nq * 4, st) == cudaSuccess;
+    }
+    // after a dense route most chunks of the caps are empty: a grid of a few CTAs per SM strides over them
+    const uint64_t max_grid = path ? (uint64_t)device_sm_count() * 16 : 0;
+    ok = ok && launch_gather_ragged_range(v, d_q, qpitch, bg, tab + 3 * nq + 1, blocks, d_label_to_id_, (uint32_t)l2i_size_,
+                                          multi_ ? d_label_rows_ : nullptr, d_radii, cap32, comp, d_counts_out, st, &lc, max_grid) == cudaSuccess;
+    ok = ok && launch_range_finish(d_labels, d_scores, d_counts_out, nq32, cap32, d_id_to_label_, order == BY_ID, st, &lc) == cudaSuccess;
+    c->d_last_ok = d_flags;
+    c->last_ok_n = nq32;
+    last_batch_coarse_ = true; // LastCoarseFlags: 1 = a dense route answered the query, 0 = the gather
+    last_batch_path_ = path;
+    if (path) coarse_batches_++;
+    dev_timing_pending_ = ok && path;
+    dev_timing_bytes_ = path == 2 ? (uint64_t)n * dim_ : (uint64_t)n * dim_ * 2;
+    launches_total_ += lc.launches;
+    return ok ? 0 : -1;
+}
+
 // ------------------------------------------------------------------------------------------------
 // request combiner for the stock single-query entry point (opt-in)
 // ------------------------------------------------------------------------------------------------

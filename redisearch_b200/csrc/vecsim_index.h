@@ -148,6 +148,11 @@ class FlatIndex {
     // the same answered per label on any index: VecSimB200_LabelRangeQueryBatchDevice (DESIGN.md §4.12)
     int label_range_batch_device(const void *d_q, size_t nq, const float *d_radii, size_t cap, VecSimQueryReply_Order order, int64_t *d_labels,
                                  float *d_scores, uint32_t *d_counts, cudaStream_t s);
+    // the same restricted to a filter per query, on the ragged gather or a filtered tensor-core route:
+    // VecSimB200_HybridRangeQueryBatchDevice (DESIGN.md §4.13)
+    int hybrid_range_batch_device(const void *d_q, size_t nq, const float *d_radii, size_t cap, VecSimQueryReply_Order order,
+                                  const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts, const size_t *caps, VecSimQueryParams *qp,
+                                  int64_t *d_labels, float *d_scores, uint32_t *d_counts_out, int *out_modes, cudaStream_t s);
     double distance_from(size_t label, const void *stored_form_blob);
     bool prefer_adhoc(size_t subset, size_t k, bool initial);
 

@@ -19,6 +19,7 @@
 #include "topk_common.cuh"
 
 #include <algorithm>
+#include <type_traits>
 #include <mutex>
 
 namespace rsb200 {
@@ -736,12 +737,23 @@ struct GatherRaggedArgs {
     const uint32_t *label_rows; // multi-value: rows of each label in insertion order
     float *scores;
 };
+// the range form's (RANGE) outputs in place of the scores: radii [nq], the [nq][cap] composite slots and their counters (zeroed
+// by the caller)
+struct GatherRangeArgs : GatherRaggedArgs {
+    const float *radii;
+    uint32_t cap;
+    uint64_t *out;
+    uint32_t *counts;
+};
 
 // One chunk = kRaggedPerBlock consecutive entries of ONE query (its blob stays in shared memory), one warp per entry, with the
 // arithmetic of gather_kernel (single-value) / gather_min_kernel's fold (multi-value).  A chunk past its query's device count ends
 // after reading the count.  CTA i takes chunks i, i + gridDim.x, ... (one each when the grid covers them all).
-template <int DT, int MT, bool MULTI>
-__global__ void __launch_bounds__(kScanThreads) gather_ragged_kernel(const GatherRaggedArgs a) {
+// RANGE (DESIGN.md §4.13): no scores; an entry whose distance is <= its query's radius appends one composite (score key, row) to
+// the query's cap slots, counted past cap.  Multi-value: the smallest composite over the label's PASSING rows (a NaN row never
+// passes, so it cannot reset the fold as it does getDistanceFrom's).
+template <int DT, int MT, bool MULTI, bool RANGE = false>
+__global__ void __launch_bounds__(kScanThreads) gather_ragged_kernel(const std::conditional_t<RANGE, GatherRangeArgs, GatherRaggedArgs> a) {
     extern __shared__ __align__(16) uint8_t smem[];
     using Tile = DistTile<DT, MT, 1, 1>;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -770,7 +782,41 @@ __global__ void __launch_bounds__(kScanThreads) gather_ragged_kernel(const Gathe
         float *out = a.scores + a.b.off[q];
         for (uint32_t w = e0 + warp; w < e1; w += kScanWarps) {
             const uint32_t l = ids[w];
-            if (MULTI) {
+            if constexpr (RANGE) {
+                const float radius = a.radii[q];
+                uint64_t best = ~0ull;
+                if (MULTI) {
+                    uint32_t r = 0, e = 0;
+                    if (l < a.table_size) {
+                        r = a.table[l];
+                        e = a.table[l + 1];
+                    }
+                    uint32_t id = r < e ? a.label_rows[r] : 0u;
+#pragma unroll 1
+                    for (; r < e; r++) {
+                        const uint32_t row = id;
+                        const uint8_t *rowb[1] = {a.rows + (size_t)row * a.pitch};
+                        if (r + 1 < e) id = a.label_rows[r + 1];
+                        float d[1];
+                        Tile::run(rowb, qb, a.dim, lane, d);
+                        if (lane == 0 && d[0] <= radius) { // brute_force.h:315 (NaN never passes)
+                            const uint64_t c = make_composite(d[0], row);
+                            best = c < best ? c : best;
+                        }
+                    }
+                } else {
+                    const uint32_t id = l < a.table_size ? a.table[l] : 0xFFFFFFFFu;
+                    if (id == 0xFFFFFFFFu) continue;
+                    const uint8_t *rowb[1] = {a.rows + (size_t)id * a.pitch};
+                    float d[1];
+                    Tile::run(rowb, qb, a.dim, lane, d);
+                    if (lane == 0 && d[0] <= radius) best = make_composite(d[0], id);
+                }
+                if (lane == 0 && best != ~0ull) {
+                    const uint32_t pos = atomicAdd(a.counts + q, 1u);
+                    if (pos < a.cap) a.out[(size_t)q * a.cap + pos] = best;
+                }
+            } else if (MULTI) {
                 uint32_t r = 0, e = 0;
                 if (l < a.table_size) {
                     r = a.table[l];
@@ -1361,21 +1407,17 @@ cudaError_t launch_gather_min_distances(const CorpusView &c, const void *d_query
     return e;
 }
 
-template <int DT, int MT, bool MULTI>
-static cudaError_t launch_gather_ragged_inst(const GatherRaggedArgs &a, uint64_t grid, cudaStream_t s) {
-    auto kern = gather_ragged_kernel<DT, MT, MULTI>;
+template <int DT, int MT, bool MULTI, bool RANGE = false, class Args>
+static cudaError_t launch_gather_ragged_inst(const Args &a, uint64_t grid, cudaStream_t s) {
+    auto kern = gather_ragged_kernel<DT, MT, MULTI, RANGE>;
     cudaError_t e = ensure_smem(kern, a.q_smem_pitch);
     if (e != cudaSuccess) return e;
     kern<<<(uint32_t)grid, kScanThreads, a.q_smem_pitch, s>>>(a);
     return cudaGetLastError();
 }
 
-cudaError_t launch_gather_ragged(const CorpusView &c, const void *d_queries, size_t qpitch, const RaggedBatch &b, const uint64_t *d_blk,
-                                 uint64_t n_blocks, const uint32_t *d_table, uint32_t table_size, const uint32_t *d_label_rows, float *d_scores,
-                                 cudaStream_t s, LaunchCounters *ctr, uint64_t max_grid) {
-    if (n_blocks == 0 || b.nq == 0) return cudaSuccess;
-    const uint64_t grid = max_grid ? std::min(n_blocks, max_grid) : n_blocks;
-    if (grid > 0x7FFFFFFFull) return cudaErrorInvalidValue;
+static GatherRaggedArgs gather_ragged_args(const CorpusView &c, const void *d_queries, size_t qpitch, const RaggedBatch &b, const uint64_t *d_blk,
+                                           uint64_t n_blocks, const uint32_t *d_table, uint32_t table_size, const uint32_t *d_label_rows) {
     GatherRaggedArgs a{};
     a.rows = static_cast<const uint8_t *>(c.rows);
     a.pitch = c.pitch;
@@ -1389,12 +1431,44 @@ cudaError_t launch_gather_ragged(const CorpusView &c, const void *d_queries, siz
     a.table = d_table;
     a.table_size = table_size;
     a.label_rows = d_label_rows;
+    return a;
+}
+
+cudaError_t launch_gather_ragged(const CorpusView &c, const void *d_queries, size_t qpitch, const RaggedBatch &b, const uint64_t *d_blk,
+                                 uint64_t n_blocks, const uint32_t *d_table, uint32_t table_size, const uint32_t *d_label_rows, float *d_scores,
+                                 cudaStream_t s, LaunchCounters *ctr, uint64_t max_grid) {
+    if (n_blocks == 0 || b.nq == 0) return cudaSuccess;
+    const uint64_t grid = max_grid ? std::min(n_blocks, max_grid) : n_blocks;
+    if (grid > 0x7FFFFFFFull) return cudaErrorInvalidValue;
+    GatherRaggedArgs a = gather_ragged_args(c, d_queries, qpitch, b, d_blk, n_blocks, d_table, table_size, d_label_rows);
     a.scores = d_scores;
     cudaError_t e = cudaErrorInvalidValue;
 #define CALL_GATHER_RAGGED(DT, MT)                                                                       \
     e = d_label_rows ? launch_gather_ragged_inst<DT, MT, true>(a, grid, s) : launch_gather_ragged_inst<DT, MT, false>(a, grid, s)
     RSB_DISPATCH_DM(c.dtype, c.metric, CALL_GATHER_RAGGED)
 #undef CALL_GATHER_RAGGED
+    if (ctr) ctr->launches++;
+    return e;
+}
+
+cudaError_t launch_gather_ragged_range(const CorpusView &c, const void *d_queries, size_t qpitch, const RaggedBatch &b, const uint64_t *d_blk,
+                                       uint64_t n_blocks, const uint32_t *d_table, uint32_t table_size, const uint32_t *d_label_rows,
+                                       const float *d_radii, uint32_t cap, uint64_t *d_out, uint32_t *d_counts, cudaStream_t s, LaunchCounters *ctr,
+                                       uint64_t max_grid) {
+    if (n_blocks == 0 || b.nq == 0) return cudaSuccess;
+    const uint64_t grid = max_grid ? std::min(n_blocks, max_grid) : n_blocks;
+    if (grid > 0x7FFFFFFFull || cap == 0) return cudaErrorInvalidValue;
+    GatherRangeArgs a;
+    static_cast<GatherRaggedArgs &>(a) = gather_ragged_args(c, d_queries, qpitch, b, d_blk, n_blocks, d_table, table_size, d_label_rows);
+    a.radii = d_radii;
+    a.cap = cap;
+    a.out = d_out;
+    a.counts = d_counts;
+    cudaError_t e = cudaErrorInvalidValue;
+#define CALL_GATHER_RANGE(DT, MT)                                                                        \
+    e = d_label_rows ? launch_gather_ragged_inst<DT, MT, true, true>(a, grid, s) : launch_gather_ragged_inst<DT, MT, false, true>(a, grid, s)
+    RSB_DISPATCH_DM(c.dtype, c.metric, CALL_GATHER_RANGE)
+#undef CALL_GATHER_RANGE
     if (ctr) ctr->launches++;
     return e;
 }

@@ -137,6 +137,14 @@ inline uint64_t ragged_blocks(size_t cap) { return (cap + kRaggedPerBlock - 1) /
 cudaError_t launch_gather_ragged(const CorpusView &c, const void *d_queries, size_t qpitch, const RaggedBatch &b, const uint64_t *d_blk,
                                  uint64_t n_blocks, const uint32_t *d_table, uint32_t table_size, const uint32_t *d_label_rows, float *d_scores,
                                  cudaStream_t s, LaunchCounters *ctr, uint64_t max_grid = 0);
+// range form (DESIGN.md §4.13): no scores; every live entry whose distance is <= d_radii[q] (a float compare, NaN never passes)
+// appends one composite (score key, row) to d_out[q * cap, ...) unordered, atomically counted in d_counts[q] (zeroed by the caller)
+// past cap too.  Multi-value: an entry passes iff one of its label's rows does, with the smallest passing (score key, row).  One
+// launch, the grid of launch_gather_ragged
+cudaError_t launch_gather_ragged_range(const CorpusView &c, const void *d_queries, size_t qpitch, const RaggedBatch &b, const uint64_t *d_blk,
+                                       uint64_t n_blocks, const uint32_t *d_table, uint32_t table_size, const uint32_t *d_label_rows,
+                                       const float *d_radii, uint32_t cap, uint64_t *d_out, uint32_t *d_counts, cudaStream_t s, LaunchCounters *ctr,
+                                       uint64_t max_grid = 0);
 // CTAs per query of the segmented select (their lists: parts * 8 per query and chunk)
 uint32_t plan_ragged_select_parts(size_t max_cap, uint32_t nq);
 // d_out [nq][k] = each query's k smallest (score, position) composites over its live scores, ascending, kEmptySlot-padded;

@@ -141,6 +141,8 @@ SIGNATURES = [
     ("VecSimB200_TopKQueryBatchDevice", C.c_int, [_P, _P, _SZ, _SZ, _P, _P, _P]),
     ("VecSimB200_RangeQueryBatchDevice", C.c_int, [_P, _P, _SZ, _P, _SZ, C.c_int, _P, _P, _P, _P]),
     ("VecSimB200_LabelRangeQueryBatchDevice", C.c_int, [_P, _P, _SZ, _P, _SZ, C.c_int, _P, _P, _P, _P]),
+    ("VecSimB200_HybridRangeQueryBatchDevice", C.c_int,
+     [_P, _P, _SZ, _P, _SZ, C.c_int, _P, _P, _P, C.POINTER(VecSimQueryParams), _P, _P, _P, _P, _P]),
     ("VecSimB200_RangeQueryBatch", C.c_int, [_P, _P, _SZ, _SZ, _P, C.POINTER(VecSimQueryParams), C.c_int, _P, _P]),
     ("VecSimB200_AddVectors", C.c_int, [_P, _P, _SZ, _SZ, _P, _SZ]),
     ("VecSimB200_AddVectorsDevice", C.c_int, [_P, _P, _SZ, _SZ]),
@@ -363,6 +365,34 @@ class VecSimIndex:
         label at its best passing row, counts in labels).  Returns (labels, scores, counts, rc); rc -2 = labels too sparse."""
         return self._range_device(self.L.VecSimB200_LabelRangeQueryBatchDevice, d_queries, d_radii, cap, order, out_labels, out_scores,
                                   out_counts, stream)
+
+    def hybrid_range_batch_device(self, d_queries, d_radii, cap, doc_ids, caps, counts=None, order=BY_SCORE, params=None, out_labels=None,
+                                  out_scores=None, out_counts=None, stream=None):
+        """VecSimB200_HybridRangeQueryBatchDevice: label_range_batch_device restricted to a filter per query.  doc_ids / counts / caps
+        as in hybrid_topk_batch_device; params: a VecSimQueryParams whose searchMode picks the policy (None = automatic).  Returns
+        (labels, scores, counts, modes, rc); modes[i] = HYBRID_ADHOC_BF or HYBRID_BATCHES, the route query i took."""
+        import torch
+
+        nq = len(caps)
+        dev = torch.device("cuda")
+        if out_labels is None:
+            out_labels = torch.empty((nq, max(cap, 0)), dtype=torch.int64, device=dev)
+        if out_scores is None:
+            out_scores = torch.empty((nq, max(cap, 0)), dtype=torch.float32, device=dev)
+        if out_counts is None:
+            out_counts = torch.empty(nq, dtype=torch.int32, device=dev)
+        n = max(1, nq)
+        ids = (C.c_void_p * n)(*[int(p) if p else None for p in doc_ids])
+        cnt = (C.c_void_p * n)(*[int(p) if p else None for p in counts]) if counts is not None else None
+        cap_arr = (C.c_size_t * n)(*[int(c) for c in caps])
+        modes = np.zeros(n, dtype=np.int32)
+        qp = d_queries.data_ptr() if hasattr(d_queries, "data_ptr") else int(d_queries)
+        rp = d_radii.data_ptr() if hasattr(d_radii, "data_ptr") else int(d_radii)
+        sh = None if stream is None else C.c_void_p(int(getattr(stream, "cuda_stream", stream)) or None)
+        rc = self.L.VecSimB200_HybridRangeQueryBatchDevice(self.h, C.c_void_p(qp), nq, C.c_void_p(rp), cap, order, ids, cnt, cap_arr,
+                                                           C.byref(params) if params is not None else None, C.c_void_p(out_labels.data_ptr()),
+                                                           C.c_void_p(out_scores.data_ptr()), C.c_void_p(out_counts.data_ptr()), _ptr(modes), sh)
+        return out_labels, out_scores, out_counts, modes[:nq], rc
 
     def _range_device(self, fn, d_queries, d_radii, cap, order, out_labels, out_scores, out_counts, stream):
         import torch
