@@ -552,6 +552,48 @@ int VecSimB200_ShardGroup_TopKBatchDevice(VecSimB200_ShardGroup *g, VecSimIndex 
  * merge, D2H inside the call).  Empty slots: label SIZE_MAX, score NaN.  The same limits on k.  Returns 0 / -1. */
 int VecSimB200_ShardGroup_TopKBatch(VecSimB200_ShardGroup *g, VecSimIndex *shard, const void *queryBlobs, size_t qstride, size_t nq,
                                     size_t k, size_t *out_labels, double *out_scores);
+/* ---- sharded filtered KNN, range and filtered range batches (DESIGN.md §6.1) ----------------------------------------------------
+ * The counted exchange block of one rank: [labels int64 x nq*w][scores float x nq*w][counts u32 x nq], padded to 16 bytes.  Row i and
+ * counts[i] are what the rank's local device call wrote for query i: KNN, the entries written (<= w); range, the true number of hits
+ * (past w the row is all -1); UINT32_MAX, the rank could not answer.  Blocks are rank-major after an all-gather. */
+size_t VecSimB200_ShardListBlockBytes(size_t nq, size_t w);
+/* Merge of G such blocks on the device into [nq][w] labels / scores and [nq] counts, enqueued on `stream` (NULL = the legacy default
+ * stream).  range == 0 (top-w, BY_SCORE only): the first w entries of the union by (score, label), count = min(w, sum of counts).
+ * range == 1: total = the sum of the counts (saturating at UINT32_MAX); total > w gives the row all -1 / NaN with count = total (the cap
+ * rule of the range calls), otherwise the union in the local calls' order (BY_SCORE: (score, label); BY_ID: label), count = total.  A
+ * rank with count UINT32_MAX makes the row empty with count UINT32_MAX.  Entries sort by the key the local calls sort by (-0.0 ties
+ * +0.0, ties break by label, then by rank) and keep their score bits, so merging the shards of a corpus whose labels each live on one
+ * shard gives, bit for bit, the rows the local call gives on one index holding the whole corpus.  Runs must be sorted, as every local
+ * call writes them.  One launch, O(G m log m) per query for runs of m entries.
+ * Returns 0; -1, before any CUDA call, for G == 0, w == 0 or w > 4096, nq > 2^31, range not 0 / 1, an order other than BY_SCORE /
+ * BY_ID, BY_ID with range == 0; -1 for a CUDA failure. */
+int VecSimB200_MergeShardListBlocks(const void *d_blocks, size_t G, size_t nq, size_t w, int range, VecSimQueryReply_Order order,
+                                    int64_t *d_out_labels, float *d_out_scores, uint32_t *d_out_counts, void *stream);
+/* Collectives: this rank's local call (VecSimB200_HybridTopKBatchDevice, VecSimB200_LabelRangeQueryBatchDevice,
+ * VecSimB200_HybridRangeQueryBatchDevice) writes straight into the group's send block, ONE ncclAllGather, the list merge; every
+ * rank receives the merged rows and counts.  Arguments mean what they mean in the local call; the filters are THIS rank's docIds (its
+ * slice of each posting list, cut at the shard boundaries), and out_modes / VecSimB200_LastCoarseFlags report this rank's routes.
+ * Shards hold disjoint labels (a multi-value label's rows all on one shard): the merged rows, scores and counts are then bit-equal to
+ * the local call on one index holding every shard's rows, with the union of the filters.  world == 1: the call IS the local call (no
+ * NCCL is loaded).  Launches: the local call's + 1 all-gather + 1 merge, enqueued on `stream`; the host waits for nothing beyond what
+ * the local call waits for.  The group's blocks grow under its mutex.  An empty shard takes part with counts 0.
+ * Failures never leave a rank waiting in the all-gather: refusals from the shared arguments (k > 1024, cap outside 1..4096, an order
+ * other than BY_SCORE / BY_ID, a bad searchMode, nq > 2^31) return -1 on every rank before anything is enqueued; a refusal of the
+ * local call itself (-2 for labels too sparse for the docId table or a cap beyond the 32-bit range, -1 for a failed flush) still
+ * takes part with a block of counts UINT32_MAX and returns its code, and every rank's merged rows come out empty with count
+ * UINT32_MAX.  A CUDA or NCCL failure after the enqueue is -1. */
+int VecSimB200_ShardGroup_HybridTopKBatchDevice(VecSimB200_ShardGroup *g, VecSimIndex *shard, const void *d_queries, size_t nq, size_t k,
+                                                const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts, const size_t *caps,
+                                                VecSimQueryParams *queryParams, int64_t *d_out_labels, float *d_out_scores,
+                                                uint32_t *d_out_counts, int *out_modes, void *stream);
+int VecSimB200_ShardGroup_RangeQueryBatchDevice(VecSimB200_ShardGroup *g, VecSimIndex *shard, const void *d_queries, size_t nq,
+                                                const float *d_radii, size_t cap, VecSimQueryReply_Order order, int64_t *d_out_labels,
+                                                float *d_out_scores, uint32_t *d_out_counts, void *stream);
+int VecSimB200_ShardGroup_HybridRangeQueryBatchDevice(VecSimB200_ShardGroup *g, VecSimIndex *shard, const void *d_queries, size_t nq,
+                                                      const float *d_radii, size_t cap, VecSimQueryReply_Order order,
+                                                      const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts, const size_t *caps,
+                                                      VecSimQueryParams *queryParams, int64_t *d_out_labels, float *d_out_scores,
+                                                      uint32_t *d_out_counts, int *out_modes, void *stream);
 /* The whole HybridIterator state machine of src/iterators/hybrid_reader.c in one call: mode choice (:668-691:
  * VecSimIndex_PreferAdHocSearch on the child's estimate unless qp->searchMode forces a policy), HYBRID_BATCHES with the
  * reference's batch-size formula (:400-404), the alternating merge of each BY_ID batch with the child (:140-169) and the

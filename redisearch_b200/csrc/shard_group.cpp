@@ -4,6 +4,7 @@
 // VS/utils/query_result_utils.h:19-23.  NCCL is bound at run time (dlopen of libnccl.so.2: the copy the host process
 // already loaded — PyTorch's, or the system library for a C host), so libvecsim_b200.so has no link-time dependency
 // on it and single-GPU users never load it.
+#include "topk_common.cuh"
 #include "vecsim_index.h"
 
 #include <dlfcn.h>
@@ -115,7 +116,105 @@ struct VecSimB200_ShardGroup {
     }
 };
 
+namespace {
+// Counted exchange block of one rank (DESIGN.md §6.1): [labels int64 x nq*w][scores float x nq*w][counts u32 x nq], padded to 16 bytes
+size_t list_block_bytes(size_t nq, size_t w) { return align16(nq * w * 12 + nq * 4); }
+
+// Refusals every rank makes alike, from the arguments they share, before anything is enqueued
+bool shared_mode_ok(const VecSimQueryParams *qp) {
+    const int m = qp ? (int)qp->searchMode : (int)EMPTY_MODE;
+    return m == EMPTY_MODE || m == HYBRID_ADHOC_BF || m == HYBRID_BATCHES;
+}
+bool shared_range_ok(size_t nq, size_t cap, VecSimQueryReply_Order order) {
+    return cap >= 1 && cap <= rsb200::kRangeDeviceMaxCap && (order == BY_SCORE || order == BY_ID) && nq <= (1ull << 31);
+}
+
+// The body of the list collectives: `local(labels, scores, counts)` is this rank's local call, writing its rows straight into the
+// send block; ONE all-gather; the list merge.  A local refusal (its shard, its filters, a failed flush) still takes part in the
+// exchange with a failed block (counts UINT32_MAX), so no rank is left waiting in the all-gather and every rank's merged rows come
+// out failed; the call then returns the local code.
+template <class Local>
+int list_collective(VecSimB200_ShardGroup *g, size_t nq, size_t w, bool range, VecSimQueryReply_Order order, int64_t *d_out_labels,
+                    float *d_out_scores, uint32_t *d_out_counts, cudaStream_t st, Local local) {
+    const size_t n = nq * w, block = list_block_bytes(nq, w);
+    {
+        std::lock_guard<std::mutex> lk(g->mu);
+        if (!g->need_block(block)) return -1;
+    }
+    const int rc = local(reinterpret_cast<int64_t *>(g->d_send), reinterpret_cast<float *>(g->d_send + n * 8),
+                         reinterpret_cast<uint32_t *>(g->d_send + n * 12));
+    if (rc != 0 && cudaMemsetAsync(g->d_send, 0xFF, block, st) != cudaSuccess) return -1;
+    if (!nccl_ok(nccl().AllGather(g->d_send, g->d_recv, block, /* ncclInt8 */ 0, g->comm, st), "ncclAllGather")) return -1;
+    if (rsb200::launch_merge_lists(g->d_recv, block, (uint32_t)g->world, (uint32_t)nq, (uint32_t)w, range, order == BY_ID, d_out_labels,
+                                   d_out_scores, d_out_counts, st, nullptr) != cudaSuccess)
+        return -1;
+    return rc;
+}
+} // namespace
+
 extern "C" {
+
+size_t VecSimB200_ShardListBlockBytes(size_t nq, size_t w) { return list_block_bytes(nq, w); }
+
+int VecSimB200_MergeShardListBlocks(const void *d_blocks, size_t G, size_t nq, size_t w, int range, VecSimQueryReply_Order order,
+                                    int64_t *d_out_labels, float *d_out_scores, uint32_t *d_out_counts, void *stream) {
+    if (G == 0 || G > 0xFFFFFFFFull || w == 0 || w > rsb200::kMaxListWidth || nq > (1ull << 31) || (range != 0 && range != 1) ||
+        (order != BY_SCORE && order != BY_ID) || (order == BY_ID && range == 0))
+        return -1;
+    return rsb200::launch_merge_lists(d_blocks, list_block_bytes(nq, w), (uint32_t)G, (uint32_t)nq, (uint32_t)w, range == 1, order == BY_ID,
+                                      d_out_labels, d_out_scores, d_out_counts, static_cast<cudaStream_t>(stream), nullptr) == cudaSuccess
+               ? 0
+               : -1;
+}
+
+int VecSimB200_ShardGroup_HybridTopKBatchDevice(VecSimB200_ShardGroup *g, VecSimIndex *shard, const void *d_queries, size_t nq, size_t k,
+                                                const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts, const size_t *caps,
+                                                VecSimQueryParams *queryParams, int64_t *d_out_labels, float *d_out_scores,
+                                                uint32_t *d_out_counts, int *out_modes, void *stream) {
+    if (!g || !shard) return -1;
+    FlatIndex *ix = reinterpret_cast<FlatIndex *>(shard);
+    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : cudaStreamLegacy;
+    if (g->world == 1)
+        return ix->hybrid_topk_batch_device(d_queries, nq, k, d_doc_ids, d_counts, caps, queryParams, d_out_labels, d_out_scores, d_out_counts,
+                                            out_modes, st);
+    if (!shared_mode_ok(queryParams) || k > (size_t)rsb200::kMaxWideK || nq > (1ull << 31)) return -1;
+    if (nq == 0 || k == 0) return 0;
+    return list_collective(g, nq, k, false, BY_SCORE, d_out_labels, d_out_scores, d_out_counts, st, [&](int64_t *l, float *s, uint32_t *c) {
+        return ix->hybrid_topk_batch_device(d_queries, nq, k, d_doc_ids, d_counts, caps, queryParams, l, s, c, out_modes, st);
+    });
+}
+
+int VecSimB200_ShardGroup_RangeQueryBatchDevice(VecSimB200_ShardGroup *g, VecSimIndex *shard, const void *d_queries, size_t nq,
+                                                const float *d_radii, size_t cap, VecSimQueryReply_Order order, int64_t *d_out_labels,
+                                                float *d_out_scores, uint32_t *d_out_counts, void *stream) {
+    if (!g || !shard) return -1;
+    FlatIndex *ix = reinterpret_cast<FlatIndex *>(shard);
+    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : cudaStreamLegacy;
+    if (g->world == 1) return ix->label_range_batch_device(d_queries, nq, d_radii, cap, order, d_out_labels, d_out_scores, d_out_counts, st);
+    if (!shared_range_ok(nq, cap, order)) return -1;
+    if (nq == 0) return 0;
+    return list_collective(g, nq, cap, true, order, d_out_labels, d_out_scores, d_out_counts, st, [&](int64_t *l, float *s, uint32_t *c) {
+        return ix->label_range_batch_device(d_queries, nq, d_radii, cap, order, l, s, c, st);
+    });
+}
+
+int VecSimB200_ShardGroup_HybridRangeQueryBatchDevice(VecSimB200_ShardGroup *g, VecSimIndex *shard, const void *d_queries, size_t nq,
+                                                      const float *d_radii, size_t cap, VecSimQueryReply_Order order,
+                                                      const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts, const size_t *caps,
+                                                      VecSimQueryParams *queryParams, int64_t *d_out_labels, float *d_out_scores,
+                                                      uint32_t *d_out_counts, int *out_modes, void *stream) {
+    if (!g || !shard) return -1;
+    FlatIndex *ix = reinterpret_cast<FlatIndex *>(shard);
+    cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : cudaStreamLegacy;
+    if (g->world == 1)
+        return ix->hybrid_range_batch_device(d_queries, nq, d_radii, cap, order, d_doc_ids, d_counts, caps, queryParams, d_out_labels,
+                                             d_out_scores, d_out_counts, out_modes, st);
+    if (!shared_mode_ok(queryParams) || !shared_range_ok(nq, cap, order)) return -1;
+    if (nq == 0) return 0;
+    return list_collective(g, nq, cap, true, order, d_out_labels, d_out_scores, d_out_counts, st, [&](int64_t *l, float *s, uint32_t *c) {
+        return ix->hybrid_range_batch_device(d_queries, nq, d_radii, cap, order, d_doc_ids, d_counts, caps, queryParams, l, s, c, out_modes, st);
+    });
+}
 
 // Exchange format of one shard: [labels int64 x nq*k][scores float x nq*k], padded to 16 bytes.
 size_t VecSimB200_ShardBlockBytes(size_t nq, size_t k) { return align16(nq * k * 12); }

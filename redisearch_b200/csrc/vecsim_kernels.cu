@@ -980,6 +980,76 @@ __global__ void merge_shards_kernel(const float *__restrict__ scores, const int6
     }
 }
 
+// Counted exchange blocks (DESIGN.md §6.1): per rank [labels int64 x nq*w][scores float x nq*w][counts u32 x nq], block_bytes
+// apart.  Entry (score key, label) of a BY_SCORE run or (label, score key) of a BY_ID run: the composite the local calls sort by.
+struct ListEntry {
+    uint32_t key;
+    uint64_t label;
+};
+__device__ __forceinline__ bool list_before(const ListEntry &a, const ListEntry &b, int by_id) {
+    return by_id ? (a.label < b.label || (a.label == b.label && a.key < b.key)) : (a.key < b.key || (a.key == b.key && a.label < b.label));
+}
+__device__ __forceinline__ ListEntry list_entry(const int64_t *labels, const float *scores, size_t i) {
+    return ListEntry{orderable_key(scores[i]), (uint64_t)labels[i]};
+}
+
+// One CTA per (query, rank): each entry of the rank's sorted run finds its place in the merged row as its index in the run plus,
+// for every other run, a lower bound of its key (ties go to the smaller rank), so the places of all runs are a permutation of
+// [0, sum of run lengths): O(G m log m) per query.  Scores are copied bit for bit.  The rank-0 CTA writes the count and pads the
+// row past the merged entries; a failed rank (count UINT32_MAX) or, for range rows, a total past w pads the whole row.
+__global__ void __launch_bounds__(256) merge_lists_kernel(const uint8_t *__restrict__ blocks, size_t block_bytes, uint32_t G, uint32_t nq,
+                                                          uint32_t w, int range, int by_id, int64_t *__restrict__ out_labels,
+                                                          float *__restrict__ out_scores, uint32_t *__restrict__ out_counts) {
+    const size_t nw = (size_t)nq * w;
+    const float nan = range ? __int_as_float(0x7fffffff) : __uint_as_float(0x7FC00000u); // the pad of range_finish / unpack_ragged
+    for (uint64_t u = blockIdx.x; u < (uint64_t)nq * G; u += gridDim.x) {
+        const uint32_t q = (uint32_t)(u / G), g = (uint32_t)(u - (uint64_t)q * G);
+        uint64_t total = 0, merged = 0;
+        bool failed = false;
+        for (uint32_t h = 0; h < G; h++) {
+            const uint32_t c = reinterpret_cast<const uint32_t *>(blocks + (size_t)h * block_bytes + nw * 12)[q];
+            failed |= c == 0xFFFFFFFFu;
+            total += c;
+            merged += min(c, w);
+        }
+        const bool blank = failed || (range && total > w);
+        int64_t *L = out_labels + (size_t)q * w;
+        float *S = out_scores + (size_t)q * w;
+        if (g == 0) {
+            if (threadIdx.x == 0)
+                out_counts[q] = failed ? 0xFFFFFFFFu : range ? (uint32_t)min(total, (uint64_t)0xFFFFFFFFu) : (uint32_t)min(total, (uint64_t)w);
+            const uint32_t from = blank ? 0u : (uint32_t)min(merged, (uint64_t)w);
+            for (uint32_t i = from + threadIdx.x; i < w; i += blockDim.x) L[i] = -1, S[i] = nan;
+        }
+        if (blank) continue;
+        const uint8_t *mine = blocks + (size_t)g * block_bytes;
+        const uint32_t m = min(reinterpret_cast<const uint32_t *>(mine + nw * 12)[q], w);
+        const int64_t *ml = reinterpret_cast<const int64_t *>(mine) + (size_t)q * w;
+        const float *ms = reinterpret_cast<const float *>(mine + nw * 8) + (size_t)q * w;
+        for (uint32_t p = threadIdx.x; p < m; p += blockDim.x) {
+            const ListEntry e = list_entry(ml, ms, p);
+            uint64_t pos = p;
+            for (uint32_t h = 0; h < G && pos < w; h++) {
+                if (h == g) continue;
+                const uint8_t *other = blocks + (size_t)h * block_bytes;
+                const int64_t *hl = reinterpret_cast<const int64_t *>(other) + (size_t)q * w;
+                const float *hs = reinterpret_cast<const float *>(other + nw * 8) + (size_t)q * w;
+                uint32_t lo = 0, hi = min(reinterpret_cast<const uint32_t *>(other + nw * 12)[q], w);
+                while (lo < hi) { // entries of run h placed before e: key <= e's for h < g, key < e's for h > g
+                    const uint32_t mid = (lo + hi) >> 1;
+                    const ListEntry o = list_entry(hl, hs, mid);
+                    if (h < g ? !list_before(e, o, by_id) : list_before(o, e, by_id))
+                        lo = mid + 1;
+                    else
+                        hi = mid;
+                }
+                pos += lo;
+            }
+            if (pos < w) L[pos] = ml[p], S[pos] = ms[p];
+        }
+    }
+}
+
 // ================================================================================================
 // host side: dispatch
 // ================================================================================================
@@ -1549,6 +1619,16 @@ cudaError_t launch_merge_shards(const float *d_scores, const int64_t *d_labels, 
     cudaError_t e = ensure_smem(merge_shards_kernel, smem);
     if (e != cudaSuccess) return e;
     merge_shards_kernel<<<nq, 256, smem, s>>>(d_scores, d_labels, G, nq, k, score_stride, label_stride, d_out_scores, d_out_labels);
+    if (ctr) ctr->launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_merge_lists(const void *d_blocks, size_t block_bytes, uint32_t G, uint32_t nq, uint32_t w, bool range, bool by_id,
+                               int64_t *d_out_labels, float *d_out_scores, uint32_t *d_out_counts, cudaStream_t s, LaunchCounters *ctr) {
+    if (nq == 0) return cudaSuccess;
+    const uint64_t grid = std::min<uint64_t>((uint64_t)nq * G, 1u << 20);
+    merge_lists_kernel<<<(unsigned)grid, 256, 0, s>>>(static_cast<const uint8_t *>(d_blocks), block_bytes, G, nq, w, range ? 1 : 0,
+                                                      by_id ? 1 : 0, d_out_labels, d_out_scores, d_out_counts);
     if (ctr) ctr->launches++;
     return cudaGetLastError();
 }

@@ -186,5 +186,10 @@ cudaError_t launch_unpack_results(const uint64_t *d_comp, uint32_t nq, uint32_t 
 cudaError_t launch_merge_shards(const float *d_scores, const int64_t *d_labels, uint32_t G, uint32_t nq,
                                 uint32_t k, float *d_out_scores, int64_t *d_out_labels, cudaStream_t s,
                                 LaunchCounters *ctr, size_t score_stride = 0, size_t label_stride = 0);
+// G counted exchange blocks, block_bytes apart (layout: VecSimB200_ShardListBlockBytes) -> the merged [nq][w] rows and counts
+// (DESIGN.md §6.1).  range: the cap rule of the range calls; by_id: runs ordered by label (range rows only).  One launch.
+constexpr uint32_t kMaxListWidth = 4096;
+cudaError_t launch_merge_lists(const void *d_blocks, size_t block_bytes, uint32_t G, uint32_t nq, uint32_t w, bool range, bool by_id,
+                               int64_t *d_out_labels, float *d_out_scores, uint32_t *d_out_counts, cudaStream_t s, LaunchCounters *ctr);
 
 } // namespace rsb200

@@ -59,6 +59,39 @@ def merge_topk_device(gath_scores, gath_labels, stream_ptr=None):
     return out_s, out_l
 
 
+def merge_shard_lists(parts, range_query=False, order=0, stream_ptr=None):
+    """Per rank the (labels [nq,w] int64, scores [nq,w] float32, counts [nq] 32-bit) CUDA tensors of its local device call
+    (HybridTopKBatchDevice, [Label|Hybrid]RangeQueryBatchDevice) -> the merged (labels, scores, counts) of all ranks.  Packs each
+    rank's result into its counted exchange block (VecSimB200_ShardListBlockBytes), rank-major as an all-gather leaves them, and
+    merges them with VecSimB200_MergeShardListBlocks on the device.  order: BY_SCORE (0) or BY_ID (1, range results only).
+    Packing and merge run on `stream_ptr` (default: torch's current stream), so the local calls must be enqueued on that stream
+    or be complete: a call left on another stream, e.g. the legacy default stream while torch's current stream is a non-blocking
+    one, races with the packing."""
+    import torch
+
+    from . import vecsim
+
+    L = vecsim.lib()
+    nq, w = parts[0][0].shape
+    dev = parts[0][0].device
+    n = nq * w
+    block = int(L.VecSimB200_ShardListBlockBytes(nq, w))
+    blocks = torch.zeros((len(parts), block), dtype=torch.uint8, device=dev)
+    for g, (labels, scores, counts) in enumerate(parts):
+        blocks[g, :n * 8] = labels.contiguous().view(torch.uint8).reshape(-1)
+        blocks[g, n * 8:n * 12] = scores.contiguous().view(torch.uint8).reshape(-1)
+        blocks[g, n * 12:n * 12 + nq * 4] = counts.contiguous().view(torch.uint8).reshape(-1)
+    out_l = torch.empty((nq, w), dtype=torch.int64, device=dev)
+    out_s = torch.empty((nq, w), dtype=torch.float32, device=dev)
+    out_c = torch.empty(nq, dtype=torch.int32, device=dev)
+    sp = C.c_void_p(stream_ptr if stream_ptr is not None else torch.cuda.current_stream().cuda_stream)
+    rc = L.VecSimB200_MergeShardListBlocks(blocks.data_ptr(), len(parts), nq, w, 1 if range_query else 0, order, out_l.data_ptr(),
+                                           out_s.data_ptr(), out_c.data_ptr(), sp)
+    if rc != 0:
+        raise RuntimeError("VecSimB200_MergeShardListBlocks failed")
+    return out_l, out_s, out_c
+
+
 # ------------------------------------------------------------------------------------------------
 # postings
 # ------------------------------------------------------------------------------------------------

@@ -167,6 +167,13 @@ SIGNATURES = [
     ("VecSimB200_ShardGroup_Size", C.c_int, [_P]),
     ("VecSimB200_ShardGroup_TopKBatchDevice", C.c_int, [_P, _P, _P, _SZ, _SZ, _P, _P, _P]),
     ("VecSimB200_ShardGroup_TopKBatch", C.c_int, [_P, _P, _P, _SZ, _SZ, _SZ, _P, _P]),
+    ("VecSimB200_ShardListBlockBytes", _SZ, [_SZ, _SZ]),
+    ("VecSimB200_MergeShardListBlocks", C.c_int, [_P, _SZ, _SZ, _SZ, C.c_int, C.c_int, _P, _P, _P, _P]),
+    ("VecSimB200_ShardGroup_HybridTopKBatchDevice", C.c_int,
+     [_P, _P, _P, _SZ, _SZ, _P, _P, _P, C.POINTER(VecSimQueryParams), _P, _P, _P, _P, _P]),
+    ("VecSimB200_ShardGroup_RangeQueryBatchDevice", C.c_int, [_P, _P, _P, _SZ, _P, _SZ, C.c_int, _P, _P, _P, _P]),
+    ("VecSimB200_ShardGroup_HybridRangeQueryBatchDevice", C.c_int,
+     [_P, _P, _P, _SZ, _P, _SZ, C.c_int, _P, _P, _P, C.POINTER(VecSimQueryParams), _P, _P, _P, _P, _P]),
 ]
 # VecSim_SetMemoryFunctions takes a struct by value; declared in the header, bound lazily.
 EXTRA_SYMBOLS = ["VecSim_SetMemoryFunctions"]
