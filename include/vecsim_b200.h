@@ -717,6 +717,9 @@ int VecSimB200_LastCoarseFlags(VecSimIndex *index, uint32_t *out_ok, size_t nq);
  * inner product, cosine or L2 — s8 / u8 wgmma integer dot products are exact and the reference's float expression is applied
  * to them (L2: float(|row|^2 + |q|^2 - 2 dot), evaluated in int32 from exact squared norms), bit-exact. */
 int VecSimB200_LastBatchPath(VecSimIndex *index);
+/* Debug: the operand copy of the fp32 rows the last route 1 query or batch read: 8 = the int8 copy (unit rows: cosine with
+ * k <= 128), 16 = the fp16 copy, 0 = none (another route, or TF32 on the fp32 rows). */
+int VecSimB200_LastCoarseShadowBits(VecSimIndex *index);
 /* Library/ABI version and the SM arch the kernels were compiled for ("sm_90a"). */
 const char *VecSimB200_Version(void);
 

@@ -723,6 +723,16 @@ __device__ __forceinline__ int range_int_bound(float r) {
     return x;
 }
 
+// int8 shadow (kOp 5): an integer bound ti with  fl(fl(sqt * a)) > tdot  =>  a > ti  for every int32 accumulator a (|a| < 2^24,
+// exact in float), so that `a > ti` never drops a row the float test keeps: tdot / sqt loosened by 1e-5 relative (the rounding of
+// the division and of the product) and one more integer.  NaN: everything passes; a bound beyond +-2^25: everything / nothing.
+__device__ __forceinline__ int q8_dot_bound(float tdot, float sqt) {
+    const float f = tdot / sqt;
+    if (!(f == f)) return INT_MIN;
+    const float c = fminf(fmaxf(f, -33554432.0f), 33554432.0f);
+    return (int)floorf(c - fabsf(c) * 1e-5f) - 1;
+}
+
 // kDirect = false: fp32 corpus, rows come from the tiled fp16 shadow (bulk copies), output = sorted candidate lists for
 //                  the exact rescoring + proof.
 // kDirect = true : fp16 / bf16 corpus, rows come straight from the row-major corpus through a 128B-swizzle tensor
@@ -757,6 +767,11 @@ __device__ __forceinline__ int range_int_bound(float r) {
 //            filtered rows; the adaptive lists and the fixed bound admit only filtered rows (the fixed bound tests the bit on
 //            its rare survivor path, after the key test).  fp32 route, and the 8-bit fixed-radius pass (DESIGN.md §4.13), which
 //            tests the bit after both the integer pre-test and the float range test.
+//   kOp = 5  the int8 shadow of unit fp32 rows (s8 wgmma, int32 accumulators): the approximate distance is
+//            1 - fl(fl(s_q s_t) acc), s_q = the query's scale (a float after its int8 payload), s_t = the row tile's scale
+//            (row_norm2[tile]).  The fixed-bound pass tests one integer bound per (query, tile) on the accumulators; the sample
+//            and adaptive-list passes turn the accumulators into those float dot products in the transpose and then run kOp 0's
+//            epilogue.  Unit vectors only; the error bound is per query (DESIGN.md §4.2)
 //   kRegKb   the fixed-bound pass over the fp16 shadow: the first kRegKb K blocks of the CTA's queries are held in registers
 //            (the wgmma A fragment, 16 per K block and thread, loaded once per consumer warpgroup) instead of shared memory,
 //            which frees kRegKb x 8 KB for the ring (DESIGN.md §4.2).  The first kRegKb / kQKbPerStage stages of a tile take
@@ -771,13 +786,16 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                     uint32_t tile_stride, const float *__restrict__ thr_fixed, uint32_t *__restrict__ overflow,
                     const uint32_t *__restrict__ filt, uint32_t filt_words, const uint32_t *__restrict__ filt_q) {
     constexpr bool kFixed = kMode == 1, kSample = kMode == 2;
-    constexpr bool kInt = kOp == 1 || kOp == 2 || kOp == 4;
+    constexpr bool kQ8 = kOp == 5;
+    constexpr bool kInt = kOp == 1 || kOp == 2 || kOp == 4 || kQ8;
+    constexpr int kOpE = kQ8 ? 0 : kOp; // the epilogue of kOp 5 past the integer bound test is kOp 0's
     constexpr int kCons = coarse_consumers(kMode), kConsThreads = 128 * kCons;
     using Acc = typename std::conditional<kInt, uint32_t, float>::type;
     // bx = row range, by = query group
     const uint32_t bx = blockIdx.x, by = blockIdx.y, gx = gridDim.x;
-    static_assert(kMode == 0 || (!kDirect && (kOp == 0 || kOp == 3)) || (kDirect && kOp == 0) || (kDirect && kFixed && kInt && kEpl == 8),
+    static_assert(kMode == 0 || (!kDirect && (kOp == 0 || kOp == 3 || kQ8)) || (kDirect && kOp == 0) || (kDirect && kFixed && kInt && kEpl == 8),
                   "fixed bound / sample pass: the fp32 route and 16-bit corpora (inner product / cosine); fixed radius: 8-bit corpora");
+    static_assert(!kQ8 || (!kDirect && !kFilt && kRegKb == 0 && kVar == 1), "int8 shadow: signed operands, no filters");
     static_assert(!kFilt || (!kDirect && (kOp == 0 || kOp == 3)) || (kDirect && kFixed && kInt && kEpl == 8),
                   "row filters: the fp32 route and the 8-bit fixed-radius pass");
     static_assert(kRegKb == 0 || (!kDirect && kFixed && kRegKb % kQKbPerStage == 0),
@@ -952,7 +970,16 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         // 8-bit fixed radius: the radius, the integer bound of the inner-product / L2 pre-test, |q|^2 (L2)
         float frad[2];
         int fix[2], fnqi[2];
-        if constexpr (kFixed && kInt) {
+        // kOp 5: the scales s_q of the two fragment queries (1 for slots without a query)
+        float fsq[2] = {1.0f, 1.0f};
+        if constexpr (kQ8) {
+#pragma unroll
+            for (int i2 = 0; i2 < 2; i2++) {
+                const uint32_t fq = q_base + 16 * ew + (lane >> 2) + 8 * i2;
+                if (fq < nq) fsq[i2] = *reinterpret_cast<const float *>(q16 + (size_t)fq * q16_pitch + row_bytes);
+            }
+        }
+        if constexpr (kFixed && kInt && !kQ8) {
 #pragma unroll
             for (int i2 = 0; i2 < 2; i2++) {
                 const uint32_t fq = q_base + 16 * ew + (lane >> 2) + 8 * i2;
@@ -968,7 +995,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                 fthr_dot[i2] = fnq[i2] * ((1.0f - frad[i2]) - 1e-6f * (1.0f + fabsf(frad[i2])));
             }
         }
-        if constexpr (kFixed && !kInt) {
+        if constexpr (kFixed && (!kInt || kQ8)) {
 #pragma unroll
             for (int i2 = 0; i2 < 2; i2++) {
                 const uint32_t fq = q_base + 16 * ew + (lane >> 2) + 8 * i2;
@@ -977,7 +1004,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                 // fixed admission bound (a distance): keep every row with approximate distance < T
                 const float T = flive ? thr_fixed[fq] : -__int_as_float(0x7f800000);
                 fthr[i2] = orderable_key(T);
-                if constexpr (kOp == 0) { // d < T  <=>  dot > 1 - T; slack: the rounding of the two subtractions
+                if constexpr (kOpE == 0) { // d < T  <=>  dot > 1 - T; slack: the rounding of the two subtractions
                     const float t = 1.0f - T;
                     fthr_dot[i2] = t - (4e-7f + 2.4e-7f * fabsf(t));
                 } else {
@@ -1104,6 +1131,53 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
             release(prev);
             wg_fence_operands(acc);
             // accumulator fragment: acc[4j + 2 i2 + c] = (query 16 ew + lane / 4 + 8 i2, row 8 j + 2 (lane % 4) + c)
+            if constexpr (kFixed && kQ8) {
+                // int8 shadow: the bound dot > fthr_dot becomes one integer bound per query on this tile's accumulators
+                // (q8_dot_bound); the rare survivors take the float distance and the exact key comparison, as kOp 0
+                const float st = __ldg(row_norm2 + tile);
+#pragma unroll
+                for (int i2 = 0; i2 < 2; i2++) {
+                    const float sqt = __fmul_rn(fsq[i2], st);
+                    const int ti = q8_dot_bound(fthr_dot[i2], sqt);
+                    int m8[8];
+#pragma unroll
+                    for (int g = 0; g < 8; g++)
+                        m8[g] = max(max((int)acc[8 * g + 2 * i2], (int)acc[8 * g + 2 * i2 + 1]), max((int)acc[8 * g + 4 + 2 * i2], (int)acc[8 * g + 5 + 2 * i2]));
+                    const int mx = max(max(max(m8[0], m8[1]), max(m8[2], m8[3])), max(max(m8[4], m8[5]), max(m8[6], m8[7])));
+                    uint32_t pass = 0; // bit 2 j + c: acc[4 j + 2 i2 + c]
+                    if (mx > ti) {
+#pragma unroll
+                        for (int j = 0; j < kQN / 8; j++)
+#pragma unroll
+                            for (int c = 0; c < 2; c++)
+                                if ((int)acc[4 * j + 2 * i2 + c] > ti) pass |= 1u << (2 * j + c);
+                    }
+                    if (pass && tile * kQN + kQN > n_rows) { // rows past the end (zero or stale shadow bytes)
+#pragma unroll
+                        for (int j = 0; j < kQN / 8; j++)
+#pragma unroll
+                            for (int c = 0; c < 2; c++)
+                                if (rbase + 8 * j + c >= n_rows) pass &= ~(1u << (2 * j + c));
+                    }
+                    while (pass) {
+                        const int b = __ffs(pass) - 1;
+                        pass &= pass - 1;
+                        uint32_t raw = 0;
+#pragma unroll
+                        for (int x = 0; x < 32; x++)
+                            if (x == b) raw = acc[4 * (x >> 1) + 2 * i2 + (x & 1)];
+                        const uint32_t row = rbase + 8 * (b >> 1) + (b & 1);
+                        const uint32_t key = orderable_key(__fsub_rn(1.0f, __fmul_rn(sqt, __int2float_rn((int)raw))));
+                        if (key < fthr[i2]) {
+                            const int qs = 16 * ew + (lane >> 2) + 8 * i2;
+                            const uint32_t slot = atomicAdd(&qcount[qs], 1u);
+                            if (slot < (uint32_t)kQListCap) lists[slot * kQListStride + qs] = ((uint64_t)key << 32) | row;
+                        }
+                    }
+                }
+                ca.add(kCaEpilogue, t_epilogue);
+                continue;
+            }
             if constexpr (kFixed && kInt) {
                 // 8-bit fixed radius: a conservative pre-test on the integer dot products (exact for inner product and L2,
                 // range_int_bound), then the epilogue's own float distance and the range test d <= r on the rare survivors.
@@ -1243,13 +1317,20 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                 continue;
             }
             asm volatile("bar.sync 1, 128;" ::: "memory"); // the previous tile's reads of sacc are done
+            float tsqt[2] = {0.0f, 0.0f}; // kOp 5: fl(s_q s_t) of the fragment's two queries on this tile
+            if constexpr (kQ8) {
+                const float st = __ldg(row_norm2 + tile);
+                tsqt[0] = __fmul_rn(fsq[0], st), tsqt[1] = __fmul_rn(fsq[1], st);
+            }
 #pragma unroll
             for (int j = 0; j < kQN / 8; j++) {
                 const int m = 16 * ew + (lane >> 2), n = 8 * j + 2 * (lane & 3);
                 uint32_t b[4];
 #pragma unroll
                 for (int x = 0; x < 4; x++) {
-                    if constexpr (kInt)
+                    if constexpr (kQ8)
+                        b[x] = __float_as_uint(__fmul_rn(tsqt[x >> 1], __int2float_rn((int)acc[4 * j + x])));
+                    else if constexpr (kInt)
                         b[x] = acc[4 * j + x];
                     else
                         b[x] = __float_as_uint(acc[4 * j + x]);
@@ -1283,10 +1364,10 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
 #pragma unroll
                         for (int j = 0; j < 32; j++) {
                             float u = __uint_as_float(v[h][j]);
-                            if constexpr (kOp != 0) u = fmaf(__shfl_sync(0xFFFFFFFFu, nrm[h], j), -0.5f, u);
+                            if constexpr (kOpE != 0) u = fmaf(__shfl_sync(0xFFFFFFFFu, nrm[h], j), -0.5f, u);
                             if ((fw >> j) & 1u) mx = fmaxf(mx, u);
                         }
-                    } else if constexpr (kOp == 0) {
+                    } else if constexpr (kOpE == 0) {
                         if (!tail) {
                             float m8[8];
 #pragma unroll
@@ -1318,7 +1399,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
 #pragma unroll
                 for (int j = 0; j < 32; j++) {
                     bool p;
-                    if constexpr (kOp == 0)
+                    if constexpr (kOpE == 0)
                         p = __uint_as_float(v[h][j]) > thr_dot;
                     else if constexpr (kOp == 1)
                         p = (float)(int)v[h][j] > thr_dot;
@@ -1340,7 +1421,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                     for (int x = 0; x < 32; x++)
                         if (x == j) raw = v[h][x];
                     float d;
-                    if constexpr (kOp == 0)
+                    if constexpr (kOpE == 0)
                         d = 1.0f - __uint_as_float(raw);
                     else if constexpr (kOp == 1)
                         d = (float)(1 - (int)raw);
@@ -1372,7 +1453,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         // d < d_thr needs dot > t = 1 - d_thr (times the norms for the integer cosine); the slack covers
                         // the rounding of the subtractions, of int -> float and of the norm product
                         const float t = 1.0f - key_to_float(thr);
-                        if constexpr (kOp == 0)
+                        if constexpr (kOpE == 0)
                             thr_dot = t - 4e-7f;
                         else if constexpr (kOp == 1)
                             thr_dot = t - (fabsf(t) * 1e-6f + 2.0f);
@@ -1419,7 +1500,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         const float m = smax[kSample ? x : 0][h];
                         uint64_t c = kEmptySlot;
                         if (m > -__int_as_float(0x7f800000)) {
-                            const float d = kOp == 0 ? 1.0f - m : __fsub_rn(nq_norm, __fmul_rn(2.0f, m));
+                            const float d = kOpE == 0 ? 1.0f - m : __fsub_rn(nq_norm, __fmul_rn(2.0f, m));
                             c = (uint64_t)orderable_key(d) << 32;
                         }
                         if ((uint32_t)(x * (kQN / 32) + h) < keep) dst[x * (kQN / 32) + h] = c;
@@ -1486,8 +1567,11 @@ __global__ void __launch_bounds__(256) to_f16_kernel(const uint8_t *__restrict__
 constexpr uint32_t kRefineMaxSurv = 2048;     // survivors rescored per query, k <= kCoarseMaxK
 constexpr uint32_t kRefineMaxSurvWide = 4096; // the same for k > kCoarseMaxK (32 KB)
 
-// |approx - exact| bound of one query (see above); q_norm2 == NULL: unit vectors
-__device__ __forceinline__ float query_eps(float eps, const float *q_norm2, uint32_t pos, float max_norm, uint32_t dim, bool l2) {
+// |approx - exact| bound of one query (see above); q_norm2 == NULL: unit vectors.  q_eps (the int8 shadow): the bound of each
+// query, computed with its quantization (quantize_queries_kernel)
+__device__ __forceinline__ float query_eps(float eps, const float *q_norm2, uint32_t pos, float max_norm, uint32_t dim, bool l2,
+                                           const float *q_eps = nullptr) {
+    if (q_eps) return q_eps[pos];
     if (!q_norm2) return eps;
     const float qn2 = q_norm2[pos], qn = sqrtf(qn2);
     float e = eps * max_norm * qn + 5.97e-8f * sqrtf((float)dim) * (max_norm + qn);
@@ -1539,14 +1623,14 @@ __device__ __forceinline__ uint32_t block_kth_key(const uint64_t *mine, uint32_t
 __global__ void __launch_bounds__(256) threshold_kernel(const uint64_t *__restrict__ cand, uint32_t nq, uint32_t lists_per_query,
                                                         uint32_t keep, uint32_t k, float eps, const float *__restrict__ q_norm2,
                                                         float max_norm, uint32_t dim, int l2, float *__restrict__ thr_out,
-                                                        uint32_t *__restrict__ overflow) {
+                                                        uint32_t *__restrict__ overflow, const float *__restrict__ q_eps) {
     __shared__ uint32_t hist[256];
     __shared__ uint32_t ctl[4];
     const uint32_t q = blockIdx.x;
     if (q >= nq) return;
     const uint32_t ak = block_kth_key(cand + (size_t)q * lists_per_query * keep, lists_per_query * keep, k, hist, ctl);
     if (threadIdx.x == 0) {
-        const float e = query_eps(eps, q_norm2, q, max_norm, dim, l2 != 0);
+        const float e = query_eps(eps, q_norm2, q, max_norm, dim, l2 != 0, q_eps);
         float T;
         if (ak == 0xFFFFFFFFu)
             T = __int_as_float(0x7f800000);
@@ -1571,7 +1655,7 @@ __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t
                                                      float max_norm, uint32_t *__restrict__ ok, uint32_t ok_value, uint64_t *__restrict__ out,
                                                      const uint32_t *__restrict__ q_index, const uint32_t *__restrict__ nq_dev,
                                                      const float *__restrict__ thr_T, const uint32_t *__restrict__ overflow,
-                                                     uint32_t smem_cap, const uint64_t *__restrict__ row_label) {
+                                                     uint32_t smem_cap, const uint64_t *__restrict__ row_label, const float *__restrict__ q_eps) {
     using Tile = DistTile<DT_F32, MT, 1, 1>;
     __shared__ uint64_t surv[kSurv];
     __shared__ uint32_t hist[256];
@@ -1583,7 +1667,7 @@ __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint64_t *mine = cand + (size_t)blockIdx.x * lists_per_query * keep;
     uint32_t total = lists_per_query * keep;
-    eps = query_eps(eps, q_norm2, blockIdx.x, max_norm, dim, MT == MT_L2);
+    eps = query_eps(eps, q_norm2, blockIdx.x, max_norm, dim, MT == MT_L2, q_eps);
     if (threadIdx.x == 0) s_nsurv = 0, s_bad = 0, s_ncomp = 0;
     __syncthreads();
     // the lists are mostly empty slots (fixed-bound pass: ~15 of 96 per list): pack the real candidates into shared memory
@@ -1974,6 +2058,12 @@ static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, int epi, int m
     const bool l2 = epi != 0;
     if (kind == CoarseDirect16 || kind == CoarseDirect8)
         return variant ? wgmma_kernel_fn_v<1>(kind, epl, epi, mode, filt) : wgmma_kernel_fn_v<0>(kind, epl, epi, mode, filt);
+    if (kind == CoarseQ8) { // int8 shadow: fixed bound with lists of 256, the sample pass, adaptive lists of 128 (second tier)
+        if (filt || reg_kb || epi) return nullptr;
+        if (mode == 1) return (const void *)coarse_wgmma_kernel<false, 8, 5, 1, 1>;
+        if (mode == 2) return (const void *)coarse_wgmma_kernel<false, 3, 5, 2, 1>;
+        return epl == 8 ? (const void *)coarse_wgmma_kernel<false, 8, 5, 0, 1> : nullptr;
+    }
     if (reg_kb) {
         if (mode != 1 || reg_kb != fixed_reg_kb(epl, l2, filt)) return nullptr;
         return (const void *)coarse_wgmma_kernel<false, 3, 0, 1, 0, false, kFixedRegKb>;
@@ -2026,6 +2116,13 @@ bool coarse_supported(const CorpusView &c, uint32_t nq, uint32_t k, CoarseKind k
         if (k > 128 || nq < 1 || c.n_rows < 65536) return false;
         return encode_fn() != nullptr;
     }
+    if (kind == CoarseQ8) { // fp32 unit rows (the caller checks), inner product on the int8 shadow
+        if (c.dtype != DT_F32 || c.metric != MT_IP || c.dim % 8 != 0 || c.dim < 32 || c.dim > 1024 || c.pitch % 16 != 0) return false;
+        if (k > kCoarseMaxK || nq < 1 || c.n_rows < 65536 || !wgmma_fits_bytes(c.dim)) return false;
+        // rows are padded to whole 256-byte stages: up to 128 dimensions the int8 row streams as many bytes and MMAs as the fp16 one
+        if (coarse_kb(c.dim) >= coarse_kb(c.dim * 2)) return false;
+        return encode_fn() != nullptr;
+    }
     // fp32: cosine / inner product (distance 1 - dot) or squared L2; the caller supplies the error bound (unit vectors or norms)
     if (c.dtype != DT_F32 || (c.metric != MT_IP && c.metric != MT_L2)) return false;
     if (kind == CoarseTF32 && c.metric != MT_IP) return false;
@@ -2045,24 +2142,25 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
     p.kind = kind;
     p.tile_stride = std::max(1u, tile_stride);
     // 8-bit corpora: the fixed-radius pass of range batches (mode 1) only
-    p.mode = (kind == CoarseF16 || (kind == CoarseDirect16 && c.metric == MT_IP)) ? mode : (kind == CoarseDirect8 && mode == 1) ? 1 : 0;
-    if (kind == CoarseF16 || kind == CoarseDirect16 || kind == CoarseDirect8) {
-        p.num_kb = coarse_kb(kind == CoarseDirect8 ? c.dim : c.dim * 2);
+    p.mode = (kind == CoarseF16 || kind == CoarseQ8 || (kind == CoarseDirect16 && c.metric == MT_IP)) ? mode : (kind == CoarseDirect8 && mode == 1) ? 1 : 0;
+    if (kind == CoarseF16 || kind == CoarseQ8 || kind == CoarseDirect16 || kind == CoarseDirect8) {
+        p.num_kb = coarse_kb(kind == CoarseDirect8 || kind == CoarseQ8 ? c.dim : c.dim * 2);
         p.tiles = ((c.n_rows + kQN - 1) / kQN + p.tile_stride - 1) / p.tile_stride; // row tiles this pass visits
         p.grid_y = (nq + kQM - 1) / kQM;
         const uint32_t sms = (uint32_t)device_sm_count();
         p.grid_x = std::max(1u, std::min(p.tiles, sms / p.grid_y));
         // direct routes: the CTA's exact top-k of its rows.  fp32 route: candidates per (row range, query) — kCoarseKeep
         // for k <= 16, 128 for larger k and for the second tier
-        p.keep = kind == CoarseF16 ? (keep_override ? keep_override : (k <= kCoarseTier1MaxK ? kCoarseKeep : kCoarseKeepWide))
+        p.keep = (kind == CoarseF16 || kind == CoarseQ8) ? (keep_override ? keep_override : (k <= kCoarseTier1MaxK ? kCoarseKeep : kCoarseKeepWide))
                                    : (k <= 32 ? 32u : 128u);
         p.epl = p.keep <= 32 ? 3 : 8;
         if (p.mode == 1 && kind == CoarseF16) // every row below the bound, up to the list capacity
             p.keep = k > kCoarseMaxK ? kCoarseFixedCapWide : kCoarseFixedCap, p.epl = k > kCoarseMaxK ? 8 : 3;
         if (p.mode == 1 && (kind == CoarseDirect16 || kind == CoarseDirect8)) p.keep = kCoarseFixedCapDirect, p.epl = 8;
+        if (p.mode == 1 && kind == CoarseQ8) p.keep = kCoarseFixedCapQ8, p.epl = 8;
         if (p.mode == 2) p.keep = kCoarseSampleSlices, p.epl = 3; // the slice minima
         p.threads = (uint32_t)coarse_threads(p.mode);
-        const int epi = kind == CoarseF16 ? (c.metric == MT_L2 ? 1 : 0) : c.metric == MT_COS ? 1 : (kind == CoarseDirect8 && c.metric == MT_L2) ? 2 : 0;
+        const int epi = kind == CoarseQ8 ? 0 : kind == CoarseF16 ? (c.metric == MT_L2 ? 1 : 0) : c.metric == MT_COS ? 1 : (kind == CoarseDirect8 && c.metric == MT_L2) ? 2 : 0;
         // the fixed-bound pass over the shadow holds the leading K blocks of its queries in registers where that frees shared
         // memory for one more ring stage and leaves at least one stage of queries in shared memory
         static int rcap = -1; // VECSIM_B200_REGKB caps the register-held K blocks (0 = none)
@@ -2090,7 +2188,8 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
                 p.csize = cs;
                 break;
             }
-        const void *kfn = wgmma_kernel_fn(kind, p.epl, epi, p.mode, (c.dtype == DT_BF16 || c.dtype == DT_I8) ? 1u : 0u, filt, p.reg_kb);
+        const void *kfn = wgmma_kernel_fn(kind, p.epl, epi, p.mode, (c.dtype == DT_BF16 || c.dtype == DT_I8 || kind == CoarseQ8) ? 1u : 0u, filt,
+                                          p.reg_kb);
         if (p.csize > 1) {
             cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem_bytes);
             cudaLaunchConfig_t cfg{};
@@ -2147,7 +2246,7 @@ cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim
                           uint64_t *d_scratch, cudaStream_t s, const uint32_t *d_nq_dev, const float *d_thr_fixed, uint32_t *d_overflow,
                           const uint32_t *d_filt, uint32_t filt_words, const uint32_t *d_filt_q) {
     if (d_filt && p.kind != CoarseF16 && !(p.kind == CoarseDirect8 && p.mode == 1)) return cudaErrorInvalidValue;
-    if (p.kind == CoarseF16 || p.kind == CoarseDirect16 || p.kind == CoarseDirect8) {
+    if (p.kind == CoarseF16 || p.kind == CoarseQ8 || p.kind == CoarseDirect16 || p.kind == CoarseDirect8) {
         if (p.mode == 1 && (!d_thr_fixed || !d_overflow)) return cudaErrorInvalidValue;
         // operand variant: 16-bit 1 = bf16 (else fp16); 8-bit 1 = int8 (else uint8); the fp16 shadow of the fp32 route: 0
         const uint32_t ev = (p.kind == CoarseDirect16 || p.kind == CoarseDirect8) && o.elem_variant ? 1u : 0u;
@@ -2164,6 +2263,8 @@ cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim
             if (!make_map(&mr, ev ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, o.rows, dim, n_rows, o.pitch, 64,
                           kQN / p.csize))
                 return cudaErrorInvalidValue;
+        } else if (p.kind == CoarseQ8) {
+            row_bytes = (uint32_t)coarse_q8_payload(dim); // the query's scale follows its payload
         } else if (p.kind == CoarseDirect8) {
             row_bytes = dim;
             if (!make_map(&mr, CU_TENSOR_MAP_DATA_TYPE_UINT8, o.rows, dim, n_rows, o.pitch, 128, kQN / p.csize)) return cudaErrorInvalidValue;
@@ -2241,6 +2342,159 @@ cudaError_t launch_to_f16_tiled(const void *src, size_t spitch, uint32_t dim, ui
     const size_t total = (size_t)n * num_kb * 8;
     const uint32_t grid = (uint32_t)std::max<size_t>(1, std::min<size_t>((total + 255) / 256, (size_t)device_sm_count() * 16));
     to_f16_tiled_kernel<<<grid, 256, 0, s>>>(static_cast<const uint8_t *>(src), spitch, dim, first, n, static_cast<uint8_t *>(dst), num_kb);
+    return cudaGetLastError();
+}
+
+// fp32 unit rows -> the tiled int8 shadow: [tile of 128 rows][K block of 128 int8][128 rows x 128 B, 128B-swizzled], the image
+// of to_f16_tiled_kernel with one-byte elements.  One CTA per tile: the tile's max |x| gives its scale s_t = max / 127 (1 for an
+// all-zero tile, so that no scale is 0), every element x becomes rint(x / s_t) (|x / s_t| <= 127 up to rounding, clamped), rows
+// past n_rows and bytes past dim are zero.  The residual norm |x - s_t x~| and the norm |x| of each row are accumulated in fp64
+// and folded, rounded up to float, into the running maxima stats[0] and stats[1] (as bits: the values are >= 0; a NaN or inf
+// element makes them NaN / inf, and the host keeps such an index off the route).
+__global__ void __launch_bounds__(256) to_i8_tiled_kernel(const uint8_t *__restrict__ src, size_t spitch, uint32_t dim, uint32_t n_rows,
+                                                          uint32_t tile0, uint32_t ntiles, uint8_t *__restrict__ dst, uint32_t num_kb,
+                                                          float *__restrict__ tscale, uint32_t *__restrict__ stats) {
+    __shared__ float s_max[8];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float w_res = 0.0f, w_nrm = 0.0f; // this warp's maxima over its rows
+    for (uint32_t t = tile0 + blockIdx.x; t < tile0 + ntiles; t += gridDim.x) {
+        float m = 0.0f;
+        for (uint32_t rr = warp; rr < (uint32_t)kQN; rr += 8) {
+            const uint32_t r = t * kQN + rr;
+            if (r >= n_rows) break;
+            const float *x = reinterpret_cast<const float *>(src + (size_t)r * spitch);
+            for (uint32_t e = lane * 4; e < dim; e += 128) {
+                const float4 v = *reinterpret_cast<const float4 *>(x + e);
+                m = fmaxf(m, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+                if (!(v.x == v.x && v.y == v.y && v.z == v.z && v.w == v.w)) m = __int_as_float(0x7f800000);
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xFFFFFFFFu, m, o));
+        if (lane == 0) s_max[warp] = m;
+        __syncthreads();
+        m = s_max[0];
+        for (int w = 1; w < 8; w++) m = fmaxf(m, s_max[w]);
+        __syncthreads(); // s_max is rewritten by the next tile
+        const float sc = m > 0.0f ? __fdiv_rn(m, 127.0f) : 1.0f;
+        if (threadIdx.x == 0) tscale[t] = sc;
+        for (uint32_t rr = warp; rr < (uint32_t)kQN; rr += 8) {
+            const uint32_t r = t * kQN + rr;
+            const bool real = r < n_rows;
+            const float *x = reinterpret_cast<const float *>(src + (size_t)(real ? r : 0) * spitch);
+            double res2 = 0.0, nrm2 = 0.0;
+            for (uint32_t ci = lane; ci < num_kb * 8; ci += 32) { // 16-element chunk ci of the row
+                uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+                for (int g = 0; g < 4; g++) {
+                    const uint32_t e = ci * 16 + g * 4;
+                    if (!real || e >= dim) continue; // dim % 8 == 0: a float4 is all in or all out
+                    const float4 v = *reinterpret_cast<const float4 *>(x + e);
+                    const float f[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                    for (int h = 0; h < 4; h++) {
+                        const float qv = fminf(fmaxf(rintf(__fdiv_rn(f[h], sc)), -127.0f), 127.0f);
+                        const double d = (double)f[h] - (double)sc * (double)qv;
+                        res2 = fma(d, d, res2);
+                        nrm2 = fma((double)f[h], (double)f[h], nrm2);
+                        w[g] |= ((uint32_t)(int)qv & 0xFFu) << (8 * h);
+                    }
+                }
+                const uint32_t kb = ci / 8, c = ci % 8;
+                uint8_t *blk = dst + ((size_t)t * num_kb + kb) * kQBlockBytes;
+                *reinterpret_cast<uint4 *>(blk + rr * 128 + ((c ^ (rr & 7)) * 16)) = make_uint4(w[0], w[1], w[2], w[3]);
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                res2 += __shfl_xor_sync(0xFFFFFFFFu, res2, o);
+                nrm2 += __shfl_xor_sync(0xFFFFFFFFu, nrm2, o);
+            }
+            const float rn = __double2float_ru(sqrt(res2));
+            w_res = (rn == rn && w_res == w_res) ? fmaxf(w_res, rn) : __int_as_float(0x7fc00000); // a NaN sticks
+            w_nrm = fmaxf(w_nrm, __double2float_ru(sqrt(nrm2)));
+        }
+    }
+    if (lane == 0) { // NaN has a larger bit pattern than any non-negative float: it wins the maximum
+        atomicMax(&stats[0], __float_as_uint(w_res));
+        atomicMax(&stats[1], __float_as_uint(w_nrm));
+    }
+}
+
+size_t coarse_shadow8_bytes(uint32_t rows, uint32_t dim) {
+    return (size_t)((rows + kQN - 1) / kQN) * coarse_kb(dim) * kQBlockBytes;
+}
+
+cudaError_t launch_to_i8_tiled(const void *src, size_t spitch, uint32_t dim, uint32_t n_rows, uint32_t first, uint32_t n, void *dst,
+                               float *d_tscale, uint32_t *d_stats, cudaStream_t s) {
+    if (n == 0) return cudaSuccess;
+    if (dim % 8 != 0 || spitch % 16 != 0) return cudaErrorInvalidValue;
+    const uint32_t tile0 = first / kQN, ntiles = (first + n - 1) / kQN - tile0 + 1;
+    const uint32_t grid = std::max(1u, std::min(ntiles, (uint32_t)device_sm_count() * 8));
+    to_i8_tiled_kernel<<<grid, 256, 0, s>>>(static_cast<const uint8_t *>(src), spitch, dim, n_rows, tile0, ntiles, static_cast<uint8_t *>(dst),
+                                            coarse_kb(dim), d_tscale, d_stats);
+    return cudaGetLastError();
+}
+
+// One warp per fp32 unit query q: its scale s_q = max |q_i| / 127 (1 for a zero query), q~ = rint(q / s_q) into the int8 row
+// (zero padded to the payload), s_q after the payload, and the bound of |approx - exact| for every stored row x:
+//   q.x - s_q s_t q~.x~ = q.delta + eta.x - eta.delta   (x = s_t x~ + delta, q = s_q q~ + eta)
+//   |.| <= |q| delta_max + |eta| x_max + |eta| delta_max                        (Cauchy-Schwarz)
+// plus the fp32 rounding of both sides: the exact scan's dot product (at most dim 2^-24 |q| |x| in any order) and the approximate
+// distance 1 - fl(fl(s_q s_t) acc) (two roundings of a value below (|q| + |eta|)(x_max + delta_max), one of 1 - it), all
+// covered by (dim + 8) 2^-23 (|q| + |eta|)(x_max + delta_max) + 2^-21; the sum is computed in fp64 and rounded up.  A query whose
+// bound is not finite gets NaN, which refine_kernel never proves.
+__global__ void __launch_bounds__(256) quantize_queries_kernel(const uint8_t *__restrict__ q, size_t qpitch, uint32_t dim, uint32_t nq,
+                                                               uint8_t *__restrict__ q8, size_t pitch8, uint32_t payload,
+                                                               float *__restrict__ eps, float delta_max, float x_max) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t i = blockIdx.x * 8 + warp;
+    if (i >= nq) return;
+    const float *x = reinterpret_cast<const float *>(q + (size_t)i * qpitch);
+    float m = 0.0f;
+    bool finite = true;
+    for (uint32_t e = lane; e < dim; e += 32) {
+        const float v = x[e];
+        m = fmaxf(m, fabsf(v));
+        finite = finite && fabsf(v) <= 3.4e38f;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xFFFFFFFFu, m, o));
+    finite = __all_sync(0xFFFFFFFFu, finite);
+    const float sc = (finite && m > 0.0f) ? __fdiv_rn(m, 127.0f) : 1.0f;
+    double qn2 = 0.0, en2 = 0.0;
+    uint8_t *dst = q8 + (size_t)i * pitch8;
+    for (uint32_t e = lane; e < payload; e += 32) {
+        int8_t b = 0;
+        if (e < dim && finite) {
+            const float v = x[e];
+            const float qv = fminf(fmaxf(rintf(__fdiv_rn(v, sc)), -127.0f), 127.0f);
+            const double d = (double)v - (double)sc * (double)qv;
+            en2 = fma(d, d, en2);
+            qn2 = fma((double)v, (double)v, qn2);
+            b = (int8_t)(int)qv;
+        }
+        dst[e] = (uint8_t)b;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        qn2 += __shfl_xor_sync(0xFFFFFFFFu, qn2, o);
+        en2 += __shfl_xor_sync(0xFFFFFFFFu, en2, o);
+    }
+    if (lane == 0) {
+        *reinterpret_cast<float *>(dst + payload) = sc;
+        const double qn = sqrt(qn2), en = sqrt(en2), X = (double)x_max, D = (double)delta_max;
+        double e = qn * D + en * X + en * D + (double)(dim + 8) * 0x1p-23 * (qn + en) * (X + D) + 0x1p-21;
+        e *= 1.0001;
+        const float ef = __double2float_ru(e);
+        eps[i] = (finite && isfinite(ef)) ? ef : __int_as_float(0x7fc00000);
+    }
+}
+
+cudaError_t launch_quantize_queries(const void *d_q, size_t qpitch, uint32_t dim, uint32_t nq, void *d_q8, float *d_eps, float delta_max,
+                                    float x_max, cudaStream_t s) {
+    if (nq == 0) return cudaSuccess;
+    quantize_queries_kernel<<<(nq + 7) / 8, 256, 0, s>>>(static_cast<const uint8_t *>(d_q), qpitch, dim, nq, static_cast<uint8_t *>(d_q8),
+                                                         coarse_q8_pitch(dim), (uint32_t)coarse_q8_payload(dim), d_eps, delta_max, x_max);
     return cudaGetLastError();
 }
 
@@ -2328,7 +2582,7 @@ cudaError_t launch_to_f16(const void *src, size_t spitch, uint32_t dim, uint32_t
 cudaError_t launch_refine(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t lists_per_query, uint32_t keep,
                           uint32_t k, const uint64_t *d_cand, float eps, const float *d_q_norm2, float max_norm, uint32_t *d_ok,
                           uint64_t *d_out, const uint32_t *d_q_index, const uint32_t *d_nq_dev, cudaStream_t s, const float *d_thr_T,
-                          const uint32_t *d_overflow, const uint64_t *d_row_label) {
+                          const uint32_t *d_overflow, const uint64_t *d_row_label, const float *d_q_eps) {
     if (nq == 0) return cudaSuccess;
     const uint32_t okv = d_q_index ? 2u : 1u;
     const uint8_t *rows = static_cast<const uint8_t *>(c.rows), *qs = static_cast<const uint8_t *>(d_queries);
@@ -2354,14 +2608,15 @@ cudaError_t launch_refine(const CorpusView &c, const void *d_queries, size_t qpi
         if (e != cudaSuccess) return e;
     }
     kern<<<nq, 256, smem, s>>>(rows, c.pitch, c.dim, qs, qpitch, nq, lists_per_query, keep, k, d_cand, eps, d_q_norm2, max_norm, d_ok, okv,
-                               d_out, d_q_index, d_nq_dev, d_thr_T, d_overflow, smem_cap, d_row_label);
+                               d_out, d_q_index, d_nq_dev, d_thr_T, d_overflow, smem_cap, d_row_label, d_q_eps);
     return cudaGetLastError();
 }
 
 cudaError_t launch_threshold(const uint64_t *d_cand, uint32_t nq, uint32_t lists_per_query, uint32_t keep, uint32_t k, float eps,
-                             const float *d_q_norm2, float max_norm, uint32_t dim, int l2, float *d_thr, uint32_t *d_overflow, cudaStream_t s) {
+                             const float *d_q_norm2, float max_norm, uint32_t dim, int l2, float *d_thr, uint32_t *d_overflow, cudaStream_t s,
+                             const float *d_q_eps) {
     if (nq == 0) return cudaSuccess;
-    threshold_kernel<<<nq, 256, 0, s>>>(d_cand, nq, lists_per_query, keep, k, eps, d_q_norm2, max_norm, dim, l2, d_thr, d_overflow);
+    threshold_kernel<<<nq, 256, 0, s>>>(d_cand, nq, lists_per_query, keep, k, eps, d_q_norm2, max_norm, dim, l2, d_thr, d_overflow, d_q_eps);
     return cudaGetLastError();
 }
 

@@ -14,6 +14,7 @@ constexpr uint32_t kCoarseMaxKWide = 1024; // largest k of the fp32 route's two-
 constexpr uint32_t kCoarseFixedCapWide = 256; // list capacity of the fp32 main pass for k > kCoarseMaxK
 constexpr uint32_t kCoarseSampleSlices = 32; // minima the sample pass publishes per (query, row range)
 constexpr uint32_t kCoarseFixedCapDirect = 256; // list capacity of the fixed-bound pass on 16-bit corpora (k up to 128)
+constexpr uint32_t kCoarseFixedCapQ8 = 256;   // list capacity of the main pass over the int8 shadow (its bound admits more rows)
 constexpr uint32_t kCoarseFixedCap = 96;   // list capacity of the fixed-bound main pass (rows below the bound per row range)
 constexpr uint32_t kRangeFoldMaxHits = 4096; // most hit rows range_label_fold_kernel sorts per query (48 KB of shared memory)
 // |approx - exact| bounds for unit vectors (Cauchy-Schwarz over the dot product: sum |a_i b_i| <= 1):
@@ -24,7 +25,8 @@ constexpr uint32_t kRangeFoldMaxHits = 4096; // most hit rows range_label_fold_k
 constexpr float kCoarseEpsTF32 = 2.5e-3f;
 constexpr float kCoarseEpsF16 = 1.2e-3f;
 
-enum CoarseKind : int { CoarseTF32 = 0, CoarseF16 = 1, CoarseDirect16 = 2, CoarseDirect8 = 3 };
+// CoarseQ8: the int8 shadow of fp32 unit rows (cosine, k <= kCoarseMaxK), one scale per 128-row tile, error bound per query
+enum CoarseKind : int { CoarseTF32 = 0, CoarseF16 = 1, CoarseDirect16 = 2, CoarseDirect8 = 3, CoarseQ8 = 4 };
 inline float coarse_eps(CoarseKind k) { return k == CoarseF16 ? kCoarseEpsF16 : kCoarseEpsTF32; }
 
 struct CoarsePlan {
@@ -68,13 +70,28 @@ cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim
                           uint32_t *d_overflow = nullptr, const uint32_t *d_filt = nullptr, uint32_t filt_words = 0,
                           const uint32_t *d_filt_q = nullptr);
 // bound of the fixed pass from the sample pass's candidate lists: d_thr[q] = k-th smallest approximate distance + 2 eps;
-// clears d_overflow[q]
+// clears d_overflow[q].  d_q_eps (nullable; the int8 shadow): eps of each query, in place of eps / d_q_norm2
 cudaError_t launch_threshold(const uint64_t *d_cand, uint32_t nq, uint32_t lists_per_query, uint32_t keep, uint32_t k, float eps,
-                             const float *d_q_norm2, float max_norm, uint32_t dim, int l2, float *d_thr, uint32_t *d_overflow, cudaStream_t s);
+                             const float *d_q_norm2, float max_norm, uint32_t dim, int l2, float *d_thr, uint32_t *d_overflow, cudaStream_t s,
+                             const float *d_q_eps = nullptr);
 // fp32 rows [first, first+n) -> the tiled fp16 shadow copy read by the CoarseF16 kernel (layout in coarse_tc.cu);
 // the buffer holds coarse_shadow_bytes(capacity_rows, dim) bytes
 size_t coarse_shadow_bytes(uint32_t rows, uint32_t dim);
 cudaError_t launch_to_f16_tiled(const void *src, size_t spitch, uint32_t dim, uint32_t first, uint32_t n, void *dst, cudaStream_t s);
+// fp32 unit rows -> the tiled int8 shadow read by the CoarseQ8 kernel: every 128-row tile that holds a row of [first, first+n) is
+// quantized whole (rows past n_rows are zero) with its scale s_t = max |x| / 127 into d_tscale[tile], round to nearest.  d_stats
+// keeps running maxima, as float bits rounded up, of the residual norm |x - s_t x~| and of |x| over the rows quantized; the buffer
+// holds coarse_shadow8_bytes(capacity_rows, dim) bytes
+size_t coarse_shadow8_bytes(uint32_t rows, uint32_t dim);
+cudaError_t launch_to_i8_tiled(const void *src, size_t spitch, uint32_t dim, uint32_t n_rows, uint32_t first, uint32_t n, void *dst,
+                               float *d_tscale, uint32_t *d_stats, cudaStream_t s);
+// bytes of one int8 query row of the CoarseQ8 kernel: the payload padded to 16, its scale s_q (float), padding
+inline size_t coarse_q8_payload(uint32_t dim) { return (dim + 15) & ~(size_t)15; }
+inline size_t coarse_q8_pitch(uint32_t dim) { return coarse_q8_payload(dim) + 16; }
+// nq fp32 unit queries -> int8 rows (coarse_q8_pitch) with their scale, and d_eps[q], a rigorous bound of |approx - exact| for
+// every stored row, from the row bounds delta_max (residual norm) and x_max (row norm) of the shadow; NaN when not finite
+cudaError_t launch_quantize_queries(const void *d_q, size_t qpitch, uint32_t dim, uint32_t nq, void *d_q8, float *d_eps, float delta_max,
+                                    float x_max, cudaStream_t s);
 // fp32 rows [first, first+n) -> row-major fp16 rows (the query batch; dim % 8 == 0)
 cudaError_t launch_to_f16(const void *src, size_t spitch, uint32_t dim, uint32_t first, uint32_t n, void *dst, size_t dpitch,
                           cudaStream_t s);
@@ -83,11 +100,12 @@ cudaError_t launch_to_f16(const void *src, size_t spitch, uint32_t dim, uint32_t
 // |approx - exact| <= eps; otherwise the bound scales with max_norm (over all rows) and |q| (refine_kernel).  Second tier:
 // d_q_index[i] = query of the original batch whose lists sit at position i (d_q_norm2 is indexed by position), *d_nq_dev
 // live positions.  d_row_label (nullable): the answer's composites carry row_label[row] (a docId) in place of the row, and ties
-// resolve by it.
+// resolve by it.  d_q_eps (nullable; the int8 shadow): the bound of each query by position, in place of eps / d_q_norm2.
 cudaError_t launch_refine(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t lists_per_query, uint32_t keep,
                           uint32_t k, const uint64_t *d_cand, float eps, const float *d_q_norm2, float max_norm, uint32_t *d_ok,
                           uint64_t *d_out, const uint32_t *d_q_index, const uint32_t *d_nq_dev, cudaStream_t s,
-                          const float *d_thr_T = nullptr, const uint32_t *d_overflow = nullptr, const uint64_t *d_row_label = nullptr);
+                          const float *d_thr_T = nullptr, const uint32_t *d_overflow = nullptr, const uint64_t *d_row_label = nullptr,
+                          const float *d_q_eps = nullptr);
 // direct 16-bit route: d_ok[q] = d_overflow[q] ? 0 : 1
 cudaError_t launch_flags_from_overflow(const uint32_t *d_overflow, uint32_t nq, uint32_t *d_ok, cudaStream_t s);
 // second tier of the direct route: row i of src ([.][k] composites) -> row d_idx[i] of dst, d_ok[d_idx[i]] = 2, for i < *d_count

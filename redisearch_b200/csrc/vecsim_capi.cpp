@@ -326,6 +326,7 @@ int VecSimB200_HybridRangeQueryBatchDevice(VecSimIndex *index, const void *d_que
                                                 d_out_scores, d_out_counts, out_modes, static_cast<cudaStream_t>(stream));
 }
 int VecSimB200_LastBatchPath(VecSimIndex *index) { return IX(index)->last_batch_path(); }
+int VecSimB200_LastCoarseShadowBits(VecSimIndex *index) { return IX(index)->last_shadow_bits(); }
 void VecSimB200_SetCoarseMode(int mode) { rsb200::set_coarse_mode(mode); }
 int VecSimB200_LastCoarseFlags(VecSimIndex *index, uint32_t *out_ok, size_t nq) { return IX(index)->last_coarse_flags(out_ok, nq); }
 const char *VecSimB200_Version(void) { return "vecsim_b200 0.1 (sm_90a)"; }

@@ -174,6 +174,9 @@ FlatIndex::~FlatIndex() {
     }
     cudaFree(d_rows_);
     cudaFree(d_shadow_);
+    cudaFree(d_shadow8_);
+    cudaFree(d_tscale_);
+    cudaFree(d_stats8_);
     cudaFree(d_norm2_);
     cudaFree(d_stats_);
     cudaFree(d_label_to_id_);
@@ -592,7 +595,7 @@ VecSimQueryReply *FlatIndex::topk(const void *q, size_t k, VecSimQueryParams *qp
     if (ok && !multi_ && std::min(k, n) <= (size_t)kMaxFusedK) {
         const uint32_t ke = (uint32_t)std::min(k, n);
         const uint64_t *d_res = nullptr;
-        if (single_query_takes_coarse(ke, reinterpret_cast<const float *>(c->h_query))) {
+        if (single_query_takes_coarse(ke, reinterpret_cast<const float *>(c->h_query), q8_route(1, ke))) {
             // an up-to-date fp16 shadow exists (a batch built it): one pass over 15 GB of it + exact rescoring + proof
             // beats the 31 GB exact scan; same answer (DESIGN.md §4)
             uint64_t *r = nullptr;
@@ -711,10 +714,12 @@ static int coarse_mode() {
     return m;
 }
 
-// Single queries (and batches below 16) take the tensor-core route only if that costs nothing extra: mode 1, an fp16
-// shadow that is already complete, fp32 cosine, k within the coarse lists.  host_query (nullable): the stored-form query; a
-// raw inner-product / L2 query whose fp16 form is not finite (|x| >= 65520 or NaN) cannot be proven and takes the exact scan.
-bool FlatIndex::single_query_takes_coarse(uint32_t ke, const float *host_query) {
+// Single queries (and batches below 16) take the tensor-core route only if that costs nothing extra: mode 1, the copy the route
+// reads already complete, fp32 cosine, k within the coarse lists.  host_query (nullable): the stored-form query; a raw
+// inner-product / L2 query whose fp16 form is not finite (|x| >= 65520 or NaN) cannot be proven and takes the exact scan.  q8:
+// the route reads the int8 copy (KNN batches where q8_route holds), else the fp16 shadow (every other KNN batch, and the range
+// and hybrid routes).
+bool FlatIndex::single_query_takes_coarse(uint32_t ke, const float *host_query, bool q8) {
     if (coarse_mode() != 1 || multi_ || coarse_disabled_ || dtype_ != DT_F32) return false;
     if (!unit_rows() && !(shadow_max_abs_ <= 60000.0f)) return false; // fp16 range (also false before the first build)
     if (!unit_rows() && host_query)
@@ -722,16 +727,22 @@ bool FlatIndex::single_query_takes_coarse(uint32_t ke, const float *host_query) 
             if (!(std::fabs(host_query[i]) < 65520.0f)) return false;
     {
         std::lock_guard<std::mutex> g(mu_);
-        if (!d_shadow_ || shadow_rows_ != count_ || !shadow_dirty_.empty() || shadow_cap_ < count_) return false;
+        if (!(q8 ? d_shadow8_ && std::isfinite(shadow8_delta_) && std::isfinite(shadow8_xmax_) : d_shadow_ != nullptr) ||
+            shadow_rows_ != count_ || !shadow_dirty_.empty() || shadow_cap_ < count_)
+            return false;
     }
-    return coarse_supported(view(), 1, ke, CoarseF16);
+    return q8 || coarse_supported(view(), 1, ke, CoarseF16);
+}
+
+bool FlatIndex::q8_route(uint32_t nq, uint32_t ke) const {
+    return coarse_mode() == 1 && !multi_ && unit_rows() && coarse_fixed_enabled() && coarse_supported(view(), nq, ke, CoarseQ8);
 }
 
 // Bring the fp16 shadow copy of the rows up to date on `st` (rows appended, overwritten or moved by a
 // swap-delete since the last coarse batch).  Returns false if HBM for the shadow cannot be had; the
 // caller then runs the TF32 variant on the fp32 rows.
 // int8 / uint8 L2 indexes keep no shadow, only the exact int32 |row|^2 of every row, under the same bookkeeping.
-bool FlatIndex::ensure_shadow(cudaStream_t st) {
+bool FlatIndex::ensure_shadow(cudaStream_t st, bool q8) {
     std::lock_guard<std::mutex> g(mu_);
     const bool inorm = int_l2();
     if (inorm && (shadow_cap_ < count_ || !d_norm2_)) {
@@ -747,15 +758,62 @@ bool FlatIndex::ensure_shadow(cudaStream_t st) {
         }
         shadow_cap_ = cap;
     }
-    if (!inorm && (shadow_cap_ < count_ || !d_shadow_)) {
-        const size_t cap = std::max(capacity_, count_);
+    bool launched = false;
+    if (!inorm && shadow_cap_ >= count_ && (q8 ? !d_shadow8_ : !d_shadow_) && (d_shadow_ || d_shadow8_)) {
+        // the other copy is kept: allocate only the missing one and build it over the rows the other covers; the refresh below
+        // brings both over dirty and appended rows
+        const size_t cap = shadow_cap_;
         uint8_t *nu = nullptr;
-        if (cudaMalloc(&nu, coarse_shadow_bytes((uint32_t)cap, (uint32_t)dim_)) != cudaSuccess) {
+        float *nsc = nullptr;
+        if (cudaMalloc(&nu, q8 ? coarse_shadow8_bytes((uint32_t)cap, (uint32_t)dim_) : coarse_shadow_bytes((uint32_t)cap, (uint32_t)dim_)) !=
+                cudaSuccess ||
+            (q8 && (cudaMalloc(&nsc, (cap + 127) / 128 * sizeof(float)) != cudaSuccess ||
+                    (!d_stats8_ && cudaMalloc(&d_stats8_, 8) != cudaSuccess)))) {
             cudaGetLastError();
+            cudaFree(nu);
+            cudaFree(nsc);
             return false;
         }
-        cudaFree(d_shadow_); // rows are re-converted below (one conversion kernel over the rows)
+        const uint32_t n = (uint32_t)std::min(shadow_rows_, count_);
+        cudaError_t e;
+        if (q8) {
+            d_shadow8_ = nu;
+            d_tscale_ = nsc;
+            e = cudaMemsetAsync(d_stats8_, 0, 8, st);
+            if (e == cudaSuccess) e = launch_to_i8_tiled(d_rows_, pitch_, (uint32_t)dim_, (uint32_t)count_, 0, n, d_shadow8_, d_tscale_, d_stats8_, st);
+        } else {
+            d_shadow_ = nu;
+            e = launch_to_f16_tiled(d_rows_, pitch_, (uint32_t)dim_, 0, n, d_shadow_, st);
+        }
+        if (e != cudaSuccess) { // the new copy does not cover the rows: every copy is rebuilt next time
+            shadow_rows_ = 0;
+            shadow_dirty_.clear();
+            return false;
+        }
+        launched = true;
+    }
+    if (!inorm && (shadow_cap_ < count_ || (q8 ? !d_shadow8_ : !d_shadow_))) {
+        // the requested copy and every copy already kept, at the capacity; rows are re-converted below
+        const size_t cap = std::max(capacity_, count_);
+        const bool k16 = !q8 || d_shadow_, k8 = q8 || d_shadow8_;
+        uint8_t *nu = nullptr, *nu8 = nullptr;
+        float *nsc = nullptr;
+        if ((k16 && cudaMalloc(&nu, coarse_shadow_bytes((uint32_t)cap, (uint32_t)dim_)) != cudaSuccess) ||
+            (k8 && (cudaMalloc(&nu8, coarse_shadow8_bytes((uint32_t)cap, (uint32_t)dim_)) != cudaSuccess ||
+                    cudaMalloc(&nsc, (cap + 127) / 128 * sizeof(float)) != cudaSuccess)) ||
+            (k8 && !d_stats8_ && cudaMalloc(&d_stats8_, 8) != cudaSuccess)) {
+            cudaGetLastError();
+            cudaFree(nu);
+            cudaFree(nu8);
+            cudaFree(nsc);
+            return false;
+        }
+        cudaFree(d_shadow_);
+        cudaFree(d_shadow8_);
+        cudaFree(d_tscale_);
         d_shadow_ = nu;
+        d_shadow8_ = nu8;
+        d_tscale_ = nsc;
         cudaFree(d_norm2_);
         d_norm2_ = nullptr;
         shadow_cap_ = cap;
@@ -776,18 +834,23 @@ bool FlatIndex::ensure_shadow(cudaStream_t st) {
         shadow_dirty_.clear();
     }
     if (shadow_rows_ > count_) shadow_rows_ = count_;
-    // rows [first, first + n) into every copy this index keeps
+    // rows [first, first + n) into every copy this index keeps (the int8 copy re-quantizes the whole tiles that hold them: a
+    // changed row may change its tile's scale)
     const auto refresh = [&](uint32_t first, uint32_t n) {
         if (inorm) return launch_int_norm2(d_rows_, pitch_, (uint32_t)dim_, first, n, dtype_ == DT_I8, reinterpret_cast<int32_t *>(d_norm2_), st) ==
                           cudaSuccess;
-        if (launch_to_f16_tiled(d_rows_, pitch_, (uint32_t)dim_, first, n, d_shadow_, st) != cudaSuccess) return false;
+        if (d_shadow_ && launch_to_f16_tiled(d_rows_, pitch_, (uint32_t)dim_, first, n, d_shadow_, st) != cudaSuccess) return false;
+        if (d_shadow8_ && launch_to_i8_tiled(d_rows_, pitch_, (uint32_t)dim_, (uint32_t)count_, first, n, d_shadow8_, d_tscale_, d_stats8_, st) !=
+                              cudaSuccess)
+            return false;
         return !d_norm2_ || launch_row_stats(d_rows_, pitch_, (uint32_t)dim_, first, n, d_norm2_, d_stats_, st) == cudaSuccess;
     };
-    bool launched = false;
     if (shadow_dirty_.size() > 256) {
         shadow_rows_ = 0;
         shadow_dirty_.clear();
     }
+    // a full rebuild recomputes the int8 copy's residual and norm maxima
+    if (d_shadow8_ && shadow_rows_ == 0 && count_ > 0 && cudaMemsetAsync(d_stats8_, 0, 8, st) != cudaSuccess) return false;
     for (idType id : shadow_dirty_)
         if (id < shadow_rows_) {
             if (!refresh(id, 1)) return false;
@@ -802,9 +865,14 @@ bool FlatIndex::ensure_shadow(cudaStream_t st) {
     // other query streams may read the shadow as soon as the lock is released
     if (launched) {
         const bool stats = d_norm2_ && !inorm;
-        uint32_t h[2] = {0, 0};
+        uint32_t h[2] = {0, 0}, h8[2] = {0, 0};
         if (stats && cudaMemcpyAsync(h, d_stats_, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) return false;
+        if (d_shadow8_ && cudaMemcpyAsync(h8, d_stats8_, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess) return false;
         if (cudaStreamSynchronize(st) != cudaSuccess) return false;
+        if (d_shadow8_) {
+            memcpy(&shadow8_delta_, &h8[0], 4);
+            memcpy(&shadow8_xmax_, &h8[1], 4);
+        }
         if (stats) { // running maxima over every row ever converted (deletes do not lower them: conservative)
             float n2, ma;
             memcpy(&n2, &h[0], 4);
@@ -820,8 +888,12 @@ void FlatIndex::disable_coarse() {
     std::lock_guard<std::mutex> g(mu_);
     coarse_disabled_ = true;
     cudaFree(d_shadow_);
+    cudaFree(d_shadow8_);
+    cudaFree(d_tscale_);
     cudaFree(d_norm2_);
     d_shadow_ = nullptr;
+    d_shadow8_ = nullptr;
+    d_tscale_ = nullptr;
     d_norm2_ = nullptr;
     shadow_cap_ = shadow_rows_ = 0;
     shadow_dirty_.clear();
@@ -956,7 +1028,11 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
     // k > kCoarseMaxK (DESIGN.md §4.5): the fp16 route's two-pass first tier, for batches of 16 queries and more
     const bool wide = ke > kCoarseMaxK;
     const bool eligible = cmode != 0 && !coarse_disabled_ && dtype_ == DT_F32 && (unit || cmode == 1) &&
-                          (nq >= 16 || (!wide && single_query_takes_coarse(ke))) && (!wide || coarse_fixed_enabled());
+                          (nq >= 16 || (!wide && single_query_takes_coarse(ke, nullptr, q8_route(nq, ke)))) && (!wide || coarse_fixed_enabled());
+    // unit rows with k <= kCoarseMaxK: the int8 copy (DESIGN.md §4.2), unless its bounds are not finite (a NaN or inf row)
+    if (eligible && kind == CoarseF16 && q8_route(nq, ke) && ensure_shadow(st, true) && std::isfinite(shadow8_delta_) &&
+        std::isfinite(shadow8_xmax_))
+        kind = CoarseQ8;
     bool coarse = eligible && coarse_supported(v, nq, ke, kind);
     if (eligible && kind == CoarseF16 && (!coarse || !ensure_shadow(st))) { // rows too wide for the 16-bit kernel's shared memory, or no HBM for the shadow
         kind = CoarseTF32;
@@ -969,6 +1045,7 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
     }
     last_batch_coarse_ = coarse;
     last_batch_path_ = coarse ? 1 : 0;
+    last_shadow_bits_ = !coarse ? 0 : kind == CoarseQ8 ? 8 : kind == CoarseF16 ? 16 : 0;
     if (!coarse && tc_only) {
         *d_result = nullptr;
         return true;
@@ -1000,7 +1077,8 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
     //   main pass     all row tiles, every row with approximate distance < T is kept (fixed bound: no running thresholds,
     //                 no list compaction, which a running threshold keeps the epilogue busy with)
     // TF32 route: one pass with adaptive lists, as before.
-    const bool two_pass = kind == CoarseF16 && coarse_fixed_enabled();
+    const bool q8 = kind == CoarseQ8, shadow = kind == CoarseF16 || q8;
+    const bool two_pass = shadow && coarse_fixed_enabled();
     CoarsePlan cp = plan_coarse(v, nq, kind, ke); // TF32 / single-pass: the adaptive lists ARE the first tier
     CoarsePlan cps{};                             // sample pass
     if (two_pass) {
@@ -1013,8 +1091,10 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
             // holds about 4 k rows (128 per visited tile).
             cps = plan_coarse(v, nq, kind, ke, kCoarseKeepWide, sample_stride(probe, ke, 128.0, 1 / 32.0), 0);
         } else {
-            // the sample holds a few times k slice minima (4 per visited tile)
-            cps = plan_coarse(v, nq, kind, ke, 0, sample_stride(probe, ke, 24.0, 2.0), 2);
+            // the sample holds a few times k slice minima (4 per visited tile).  The int8 copy's bound is about 7x the fp16 one's, and
+            // the rows within 2 eps of the k-th distance, not k / f, fill most of its lists of 256: it samples about 4 % at k = 10 over
+            // 30 ranges (aim 8), which keeps the rows below the bound near a quarter of a list on uniform unit rows
+            cps = plan_coarse(v, nq, kind, ke, 0, sample_stride(probe, ke, q8 ? 8.0 : 24.0, 2.0), 2);
         }
         cp = probe;
     }
@@ -1022,17 +1102,18 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
     // rows of one range within the bound — clustered corpora) are packed to the front and run once more with adaptive
     // lists of 128 per row range.  Nothing is known on the host: the tier's kernels read the count of open queries from
     // device memory and leave at once when it is zero.
-    const bool tier2 = kind == CoarseF16 && coarse_tier2_enabled();
+    const bool tier2 = shadow && coarse_tier2_enabled();
     CoarsePlan cp2{};
     if (tier2) cp2 = plan_coarse(v, nq, kind, ke, kCoarseKeepWide);
     const size_t nO = (size_t)nq * ke;
-    const size_t q16_pitch = (dim_ * 2 + 15) & ~(size_t)15;
-    const size_t q16_bytes = kind == CoarseF16 ? (size_t)nq * q16_pitch : 0;
+    // the queries in the operand type of the copy: fp16 rows, or int8 rows with their scale (coarse_q8_pitch)
+    const size_t q16_pitch = q8 ? coarse_q8_pitch((uint32_t)dim_) : (dim_ * 2 + 15) & ~(size_t)15;
+    const size_t q16_bytes = shadow ? (size_t)nq * q16_pitch : 0;
     const size_t scratch = std::max(std::max(cp.scratch_elems, two_pass ? cps.scratch_elems : 0), tier2 ? cp2.scratch_elems : 0);
     const size_t nO12 = wide ? 0 : nO; // k > kMaxFusedK: the tiers write the answer rows in place, no out1 / out2
     uint64_t *coarse_cand, *cand_s, *cand_t2, *out1, *out2, *cand2, *list_scratch;
     uint8_t *q16, *q16_t2;
-    float *d_qn2, *d_qn2_t2, *d_thr;
+    float *d_qn2, *d_qn2_t2, *d_thr, *d_qeps, *d_qeps_t2;
     uint32_t *d_ok, *d_idx, *d_n2, *d_ovf;
     const auto layout = [&](void *base) {
         BatchScratch s(base);
@@ -1048,6 +1129,8 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
         list_scratch = s.take<uint64_t>(scratch);
         d_qn2 = s.take<float>(unit ? 0 : nq); // |q|^2 per query
         d_qn2_t2 = s.take<float>(unit || !tier2 ? 0 : nq);
+        d_qeps = s.take<float>(q8 ? nq : 0); // int8 copy: the error bound of each query
+        d_qeps_t2 = s.take<float>(q8 && tier2 ? nq : 0);
         d_ok = s.take<uint32_t>(nq);
         d_idx = s.take<uint32_t>(nq); // tier 2: indices of the open queries
         d_n2 = s.take<uint32_t>(1);   //         and their count
@@ -1067,12 +1150,16 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
         ops = CoarseOperands{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
         if (!unit) ok = ok && launch_row_stats(d_q, qpitch, (uint32_t)dim_, 0, nq, d_qn2, nullptr, st) == cudaSuccess;
         lc.launches += unit ? 1 : 2;
+    } else if (q8) {
+        ok = launch_quantize_queries(d_q, qpitch, (uint32_t)dim_, nq, q16, d_qeps, shadow8_delta_, shadow8_xmax_, st) == cudaSuccess;
+        ops = CoarseOperands{d_shadow8_, 0, q16, q16_pitch, 1, 0, d_tscale_, nullptr};
+        lc.launches++;
     }
     const float eps = coarse_eps(kind);
     if (two_pass) {
         ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq, cps, cand_s, list_scratch, st) == cudaSuccess;
         ok = ok && launch_threshold(cand_s, nq, cps.grid_x, cps.keep, ke, eps, d_qn2, shadow_max_norm_, (uint32_t)dim_, mkind_ == MT_L2 ? 1 : 0, d_thr,
-                                    d_ovf, st) == cudaSuccess;
+                                    d_ovf, st, q8 ? d_qeps : nullptr) == cudaSuccess;
         lc.launches += 2;
     }
     cudaEventRecord(c.ev_start, st);
@@ -1081,17 +1168,18 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
     cudaEventRecord(c.ev_stop, st);
     // exact rescoring of the few candidates that can still matter + exact top-k + proof, one CTA per query
     ok = ok && launch_refine(v, d_q, qpitch, nq, cp.grid_x, cp.keep, ke, coarse_cand, eps, d_qn2, shadow_max_norm_, d_ok, out1, nullptr, nullptr,
-                             st, two_pass ? d_thr : nullptr, two_pass ? d_ovf : nullptr) == cudaSuccess;
+                             st, two_pass ? d_thr : nullptr, two_pass ? d_ovf : nullptr, nullptr, q8 ? d_qeps : nullptr) == cudaSuccess;
     lc.launches += 2;
     if (tier2) {
         ok = ok && launch_compact_unproven(d_ok, nq, d_idx, d_n2, st) == cudaSuccess;
-        ok = ok && launch_gather_queries(q16, q16_pitch, d_qn2, d_idx, d_n2, nq, q16_t2, d_qn2_t2, st) == cudaSuccess;
+        // the open queries' operand rows with their |q|^2 (fp16 copy) or error bound (int8 copy)
+        ok = ok && launch_gather_queries(q16, q16_pitch, q8 ? d_qeps : d_qn2, d_idx, d_n2, nq, q16_t2, q8 ? d_qeps_t2 : d_qn2_t2, st) == cudaSuccess;
         CoarseOperands ops2 = ops;
         ops2.queries = q16_t2;
-        ops2.q_norm2 = d_qn2_t2;
+        if (!q8) ops2.q_norm2 = d_qn2_t2;
         ok = ok && launch_coarse(ops2, v.n_rows, v.dim, nq, cp2, cand_t2, list_scratch, st, d_n2) == cudaSuccess;
         ok = ok && launch_refine(v, d_q, qpitch, nq, cp2.grid_x, cp2.keep, ke, cand_t2, eps, d_qn2_t2, shadow_max_norm_, d_ok, out1, d_idx, d_n2,
-                                 st) == cudaSuccess;
+                                 st, nullptr, nullptr, nullptr, q8 ? d_qeps_t2 : nullptr) == cudaSuccess;
         lc.launches += 4;
     }
     if (wide) {

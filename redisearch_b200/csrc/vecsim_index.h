@@ -250,6 +250,14 @@ class FlatIndex {
     // valid except shadow_dirty_
     uint8_t *d_shadow_ = nullptr;
     size_t shadow_cap_ = 0, shadow_rows_ = 0;
+    // int8 copy of unit rows for the cosine batches with k <= kCoarseMaxK (DESIGN.md §4.2), the same tiled layout with one byte per
+    // element and one scale per 128-row tile (d_tscale_); built lazily by the first batch that takes it and kept by the same
+    // bookkeeping as the fp16 copy.  d_stats8_ = running maxima (float bits) of the quantization residual norm and of the row norm
+    // over every row quantized since the last full rebuild, mirrored on the host after each refresh
+    uint8_t *d_shadow8_ = nullptr;
+    float *d_tscale_ = nullptr;
+    uint32_t *d_stats8_ = nullptr;
+    float shadow8_delta_ = 0.0f, shadow8_xmax_ = 0.0f;
     // L2 / raw inner-product indexes: |row|^2 per row and the running maxima the error bound needs.  int8 / uint8 L2 indexes keep
     // the exact int32 |row|^2 here (stored as int32, no shadow, no maxima) for the integer tensor-core route; the same
     // shadow_rows_ / shadow_dirty_ / shadow_cap_ bookkeeping tracks it
@@ -263,12 +271,15 @@ class FlatIndex {
     bool unit_rows() const { return metric_ == VecSimMetric_Cosine && !raw_rows_; }
     std::vector<idType> shadow_dirty_;
     // a per-row copy (the fp16 shadow and / or |row|^2) exists: in-place overwrites and swap-deletes go to shadow_dirty_
-    bool keeps_row_copies() const { return d_shadow_ || d_norm2_; }
+    bool keeps_row_copies() const { return d_shadow_ || d_shadow8_ || d_norm2_; }
     bool int_l2() const { return (dtype_ == DT_I8 || dtype_ == DT_U8) && mkind_ == MT_L2; }
     // fp32: the fp16 shadow (+ |row|^2 unless unit rows); int8 / uint8 L2: only the int32 |row|^2 table
-    bool ensure_shadow(cudaStream_t st);
+    // q8: the int8 copy instead (unit rows); every copy the index already keeps is brought up to date either way
+    bool ensure_shadow(cudaStream_t st, bool q8 = false);
+    // a KNN batch of this k on this single-value index of unit rows runs on the int8 copy (its bounds are finite once built)
+    bool q8_route(uint32_t nq, uint32_t ke) const;
     void disable_coarse(); // rows outside the fp16 range: exact scans from now on, the shadow's HBM is given back
-    bool single_query_takes_coarse(uint32_t ke, const float *host_query = nullptr);
+    bool single_query_takes_coarse(uint32_t ke, const float *host_query = nullptr, bool q8 = false);
     size_t capacity_ = 0; // rows of HBM allocated
     size_t count_ = 0;    // rows in the index (incl. staged)
     size_t resident_ = 0; // rows already copied to HBM
@@ -311,6 +322,8 @@ class FlatIndex {
     int last_batch_path_ = 0; // 0 exact scan, 1 tensor-core coarse pass + proof, 2 tensor-core direct (16-bit corpora); multi-value: the row stage's
   public:
     int last_batch_path() const { return last_batch_path_; }
+    int last_shadow_bits_ = 0; // the copy route 1 read: 8 int8, 16 fp16, 0 none
+    int last_shadow_bits() const { return last_shadow_bits_; }
   private:
     std::unique_ptr<QueryCtx> dev_ctx_; // scratch of topk_batch_device / topk_filtered_batch_device (stream-ordered)
     std::mutex dev_mu_;

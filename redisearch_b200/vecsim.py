@@ -155,6 +155,7 @@ SIGNATURES = [
     ("VecSimB200_TopKFiltered", C.c_int, [_P, _P, _SZ, _P, _SZ, C.c_int, _P, _P, C.POINTER(_SZ)]),
     ("VecSimB200_HybridTopK", C.c_int, [_P, _P, _SZ, _P, C.POINTER(VecSimQueryParams), _P, _P, C.POINTER(_SZ), C.POINTER(C.c_int), C.POINTER(_SZ)]),
     ("VecSimB200_LastBatchPath", C.c_int, [_P]),
+    ("VecSimB200_LastCoarseShadowBits", C.c_int, [_P]),
     ("VecSimB200_SetCoarseMode", None, [C.c_int]),
     ("VecSimB200_LastCoarseFlags", C.c_int, [_P, _P, _SZ]),
     ("VecSimB200_Version", C.c_char_p, []),
