@@ -562,7 +562,8 @@ coarse_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
 // QUERY: its threshold lives in a register and its candidate list needs no atomics.  64 queries per CTA (not 128) so
 // that the resident queries fit shared memory next to the ring up to 1024 dimensions (16 KB per 128 dimensions per 128
 // queries would leave no room for the ring at 768); threads 64-127 of the warpgroup take part in the MMAs and the
-// warp-wide selections but own no query.
+// warp-wide selections but own no query.  The fixed-bound pass over the int8 shadow, whose queries take half the bytes,
+// holds 128 (coarse_cta_queries).
 //   The candidate lists live in global memory (L2): appends are rare once the thresholds have settled, and shared
 //   memory goes to the row-tile ring.
 // ------------------------------------------------------------------------------------------------
@@ -578,7 +579,6 @@ constexpr int kQKbPerStage = 2;     // K blocks per pipeline stage: amortises th
 constexpr int kQListStride = 129;   // lists[slot * stride + query slot]: conflict-free appends
 constexpr uint32_t kQBlockBytes = kQN * 128;                    // one K block of a row tile: 128 rows x 128 bytes
 constexpr uint32_t kQStageBytes = kQKbPerStage * kQBlockBytes; // 32 KB
-constexpr uint32_t kQABlockBytes = kQM * 128;                   // one K block of the queries: 64 x 128 bytes
 // K blocks of `bytes_per_row` bytes of operand (128 per block), padded to whole stages: the padding blocks are zero in the
 // queries (and in the fp16 shadow; tensor-map loads past the row fill zeros), so they add nothing to the dot products
 __host__ __device__ constexpr uint32_t coarse_kb(uint32_t bytes_per_row) {
@@ -591,6 +591,12 @@ constexpr uint32_t kQAccBytes = kQM * kQAccStride * 4;
 // (DESIGN.md §4.2: 5,022 -> 4,294 clk per tile at 10M x 768).  The other modes keep one: their epilogue transposes
 // through shared memory and compacts lists, which a second warpgroup would have to double.
 __host__ __device__ constexpr int coarse_consumers(int mode) { return mode == 1 ? 2 : 1; }
+// Queries per CTA.  The fixed-bound pass over the int8 shadow (kOp 5, mode 1) holds 128: each consumer warpgroup owns 64 of
+// them and both run their MMAs against every ring stage, so a row tile is copied into shared memory once per 128 queries
+// instead of once per 64 (384 instead of 480 KB of shared-memory traffic per 128 queries x 128 rows, DESIGN.md §4.2), and
+// at a batch of 256 the two query groups of a row range form clusters of two, which fill all the SMs.  Its int8 queries
+// take 128 B per K block and query, so 128 of them leave at least three ring stages up to 1024 dimensions
+__host__ __device__ constexpr int coarse_cta_queries(bool q8, int mode) { return q8 && mode == 1 ? 2 * kQM : kQM; }
 // warp 0 produces, warps 1-3 idle, warps 4.. are the consumer warpgroups
 __host__ __device__ constexpr int coarse_threads(int mode) { return 128 * (1 + coarse_consumers(mode)); }
 
@@ -790,6 +796,11 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
     constexpr bool kInt = kOp == 1 || kOp == 2 || kOp == 4 || kQ8;
     constexpr int kOpE = kQ8 ? 0 : kOp; // the epilogue of kOp 5 past the integer bound test is kOp 0's
     constexpr int kCons = coarse_consumers(kMode), kConsThreads = 128 * kCons;
+    // kWide: 128 queries per CTA, warpgroup cw takes the MMAs and the epilogue of queries 64 cw .. 64 cw + 63 of every tile
+    constexpr int kCtaQ = coarse_cta_queries(kQ8, kMode);
+    constexpr bool kWide = kCtaQ > kQM;
+    static_assert(!kWide || (kCons == 2 && kCtaQ == kCons * kQM), "a wide CTA: one consumer warpgroup per 64 queries");
+    constexpr uint32_t kQKbBytes = kCtaQ * 128; // one K block of the resident queries
     using Acc = typename std::conditional<kInt, uint32_t, float>::type;
     // bx = row range, by = query group
     const uint32_t bx = blockIdx.x, by = blockIdx.y, gx = gridDim.x;
@@ -814,28 +825,30 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
     // so their accesses compile to STS / LDS rather than generic stores and loads
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t *sB = smem;                                                   // nstages x kQKbPerStage x [128 rows x 128B]
-    uint8_t *sQ = sB + (size_t)nstages * kQStageBytes;                    // K blocks kRegKb .. num_kb - 1 x [64 queries x 128B], swizzled
-    uint32_t *sacc = reinterpret_cast<uint32_t *>(sQ + (size_t)(num_kb - kRegKb) * kQABlockBytes); // [kQM][kQAccStride]; not kFixed
+    // K blocks kRegKb .. num_kb - 1 x [64 queries x 128B], swizzled; kWide: two such 64-query halves per K block
+    uint8_t *sQ = sB + (size_t)nstages * kQStageBytes;
+    uint32_t *sacc = reinterpret_cast<uint32_t *>(sQ + (size_t)(num_kb - kRegKb) * kQKbBytes); // [kQM][kQAccStride]; not kFixed
     uint64_t *bars = reinterpret_cast<uint64_t *>(sacc + (kFixed ? 0 : kQM * kQAccStride));
     uint64_t *full = bars, *empty = bars + kQMaxStages;
-    uint32_t *qcount = reinterpret_cast<uint32_t *>(bars + 2 * kQMaxStages); // kFixed: [kQM] appends per query
+    uint32_t *qcount = reinterpret_cast<uint32_t *>(bars + 2 * kQMaxStages); // kFixed: [kCtaQ] appends per query
     // this CTA's candidate lists [kQListCap][kQListStride]
     uint64_t *lists = list_scratch + (size_t)(by * gx + bx) * (kQListCap * kQListStride);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t q_base = by * kQM;
+    const uint32_t q_base = by * kCtaQ;
     const uint32_t my_tiles = (tiles_total > bx) ? (tiles_total - bx + gx - 1) / gx : 0;
 
     if (threadIdx.x == 0) {
         for (uint32_t s = 0; s < nstages; s++) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], csize); // multicast clusters: every CTA of the cluster reads the stage and releases it
+            // multicast clusters: every CTA of the cluster reads the stage and releases it (kWide: each of its warpgroups)
+            mbar_init(&empty[s], kWide ? kCons * csize : csize);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
     __syncthreads();
-    // cluster mode: the csize CTAs that share blockIdx.x (one per group of 64 queries) walk the SAME row tiles.
+    // cluster mode: the csize CTAs that share blockIdx.x (one per query group) walk the SAME row tiles.
     // Each fetches 1/csize of every stage and multicasts it into all csize shared memories, so a tile leaves
     // HBM/L2 once per cluster instead of once per query group.
     const uint32_t crank = (csize > 1) ? cluster_ctarank() : 0;
@@ -851,6 +864,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         const long long t_pass = ca.now();
         for (uint32_t i = 0; i < my_tiles; i++) {
             const uint32_t tile = (bx + i * gx) * tile_stride;
+            ca.count(kCaTiles);
             for (uint32_t kb0 = 0; kb0 < num_kb; kb0 += kQKbPerStage) {
                 const uint32_t kbn = min((uint32_t)kQKbPerStage, num_kb - kb0);
                 const long long t_wait = ca.now();
@@ -898,14 +912,17 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         const int ew = kCons > 1 ? (warp - 4) & 3 : warp - 4; // warp of the warpgroup: accumulator rows (queries) 16 ew .. 16 ew + 15
         // 0..127 within the warpgroup; the query slot in the epilogue (slots >= kQM own no query)
         const int et = kCons > 1 ? (threadIdx.x - 128) & 127 : threadIdx.x - 128;
-        const uint32_t q = q_base + et;
+        // kWide: the CTA's query slots of this warpgroup start at wq, its queries at qw
+        const int wq = kWide ? kQM * cw : 0;
+        const uint32_t qw = q_base + wq;
+        const uint32_t q = qw + et;
         const bool live = et < kQM && q < nq;
-        // ===== queries -> shared memory (zero padded to num_kb * 128 bytes and to 64 queries) =====
-        if (cw == 0 && et < kQM) {
+        // ===== queries -> shared memory (zero padded to num_kb * 128 bytes and to kCtaQ queries) =====
+        if ((kWide || cw == 0) && et < kQM) {
             const uint4 *src = reinterpret_cast<const uint4 *>(q16 + (size_t)q * q16_pitch);
             for (uint32_t kb = kRegKb; kb < num_kb; kb++) {
                 // row `et` of a K-major 128B-swizzled operand tile: chunk u at et*128 + ((u ^ (et & 7)) * 16)
-                uint8_t *row = sQ + (size_t)(kb - kRegKb) * kQABlockBytes + et * 128;
+                uint8_t *row = sQ + (size_t)(kb - kRegKb) * kQKbBytes + wq * 128 + et * 128;
 #pragma unroll
                 for (int u = 0; u < 8; u++) {
                     uint4 x = make_uint4(0, 0, 0, 0);
@@ -913,7 +930,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                     *reinterpret_cast<uint4 *>(row + ((u ^ (et & 7)) * 16)) = x;
                 }
             }
-            if constexpr (kFixed) qcount[et] = 0;
+            if constexpr (kFixed) qcount[wq + et] = 0;
         }
         // kRegKb: this thread's A fragments of K blocks 0 .. kRegKb - 1 (k16 step t = 4 kb + kk), straight from q16 in every
         // consumer warpgroup, zero padded as sQ is (query slots >= nq, bytes past the row).  The wgmma.fence in front of
@@ -922,7 +939,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         if constexpr (kRegKb > 0) {
 #pragma unroll
             for (int i2 = 0; i2 < 2; i2++) {
-                const uint32_t fq = q_base + 16 * ew + (lane >> 2) + 8 * i2;
+                const uint32_t fq = qw + 16 * ew + (lane >> 2) + 8 * i2;
                 const uint8_t *src = q16 + (size_t)fq * q16_pitch;
 #pragma unroll
                 for (int t = 0; t < 4 * kRegKb; t++)
@@ -975,14 +992,14 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         if constexpr (kQ8) {
 #pragma unroll
             for (int i2 = 0; i2 < 2; i2++) {
-                const uint32_t fq = q_base + 16 * ew + (lane >> 2) + 8 * i2;
+                const uint32_t fq = qw + 16 * ew + (lane >> 2) + 8 * i2;
                 if (fq < nq) fsq[i2] = *reinterpret_cast<const float *>(q16 + (size_t)fq * q16_pitch + row_bytes);
             }
         }
         if constexpr (kFixed && kInt && !kQ8) {
 #pragma unroll
             for (int i2 = 0; i2 < 2; i2++) {
-                const uint32_t fq = q_base + 16 * ew + (lane >> 2) + 8 * i2;
+                const uint32_t fq = qw + 16 * ew + (lane >> 2) + 8 * i2;
                 const bool flive = fq < nq;
                 frad[i2] = flive ? thr_fixed[fq] : __int_as_float(0x7fffffff); // slots without a query: a NaN radius keeps nothing
                 fix[i2] = range_int_bound(frad[i2]);
@@ -998,7 +1015,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         if constexpr (kFixed && (!kInt || kQ8)) {
 #pragma unroll
             for (int i2 = 0; i2 < 2; i2++) {
-                const uint32_t fq = q_base + 16 * ew + (lane >> 2) + 8 * i2;
+                const uint32_t fq = qw + 16 * ew + (lane >> 2) + 8 * i2;
                 const bool flive = fq < nq;
                 fnq[i2] = (kOp == 3 && flive) ? q_norm2[fq] : 0.0f; // |q|^2
                 // fixed admission bound (a distance): keep every row with approximate distance < T
@@ -1015,20 +1032,24 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
             }
         }
         uint32_t s = 0, ph = 0;
-        const uint64_t bdesc_first = make_smem_desc(smem_u32(sB)), adesc_first = make_smem_desc(smem_u32(sQ));
-        constexpr uint64_t kStageStep = kQStageBytes >> 4, kBlockStep = kQBlockBytes >> 4, kABlockStep = kQABlockBytes >> 4;
+        const uint64_t bdesc_first = make_smem_desc(smem_u32(sB)), adesc_first = make_smem_desc(smem_u32(sQ + wq * 128));
+        constexpr uint64_t kStageStep = kQStageBytes >> 4, kBlockStep = kQBlockBytes >> 4, kAKbStep = kQKbBytes >> 4;
         // kCons warpgroups take tiles i = cw, cw + kCons, ...; a warpgroup steps its ring position past the stages of
         // the tiles the others take.  MMA issue stays in ring order: a warpgroup waits on a stage's `full` barrier only
         // once every earlier stage has been waited on, so that barrier is never more than one phase ahead of the wait.
+        // kWide: both warpgroups take every tile, each against its own 64 queries, and walk the ring independently: the
+        // producer refills a stage once both have released it, so neither is ever more than one ring ahead of the other, and
+        // one warpgroup's drain and bound test run under the other's MMAs.  (Issuing every stage in turn, warpgroup 0 first,
+        // left each one waiting through the other's bound test: DESIGN.md §4.2.)
         const uint32_t stages_per_tile = num_kb / kQKbPerStage;
         auto skip = [&](uint32_t n) {
             for (s += n; s >= nstages; s -= nstages) ph ^= 1;
         };
-        if (kCons > 1) skip(stages_per_tile * cw);
+        if (kCons > 1 && !kWide) skip(stages_per_tile * cw);
         const long long t_pass = ca.now();
-        for (uint32_t i = cw; i < my_tiles; i += kCons) {
+        for (uint32_t i = kWide ? 0 : cw; i < my_tiles; i += kWide ? 1 : kCons) {
             const uint32_t tile = (bx + i * gx) * tile_stride;
-            if (kCons > 1 && i >= (uint32_t)kCons) skip(stages_per_tile * (kCons - 1));
+            if (kCons > 1 && !kWide && i >= (uint32_t)kCons) skip(stages_per_tile * (kCons - 1));
             ca.count(kCaTiles);
             float nrm[kQN / 32]; // kOp 2 / 3: lane l holds the norm / squared norm of rows h*32 + l of the tile
             int inrm[kQN / 32];  // kOp 4: the same, int32
@@ -1067,7 +1088,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         rn[j] = make_float2(r < n_rows ? __ldg(row_norm2 + r) : 0.0f, 0.0f);
                 }
             }
-            if constexpr (kCons > 1) {
+            if constexpr (kCons > 1 && !kWide) {
                 static_assert(kCons == 2, "the hand-off pairs two warpgroups");
                 // hand-off: the warpgroup of tile i - 1 has issued its last MMAs (warpgroup cw waits on barrier 2 + cw)
                 const long long t_handoff = ca.now();
@@ -1079,7 +1100,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                 }
                 ca.add(kCaHandoff, t_handoff);
             }
-            // ===== D[64 queries x 128 rows] (+)= Q[smem] * rows[smem]^T =====
+            // ===== D[64 queries x 128 rows] (+)= Q[smem] * rows[smem]^T, per warpgroup =====
             Acc acc[64];
             uint32_t prev = 0;
             // one ring stage (K blocks kb0, kb0 + 1): wait for it, issue(bd) its MMAs against the stage's B descriptor, hand
@@ -1092,7 +1113,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                 wg_fence(); // the accumulator registers are handed to the MMA pipe for this stage's run
                 issue(bdesc_first + (uint64_t)s * kStageStep);
                 wg_commit();
-                if constexpr (kCons > 1) { // the tile's last MMAs are issued: the other warpgroup may start the next tile
+                if constexpr (kCons > 1 && !kWide) { // the tile's last MMAs are issued: the other warpgroup may start the next tile
                     if (kb0 + kQKbPerStage >= num_kb && i + 1 < my_tiles) {
                         if (cw == 0)
                             named_arrive<3, 2 * 128>();
@@ -1120,10 +1141,10 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
             }
             for (uint32_t kb0 = kRegKb; kb0 < num_kb; kb0 += kQKbPerStage)
                 stage(kb0, [&](uint64_t bd) {
-                    const uint64_t ad = adesc_first + (uint64_t)(kb0 - kRegKb) * kABlockStep;
+                    const uint64_t ad = adesc_first + (uint64_t)(kb0 - kRegKb) * kAKbStep;
 #pragma unroll
                     for (int x = 0; x < 4 * kQKbPerStage; x++)
-                        wgmma_n128<kInt, kVar>(acc, ad + (x >> 2) * kABlockStep + 2 * (x & 3), bd + (x >> 2) * kBlockStep + 2 * (x & 3),
+                        wgmma_n128<kInt, kVar>(acc, ad + (x >> 2) * kAKbStep + 2 * (x & 3), bd + (x >> 2) * kBlockStep + 2 * (x & 3),
                                                (kb0 | (uint32_t)x) != 0);
                 });
             const long long t_epilogue = ca.now();
@@ -1169,7 +1190,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         const uint32_t row = rbase + 8 * (b >> 1) + (b & 1);
                         const uint32_t key = orderable_key(__fsub_rn(1.0f, __fmul_rn(sqt, __int2float_rn((int)raw))));
                         if (key < fthr[i2]) {
-                            const int qs = 16 * ew + (lane >> 2) + 8 * i2;
+                            const int qs = wq + 16 * ew + (lane >> 2) + 8 * i2;
                             const uint32_t slot = atomicAdd(&qcount[qs], 1u);
                             if (slot < (uint32_t)kQListCap) lists[slot * kQListStride + qs] = ((uint64_t)key << 32) | row;
                         }
@@ -1244,7 +1265,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                             if (hit) hit = (__ldg(filt_row(q_base + 16 * ew + (lane >> 2) + 8 * i2) + (row >> 5)) >> (row & 31)) & 1u;
                         }
                         if (hit) {
-                            const int qs = 16 * ew + (lane >> 2) + 8 * i2;
+                            const int qs = wq + 16 * ew + (lane >> 2) + 8 * i2;
                             const uint32_t slot = atomicAdd(&qcount[qs], 1u);
                             if (slot < (uint32_t)kQListCap) lists[slot * kQListStride + qs] = ((uint64_t)orderable_key(d) << 32) | row;
                         }
@@ -1307,7 +1328,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                             if (admit) admit = (__ldg(filt_row(q_base + 16 * ew + (lane >> 2) + 8 * i2) + (row >> 5)) >> (row & 31)) & 1u;
                         }
                         if (admit) {
-                            const int qs = 16 * ew + (lane >> 2) + 8 * i2;
+                            const int qs = wq + 16 * ew + (lane >> 2) + 8 * i2;
                             const uint32_t slot = atomicAdd(&qcount[qs], 1u);
                             if (slot < (uint32_t)kQListCap) lists[slot * kQListStride + qs] = ((uint64_t)key << 32) | row;
                         }
@@ -1475,11 +1496,11 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         // publish: cand_out[q][blockIdx.x][keep], kEmptySlot padded
         __syncwarp();
         if constexpr (kFixed) {
-            // every append of the CTA is done; consumer warp pw publishes queries per * pw .. per * pw + per - 1.
+            // every append of the CTA is done; consumer warp pw publishes query slots per * pw .. per * pw + per - 1.
             // keep == kQListCap here (plan_coarse), so a list that did not overflow is published whole.  More rows below
             // the bound than the list holds: overflow, the query goes to the next tier.
             named_sync<1, kConsThreads>();
-            constexpr int per = kQM / (4 * kCons);
+            constexpr int per = kCtaQ / (4 * kCons);
             const int pw = 4 * cw + ew;
             for (int qs = per * pw; qs < per * pw + per; qs++) {
                 const uint32_t qq = q_base + qs;
@@ -2084,17 +2105,19 @@ static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, int epi, int m
     if (l2) return epl == 3 ? (const void *)coarse_wgmma_kernel<false, 3, 3, 0> : (const void *)coarse_wgmma_kernel<false, 8, 3, 0>;
     return epl == 3 ? (const void *)coarse_wgmma_kernel<false, 3, 0, 0> : (const void *)coarse_wgmma_kernel<false, 8, 0, 0>;
 }
-// shared memory of coarse_wgmma_kernel besides the ring: the resident queries (less the reg_kb K blocks held in registers), the
-// accumulator transpose (the fixed-bound pass, mode 1, tests the accumulators in registers and keeps a counter per query
-// instead), the barriers
-static size_t wgmma_fixed_smem(uint32_t num_kb, int mode = 0, uint32_t reg_kb = 0) {
-    return 1024 + (size_t)(num_kb - reg_kb) * kQABlockBytes + (mode == 1 ? kQM * 4 : kQAccBytes) + 2 * kQMaxStages * 8 + 64;
+// shared memory of coarse_wgmma_kernel besides the ring: the resident queries (cta_q per CTA, less the reg_kb K blocks held in
+// registers), the accumulator transpose (the fixed-bound pass, mode 1, tests the accumulators in registers and keeps a counter
+// per query instead), the barriers
+static size_t wgmma_fixed_smem(uint32_t num_kb, int mode = 0, uint32_t reg_kb = 0, uint32_t cta_q = kQM) {
+    return 1024 + (size_t)(num_kb - reg_kb) * cta_q * 128 + (mode == 1 ? cta_q * 4 : kQAccBytes) + 2 * kQMaxStages * 8 + 64;
 }
-static uint32_t wgmma_stages(uint32_t num_kb, int mode, uint32_t reg_kb) {
-    return (uint32_t)std::min<size_t>(kQMaxStages, (kSmemLimit - wgmma_fixed_smem(num_kb, mode, reg_kb)) / kQStageBytes);
+static uint32_t wgmma_stages(uint32_t num_kb, int mode, uint32_t reg_kb, uint32_t cta_q = kQM) {
+    return (uint32_t)std::min<size_t>(kQMaxStages, (kSmemLimit - wgmma_fixed_smem(num_kb, mode, reg_kb, cta_q)) / kQStageBytes);
 }
 // the 16/8-bit kernel needs at least two ring stages next to the resident queries (1024 fp16 dimensions fit)
-static bool wgmma_fits_bytes(uint32_t row_bytes) { return wgmma_fixed_smem(coarse_kb(row_bytes)) + 2 * (size_t)kQStageBytes <= kSmemLimit; }
+static bool wgmma_fits_bytes(uint32_t row_bytes, uint32_t cta_q = kQM) {
+    return wgmma_fixed_smem(coarse_kb(row_bytes), 0, 0, cta_q) + 2 * (size_t)kQStageBytes <= kSmemLimit;
+}
 static bool wgmma_fits(uint32_t dim) { return wgmma_fits_bytes(dim * 2); }
 
 static size_t fixed_smem(uint32_t num_kb) {
@@ -2118,7 +2141,7 @@ bool coarse_supported(const CorpusView &c, uint32_t nq, uint32_t k, CoarseKind k
     }
     if (kind == CoarseQ8) { // fp32 unit rows (the caller checks), inner product on the int8 shadow
         if (c.dtype != DT_F32 || c.metric != MT_IP || c.dim % 8 != 0 || c.dim < 32 || c.dim > 1024 || c.pitch % 16 != 0) return false;
-        if (k > kCoarseMaxK || nq < 1 || c.n_rows < 65536 || !wgmma_fits_bytes(c.dim)) return false;
+        if (k > kCoarseMaxK || nq < 1 || c.n_rows < 65536 || !wgmma_fits_bytes(c.dim, coarse_cta_queries(true, 1))) return false;
         // rows are padded to whole 256-byte stages: up to 128 dimensions the int8 row streams as many bytes and MMAs as the fp16 one
         if (coarse_kb(c.dim) >= coarse_kb(c.dim * 2)) return false;
         return encode_fn() != nullptr;
@@ -2146,7 +2169,8 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
     if (kind == CoarseF16 || kind == CoarseQ8 || kind == CoarseDirect16 || kind == CoarseDirect8) {
         p.num_kb = coarse_kb(kind == CoarseDirect8 || kind == CoarseQ8 ? c.dim : c.dim * 2);
         p.tiles = ((c.n_rows + kQN - 1) / kQN + p.tile_stride - 1) / p.tile_stride; // row tiles this pass visits
-        p.grid_y = (nq + kQM - 1) / kQM;
+        const uint32_t cta_q = (uint32_t)coarse_cta_queries(kind == CoarseQ8, p.mode);
+        p.grid_y = (nq + cta_q - 1) / cta_q;
         const uint32_t sms = (uint32_t)device_sm_count();
         p.grid_x = std::max(1u, std::min(p.tiles, sms / p.grid_y));
         // direct routes: the CTA's exact top-k of its rows.  fp32 route: candidates per (row range, query) — kCoarseKeep
@@ -2174,16 +2198,17 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
             if (rk && (int)rk <= rcap && p.num_kb >= rk + kQKbPerStage && wgmma_stages(p.num_kb, p.mode, rk) > wgmma_stages(p.num_kb, p.mode, 0))
                 p.reg_kb = rk;
         }
-        p.stages = wgmma_stages(p.num_kb, p.mode, p.reg_kb);
-        p.smem_bytes = wgmma_fixed_smem(p.num_kb, p.mode, p.reg_kb) + (size_t)p.stages * kQStageBytes;
-        // the query groups of a row range form a thread-block cluster (multicast of the row tiles)
+        p.stages = wgmma_stages(p.num_kb, p.mode, p.reg_kb, cta_q);
+        p.smem_bytes = wgmma_fixed_smem(p.num_kb, p.mode, p.reg_kb, cta_q) + (size_t)p.stages * kQStageBytes;
+        // the query groups of a row range form a thread-block cluster (multicast of the row tiles).  128 queries per CTA: pairs at
+        // most, which can fill all 132 SMs where clusters of four leave 12 idle (DESIGN.md §4.2)
         p.csize = 1;
         static int ccap = -1; // VECSIM_B200_CLUSTER caps the cluster size (1 = no clusters)
         if (ccap < 0) {
             const char *e = getenv("VECSIM_B200_CLUSTER");
             ccap = e ? std::max(1, atoi(e)) : 4;
         }
-        for (uint32_t cs = 4; cs > 1; cs >>= 1)
+        for (uint32_t cs = cta_q > kQM ? 2 : 4; cs > 1; cs >>= 1)
             if ((int)cs <= ccap && p.grid_y % cs == 0 && (kQStageBytes / kQKbPerStage) % (16 * cs) == 0) {
                 p.csize = cs;
                 break;

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Cycle account of the fixed-bound main pass of the batched fp32 KNN scan (coarse_wgmma_kernel<false,*,*,1>).
+"""Cycle account of the fixed-bound main pass of the batched fp32 KNN scan (coarse_wgmma_kernel<false,*,*,1>, over the int8
+copy at the flagship shape).
 
 Builds libvecsim_b200.so with -DCOARSE_CYCLE_ACCOUNT into a directory of its own (never redisearch_b200/lib/), runs the
 flagship shape of bench.py (FLAT 10M x 768 fp32 cosine, k=10, batch 256; bench.py's generators and seeds) and prints,
@@ -89,8 +90,8 @@ def main():
         live = [c for c in ctas if at(c, role, "pass") > 0]
         if not live:
             continue
-        # the producer fills the ring for every tile of the CTA
-        tiles = [at(c, 0, "tiles") + at(c, 1, "tiles") if role == 2 else at(c, role, "tiles") for c in live]
+        # the producer fills the ring once for every tile of the CTA; a consumer warpgroup counts the tiles it multiplies
+        tiles = [at(c, role, "tiles") for c in live]
         rows = {}
         for slot in SLOTS[:-1]:
             share = [at(c, role, slot) / at(c, role, "pass") for c in live]
