@@ -729,12 +729,17 @@ __device__ __forceinline__ int range_int_bound(float r) {
     return x;
 }
 
-// int8 shadow (kOp 5): an integer bound ti with  fl(fl(sqt * a)) > tdot  =>  a > ti  for every int32 accumulator a (|a| < 2^24,
-// exact in float), so that `a > ti` never drops a row the float test keeps: tdot / sqt loosened by 1e-5 relative (the rounding of
-// the division and of the product) and one more integer.  NaN: everything passes; a bound beyond +-2^25: everything / nothing.
-__device__ __forceinline__ int q8_dot_bound(float tdot, float sqt) {
-    const float f = tdot / sqt;
-    if (!(f == f)) return INT_MIN;
+// int8 shadow (kOp 5): an integer bound ti with  fl(sqt * a) > tdot  =>  a > ti  for every int32 accumulator a (|a| < 2^24,
+// exact in float), sqt = fl(s_q s_t), so that `a > ti` never drops a row the float test keeps.  No division: rq = fl(1 / s_q) is
+// taken once per query and rt = fl(1 / s_t) once per tile, and f = fl(tdot fl(rq rt)) is tdot / sqt up to six roundings of
+// 2^-24 relative (rq, rt, their product and f; sqt and fl(sqt a) on the test's side), under 3.6e-7 in all, which the 1e-5
+// relative loosening covers many times over; one more integer covers the rounding of the loosening and a subnormal f.  The
+// argument needs fl(rq rt) in [2^-125, 2^125], which keeps s_q s_t normal: outside it, and for NaN, everything passes.  A bound
+// beyond +-2^25: everything / nothing.
+__device__ __forceinline__ int q8_dot_bound(float tdot, float rq, float rt) {
+    const float r = __fmul_rn(rq, rt);
+    const float f = __fmul_rn(tdot, r);
+    if (!(f == f) || !(r >= 0x1p-125f && r <= 0x1p125f)) return INT_MIN;
     const float c = fminf(fmaxf(f, -33554432.0f), 33554432.0f);
     return (int)floorf(c - fabsf(c) * 1e-5f) - 1;
 }
@@ -989,11 +994,13 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
         int fix[2], fnqi[2];
         // kOp 5: the scales s_q of the two fragment queries (1 for slots without a query)
         float fsq[2] = {1.0f, 1.0f};
+        float frq[2] = {1.0f, 1.0f}; // kFixed: fl(1 / s_q) (q8_dot_bound)
         if constexpr (kQ8) {
 #pragma unroll
             for (int i2 = 0; i2 < 2; i2++) {
                 const uint32_t fq = qw + 16 * ew + (lane >> 2) + 8 * i2;
                 if (fq < nq) fsq[i2] = *reinterpret_cast<const float *>(q16 + (size_t)fq * q16_pitch + row_bytes);
+                if constexpr (kFixed) frq[i2] = __frcp_rn(fsq[i2]);
             }
         }
         if constexpr (kFixed && kInt && !kQ8) {
@@ -1077,6 +1084,10 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
             // kFixed: acc[4 j + 2 i2 + c] holds row rbase + 8 j + c of the tile; squared L2 loads the squared norms of
             // each row pair (j) at once
             const uint32_t rbase = tile * kQN + 2 * (lane & 3);
+            // kOp 5, fixed bound: the tile's scale s_t, loaded before the MMAs so that the bound test after the drain does not
+            // wait for it
+            float q8_st = 0.0f;
+            if constexpr (kFixed && kQ8) q8_st = __ldg(row_norm2 + tile);
             float2 rn[(kFixed && kOp == 3) ? kQN / 8 : 1];
             if constexpr (kFixed && kOp == 3) {
 #pragma unroll
@@ -1155,16 +1166,21 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
             if constexpr (kFixed && kQ8) {
                 // int8 shadow: the bound dot > fthr_dot becomes one integer bound per query on this tile's accumulators
                 // (q8_dot_bound); the rare survivors take the float distance and the exact key comparison, as kOp 0
-                const float st = __ldg(row_norm2 + tile);
+                const float st = q8_st, rst = __frcp_rn(st);
 #pragma unroll
                 for (int i2 = 0; i2 < 2; i2++) {
                     const float sqt = __fmul_rn(fsq[i2], st);
-                    const int ti = q8_dot_bound(fthr_dot[i2], sqt);
-                    int m8[8];
+                    const int ti = q8_dot_bound(fthr_dot[i2], frq[i2], rst);
+                    // the max of the query's 32 values: a tree of three-input maxima
+                    int m3[11];
 #pragma unroll
-                    for (int g = 0; g < 8; g++)
-                        m8[g] = max(max((int)acc[8 * g + 2 * i2], (int)acc[8 * g + 2 * i2 + 1]), max((int)acc[8 * g + 4 + 2 * i2], (int)acc[8 * g + 5 + 2 * i2]));
-                    const int mx = max(max(max(m8[0], m8[1]), max(m8[2], m8[3])), max(max(m8[4], m8[5]), max(m8[6], m8[7])));
+                    for (int g = 0; g < 10; g++)
+                        m3[g] = __vimax3_s32((int)acc[4 * ((3 * g) >> 1) + 2 * i2 + ((3 * g) & 1)],
+                                             (int)acc[4 * ((3 * g + 1) >> 1) + 2 * i2 + ((3 * g + 1) & 1)],
+                                             (int)acc[4 * ((3 * g + 2) >> 1) + 2 * i2 + ((3 * g + 2) & 1)]);
+                    m3[10] = max((int)acc[4 * 15 + 2 * i2], (int)acc[4 * 15 + 2 * i2 + 1]); // values 30, 31
+                    const int mx = __vimax3_s32(__vimax3_s32(m3[0], m3[1], m3[2]), __vimax3_s32(m3[3], m3[4], m3[5]),
+                                                __vimax3_s32(__vimax3_s32(m3[6], m3[7], m3[8]), m3[9], m3[10]));
                     uint32_t pass = 0; // bit 2 j + c: acc[4 j + 2 i2 + c]
                     if (mx > ti) {
 #pragma unroll
