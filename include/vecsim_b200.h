@@ -469,19 +469,23 @@ int VecSimB200_RangeQueryBatch(VecSimIndex *index, const void *queryBlobs, size_
  * (re-issue the query with a larger cap, or use VecSimB200_RangeQueryBatch).
  * Routes: single-value fp32 batches the fp32 route of VecSimB200_RangeQueryBatch serves take it; int8 / uint8 batches of
  * >= 16 queries (dim % 16 == 0, 32..2048, >= 65536 rows, coarse mode 1 or 2, VECSIM_B200_FIXED not 0) take a fixed-radius
- * pass on the integer tensor cores, whose distances are the reference's; every other query, and every query a route cannot
+ * pass on the integer tensor cores, whose distances are the reference's; fp16 / bf16 inner-product or cosine batches of >= 16
+ * queries (dim % 8 == 0, 32..1024, >= 65536 rows, coarse mode 1 or 2, VECSIM_B200_FIXED not 0, a finite largest row norm)
+ * take the direct 16-bit pass with the bound radius + eps16_q and CUDA-core rescoring, which gives the exact scan's bits; every
+ * other query (fp16 / bf16 L2, a query with an inf or NaN component, a NaN or infinite radius), and every query a route cannot
  * complete, takes the exact scan on the device.  The call only enqueues on `stream` (NULL = the legacy default stream); the
- * host waits only for the first build of the fp16 shadow / the int32 |row|^2 table of 8-bit L2 indexes or their refresh
- * after mutations.  After a synchronise, VecSimB200_LastCoarseFlags gives 1 per query a tensor-core route answered and 0 per
- * query the exact scan answered; VecSimB200_LastBatchPath is 1 (fp32 route), 2 (8-bit route) or 0 (exact scan only).  The
- * scratch is that of VecSimB200_TopKQueryBatchDevice.
+ * host waits only for the first build of the fp16 shadow / the int32 |row|^2 table of 8-bit L2 indexes / the |row|^2 table of
+ * 16-bit indexes or their refresh after mutations.  After a synchronise, VecSimB200_LastCoarseFlags gives 1 per query a
+ * tensor-core route answered and 0 per query the exact scan answered; VecSimB200_LastBatchPath is 1 (fp32 route), 2 (8-bit or
+ * 16-bit route) or 0 (exact scan only).  The scratch is that of VecSimB200_TopKQueryBatchDevice.
  * Returns 0 (0 with nothing enqueued for nq == 0); -1 for a multi-value index, cap == 0 or cap > 4096, an order other than
  * BY_ID / BY_SCORE, or a CUDA failure. */
 int VecSimB200_RangeQueryBatchDevice(VecSimIndex *index, const void *d_queries, size_t nq, const float *d_radii, size_t cap,
                                      VecSimQueryReply_Order order, int64_t *d_out_labels, float *d_out_scores,
                                      uint32_t *d_out_counts, void *stream);
 /* nq range queries, device pointers end to end, answered per LABEL as VecSimIndex_RangeQuery answers them on any FLAT index
- * (DESIGN.md §4.12).  Arguments, outputs, cap rule, orders, stream and host waits as VecSimB200_RangeQueryBatchDevice.
+ * (DESIGN.md §4.12).  Arguments, outputs, cap rule, orders, stream, host waits and routes (fp32, 8-bit and 16-bit) as
+ * VecSimB200_RangeQueryBatchDevice.
  * Multi-value index: a label is in query i's answer iff one of its rows has score <= d_radii[i] (float compare; a NaN score
  * never passes); its score is the smallest such row score; d_out_counts[i] is the true number of such LABELS.  The first call
  * after a mutation also waits for the rebuild of the label tables.  After a synchronise, VecSimB200_LastCoarseFlags gives 1 per

@@ -1822,21 +1822,74 @@ __global__ void range_bound_kernel(const float *__restrict__ radius, uint32_t nq
     overflow[q] = 0;
 }
 
+// The direct 16-bit range route (DESIGN.md §4.11): eps16_q bounds |tc - cc| for every stored row and query q, tc = the
+// epilogue's 1 - acc of the wgmma pass and cc = the CUDA-core distance (DistTile16).  With mag = sum |x_i q_i| <= M = X |q|
+// (X the running maximum row norm) and |e| <= 1 + M for the float64 distance e of the stored values:
+//   B_tc = dim 2^-22 M + u (1 + M)                       (DESIGN.md §4, an assumption about the wgmma adder)
+//   B_cc = gamma_{m+7} M + u (1 + M) + dim 2^-149        (DESIGN.md §3.1, m = the lane's fmaf chain)
+//   eps16_q = 2 (B_tc + B_cc + dim 2^-126)               (2^-126: bf16 products the tensor core may flush from the subnormals)
+// evaluated in float64 with every operation rounded up.
+constexpr double kR16U = 0x1p-24;         // u, the unit roundoff of fp32
+constexpr double kR16TcStep = 0x1p-22;    // B_tc per dimension and unit of M
+constexpr double kR16Underflow = 0x1p-149; // B_cc per dimension: fp32 underflow of a product or a partial sum
+constexpr double kR16Flush = 0x1p-126;    // per dimension: a product or partial sum flushed to zero by the tensor core
+constexpr double kR16Margin = 2.0;        // the factor over B_tc + B_cc
+constexpr double kR16MaxMag = 0x1p120;    // M at or above this: never proven (no fp32 overflow in either sum below it)
+
+// One warp per query: |q| from the stored 16-bit query (float64, rounded up), X from max_norm (the float sqrt of the largest
+// fp32 |row|^2 row_stats_kernel<DT> found, raised to cover that sum's rounding and underflow), then eps16_q and
+// thr[q] = radius[q] + eps16_q rounded up to float.  A query whose |q|, X, M or thr is not finite (or M >= kR16MaxMag) gets
+// thr[q] = -inf: the main pass keeps nothing for it and range_refine_kernel never proves it.  Clears overflow[q].
+template <int DT>
+__global__ void __launch_bounds__(256) range_bound16_kernel(const uint8_t *__restrict__ queries, size_t qpitch, uint32_t nq, uint32_t dim,
+                                                            const float *__restrict__ radius, float max_norm, float *__restrict__ thr,
+                                                            uint32_t *__restrict__ overflow) {
+    const uint32_t q = blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (q >= nq) return;
+    const uint8_t *qb = queries + (size_t)q * qpitch;
+    double s = 0.0;
+    for (uint32_t i = lane; i < dim; i += 32) {
+        const double v = (double)load16<DT>(qb, i);
+        s = __fma_ru(v, v, s);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s = __dadd_ru(s, __shfl_xor_sync(0xFFFFFFFFu, s, o));
+    if (lane != 0) return;
+    const double d = (double)dim;
+    const double qn = __dsqrt_ru(s);
+    // max |row|^2 in fp32: at most dim / 32 + 6 roundings of 2^-24 (<= dim 2^-20 relative) and dim 2^-150 of underflow;
+    // sqrtf rounds once more
+    const double x = __dadd_ru(__dmul_ru(__dmul_ru((double)max_norm, 1.0 + 0x1p-23), __dsqrt_ru(__fma_ru(d, 0x1p-20, 1.0))),
+                               __dsqrt_ru(__dmul_ru(d, 0x1p-149)));
+    const double mag = __dmul_ru(x, qn);
+    const double chain = 8.0 * ((dim / 8 + 31) / 32) + (double)((dim % 8 + 31) / 32) + 7.0; // m + 7
+    const double gamma = __ddiv_ru(chain * kR16U, __dsub_rd(1.0, chain * kR16U));
+    const double ue = __dmul_ru(kR16U, __dadd_ru(1.0, mag));                         // u |e|
+    const double b_tc = __dadd_ru(__dmul_ru(__dmul_ru(d, kR16TcStep), mag), ue);
+    const double b_cc = __dadd_ru(__dadd_ru(__dmul_ru(gamma, mag), ue), __dmul_ru(d, kR16Underflow));
+    const double eps = __dmul_ru(kR16Margin, __dadd_ru(__dadd_ru(b_tc, b_cc), __dmul_ru(d, kR16Flush)));
+    const float t = __double2float_ru(__dadd_ru((double)radius[q], eps));
+    const bool ok = isfinite(qn) && isfinite(x) && mag < kR16MaxMag && isfinite(t);
+    thr[q] = ok ? t : -__int_as_float(0x7f800000);
+    overflow[q] = 0;
+}
+
 // One CTA per query.  Packs the real candidates of the query's `slots` list entries into shared memory a window at a
-// time, rescores them from the fp32 rows (one warp per row, the scan's own arithmetic) and keeps a row iff
-// d <= radius (the reference's inclusive test, brute_force.h range query).  Kept composites are appended to the front
+// time, rescores them from the stored rows (fp32, or 16-bit on the direct route; one warp per row, the scan's own
+// arithmetic) and keeps a row iff d <= radius (the reference's inclusive test, brute_force.h range query).  Kept composites are appended to the front
 // of the query's own list segment: the count kept so far never exceeds the slots already read, so this overwrites
 // only consumed entries.  The segment is then copied to out[off[q], off[q] + cnt[q]) in the dense result buffer, at an
 // offset reserved from *total.  ok[q] = 1 unless a list overflowed, the query's fp16 form is not finite (|q|^2 NaN,
 // row_stats_kernel) or its bound is not finite; an unproven query writes cnt[q] = 0 and skips the rescoring.
-template <int MT>
+template <int DT, int MT>
 __global__ void __launch_bounds__(256) range_refine_kernel(const uint8_t *rows, size_t pitch, uint32_t dim, const uint8_t *queries,
                                                            size_t qpitch, uint32_t slots, uint64_t *cand, const float *__restrict__ radius,
                                                            const float *__restrict__ q_norm2, const float *__restrict__ thr,
                                                            const uint32_t *__restrict__ overflow, uint64_t *__restrict__ out,
                                                            uint32_t *__restrict__ total, uint32_t *__restrict__ ok, uint32_t *__restrict__ cnt,
                                                            uint32_t *__restrict__ off, uint32_t cap) {
-    using Tile = DistTile<DT_F32, MT, 1, 1>;
+    using Tile = DistTile<DT, MT, 1, 1>;
     __shared__ uint64_t s_cand[kRangeWindow];
     __shared__ uint32_t s_n, s_kept, s_base;
     const uint32_t q = blockIdx.x;
@@ -2544,14 +2597,17 @@ cudaError_t launch_quantize_queries(const void *d_q, size_t qpitch, uint32_t dim
 // A row (in practice a query: rows outside the fp16 range keep their index off the route) whose fp16 form is not finite
 // — a component with |x| >= 65520 rounds to inf, or is NaN — gets norm2 = NaN: its approximate distances are inf or NaN,
 // query_eps does not bound them, and refine_kernel never proves such a query.
+// DT_F16 / DT_BF16: the stored 16-bit rows of the direct range route (DESIGN.md §4.11), which reads only the running maximum of
+// the squared norm (a NaN or inf component makes it NaN or inf, and the route then leaves the batch to the exact scan).
+template <int DT>
 __global__ void __launch_bounds__(256) row_stats_kernel(const uint8_t *__restrict__ rows, size_t pitch, uint32_t dim, uint32_t first,
                                                         uint32_t n, float *__restrict__ norm2, uint32_t *__restrict__ stats) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (uint32_t r = blockIdx.x * 8 + warp; r < n; r += gridDim.x * 8) {
-        const float *x = reinterpret_cast<const float *>(rows + (size_t)(first + r) * pitch);
+        const uint8_t *x = rows + (size_t)(first + r) * pitch;
         float s = 0.0f, m = 0.0f;
         for (uint32_t i = lane; i < dim; i += 32) {
-            const float v = x[i];
+            const float v = DT == DT_F32 ? reinterpret_cast<const float *>(x)[i] : load16<DT>(x, i);
             s = fmaf(v, v, s);
             m = fmaxf(m, fabsf(v));
             if (v != v) m = __int_as_float(0x7f800000);
@@ -2571,10 +2627,18 @@ __global__ void __launch_bounds__(256) row_stats_kernel(const uint8_t *__restric
     }
 }
 cudaError_t launch_row_stats(const void *rows, size_t pitch, uint32_t dim, uint32_t first, uint32_t n, float *d_norm2, uint32_t *d_stats,
-                             cudaStream_t s) {
+                             cudaStream_t s, int dtype) {
     if (n == 0) return cudaSuccess;
     const uint32_t grid = std::max(1u, std::min((n + 7) / 8, (uint32_t)device_sm_count() * 8));
-    row_stats_kernel<<<grid, 256, 0, s>>>(static_cast<const uint8_t *>(rows), pitch, dim, first, n, d_norm2, d_stats);
+    const uint8_t *r = static_cast<const uint8_t *>(rows);
+    if (dtype == DT_F32)
+        row_stats_kernel<DT_F32><<<grid, 256, 0, s>>>(r, pitch, dim, first, n, d_norm2, d_stats);
+    else if (dtype == DT_F16)
+        row_stats_kernel<DT_F16><<<grid, 256, 0, s>>>(r, pitch, dim, first, n, d_norm2, d_stats);
+    else if (dtype == DT_BF16)
+        row_stats_kernel<DT_BF16><<<grid, 256, 0, s>>>(r, pitch, dim, first, n, d_norm2, d_stats);
+    else
+        return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
 
@@ -2696,17 +2760,37 @@ cudaError_t launch_range_bound(const float *d_radius, uint32_t nq, float eps, co
     range_bound_kernel<<<(nq + 255) / 256, 256, 0, s>>>(d_radius, nq, eps, d_q_norm2, max_norm, dim, l2, d_thr, d_overflow, d_total);
     return cudaGetLastError();
 }
+cudaError_t launch_range_bound16(const void *d_queries, size_t qpitch, uint32_t nq, uint32_t dim, int dtype, const float *d_radius,
+                                 float max_norm, float *d_thr, uint32_t *d_overflow, cudaStream_t s) {
+    if (nq == 0) return cudaSuccess;
+    const uint8_t *qs = static_cast<const uint8_t *>(d_queries);
+    if (dtype == DT_F16)
+        range_bound16_kernel<DT_F16><<<(nq + 7) / 8, 256, 0, s>>>(qs, qpitch, nq, dim, d_radius, max_norm, d_thr, d_overflow);
+    else if (dtype == DT_BF16)
+        range_bound16_kernel<DT_BF16><<<(nq + 7) / 8, 256, 0, s>>>(qs, qpitch, nq, dim, d_radius, max_norm, d_thr, d_overflow);
+    else
+        return cudaErrorInvalidValue;
+    return cudaGetLastError();
+}
 cudaError_t launch_range_refine(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t slots, uint64_t *d_cand,
                                 const float *d_radius, const float *d_q_norm2, const float *d_thr, const uint32_t *d_overflow, uint64_t *d_out,
                                 uint32_t *d_total, uint32_t *d_ok, uint32_t *d_cnt, uint32_t *d_off, cudaStream_t s, uint32_t cap) {
     if (nq == 0) return cudaSuccess;
     const uint8_t *rows = static_cast<const uint8_t *>(c.rows), *qs = static_cast<const uint8_t *>(d_queries);
-    if (c.metric == MT_L2)
-        range_refine_kernel<MT_L2><<<nq, 256, 0, s>>>(rows, c.pitch, c.dim, qs, qpitch, slots, d_cand, d_radius, d_q_norm2, d_thr, d_overflow,
-                                                      d_out, d_total, d_ok, d_cnt, d_off, cap);
+    if (c.dtype == DT_F32 && c.metric == MT_L2)
+        range_refine_kernel<DT_F32, MT_L2><<<nq, 256, 0, s>>>(rows, c.pitch, c.dim, qs, qpitch, slots, d_cand, d_radius, d_q_norm2, d_thr,
+                                                              d_overflow, d_out, d_total, d_ok, d_cnt, d_off, cap);
+    else if (c.dtype == DT_F32 && c.metric == MT_IP)
+        range_refine_kernel<DT_F32, MT_IP><<<nq, 256, 0, s>>>(rows, c.pitch, c.dim, qs, qpitch, slots, d_cand, d_radius, d_q_norm2, d_thr,
+                                                              d_overflow, d_out, d_total, d_ok, d_cnt, d_off, cap);
+    else if (c.dtype == DT_F16 && c.metric == MT_IP) // the direct 16-bit route: inner product / cosine (normalised rows)
+        range_refine_kernel<DT_F16, MT_IP><<<nq, 256, 0, s>>>(rows, c.pitch, c.dim, qs, qpitch, slots, d_cand, d_radius, d_q_norm2, d_thr,
+                                                              d_overflow, d_out, d_total, d_ok, d_cnt, d_off, cap);
+    else if (c.dtype == DT_BF16 && c.metric == MT_IP)
+        range_refine_kernel<DT_BF16, MT_IP><<<nq, 256, 0, s>>>(rows, c.pitch, c.dim, qs, qpitch, slots, d_cand, d_radius, d_q_norm2, d_thr,
+                                                               d_overflow, d_out, d_total, d_ok, d_cnt, d_off, cap);
     else
-        range_refine_kernel<MT_IP><<<nq, 256, 0, s>>>(rows, c.pitch, c.dim, qs, qpitch, slots, d_cand, d_radius, d_q_norm2, d_thr, d_overflow,
-                                                      d_out, d_total, d_ok, d_cnt, d_off, cap);
+        return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
 cudaError_t launch_range_pack(const uint64_t *d_cand, uint32_t nq, uint32_t slots, const uint32_t *d_overflow, uint32_t cap, uint64_t *d_out,

@@ -120,10 +120,15 @@ cudaError_t launch_gather_queries(const void *d_src, size_t pitch, const float *
 // *d_total
 cudaError_t launch_range_bound(const float *d_radius, uint32_t nq, float eps, const float *d_q_norm2, float max_norm, uint32_t dim, int l2,
                                float *d_thr, uint32_t *d_overflow, uint32_t *d_total, cudaStream_t s);
+// device range batches on fp16 / bf16 (dtype) inner product or cosine (the direct route, DESIGN.md §4.11): d_thr[q] = d_radius[q] +
+// eps16_q rounded up, eps16_q from |q| of the stored query and max_norm = X, the running maximum row norm; -inf where |q|, X or the
+// bound is not finite (the query is then never proven).  Clears d_overflow[q]
+cudaError_t launch_range_bound16(const void *d_queries, size_t qpitch, uint32_t nq, uint32_t dim, int dtype, const float *d_radius,
+                                 float max_norm, float *d_thr, uint32_t *d_overflow, cudaStream_t s);
 // range batches, one CTA per query over its `slots` list entries of the main pass (d_cand, overwritten): exact rescoring and
 // the inclusive test d <= d_radius[q].  Query q's hits go to d_out[d_off[q], d_off[q] + d_cnt[q]) (composites, unordered;
 // d_out holds nq * slots); d_ok[q] = 1 if the answer is proven complete, else 0 with d_cnt[q] = 0.  d_q_norm2 == NULL: unit
-// rows.  cap != 0 (device range batches): query q's hits go to d_out[q * cap, q * cap + min(d_cnt[q], cap)) instead, d_cnt[q] the
+// rows.  fp32 rows (L2 / inner product), or fp16 / bf16 rows (inner product) rescored with DistTile16.  cap != 0 (device range batches): query q's hits go to d_out[q * cap, q * cap + min(d_cnt[q], cap)) instead, d_cnt[q] the
 // true count; d_total and d_off are not used.
 cudaError_t launch_range_refine(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t slots, uint64_t *d_cand,
                                 const float *d_radius, const float *d_q_norm2, const float *d_thr, const uint32_t *d_overflow, uint64_t *d_out,
@@ -144,9 +149,10 @@ cudaError_t launch_range_label_fold(const uint64_t *d_cand, uint32_t nq, uint32_
                                     const uint64_t *d_id_to_label, uint32_t cap, uint64_t *d_out, uint32_t *d_cnt, uint32_t *d_ok,
                                     uint32_t *d_flags, cudaStream_t s);
 // |row|^2 of fp32 rows [first, first+n) into d_norm2[first..], NaN for a row whose fp16 form is not finite (a component
-// with |x| >= 65520, or NaN: refine_kernel never proves such a query); d_stats (nullable) = {max |row|^2, max |x|} as float bits
+// with |x| >= 65520, or NaN: refine_kernel never proves such a query); d_stats (nullable) = {max |row|^2, max |x|} as float bits.
+// dtype DT_F16 / DT_BF16: the same over stored 16-bit rows
 cudaError_t launch_row_stats(const void *rows, size_t pitch, uint32_t dim, uint32_t first, uint32_t n, float *d_norm2, uint32_t *d_stats,
-                             cudaStream_t s);
+                             cudaStream_t s, int dtype = DT_F32);
 // exact int32 |x|^2 of int8 (is_signed) / uint8 rows [first, first+n) into d_norm2[first..] (dim <= 2048: no overflow); serves
 // the corpus rows and the query batch of the 8-bit L2 route
 cudaError_t launch_int_norm2(const void *rows, size_t pitch, uint32_t dim, uint32_t first, uint32_t n, bool is_signed, int32_t *d_norm2,

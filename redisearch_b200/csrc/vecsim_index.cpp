@@ -741,11 +741,13 @@ bool FlatIndex::q8_route(uint32_t nq, uint32_t ke) const {
 // Bring the fp16 shadow copy of the rows up to date on `st` (rows appended, overwritten or moved by a
 // swap-delete since the last coarse batch).  Returns false if HBM for the shadow cannot be had; the
 // caller then runs the TF32 variant on the fp32 rows.
-// int8 / uint8 L2 indexes keep no shadow, only the exact int32 |row|^2 of every row, under the same bookkeeping.
+// int8 / uint8 L2 indexes keep no shadow, only the exact int32 |row|^2 of every row, under the same bookkeeping.  fp16 / bf16
+// indexes keep no shadow either, only |row|^2 of the stored rows and its running maximum (the direct range route's X).
 bool FlatIndex::ensure_shadow(cudaStream_t st, bool q8) {
     std::lock_guard<std::mutex> g(mu_);
-    const bool inorm = int_l2();
-    if (inorm && (shadow_cap_ < count_ || !d_norm2_)) {
+    const bool inorm = int_l2(), rows16 = dtype_ == DT_F16 || dtype_ == DT_BF16;
+    const bool norms_only = inorm || rows16;
+    if (norms_only && (shadow_cap_ < count_ || !d_norm2_)) {
         const size_t cap = std::max(capacity_, count_);
         cudaFree(d_norm2_);
         d_norm2_ = nullptr;
@@ -758,8 +760,12 @@ bool FlatIndex::ensure_shadow(cudaStream_t st, bool q8) {
         }
         shadow_cap_ = cap;
     }
+    if (rows16 && !d_stats_ && (cudaMalloc(&d_stats_, 8) != cudaSuccess || cudaMemset(d_stats_, 0, 8) != cudaSuccess)) {
+        cudaGetLastError();
+        return false;
+    }
     bool launched = false;
-    if (!inorm && shadow_cap_ >= count_ && (q8 ? !d_shadow8_ : !d_shadow_) && (d_shadow_ || d_shadow8_)) {
+    if (!norms_only && shadow_cap_ >= count_ && (q8 ? !d_shadow8_ : !d_shadow_) && (d_shadow_ || d_shadow8_)) {
         // the other copy is kept: allocate only the missing one and build it over the rows the other covers; the refresh below
         // brings both over dirty and appended rows
         const size_t cap = shadow_cap_;
@@ -792,7 +798,7 @@ bool FlatIndex::ensure_shadow(cudaStream_t st, bool q8) {
         }
         launched = true;
     }
-    if (!inorm && (shadow_cap_ < count_ || (q8 ? !d_shadow8_ : !d_shadow_))) {
+    if (!norms_only && (shadow_cap_ < count_ || (q8 ? !d_shadow8_ : !d_shadow_))) {
         // the requested copy and every copy already kept, at the capacity; rows are re-converted below
         const size_t cap = std::max(capacity_, count_);
         const bool k16 = !q8 || d_shadow_, k8 = q8 || d_shadow8_;
@@ -820,8 +826,8 @@ bool FlatIndex::ensure_shadow(cudaStream_t st, bool q8) {
         shadow_rows_ = 0;
         shadow_dirty_.clear();
     }
-    if (!inorm && !unit_rows() && !d_norm2_) { // L2 / raw inner product / cosine after a raw overwrite: the error bound (and the L2
-                                               // epilogue) need |row|^2 of every row
+    if (!norms_only && !unit_rows() && !d_norm2_) { // L2 / raw inner product / cosine after a raw overwrite: the error bound (and
+                                                    // the L2 epilogue) need |row|^2 of every row
         if (!d_stats_ && (cudaMalloc(&d_stats_, 8) != cudaSuccess || cudaMemset(d_stats_, 0, 8) != cudaSuccess)) {
             cudaGetLastError();
             return false;
@@ -843,7 +849,7 @@ bool FlatIndex::ensure_shadow(cudaStream_t st, bool q8) {
         if (d_shadow8_ && launch_to_i8_tiled(d_rows_, pitch_, (uint32_t)dim_, (uint32_t)count_, first, n, d_shadow8_, d_tscale_, d_stats8_, st) !=
                               cudaSuccess)
             return false;
-        return !d_norm2_ || launch_row_stats(d_rows_, pitch_, (uint32_t)dim_, first, n, d_norm2_, d_stats_, st) == cudaSuccess;
+        return !d_norm2_ || launch_row_stats(d_rows_, pitch_, (uint32_t)dim_, first, n, d_norm2_, d_stats_, st, dtype_) == cudaSuccess;
     };
     if (shadow_dirty_.size() > 256) {
         shadow_rows_ = 0;
@@ -1627,11 +1633,15 @@ int FlatIndex::range_device(const void *d_q, size_t nq, const float *d_radii, si
     const size_t qpitch = query_pitch();
     const CorpusView v = view();
     const int cmode = coarse_mode();
-    const bool is8 = dtype_ == DT_I8 || dtype_ == DT_U8;
-    // 1: the fp32 route of range_batch (same eligibility); 2: the fixed-radius pass over 8-bit rows; 0: the exact scan only
+    const bool is8 = dtype_ == DT_I8 || dtype_ == DT_U8, is16 = dtype_ == DT_F16 || dtype_ == DT_BF16;
+    // 1: the fp32 route of range_batch (same eligibility); 2: the fixed-radius pass over 8-bit rows, or the fixed-bound pass over
+    // 16-bit rows with the margin eps16_q and CUDA-core rescoring (r16, finite X only); 0: the exact scan only
     int path = 0;
     if (n > 0 && is8 && cmode != 0 && nq >= 16 && coarse_fixed_enabled() && coarse_supported(v, nq32, 1, CoarseDirect8) &&
         (!int_l2() || ensure_shadow(st))) {
+        path = 2;
+    } else if (n > 0 && is16 && cmode != 0 && nq >= 16 && coarse_fixed_enabled() && coarse_supported(v, nq32, 1, CoarseDirect16) &&
+               ensure_shadow(st) && std::isfinite(shadow_max_norm_)) {
         path = 2;
     } else if (n > 0 && cmode == 1 && dtype_ == DT_F32 && !coarse_disabled_ && coarse_fixed_enabled() && coarse_supported(v, nq32, 1, CoarseF16) &&
                (nq >= 16 || single_query_takes_coarse(1)) && ensure_shadow(st)) {
@@ -1641,9 +1651,10 @@ int FlatIndex::range_device(const void *d_q, size_t nq, const float *d_radii, si
             path = 0;
         }
     }
-    const bool unit = unit_rows();
-    const CoarsePlan cp = path == 1 ? plan_coarse(v, nq32, CoarseF16, 1, 0, 1, 1) : path == 2 ? plan_coarse(v, nq32, CoarseDirect8, 1, 0, 1, 1)
-                                                                                             : CoarsePlan{};
+    const bool unit = unit_rows(), r16 = path == 2 && is16, refine = path == 1 || r16; // refine: rescored by range_refine_kernel
+    const CoarsePlan cp = path == 1 ? plan_coarse(v, nq32, CoarseF16, 1, 0, 1, 1)
+                          : path == 2 ? plan_coarse(v, nq32, is16 ? CoarseDirect16 : CoarseDirect8, 1, 0, 1, 1)
+                                      : CoarsePlan{};
     const size_t slots = (size_t)cp.grid_x * cp.keep, q16_pitch = (dim_ * 2 + 15) & ~(size_t)15;
     const WidePlan wp = n > 0 ? plan_topk_wide(v.n_rows, nq32) : WidePlan{};
     uint64_t *cand, *list_scratch;
@@ -1657,14 +1668,14 @@ int FlatIndex::range_device(const void *d_q, size_t nq, const float *d_radii, si
         list_scratch = sc.take<uint64_t>(path ? cp.scratch_elems : 0);
         q16 = sc.take<uint8_t>(path == 1 ? nq * q16_pitch : 0);
         d_qn2 = sc.take<float>((path == 1 && !unit) || (path == 2 && int_l2()) ? nq : 0); // |q|^2 (fp32), or int32 for 8-bit L2
-        d_thr = sc.take<float>(path == 1 ? nq : 0);
+        d_thr = sc.take<float>(refine ? nq : 0);
         d_ovf = sc.take<uint32_t>(path ? nq : 0);
         d_total = sc.take<uint32_t>(1);
         d_ok = sc.take<uint32_t>(nq);  // reported flags
         d_idx = sc.take<uint32_t>(nq); // the open queries
         d_n2 = sc.take<uint32_t>(1);   // and their count
         d_flags = sc.take<uint32_t>(fold ? nq : 0);          // multi-value: the reported flags (d_ok: 1 = folded, 0 = open)
-        d_front = sc.take<uint32_t>(fold && path == 1 ? nq : 0); // multi-value fp32 route: the hit rows at the front of each list segment
+        d_front = sc.take<uint32_t>(fold && refine ? nq : 0); // multi-value fp32 / 16-bit route: the hit rows at the front of each list segment
         return sc.words();
     };
     if (!c->need_cand(layout(nullptr)) || (n > 0 && !c->need_scores(wp.score_elems))) return -1;
@@ -1673,12 +1684,17 @@ int FlatIndex::range_device(const void *d_q, size_t nq, const float *d_radii, si
     uint64_t *comp = reinterpret_cast<uint64_t *>(d_labels);
     bool ok = cudaMemsetAsync(d_counts, 0, nq * 4, st) == cudaSuccess && cudaMemsetAsync(d_ok, 0, nq * 4, st) == cudaSuccess;
     // the timed span (VecSimB200_GetStats): the route's main pass, or the exact scan of a batch no route serves
-    if (path == 1) {
-        ok = ok && launch_to_f16(d_q, qpitch, (uint32_t)dim_, 0, nq32, q16, q16_pitch, st) == cudaSuccess;
-        if (!unit) ok = ok && launch_row_stats(d_q, qpitch, (uint32_t)dim_, 0, nq32, d_qn2, nullptr, st) == cudaSuccess;
-        ok = ok && launch_range_bound(d_radii, nq32, kCoarseEpsF16, d_qn2, shadow_max_norm_, (uint32_t)dim_, mkind_ == MT_L2 ? 1 : 0, d_thr, d_ovf,
-                                      d_total, st) == cudaSuccess;
-        const CoarseOperands ops{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
+    if (refine) {
+        CoarseOperands ops{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
+        if (r16) {
+            ok = ok && launch_range_bound16(d_q, qpitch, nq32, (uint32_t)dim_, dtype_, d_radii, shadow_max_norm_, d_thr, d_ovf, st) == cudaSuccess;
+            ops = CoarseOperands{v.rows, v.pitch, d_q, qpitch, dtype_ == DT_BF16 ? 1 : 0, 0, nullptr, nullptr};
+        } else {
+            ok = ok && launch_to_f16(d_q, qpitch, (uint32_t)dim_, 0, nq32, q16, q16_pitch, st) == cudaSuccess;
+            if (!unit) ok = ok && launch_row_stats(d_q, qpitch, (uint32_t)dim_, 0, nq32, d_qn2, nullptr, st) == cudaSuccess;
+            ok = ok && launch_range_bound(d_radii, nq32, kCoarseEpsF16, d_qn2, shadow_max_norm_, (uint32_t)dim_, mkind_ == MT_L2 ? 1 : 0, d_thr,
+                                          d_ovf, d_total, st) == cudaSuccess;
+        }
         cudaEventRecord(c->ev_start, st);
         ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_thr, d_ovf) == cudaSuccess;
         cudaEventRecord(c->ev_stop, st);
@@ -1692,7 +1708,7 @@ int FlatIndex::range_device(const void *d_q, size_t nq, const float *d_radii, si
             ok = ok && launch_range_refine(v, d_q, qpitch, nq32, (uint32_t)slots, cand, d_radii, d_qn2, d_thr, d_ovf, comp, d_total, d_ok,
                                            d_counts, nullptr, st, cap32) == cudaSuccess;
         }
-        lc.launches += unit ? 4 : 5;
+        lc.launches += r16 ? 3 : unit ? 4 : 5;
     } else if (path == 2) {
         CoarseOperands ops{v.rows, v.pitch, d_q, qpitch, dtype_ == DT_I8 ? 1 : 0, mkind_ == MT_COS ? 1 : int_l2() ? 2 : 0, nullptr, nullptr};
         ok = ok && cudaMemsetAsync(d_ovf, 0, nq * 4, st) == cudaSuccess;

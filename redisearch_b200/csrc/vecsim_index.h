@@ -259,8 +259,9 @@ class FlatIndex {
     uint32_t *d_stats8_ = nullptr;
     float shadow8_delta_ = 0.0f, shadow8_xmax_ = 0.0f;
     // L2 / raw inner-product indexes: |row|^2 per row and the running maxima the error bound needs.  int8 / uint8 L2 indexes keep
-    // the exact int32 |row|^2 here (stored as int32, no shadow, no maxima) for the integer tensor-core route; the same
-    // shadow_rows_ / shadow_dirty_ / shadow_cap_ bookkeeping tracks it
+    // the exact int32 |row|^2 here (stored as int32, no shadow, no maxima) for the integer tensor-core route; fp16 / bf16 indexes
+    // keep |row|^2 of their stored rows and its running maximum (no shadow) once a range batch takes the direct 16-bit route.
+    // The same shadow_rows_ / shadow_dirty_ / shadow_cap_ bookkeeping tracks it
     float *d_norm2_ = nullptr;
     uint32_t *d_stats_ = nullptr;
     float shadow_max_norm_ = 0.0f, shadow_max_abs_ = std::numeric_limits<float>::infinity();
@@ -273,7 +274,7 @@ class FlatIndex {
     // a per-row copy (the fp16 shadow and / or |row|^2) exists: in-place overwrites and swap-deletes go to shadow_dirty_
     bool keeps_row_copies() const { return d_shadow_ || d_shadow8_ || d_norm2_; }
     bool int_l2() const { return (dtype_ == DT_I8 || dtype_ == DT_U8) && mkind_ == MT_L2; }
-    // fp32: the fp16 shadow (+ |row|^2 unless unit rows); int8 / uint8 L2: only the int32 |row|^2 table
+    // fp32: the fp16 shadow (+ |row|^2 unless unit rows); int8 / uint8 L2: only the int32 |row|^2 table; fp16 / bf16: only |row|^2
     // q8: the int8 copy instead (unit rows); every copy the index already keeps is brought up to date either way
     bool ensure_shadow(cudaStream_t st, bool q8 = false);
     // a KNN batch of this k on this single-value index of unit rows runs on the int8 copy (its bounds are finite once built)
