@@ -258,7 +258,11 @@ def _metric_code(vs, metric):
 def test_worst_case_rounding_at_the_kth_boundary(case, dim, k):
     """Per query: row A is in the true top-k but its operand form rounds it behind k + 1 rows B it beats in exact
     arithmetic (by at least eps / 2 in the emulated GEMM; TF32: eps / 4).  The refine cut a_k + 2 eps must still reach A,
-    and the proof must hold; with a smaller eps A is dropped and the proof passes on a wrong answer."""
+    and the proof must hold; with a smaller eps A is dropped and the proof passes on a wrong answer.  The batch must read
+    the copy the emulation models (fp16: 16 bits; TF32 reads the fp32 rows: 0).  Unit cosine rows wider than 128 dimensions
+    take the int8 copy on a single-value index (test_coarse_int8_shadow.py holds that route to its own worst case), so
+    cos_f16 at 768 runs on a multi-value index with one row per label: it keeps the fp16 copy and answers what the
+    single-value index answers."""
     from redisearch_b200 import vecsim as vs
 
     metric = {"cos_f16": ol.COS, "cos_tf32": ol.COS, "ip": ol.IP, "l2": ol.L2}[case]
@@ -279,14 +283,16 @@ def test_worst_case_rounding_at_the_kth_boundary(case, dim, k):
         a, b = adversarial_unit_rows(qn[i], nb, kind)
         rows[pos[i, 0]] = (a.astype(np.float64) * scale).astype(np.float32)
         rows[pos[i, 1:]] = (b.astype(np.float64) * scale).astype(np.float32)
-    g = vs.VecSimIndex(vs.VecSimType_FLOAT32, dim, _metric_code(vs, metric))
+    multi = case == "cos_f16" and dim > 128
+    g = vs.VecSimIndex(vs.VecSimType_FLOAT32, dim, _metric_code(vs, metric), multi=multi)
     p = _checker(metric, dim)
     assert g.add_many(rows, label0=1) == n
     p.add_many(rows, 1)
     qs_raw = raw_q if metric == ol.COS else qdev
     labels, scores, flags = _device_batch(vs, g, qdev, k)
     assert flags is not None and vs.lib().VecSimB200_LastBatchPath(g.h) == 1
-    assert (flags != 0).sum() >= nq * 0.9, np.bincount(flags, minlength=3).tolist()
+    assert vs.lib().VecSimB200_LastCoarseShadowBits(g.h) == (0 if kind == "tf32" else 16)
+    assert (flags != 0).sum() >= nq * 0.9, np.bincount(flags, minlength=4).tolist()
     _assert_exact(labels, scores, p, qs_raw, k, flags, case)
     # the construction has power on the rows the index actually stores (cosine: after its normalisation)
     if metric == ol.COS:
