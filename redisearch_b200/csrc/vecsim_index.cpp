@@ -905,6 +905,88 @@ void FlatIndex::disable_coarse() {
     shadow_dirty_.clear();
 }
 
+bool FlatIndex::shadow_values_in_range() {
+    if (unit_rows() || shadow_max_abs_ <= 60000.0f) return true;
+    disable_coarse(); // the shadow's HBM is given back
+    return false;
+}
+
+bool FlatIndex::shadow_operands(const void *d_q, size_t qpitch, uint32_t nq, uint8_t *q16, float *d_qn2, cudaStream_t st, LaunchCounters &lc,
+                                CoarseOperands &ops) {
+    const size_t q16_pitch = f16_query_pitch();
+    ops = CoarseOperands{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
+    bool ok = launch_to_f16(d_q, qpitch, (uint32_t)dim_, 0, nq, q16, q16_pitch, st) == cudaSuccess;
+    if (d_qn2) ok = ok && launch_row_stats(d_q, qpitch, (uint32_t)dim_, 0, nq, d_qn2, nullptr, st) == cudaSuccess;
+    lc.launches += d_qn2 ? 2 : 1;
+    return ok;
+}
+
+// int8 / uint8: s8 / u8 wgmma dot products are exact integers and the epilogue applies the reference's own float expression, so
+// the 8-bit routes are bit-exact.  L2: |row|^2 + |q|^2 - 2 dot in int32, rounded once to float, is the reference's float(sum of
+// squared differences) bit for bit
+bool FlatIndex::direct8_operands(const void *d_q, size_t qpitch, uint32_t nq, int32_t *d_qn, cudaStream_t st, LaunchCounters &lc,
+                                 CoarseOperands &ops) {
+    ops = CoarseOperands{d_rows_, pitch_, d_q, qpitch, dtype_ == DT_I8 ? 1 : 0, mkind_ == MT_COS ? 1 : int_l2() ? 2 : 0, nullptr, nullptr};
+    if (!int_l2()) return true;
+    ops.row_norm2 = reinterpret_cast<const float *>(d_norm2_); // int32 values (CoarseOperands)
+    ops.q_norm2 = reinterpret_cast<const float *>(d_qn);
+    lc.launches++;
+    return launch_int_norm2(d_q, qpitch, (uint32_t)dim_, 0, nq, dtype_ == DT_I8, d_qn, st) == cudaSuccess;
+}
+
+void FlatIndex::RangeScratch::take(BatchScratch &s, const FlatIndex &ix, CoarseKind kind, const CoarsePlan &cp, uint32_t nq, bool fold) {
+    const bool shadow = kind == CoarseF16, refine = kind != CoarseDirect8; // refine: rescored by range_refine_kernel
+    cand = s.take<uint64_t>((size_t)nq * cp.grid_x * cp.keep);
+    list_scratch = s.take<uint64_t>(cp.scratch_elems);
+    q16 = s.take<uint8_t>(shadow ? nq * ix.f16_query_pitch() : 0);
+    qn2 = s.take<float>((shadow && !ix.unit_rows()) || (kind == CoarseDirect8 && ix.int_l2()) ? nq : 0); // |q|^2 (fp32), or int32 for 8-bit L2
+    thr = s.take<float>(refine ? nq : 0);                 // bound of the main pass per query
+    ovf = s.take<uint32_t>(nq);                           // a list of the main pass ran full
+    front = s.take<uint32_t>(fold && refine ? nq : 0);    // multi-value: the hit rows at the front of each list segment
+}
+
+// CoarseF16: T_q = radius_q + eps_q over the fp16 shadow, then exact rescoring (DESIGN.md §4).  CoarseDirect16: the margin eps16_q
+// over the stored rows and CUDA-core rescoring (§4.11).  CoarseDirect8: the radii themselves over exact integer distances, packed.
+// Launches: 4 (+1 for |q|^2 of rows not all unit), 3, 2 (+1 for L2); one more for a fold after rescoring
+bool FlatIndex::enqueue_range_route(QueryCtx &c, const CorpusView &v, CoarseKind kind, const CoarsePlan &cp, const RangeScratch &r,
+                                    const void *d_q, size_t qpitch, uint32_t nq, const float *d_radii, const uint32_t *bm, uint32_t words,
+                                    const RangeOut &out, cudaStream_t st, LaunchCounters &lc) {
+    const uint32_t slots = cp.grid_x * cp.keep;
+    CoarseOperands ops{};
+    bool ok;
+    if (kind == CoarseDirect8) {
+        ok = cudaMemsetAsync(r.ovf, 0, nq * 4, st) == cudaSuccess;
+        ok = ok && direct8_operands(d_q, qpitch, nq, reinterpret_cast<int32_t *>(r.qn2), st, lc, ops);
+    } else if (kind == CoarseDirect16) {
+        ok = launch_range_bound16(d_q, qpitch, nq, (uint32_t)dim_, dtype_, d_radii, shadow_max_norm_, r.thr, r.ovf, st) == cudaSuccess;
+        ops = CoarseOperands{v.rows, v.pitch, d_q, qpitch, dtype_ == DT_BF16 ? 1 : 0, 0, nullptr, nullptr};
+        lc.launches++;
+    } else {
+        ok = shadow_operands(d_q, qpitch, nq, r.q16, r.qn2, st, lc, ops);
+        ok = ok && launch_range_bound(d_radii, nq, kCoarseEpsF16, r.qn2, shadow_max_norm_, (uint32_t)dim_, mkind_ == MT_L2 ? 1 : 0, r.thr, r.ovf,
+                                      out.total, st) == cudaSuccess;
+        lc.launches++;
+    }
+    cudaEventRecord(c.ev_start, st);
+    ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq, cp, r.cand, r.list_scratch, st, nullptr, kind == CoarseDirect8 ? d_radii : r.thr, r.ovf, bm,
+                             words) == cudaSuccess;
+    cudaEventRecord(c.ev_stop, st);
+    lc.launches += 2;
+    if (kind == CoarseDirect8)
+        return ok && (out.flags ? launch_range_label_fold(r.cand, nq, slots, nullptr, r.ovf, d_id_to_label_, out.cap, out.hits, out.cnt, out.ok,
+                                                          out.flags, st)
+                                : launch_range_pack(r.cand, nq, slots, r.ovf, out.cap, out.hits, out.cnt, out.ok, st)) == cudaSuccess;
+    if (!out.flags)
+        return ok && launch_range_refine(v, d_q, qpitch, nq, slots, r.cand, d_radii, r.qn2, r.thr, r.ovf, out.hits, out.total, out.ok, out.cnt,
+                                         out.off, st, out.cap) == cudaSuccess;
+    // the kept rows stay at the front of each list segment (cap = slots onto cand itself: a copy onto itself)
+    ok = ok && launch_range_refine(v, d_q, qpitch, nq, slots, r.cand, d_radii, r.qn2, r.thr, r.ovf, r.cand, out.total, out.ok, r.front, nullptr, st,
+                                   slots) == cudaSuccess;
+    lc.launches++;
+    return ok && launch_range_label_fold(r.cand, nq, slots, r.front, nullptr, d_id_to_label_, out.cap, out.hits, out.cnt, out.ok, out.flags, st) ==
+                     cudaSuccess;
+}
+
 // Enqueue on `st`: the `ke` best composites of each of `nq` device-resident stored-form queries into
 // d_out [nq][ke].  Cosine fp32 batches take the tensor-core coarse pass + exact rescoring + proof, with
 // the exact scan as an on-device fallback for unverified queries; everything else takes the exact
@@ -923,6 +1005,93 @@ static uint32_t sample_stride(const CoarsePlan &probe, uint32_t ke, double aim, 
     return (uint32_t)std::max(1.0, std::min(std::floor(1.0 / f), std::floor(probe.tiles / (tiles_per_k * ke))));
 }
 
+// The shadow copies run the first tier in two passes:
+//   sample pass   every `stride`-th row tile, per (query, row range) the smallest approximate distance of 8 interleaved
+//                 slices -> per query the bound T = (k-th smallest of its ranges x 8 minima) + 2 eps: k distinct rows
+//                 lie at or below it, so it bounds the k-th best distance from above
+//   main pass     all row tiles, every row with approximate distance < T is kept (fixed bound: no running thresholds,
+//                 no list compaction, which a running threshold keeps the epilogue busy with)
+// TF32 route: one pass with adaptive lists.  aim: the slots per (query, row range) of the main pass that should fall below the
+// bound; filt: the main pass runs with row filters.
+FlatIndex::KnnTiers FlatIndex::plan_knn_tiers(const CorpusView &v, uint32_t nq, CoarseKind kind, uint32_t ke, double aim, double tiles_per_k,
+                                              bool filt) {
+    KnnTiers t;
+    const bool shadow = kind == CoarseF16 || kind == CoarseQ8;
+    t.two_pass = shadow && coarse_fixed_enabled();
+    t.tier2 = shadow && coarse_tier2_enabled();
+    if (!t.two_pass) {
+        t.main = plan_coarse(v, nq, kind, ke); // the adaptive lists ARE the first tier
+    } else {
+        t.main = plan_coarse(v, nq, kind, ke, 0, 1, 1, filt);
+        // k in the hundreds: ranges x 32 slice minima barely hold k values.  The sample pass keeps adaptive lists of 128 per (query,
+        // row range) instead; their union holds at least k distinct rows at or below its k-th smallest approximate distance, so
+        // threshold_kernel's bound stands
+        t.sample = ke > kCoarseMaxK ? plan_coarse(v, nq, kind, ke, kCoarseKeepWide, sample_stride(t.main, ke, aim, tiles_per_k), 0)
+                                    : plan_coarse(v, nq, kind, ke, 0, sample_stride(t.main, ke, aim, tiles_per_k), 2);
+    }
+    // second tier: the queries whose first-tier proof failed (a list of the main pass overflowed: more than its capacity of rows of
+    // one range within the bound — clustered corpora) are packed to the front and run once more with adaptive lists of 128 per row
+    // range.  Nothing is known on the host: the tier's kernels read the count of open queries from device memory and leave at once
+    // when it is zero.
+    if (t.tier2) t.second = plan_coarse(v, nq, kind, ke, kCoarseKeepWide);
+    return t;
+}
+
+void FlatIndex::KnnScratch::take(BatchScratch &s, const KnnTiers &t, uint32_t nq, size_t q_pitch, bool norms, bool q8) {
+    cand = s.take<uint64_t>((size_t)nq * t.main.grid_x * t.main.keep);
+    cand_s = s.take<uint64_t>(t.two_pass ? (size_t)nq * t.sample.grid_x * t.sample.keep : 0);
+    cand_t2 = s.take<uint64_t>(t.tier2 ? (size_t)nq * t.second.grid_x * t.second.keep : 0);
+    list_scratch = s.take<uint64_t>(std::max(std::max(t.main.scratch_elems, t.two_pass ? t.sample.scratch_elems : 0),
+                                             t.tier2 ? t.second.scratch_elems : 0));
+    q = s.take<uint8_t>(nq * q_pitch);
+    q_t2 = s.take<uint8_t>(t.tier2 ? nq * q_pitch : 0);
+    qn2 = s.take<float>(norms ? nq : 0); // |q|^2 per query
+    qn2_t2 = s.take<float>(norms && t.tier2 ? nq : 0);
+    qeps = s.take<float>(q8 ? nq : 0); // int8 copy: the error bound of each query
+    qeps_t2 = s.take<float>(q8 && t.tier2 ? nq : 0);
+    ok = s.take<uint32_t>(nq);
+    idx = s.take<uint32_t>(nq);         // tier 2: indices of the open queries
+    n2 = s.take<uint32_t>(nq ? 1 : 0);  //         and their count
+    thr = s.take<float>(nq);            // fixed bound per query
+    ovf = s.take<uint32_t>(nq);         // a list of the main pass ran full
+}
+
+bool FlatIndex::enqueue_knn_tiers(QueryCtx &c, const CorpusView &v, CoarseKind kind, const KnnTiers &t, const KnnScratch &s,
+                                  const CoarseOperands &ops, const void *d_q32, size_t qpitch, uint32_t nq, uint32_t ke, uint64_t *out,
+                                  const uint32_t *bm, uint32_t words, const uint64_t *row_label, cudaStream_t st, LaunchCounters &lc) {
+    const float eps = coarse_eps(kind);
+    bool ok = true;
+    if (t.two_pass) {
+        ok = launch_coarse(ops, v.n_rows, v.dim, nq, t.sample, s.cand_s, s.list_scratch, st, nullptr, nullptr, nullptr, bm, words) == cudaSuccess;
+        ok = ok && launch_threshold(s.cand_s, nq, t.sample.grid_x, t.sample.keep, ke, eps, s.qn2, shadow_max_norm_, (uint32_t)dim_,
+                                    mkind_ == MT_L2 ? 1 : 0, s.thr, s.ovf, st, s.qeps) == cudaSuccess;
+        lc.launches += 2;
+    }
+    const float *thr = t.two_pass ? s.thr : nullptr;
+    uint32_t *ovf = t.two_pass ? s.ovf : nullptr;
+    cudaEventRecord(c.ev_start, st);
+    ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq, t.main, s.cand, s.list_scratch, st, nullptr, thr, ovf, bm, words) == cudaSuccess;
+    cudaEventRecord(c.ev_stop, st);
+    // exact rescoring of the few candidates that can still matter + exact top-k + proof, one CTA per query
+    ok = ok && launch_refine(v, d_q32, qpitch, nq, t.main.grid_x, t.main.keep, ke, s.cand, eps, s.qn2, shadow_max_norm_, s.ok, out, nullptr,
+                             nullptr, st, thr, ovf, row_label, s.qeps) == cudaSuccess;
+    lc.launches += 2;
+    if (!t.tier2) return ok;
+    ok = ok && launch_compact_unproven(s.ok, nq, s.idx, s.n2, st) == cudaSuccess;
+    // the open queries' operand rows with their |q|^2 (fp16 copy) or error bound (int8 copy)
+    ok = ok && launch_gather_queries(ops.queries, ops.qpitch, s.qeps ? s.qeps : s.qn2, s.idx, s.n2, nq, s.q_t2, s.qeps ? s.qeps_t2 : s.qn2_t2,
+                                     st) == cudaSuccess;
+    CoarseOperands ops2 = ops;
+    ops2.queries = s.q_t2;
+    if (ops.q_norm2) ops2.q_norm2 = s.qn2_t2;
+    ok = ok && launch_coarse(ops2, v.n_rows, v.dim, nq, t.second, s.cand_t2, s.list_scratch, st, s.n2, nullptr, nullptr, bm, words,
+                             bm ? s.idx : nullptr) == cudaSuccess;
+    ok = ok && launch_refine(v, d_q32, qpitch, nq, t.second.grid_x, t.second.keep, ke, s.cand_t2, eps, s.qn2_t2, shadow_max_norm_, s.ok, out,
+                             s.idx, s.n2, st, nullptr, nullptr, row_label, s.qeps_t2) == cudaSuccess;
+    lc.launches += 4;
+    return ok;
+}
+
 bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t nq, uint32_t ke, cudaStream_t st,
                                 LaunchCounters &lc, uint64_t **d_result, bool tc_only) {
     const CorpusView v = view();
@@ -934,11 +1103,7 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
     const CoarseKind dkind = is16 ? CoarseDirect16 : CoarseDirect8;
     // int8 / uint8 L2: the int32 |row|^2 table is brought up to date on `st` first (no HBM for it: the exact scan)
     if (cmode != 0 && nq >= 16 && (is16 || is8) && coarse_supported(v, nq, ke, dkind) && (!int_l2() || ensure_shadow(st))) {
-        // int8 / uint8: s8 / u8 wgmma dot products are exact integers and the epilogue applies the reference's own
-        // float expression, so that route is bit-exact.  L2: |row|^2 + |q|^2 - 2 dot in int32, rounded once to float, is the
-        // reference's float(sum of squared differences) bit for bit
-        CoarseOperands ops{v.rows, v.pitch, d_q, qpitch, (dtype_ == DT_BF16 || dtype_ == DT_I8) ? 1 : 0,
-                           mkind_ == MT_COS ? 1 : int_l2() ? 2 : 0, nullptr, nullptr};
+        const CoarseOperands ops16{v.rows, v.pitch, d_q, qpitch, dtype_ == DT_BF16 ? 1 : 0, mkind_ == MT_COS ? 1 : 0, nullptr, nullptr};
         last_batch_coarse_ = true;
         last_batch_path_ = 2;
         c.d_last_ok = nullptr;
@@ -978,10 +1143,10 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
             layout(c.d_cand);
             c.d_last_ok = d_ok;
             c.last_ok_n = nq;
-            bool ok = launch_coarse(ops, v.n_rows, v.dim, nq, cps, cand_s, list_scratch, st) == cudaSuccess;
+            bool ok = launch_coarse(ops16, v.n_rows, v.dim, nq, cps, cand_s, list_scratch, st) == cudaSuccess;
             ok = ok && launch_threshold(cand_s, nq, cps.grid_x, cps.keep, ke, 0.0f, nullptr, 0.0f, (uint32_t)dim_, 0, d_thr, d_ovf, st) == cudaSuccess;
             cudaEventRecord(c.ev_start, st);
-            ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq, probe, cand_m, list_scratch, st, nullptr, d_thr, d_ovf) == cudaSuccess;
+            ok = ok && launch_coarse(ops16, v.n_rows, v.dim, nq, probe, cand_m, list_scratch, st, nullptr, d_thr, d_ovf) == cudaSuccess;
             cudaEventRecord(c.ev_stop, st);
             ok = ok && launch_final_select(cand_m, nq, (uint32_t)(probe.grid_x * probe.keep), ke, c.d_out, st, &lc) == cudaSuccess;
             ok = ok && launch_flags_from_overflow(d_ovf, nq, d_ok, st) == cudaSuccess;
@@ -989,7 +1154,7 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
             if (tier2) {
                 ok = ok && launch_compact_unproven(d_ok, nq, d_idx, d_n2, st) == cudaSuccess;
                 ok = ok && launch_gather_queries(d_q, qpitch, nullptr, d_idx, d_n2, nq, q_t2, nullptr, st) == cudaSuccess;
-                CoarseOperands ops2 = ops;
+                CoarseOperands ops2 = ops16;
                 ops2.queries = q_t2;
                 ok = ok && launch_coarse(ops2, v.n_rows, v.dim, nq, cp, cand_t2, list_scratch, st, d_n2) == cudaSuccess;
                 ok = ok && launch_final_select(cand_t2, nq, (uint32_t)(cp.grid_x * cp.keep), ke, out2, st, &lc, d_n2) == cudaSuccess;
@@ -1011,13 +1176,8 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
         };
         if (!c.need_cand(layout(nullptr)) || !c.need_out((size_t)nq * ke)) return false;
         layout(c.d_cand);
-        bool ok = true;
-        if (int_l2()) {
-            ok = launch_int_norm2(d_q, qpitch, v.dim, 0, nq, dtype_ == DT_I8, d_qn, st) == cudaSuccess;
-            ops.row_norm2 = reinterpret_cast<const float *>(d_norm2_); // int32 values (CoarseOperands)
-            ops.q_norm2 = reinterpret_cast<const float *>(d_qn);
-            lc.launches++;
-        }
+        CoarseOperands ops = ops16;
+        bool ok = !is8 || direct8_operands(d_q, qpitch, nq, d_qn, st, lc, ops);
         cudaEventRecord(c.ev_start, st);
         ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq, cp, cand, list_scratch, st) == cudaSuccess;
         cudaEventRecord(c.ev_stop, st);
@@ -1044,11 +1204,7 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
         kind = CoarseTF32;
         coarse = unit && coarse_supported(v, nq, ke, kind);
     }
-    if (coarse && !unit && !(shadow_max_abs_ <= 60000.0f)) {
-        // values outside the fp16 range (or NaN): this index stays on the exact scan; give the shadow's HBM back
-        coarse = false;
-        disable_coarse();
-    }
+    if (coarse && !shadow_values_in_range()) coarse = false;
     last_batch_coarse_ = coarse;
     last_batch_path_ = coarse ? 1 : 0;
     last_shadow_bits_ = !coarse ? 0 : kind == CoarseQ8 ? 8 : kind == CoarseF16 ? 16 : 0;
@@ -1076,131 +1232,56 @@ bool FlatIndex::batch_scan_rows(QueryCtx &c, const void *d_q, size_t qpitch, uin
         *d_result = c.d_out;
         return ok;
     }
-    // fp16 route, first tier in two passes over the shadow rows:
-    //   sample pass   every `stride`-th row tile, per (query, row range) the smallest approximate distance of 8 interleaved
-    //                 slices -> per query the bound T = (k-th smallest of its ranges x 8 minima) + 2 eps: k distinct rows
-    //                 lie at or below it, so it bounds the k-th best distance from above
-    //   main pass     all row tiles, every row with approximate distance < T is kept (fixed bound: no running thresholds,
-    //                 no list compaction, which a running threshold keeps the epilogue busy with)
-    // TF32 route: one pass with adaptive lists, as before.
     const bool q8 = kind == CoarseQ8, shadow = kind == CoarseF16 || q8;
-    const bool two_pass = shadow && coarse_fixed_enabled();
-    CoarsePlan cp = plan_coarse(v, nq, kind, ke); // TF32 / single-pass: the adaptive lists ARE the first tier
-    CoarsePlan cps{};                             // sample pass
-    if (two_pass) {
-        // expected rows below T per (query, row range) = k / (sample fraction * ranges): aim at 24 of the 96 slots
-        const CoarsePlan probe = plan_coarse(v, nq, kind, ke, 0, 1, 1);
-        if (wide) {
-            // k in the hundreds: ranges x 32 slice minima barely hold k values.  The sample pass keeps adaptive lists of 128 per
-            // (query, row range) instead; their union holds at least k distinct rows at or below its k-th smallest
-            // approximate distance, so threshold_kernel's bound stands.  Aim at 128 of the 256 slots of the main pass; the sample
-            // holds about 4 k rows (128 per visited tile).
-            cps = plan_coarse(v, nq, kind, ke, kCoarseKeepWide, sample_stride(probe, ke, 128.0, 1 / 32.0), 0);
-        } else {
-            // the sample holds a few times k slice minima (4 per visited tile).  The int8 copy's bound is about 7x the fp16 one's, and
-            // the rows within 2 eps of the k-th distance, not k / f, fill most of its lists of 256: it samples about 4 % at k = 10 over
-            // 30 ranges (aim 8), which keeps the rows below the bound near a quarter of a list on uniform unit rows
-            cps = plan_coarse(v, nq, kind, ke, 0, sample_stride(probe, ke, q8 ? 8.0 : 24.0, 2.0), 2);
-        }
-        cp = probe;
-    }
-    // second tier (fp16 route): the queries whose first-tier proof failed (a list of the main pass overflowed: more than 96
-    // rows of one range within the bound — clustered corpora) are packed to the front and run once more with adaptive
-    // lists of 128 per row range.  Nothing is known on the host: the tier's kernels read the count of open queries from
-    // device memory and leave at once when it is zero.
-    const bool tier2 = shadow && coarse_tier2_enabled();
-    CoarsePlan cp2{};
-    if (tier2) cp2 = plan_coarse(v, nq, kind, ke, kCoarseKeepWide);
+    // expected rows below T per (query, row range) = k / (sample fraction * ranges): aim at 24 of the 96 slots; the sample holds a
+    // few times k slice minima (4 per visited tile).  The int8 copy's bound is about 7x the fp16 one's, and the rows within 2 eps
+    // of the k-th distance, not k / f, fill most of its lists of 256: it samples about 4 % at k = 10 over 30 ranges (aim 8), which
+    // keeps the rows below the bound near a quarter of a list on uniform unit rows.  k in the hundreds: aim at 128 of the 256
+    // slots of the main pass; the sample holds about 4 k rows (128 per visited tile).
+    const KnnTiers t = plan_knn_tiers(v, nq, kind, ke, wide ? 128.0 : q8 ? 8.0 : 24.0, wide ? 1 / 32.0 : 2.0, false);
     const size_t nO = (size_t)nq * ke;
     // the queries in the operand type of the copy: fp16 rows, or int8 rows with their scale (coarse_q8_pitch)
-    const size_t q16_pitch = q8 ? coarse_q8_pitch((uint32_t)dim_) : (dim_ * 2 + 15) & ~(size_t)15;
-    const size_t q16_bytes = shadow ? (size_t)nq * q16_pitch : 0;
-    const size_t scratch = std::max(std::max(cp.scratch_elems, two_pass ? cps.scratch_elems : 0), tier2 ? cp2.scratch_elems : 0);
+    const size_t q_pitch = !shadow ? 0 : q8 ? coarse_q8_pitch((uint32_t)dim_) : f16_query_pitch();
     const size_t nO12 = wide ? 0 : nO; // k > kMaxFusedK: the tiers write the answer rows in place, no out1 / out2
-    uint64_t *coarse_cand, *cand_s, *cand_t2, *out1, *out2, *cand2, *list_scratch;
-    uint8_t *q16, *q16_t2;
-    float *d_qn2, *d_qn2_t2, *d_thr, *d_qeps, *d_qeps_t2;
-    uint32_t *d_ok, *d_idx, *d_n2, *d_ovf;
+    KnnScratch ks;
+    uint64_t *out1, *out2, *cand2;
     const auto layout = [&](void *base) {
         BatchScratch s(base);
-        coarse_cand = s.take<uint64_t>((size_t)nq * cp.grid_x * cp.keep);
-        cand_s = s.take<uint64_t>(two_pass ? (size_t)nq * cps.grid_x * cps.keep : 0);
-        cand_t2 = s.take<uint64_t>(tier2 ? (size_t)nq * cp2.grid_x * cp2.keep : 0);
+        ks.take(s, t, nq, q_pitch, !unit, q8);
         out1 = s.take<uint64_t>(nO12);
         out2 = s.take<uint64_t>(nO12);
         // k > kMaxFusedK: the exact fallback's chunk-select lists take the place of the fused scan's
         cand2 = s.take<uint64_t>(wide ? wp.cand_elems : sp.cand_elems);
-        q16 = s.take<uint8_t>(q16_bytes);
-        q16_t2 = s.take<uint8_t>(tier2 ? q16_bytes : 0);
-        list_scratch = s.take<uint64_t>(scratch);
-        d_qn2 = s.take<float>(unit ? 0 : nq); // |q|^2 per query
-        d_qn2_t2 = s.take<float>(unit || !tier2 ? 0 : nq);
-        d_qeps = s.take<float>(q8 ? nq : 0); // int8 copy: the error bound of each query
-        d_qeps_t2 = s.take<float>(q8 && tier2 ? nq : 0);
-        d_ok = s.take<uint32_t>(nq);
-        d_idx = s.take<uint32_t>(nq); // tier 2: indices of the open queries
-        d_n2 = s.take<uint32_t>(1);   //         and their count
-        d_thr = s.take<float>(nq);    // fixed bound per query
-        d_ovf = s.take<uint32_t>(nq); // a list of the main pass ran full
         return s.words();
     };
     if (!c.need_cand(layout(nullptr)) || !c.need_out(nO) || (wide && !c.need_scores(wp.score_elems))) return false;
     layout(c.d_cand);
     if (wide) out1 = c.d_out; // both tiers and the exact fallback write their rows of the answer in place (no blend)
-    c.d_last_ok = d_ok;
+    c.d_last_ok = ks.ok;
     c.last_ok_n = nq;
     CoarseOperands ops{v.rows, v.pitch, d_q, qpitch, 0, 0, nullptr, nullptr};
     bool ok = true;
     if (kind == CoarseF16) {
-        ok = launch_to_f16(d_q, qpitch, (uint32_t)dim_, 0, nq, q16, q16_pitch, st) == cudaSuccess;
-        ops = CoarseOperands{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
-        if (!unit) ok = ok && launch_row_stats(d_q, qpitch, (uint32_t)dim_, 0, nq, d_qn2, nullptr, st) == cudaSuccess;
-        lc.launches += unit ? 1 : 2;
+        ok = shadow_operands(d_q, qpitch, nq, ks.q, ks.qn2, st, lc, ops);
     } else if (q8) {
-        ok = launch_quantize_queries(d_q, qpitch, (uint32_t)dim_, nq, q16, d_qeps, shadow8_delta_, shadow8_xmax_, st) == cudaSuccess;
-        ops = CoarseOperands{d_shadow8_, 0, q16, q16_pitch, 1, 0, d_tscale_, nullptr};
+        ok = launch_quantize_queries(d_q, qpitch, (uint32_t)dim_, nq, ks.q, ks.qeps, shadow8_delta_, shadow8_xmax_, st) == cudaSuccess;
+        ops = CoarseOperands{d_shadow8_, 0, ks.q, q_pitch, 1, 0, d_tscale_, nullptr};
         lc.launches++;
     }
-    const float eps = coarse_eps(kind);
-    if (two_pass) {
-        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq, cps, cand_s, list_scratch, st) == cudaSuccess;
-        ok = ok && launch_threshold(cand_s, nq, cps.grid_x, cps.keep, ke, eps, d_qn2, shadow_max_norm_, (uint32_t)dim_, mkind_ == MT_L2 ? 1 : 0, d_thr,
-                                    d_ovf, st, q8 ? d_qeps : nullptr) == cudaSuccess;
-        lc.launches += 2;
-    }
-    cudaEventRecord(c.ev_start, st);
-    ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq, cp, coarse_cand, list_scratch, st, nullptr, two_pass ? d_thr : nullptr,
-                             two_pass ? d_ovf : nullptr) == cudaSuccess;
-    cudaEventRecord(c.ev_stop, st);
-    // exact rescoring of the few candidates that can still matter + exact top-k + proof, one CTA per query
-    ok = ok && launch_refine(v, d_q, qpitch, nq, cp.grid_x, cp.keep, ke, coarse_cand, eps, d_qn2, shadow_max_norm_, d_ok, out1, nullptr, nullptr,
-                             st, two_pass ? d_thr : nullptr, two_pass ? d_ovf : nullptr, nullptr, q8 ? d_qeps : nullptr) == cudaSuccess;
-    lc.launches += 2;
-    if (tier2) {
-        ok = ok && launch_compact_unproven(d_ok, nq, d_idx, d_n2, st) == cudaSuccess;
-        // the open queries' operand rows with their |q|^2 (fp16 copy) or error bound (int8 copy)
-        ok = ok && launch_gather_queries(q16, q16_pitch, q8 ? d_qeps : d_qn2, d_idx, d_n2, nq, q16_t2, q8 ? d_qeps_t2 : d_qn2_t2, st) == cudaSuccess;
-        CoarseOperands ops2 = ops;
-        ops2.queries = q16_t2;
-        if (!q8) ops2.q_norm2 = d_qn2_t2;
-        ok = ok && launch_coarse(ops2, v.n_rows, v.dim, nq, cp2, cand_t2, list_scratch, st, d_n2) == cudaSuccess;
-        ok = ok && launch_refine(v, d_q, qpitch, nq, cp2.grid_x, cp2.keep, ke, cand_t2, eps, d_qn2_t2, shadow_max_norm_, d_ok, out1, d_idx, d_n2,
-                                 st, nullptr, nullptr, nullptr, q8 ? d_qeps_t2 : nullptr) == cudaSuccess;
-        lc.launches += 4;
-    }
+    ok = ok && enqueue_knn_tiers(c, v, kind, t, ks, ops, d_q, qpitch, nq, ke, out1, nullptr, 0, nullptr, st, lc);
     if (wide) {
         // exact fallback of the open queries, entirely on device; with none open, every launch exits at once
-        ok = ok && launch_compact_unproven(d_ok, nq, d_idx, d_n2, st) == cudaSuccess;
-        ok = ok && launch_topk_wide(v, d_q, qpitch, nq, ke, d_idx, d_n2, wp, c.d_scores, cand2, c.d_out, c.d_abort, st, &lc) == cudaSuccess;
+        ok = ok && launch_compact_unproven(ks.ok, nq, ks.idx, ks.n2, st) == cudaSuccess;
+        ok = ok && launch_topk_wide(v, d_q, qpitch, nq, ke, ks.idx, ks.n2, wp, c.d_scores, cand2, c.d_out, c.d_abort, st, &lc) == cudaSuccess;
         lc.launches++;
         coarse_batches_++;
         *d_result = c.d_out;
         return ok;
     }
     // exact fallback, entirely on device: CTAs whose queries are all verified exit at once
-    ok = ok && launch_scan_topk(v, d_q, qpitch, nq, ke, sp, cand2, st, &lc, d_ok, c.d_abort) == cudaSuccess;
+    ok = ok && launch_scan_topk(v, d_q, qpitch, nq, ke, sp, cand2, st, &lc, ks.ok, c.d_abort) == cudaSuccess;
     ok = ok && launch_final_select(cand2, nq, sp.lists_per_query * ke, ke, out2, st, &lc) == cudaSuccess;
-    ok = ok && launch_blend(d_ok, out1, out2, nq, ke, c.d_out, st, &lc) == cudaSuccess;
+    ok = ok && launch_blend(ks.ok, out1, out2, nq, ke, c.d_out, st, &lc) == cudaSuccess;
     coarse_batches_++;
     *d_result = c.d_out;
     return ok;
@@ -1497,53 +1578,33 @@ int FlatIndex::range_batch(const void *qs, size_t qstride, size_t nq, const doub
         c = checkout();
         route = c && ensure_shadow(c->stream);
     }
-    if (route && !unit_rows() && !(shadow_max_abs_ <= 60000.0f)) { // values outside the fp16 range: exact scans from now on
-        disable_coarse();
-        route = false;
-    }
+    if (route && !shadow_values_in_range()) route = false;
     if (route) {
         const uint32_t nq32 = (uint32_t)nq;
         cudaStream_t st = c->stream;
         LaunchCounters lc;
-        const bool unit = unit_rows();
         // stored-form queries, then the radii as float (the reference compares score <= DistType(radius))
         const size_t qpitch = query_pitch();
         const std::vector<float> radii_f(radii, radii + nq);
         bool ok = stage_queries(*c, qs, qstride, nq, true, radii_f.data(), nq * sizeof(float));
         const float *d_radius = reinterpret_cast<const float *>(c->d_query + qpitch * nq);
         const CoarsePlan cp = plan_coarse(v, nq32, CoarseF16, 1, 0, 1, 1);
-        const size_t slots = (size_t)cp.grid_x * cp.keep, q16_pitch = (dim_ * 2 + 15) & ~(size_t)15;
-        uint64_t *cand, *hits, *list_scratch;
-        uint8_t *q16;
-        float *d_qn2, *d_thr;
-        uint32_t *d_ovf, *d_res;
+        const size_t slots = (size_t)cp.grid_x * cp.keep;
+        RangeScratch rs;
+        uint64_t *hits;
+        uint32_t *d_res;
         const auto layout = [&](void *base) {
             BatchScratch s(base);
-            cand = s.take<uint64_t>(nq * slots);
+            rs.take(s, *this, CoarseF16, cp, nq32, false);
             hits = s.take<uint64_t>(nq * slots);
-            q16 = s.take<uint8_t>(nq * q16_pitch);
-            list_scratch = s.take<uint64_t>(cp.scratch_elems);
-            d_qn2 = s.take<float>(unit ? 0 : nq);  // |q|^2 per query
-            d_thr = s.take<float>(nq);             // bound of the main pass per query
-            d_ovf = s.take<uint32_t>(nq);          // a list of the main pass ran full
-            d_res = s.take<uint32_t>(3 * nq + 1);  // [ok nq][count nq][offset nq][hits in total]
+            d_res = s.take<uint32_t>(3 * nq + 1); // [ok nq][count nq][offset nq][hits in total]
             return s.words();
         };
         ok = ok && c->need_cand(layout(nullptr)) && c->need_ids(3 * nq + 1);
         layout(c->d_cand);
-        uint32_t *d_total = d_res + 3 * nq;
-        ok = ok && launch_to_f16(c->d_query, qpitch, (uint32_t)dim_, 0, nq32, q16, q16_pitch, st) == cudaSuccess;
-        if (!unit) ok = ok && launch_row_stats(c->d_query, qpitch, (uint32_t)dim_, 0, nq32, d_qn2, nullptr, st) == cudaSuccess;
-        ok = ok && launch_range_bound(d_radius, nq32, kCoarseEpsF16, d_qn2, shadow_max_norm_, (uint32_t)dim_, mkind_ == MT_L2 ? 1 : 0, d_thr, d_ovf,
-                                      d_total, st) == cudaSuccess;
-        const CoarseOperands ops{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
-        cudaEventRecord(c->ev_start, st);
-        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_thr, d_ovf) == cudaSuccess;
-        cudaEventRecord(c->ev_stop, st);
-        ok = ok && launch_range_refine(v, c->d_query, qpitch, nq32, (uint32_t)slots, cand, d_radius, d_qn2, d_thr, d_ovf, hits, d_total, d_res,
-                                       d_res + nq, d_res + 2 * nq, st) == cudaSuccess;
+        ok = ok && enqueue_range_route(*c, v, CoarseF16, cp, rs, c->d_query, qpitch, nq32, d_radius, nullptr, 0,
+                                       RangeOut{hits, 0, d_res, d_res + nq, d_res + 2 * nq, d_res + 3 * nq, nullptr}, st, lc);
         ok = ok && cudaMemcpyAsync(c->h_ids, d_res, (3 * nq + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st) == cudaSuccess;
-        lc.launches += unit ? 4 : 5;
         launches_total_ += lc.launches;
         coarse_batches_++;
         if (ok) {
@@ -1635,7 +1696,7 @@ int FlatIndex::range_device(const void *d_q, size_t nq, const float *d_radii, si
     const int cmode = coarse_mode();
     const bool is8 = dtype_ == DT_I8 || dtype_ == DT_U8, is16 = dtype_ == DT_F16 || dtype_ == DT_BF16;
     // 1: the fp32 route of range_batch (same eligibility); 2: the fixed-radius pass over 8-bit rows, or the fixed-bound pass over
-    // 16-bit rows with the margin eps16_q and CUDA-core rescoring (r16, finite X only); 0: the exact scan only
+    // 16-bit rows with the margin eps16_q and CUDA-core rescoring (finite X only); 0: the exact scan only
     int path = 0;
     if (n > 0 && is8 && cmode != 0 && nq >= 16 && coarse_fixed_enabled() && coarse_supported(v, nq32, 1, CoarseDirect8) &&
         (!int_l2() || ensure_shadow(st))) {
@@ -1644,38 +1705,23 @@ int FlatIndex::range_device(const void *d_q, size_t nq, const float *d_radii, si
                ensure_shadow(st) && std::isfinite(shadow_max_norm_)) {
         path = 2;
     } else if (n > 0 && cmode == 1 && dtype_ == DT_F32 && !coarse_disabled_ && coarse_fixed_enabled() && coarse_supported(v, nq32, 1, CoarseF16) &&
-               (nq >= 16 || single_query_takes_coarse(1)) && ensure_shadow(st)) {
+               (nq >= 16 || single_query_takes_coarse(1)) && ensure_shadow(st) && shadow_values_in_range()) {
         path = 1;
-        if (!unit_rows() && !(shadow_max_abs_ <= 60000.0f)) { // values outside the fp16 range: exact scans from now on
-            disable_coarse();
-            path = 0;
-        }
     }
-    const bool unit = unit_rows(), r16 = path == 2 && is16, refine = path == 1 || r16; // refine: rescored by range_refine_kernel
-    const CoarsePlan cp = path == 1 ? plan_coarse(v, nq32, CoarseF16, 1, 0, 1, 1)
-                          : path == 2 ? plan_coarse(v, nq32, is16 ? CoarseDirect16 : CoarseDirect8, 1, 0, 1, 1)
-                                      : CoarsePlan{};
-    const size_t slots = (size_t)cp.grid_x * cp.keep, q16_pitch = (dim_ * 2 + 15) & ~(size_t)15;
+    const CoarseKind kind = path == 1 ? CoarseF16 : is16 ? CoarseDirect16 : CoarseDirect8;
+    const CoarsePlan cp = path ? plan_coarse(v, nq32, kind, 1, 0, 1, 1) : CoarsePlan{};
     const WidePlan wp = n > 0 ? plan_topk_wide(v.n_rows, nq32) : WidePlan{};
-    uint64_t *cand, *list_scratch;
-    uint8_t *q16;
-    float *d_qn2, *d_thr;
-    uint32_t *d_ok, *d_idx, *d_n2, *d_ovf, *d_total, *d_flags, *d_front;
+    RangeScratch rs;
+    uint32_t *d_ok, *d_idx, *d_n2, *d_total, *d_flags;
     const bool fold = multi_ && path; // a route's rows -> labels
     const auto layout = [&](void *base) {
         BatchScratch sc(base);
-        cand = sc.take<uint64_t>(path ? nq * slots : 0);
-        list_scratch = sc.take<uint64_t>(path ? cp.scratch_elems : 0);
-        q16 = sc.take<uint8_t>(path == 1 ? nq * q16_pitch : 0);
-        d_qn2 = sc.take<float>((path == 1 && !unit) || (path == 2 && int_l2()) ? nq : 0); // |q|^2 (fp32), or int32 for 8-bit L2
-        d_thr = sc.take<float>(refine ? nq : 0);
-        d_ovf = sc.take<uint32_t>(path ? nq : 0);
+        if (path) rs.take(sc, *this, kind, cp, nq32, fold);
         d_total = sc.take<uint32_t>(1);
         d_ok = sc.take<uint32_t>(nq);  // reported flags
         d_idx = sc.take<uint32_t>(nq); // the open queries
         d_n2 = sc.take<uint32_t>(1);   // and their count
-        d_flags = sc.take<uint32_t>(fold ? nq : 0);          // multi-value: the reported flags (d_ok: 1 = folded, 0 = open)
-        d_front = sc.take<uint32_t>(fold && refine ? nq : 0); // multi-value fp32 / 16-bit route: the hit rows at the front of each list segment
+        d_flags = sc.take<uint32_t>(fold ? nq : 0); // multi-value: the reported flags (d_ok: 1 = folded, 0 = open)
         return sc.words();
     };
     if (!c->need_cand(layout(nullptr)) || (n > 0 && !c->need_scores(wp.score_elems))) return -1;
@@ -1684,50 +1730,9 @@ int FlatIndex::range_device(const void *d_q, size_t nq, const float *d_radii, si
     uint64_t *comp = reinterpret_cast<uint64_t *>(d_labels);
     bool ok = cudaMemsetAsync(d_counts, 0, nq * 4, st) == cudaSuccess && cudaMemsetAsync(d_ok, 0, nq * 4, st) == cudaSuccess;
     // the timed span (VecSimB200_GetStats): the route's main pass, or the exact scan of a batch no route serves
-    if (refine) {
-        CoarseOperands ops{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
-        if (r16) {
-            ok = ok && launch_range_bound16(d_q, qpitch, nq32, (uint32_t)dim_, dtype_, d_radii, shadow_max_norm_, d_thr, d_ovf, st) == cudaSuccess;
-            ops = CoarseOperands{v.rows, v.pitch, d_q, qpitch, dtype_ == DT_BF16 ? 1 : 0, 0, nullptr, nullptr};
-        } else {
-            ok = ok && launch_to_f16(d_q, qpitch, (uint32_t)dim_, 0, nq32, q16, q16_pitch, st) == cudaSuccess;
-            if (!unit) ok = ok && launch_row_stats(d_q, qpitch, (uint32_t)dim_, 0, nq32, d_qn2, nullptr, st) == cudaSuccess;
-            ok = ok && launch_range_bound(d_radii, nq32, kCoarseEpsF16, d_qn2, shadow_max_norm_, (uint32_t)dim_, mkind_ == MT_L2 ? 1 : 0, d_thr,
-                                          d_ovf, d_total, st) == cudaSuccess;
-        }
-        cudaEventRecord(c->ev_start, st);
-        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_thr, d_ovf) == cudaSuccess;
-        cudaEventRecord(c->ev_stop, st);
-        if (fold) { // the kept rows stay at the front of each list segment (cap = slots onto cand itself: a copy onto itself)
-            ok = ok && launch_range_refine(v, d_q, qpitch, nq32, (uint32_t)slots, cand, d_radii, d_qn2, d_thr, d_ovf, cand, d_total, d_ok,
-                                           d_front, nullptr, st, (uint32_t)slots) == cudaSuccess;
-            ok = ok && launch_range_label_fold(cand, nq32, (uint32_t)slots, d_front, nullptr, d_id_to_label_, cap32, comp, d_counts, d_ok, d_flags,
-                                               st) == cudaSuccess;
-            lc.launches++;
-        } else {
-            ok = ok && launch_range_refine(v, d_q, qpitch, nq32, (uint32_t)slots, cand, d_radii, d_qn2, d_thr, d_ovf, comp, d_total, d_ok,
-                                           d_counts, nullptr, st, cap32) == cudaSuccess;
-        }
-        lc.launches += r16 ? 3 : unit ? 4 : 5;
-    } else if (path == 2) {
-        CoarseOperands ops{v.rows, v.pitch, d_q, qpitch, dtype_ == DT_I8 ? 1 : 0, mkind_ == MT_COS ? 1 : int_l2() ? 2 : 0, nullptr, nullptr};
-        ok = ok && cudaMemsetAsync(d_ovf, 0, nq * 4, st) == cudaSuccess;
-        if (int_l2()) {
-            ok = ok && launch_int_norm2(d_q, qpitch, v.dim, 0, nq32, dtype_ == DT_I8, reinterpret_cast<int32_t *>(d_qn2), st) == cudaSuccess;
-            ops.row_norm2 = reinterpret_cast<const float *>(d_norm2_); // int32 values (CoarseOperands)
-            ops.q_norm2 = d_qn2;
-            lc.launches++;
-        }
-        cudaEventRecord(c->ev_start, st);
-        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_radii, d_ovf) == cudaSuccess;
-        cudaEventRecord(c->ev_stop, st);
-        if (fold)
-            ok = ok && launch_range_label_fold(cand, nq32, (uint32_t)slots, nullptr, d_ovf, d_id_to_label_, cap32, comp, d_counts, d_ok, d_flags,
-                                               st) == cudaSuccess;
-        else
-            ok = ok && launch_range_pack(cand, nq32, (uint32_t)slots, d_ovf, cap32, comp, d_counts, d_ok, st) == cudaSuccess;
-        lc.launches += 2;
-    }
+    if (path)
+        ok = ok && enqueue_range_route(*c, v, kind, cp, rs, d_q, qpitch, nq32, d_radii, nullptr, 0,
+                                       RangeOut{comp, cap32, d_ok, d_counts, nullptr, d_total, fold ? d_flags : nullptr}, st, lc);
     if (n > 0) {
         // the exact scan: the queries a route left open (compacted on the device; none open = every launch exits at once), or all
         if (path) {
@@ -2168,46 +2173,32 @@ FlatIndex::TableSlot *FlatIndex::table_slot(size_t elems) {
     return &table_ring_.back();
 }
 
-// The same batch with device pointers end to end (DESIGN.md §4.6): no filter length comes back to the host.  One ragged gather over
-// the flat space of the caps, 2 ceil(k / 128) segmented selects, one unpack: 2 + 2 ceil(k / 128) launches whatever nq.  Selection is
-// by (distance, position in the filter) as in topk_filtered, so every row equals its answer.
-int FlatIndex::topk_filtered_batch_device(const void *d_q, size_t nq, size_t k, const uint32_t *const *d_doc_ids,
-                                          const uint32_t *const *d_counts, const size_t *caps, int64_t *d_labels, float *d_scores,
-                                          uint32_t *d_counts_out, cudaStream_t s) {
-    last_mode_ = HYBRID_ADHOC_BF;
-    if (nq == 0 || k == 0) return 0;
-    if (k > (size_t)kMaxWideK || nq > 0x7FFFFFFFull) return -1;
+// The caps of a ragged batch: their sum, their largest and the gather's chunks.  ok = false when a cap exceeds 0xFFFFFFF0 (the entry
+// points return -2)
+struct RaggedCaps {
+    bool ok = true;
     size_t total = 0, max_cap = 0;
     uint64_t blocks = 0;
+};
+static RaggedCaps scan_caps(const size_t *caps, size_t nq) {
+    RaggedCaps r;
     for (size_t i = 0; i < nq; i++) {
-        if (caps[i] > 0xFFFFFFF0ull) return -2;
-        total += caps[i];
-        max_cap = std::max(max_cap, caps[i]);
-        blocks += ragged_blocks(caps[i]);
+        if (caps[i] > 0xFFFFFFF0ull) {
+            r.ok = false;
+            return r;
+        }
+        r.total += caps[i];
+        r.max_cap = std::max(r.max_cap, caps[i]);
+        r.blocks += ragged_blocks(caps[i]);
     }
-    if (!flush()) return -1;
-    if (!sync_label_table()) return -2;
-    const uint32_t nq32 = (uint32_t)nq, chunk = (uint32_t)std::min<size_t>(k, kMaxFusedK);
-    const uint32_t parts = plan_ragged_select_parts(max_cap, nq32);
-    std::lock_guard<std::mutex> dg(dev_mu_);
-    if (!dev_ctx_) dev_ctx_ = checkout();
-    QueryCtx *c = dev_ctx_.get();
-    if (!c) return -1;
-    const size_t tab_elems = 4 * nq + 2; // [docId pointers nq][count pointers nq][score offsets nq + 1][first CTAs nq + 1]
-    uint64_t *tab, *cand, *out;
-    float *scores;
-    const auto layout = [&](void *base) {
-        BatchScratch sc(base);
-        tab = sc.take<uint64_t>(tab_elems);
-        scores = sc.take<float>(total);
-        cand = sc.take<uint64_t>((size_t)nq * parts * 8 * chunk); // 8 lists (one per warp) per select CTA
-        out = sc.take<uint64_t>(nq * k);
-        return sc.words();
-    };
-    if (!c->need_cand(layout(nullptr))) return -1;
-    layout(c->d_cand);
-    TableSlot *slot = table_slot(tab_elems);
-    if (!slot) return -1;
+    return r;
+}
+
+bool FlatIndex::upload_ragged_table(uint64_t *d_tab, const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts, const size_t *caps,
+                                    uint32_t nq, const std::vector<uint32_t> &tail, cudaStream_t st, RaggedBatch &b, bool &ok) {
+    const size_t elems = ragged_table_elems(nq, tail.size());
+    TableSlot *slot = table_slot(elems);
+    if (!slot) return false;
     uint64_t *h = slot->h, off = 0, blk = 0;
     for (size_t i = 0; i < nq; i++) {
         h[i] = (uint64_t)(uintptr_t)d_doc_ids[i];
@@ -2219,12 +2210,51 @@ int FlatIndex::topk_filtered_batch_device(const void *d_q, size_t nq, size_t k, 
     }
     h[3 * nq] = off;
     h[4 * nq + 1] = blk;
-    cudaStream_t st = s ? s : cudaStreamLegacy; // NULL = the legacy default stream, as everywhere in CUDA
-    bool ok = cudaMemcpyAsync(tab, h, tab_elems * 8, cudaMemcpyHostToDevice, st) == cudaSuccess;
+    if (!tail.empty()) memcpy(h + 4 * nq + 2, tail.data(), tail.size() * sizeof(uint32_t));
+    ok = ok && cudaMemcpyAsync(d_tab, h, elems * 8, cudaMemcpyHostToDevice, st) == cudaSuccess;
     ok = ok && cudaEventRecord(slot->ev, st) == cudaSuccess;
-    const RaggedBatch b{reinterpret_cast<const uint32_t *const *>(tab), reinterpret_cast<const uint32_t *const *>(tab + nq), tab + 2 * nq, nq32};
+    b = RaggedBatch{reinterpret_cast<const uint32_t *const *>(d_tab), reinterpret_cast<const uint32_t *const *>(d_tab + nq), d_tab + 2 * nq, nq};
+    return true;
+}
+
+// The same batch with device pointers end to end (DESIGN.md §4.6): no filter length comes back to the host.  One ragged gather over
+// the flat space of the caps, 2 ceil(k / 128) segmented selects, one unpack: 2 + 2 ceil(k / 128) launches whatever nq.  Selection is
+// by (distance, position in the filter) as in topk_filtered, so every row equals its answer.
+int FlatIndex::topk_filtered_batch_device(const void *d_q, size_t nq, size_t k, const uint32_t *const *d_doc_ids,
+                                          const uint32_t *const *d_counts, const size_t *caps, int64_t *d_labels, float *d_scores,
+                                          uint32_t *d_counts_out, cudaStream_t s) {
+    last_mode_ = HYBRID_ADHOC_BF;
+    if (nq == 0 || k == 0) return 0;
+    if (k > (size_t)kMaxWideK || nq > 0x7FFFFFFFull) return -1;
+    const RaggedCaps rc = scan_caps(caps, nq);
+    if (!rc.ok) return -2;
+    if (!flush()) return -1;
+    if (!sync_label_table()) return -2;
+    const uint32_t nq32 = (uint32_t)nq, chunk = (uint32_t)std::min<size_t>(k, kMaxFusedK);
+    const uint32_t parts = plan_ragged_select_parts(rc.max_cap, nq32);
+    std::lock_guard<std::mutex> dg(dev_mu_);
+    if (!dev_ctx_) dev_ctx_ = checkout();
+    QueryCtx *c = dev_ctx_.get();
+    if (!c) return -1;
+    const size_t tab_elems = ragged_table_elems(nq, 0);
+    uint64_t *tab, *cand, *out;
+    float *scores;
+    const auto layout = [&](void *base) {
+        BatchScratch sc(base);
+        tab = sc.take<uint64_t>(tab_elems);
+        scores = sc.take<float>(rc.total);
+        cand = sc.take<uint64_t>((size_t)nq * parts * 8 * chunk); // 8 lists (one per warp) per select CTA
+        out = sc.take<uint64_t>(nq * k);
+        return sc.words();
+    };
+    if (!c->need_cand(layout(nullptr))) return -1;
+    layout(c->d_cand);
+    cudaStream_t st = s ? s : cudaStreamLegacy; // NULL = the legacy default stream, as everywhere in CUDA
+    RaggedBatch b;
+    bool ok = true;
+    if (!upload_ragged_table(tab, d_doc_ids, d_counts, caps, nq32, {}, st, b, ok)) return -1;
     LaunchCounters lc;
-    ok = ok && launch_gather_ragged(view(), d_q, query_pitch(), b, tab + 3 * nq + 1, blocks, d_label_to_id_, (uint32_t)l2i_size_,
+    ok = ok && launch_gather_ragged(view(), d_q, query_pitch(), b, tab + 3 * nq + 1, rc.blocks, d_label_to_id_, (uint32_t)l2i_size_,
                                     multi_ ? d_label_rows_ : nullptr, scores, st, &lc) == cudaSuccess;
     ok = ok && launch_topk_ragged(b, scores, (uint32_t)k, parts, cand, out, st, &lc) == cudaSuccess;
     ok = ok && launch_unpack_ragged(b, out, (uint32_t)k, d_labels, d_scores, d_counts_out, st, &lc) == cudaSuccess;
@@ -2251,14 +2281,8 @@ int FlatIndex::hybrid_topk_batch_device(const void *d_q, size_t nq, size_t k, co
     last_mode_ = HYBRID_ADHOC_BF;
     if (nq == 0 || k == 0) return 0;
     if (k > (size_t)kMaxWideK || nq > 0x7FFFFFFFull) return -1;
-    size_t total = 0, max_cap = 0;
-    uint64_t blocks = 0;
-    for (size_t i = 0; i < nq; i++) {
-        if (caps[i] > 0xFFFFFFF0ull) return -2;
-        total += caps[i];
-        max_cap = std::max(max_cap, caps[i]);
-        blocks += ragged_blocks(caps[i]);
-    }
+    const RaggedCaps rc = scan_caps(caps, nq);
+    if (!rc.ok) return -2;
     if (!flush()) return -1;
     if (!sync_label_table()) return -2;
     const size_t n = count_;
@@ -2286,10 +2310,7 @@ int FlatIndex::hybrid_topk_batch_device(const void *d_q, size_t nq, size_t k, co
         // a subset below the batch route's own 16 queries does not pay for a first shadow build
         if (dense_q.size() < 16 && !d_shadow_) dense_q.clear();
         if (!dense_q.empty() && !ensure_shadow(st)) dense_q.clear();
-        if (!dense_q.empty() && !unit && !(shadow_max_abs_ <= 60000.0f)) {
-            dense_q.clear();
-            disable_coarse(); // values outside the fp16 range (or NaN): exact scans from now on, as batch_scan_rows
-        }
+        if (!dense_q.empty() && !shadow_values_in_range()) dense_q.clear();
         if (!dense_q.empty() && !sync_labels_to_device()) return -1;
     }
     const uint32_t nd = (uint32_t)dense_q.size();
@@ -2297,39 +2318,38 @@ int FlatIndex::hybrid_topk_batch_device(const void *d_q, size_t nq, size_t k, co
         for (uint32_t p : dense_q) out_modes[p] = HYBRID_BATCHES;
     last_mode_ = nd ? HYBRID_BATCHES : HYBRID_ADHOC_BF;
     const uint32_t chunk = (uint32_t)std::min<size_t>(k, kMaxFusedK);
-    const uint32_t parts = plan_ragged_select_parts(max_cap, nq32);
+    const uint32_t parts = plan_ragged_select_parts(rc.max_cap, nq32);
     std::lock_guard<std::mutex> dg(dev_mu_);
     if (!dev_ctx_) dev_ctx_ = checkout();
     QueryCtx *c = dev_ctx_.get();
     if (!c) return -1;
     // dense-route plans (positions 0 .. nd - 1 = the dense queries in batch order)
-    const bool wide = ke > kCoarseMaxK, tier2 = coarse_tier2_enabled();
-    CoarsePlan cp{}, cps{}, cp2{};
+    KnnTiers t;
     const uint32_t words = (uint32_t)((n + 31) / 32);
     if (nd) {
-        cp = plan_coarse(v, nd, CoarseF16, ke, 0, 1, 1, true);
         // the sample must hold a few times k FILTERED rows: at the smallest filtered fraction among the dense queries it visits
         // tiles_per_k / f times the tiles of the unfiltered route (caps bound the counts from above: a low count only costs time)
         double fmin = 1.0;
         for (uint32_t q : dense_q) fmin = std::min(fmin, std::max((double)caps[q] / (double)n, 1e-9));
-        const double tpk = hybrid_tiles_per_k(ke) / fmin;
-        cps = wide ? plan_coarse(v, nd, CoarseF16, ke, kCoarseKeepWide, sample_stride(cp, ke, 128.0, tpk), 0)
-                   : plan_coarse(v, nd, CoarseF16, ke, 0, sample_stride(cp, ke, 24.0, tpk), 2);
-        if (tier2) cp2 = plan_coarse(v, nd, CoarseF16, ke, kCoarseKeepWide);
+        t = plan_knn_tiers(v, nd, CoarseF16, ke, ke > kCoarseMaxK ? 128.0 : 24.0, hybrid_tiles_per_k(ke) / fmin, true);
     }
-    const size_t qpitch = query_pitch(), q16_pitch = (dim_ * 2 + 15) & ~(size_t)15;
-    // pinned table: [docId pointers nq][count pointers nq][score offsets nq + 1][first chunks nq + 1], then u32 words:
-    // [dense queries nd][dense count 1][dense position of each query nq]
-    const size_t tab_elems = 4 * nq + 2 + (nd + 1 + nq + 1) / 2;
-    uint64_t *tab, *cand, *out, *cand_m, *cand_s, *cand_t2, *out_d, *list_scratch;
-    float *scores, *d_qn2, *d_qn2_t2, *d_thr;
-    uint8_t *q32, *q16, *q16_t2;
-    uint32_t *bm, *d_ok_d, *d_idx, *d_n2, *d_ovf, *d_flags, *d_live;
+    const size_t qpitch = query_pitch();
+    // u32 words after the pinned table: [dense queries nd][dense count 1][dense position of each query nq]
+    std::vector<uint32_t> tail(dense_q);
+    tail.push_back(nd);
+    tail.resize(nd + 1 + nq, 0xFFFFFFFFu);
+    for (uint32_t p = 0; p < nd; p++) tail[nd + 1 + dense_q[p]] = p;
+    const size_t tab_elems = ragged_table_elems(nq, tail.size());
+    uint64_t *tab, *cand, *out, *out_d;
+    float *scores;
+    uint8_t *q32;
+    uint32_t *bm, *d_flags, *d_live;
     const uint32_t **d_live_ptr;
+    KnnScratch ks;
     const auto layout = [&](void *base) {
         BatchScratch sc(base);
         tab = sc.take<uint64_t>(tab_elems);
-        scores = sc.take<float>(total);
+        scores = sc.take<float>(rc.total);
         cand = sc.take<uint64_t>((size_t)nq * parts * 8 * chunk); // 8 lists (one per warp) per select CTA
         out = sc.take<uint64_t>(nq * k);
         d_flags = sc.take<uint32_t>(nq);
@@ -2337,85 +2357,32 @@ int FlatIndex::hybrid_topk_batch_device(const void *d_q, size_t nq, size_t k, co
         d_live_ptr = sc.take<const uint32_t *>(nd ? nq : 0);
         bm = sc.take<uint32_t>((size_t)nd * words);
         q32 = sc.take<uint8_t>((size_t)nd * qpitch);
-        q16 = sc.take<uint8_t>((size_t)nd * q16_pitch);
-        q16_t2 = sc.take<uint8_t>(tier2 ? (size_t)nd * q16_pitch : 0);
-        cand_m = sc.take<uint64_t>((size_t)nd * cp.grid_x * cp.keep);
-        cand_s = sc.take<uint64_t>((size_t)nd * cps.grid_x * cps.keep);
-        cand_t2 = sc.take<uint64_t>(tier2 ? (size_t)nd * cp2.grid_x * cp2.keep : 0);
-        list_scratch = sc.take<uint64_t>(std::max(std::max(cp.scratch_elems, cps.scratch_elems), cp2.scratch_elems));
+        ks.take(sc, t, nd, f16_query_pitch(), !unit, false);
         out_d = sc.take<uint64_t>((size_t)nd * ke);
-        d_qn2 = sc.take<float>(unit ? 0 : nd);
-        d_qn2_t2 = sc.take<float>(unit || !tier2 ? 0 : nd);
-        d_ok_d = sc.take<uint32_t>(nd);
-        d_idx = sc.take<uint32_t>(nd);
-        d_n2 = sc.take<uint32_t>(nd ? 1 : 0);
-        d_thr = sc.take<float>(nd);
-        d_ovf = sc.take<uint32_t>(nd);
         return sc.words();
     };
     if (!c->need_cand(layout(nullptr))) return -1;
     layout(c->d_cand);
-    TableSlot *slot = table_slot(tab_elems);
-    if (!slot) return -1;
-    uint64_t *h = slot->h, off = 0, blk = 0;
-    for (size_t i = 0; i < nq; i++) {
-        h[i] = (uint64_t)(uintptr_t)d_doc_ids[i];
-        h[nq + i] = d_counts ? (uint64_t)(uintptr_t)d_counts[i] : 0;
-        h[2 * nq + i] = off;
-        h[3 * nq + 1 + i] = blk;
-        off += caps[i];
-        blk += ragged_blocks(caps[i]);
-    }
-    h[3 * nq] = off;
-    h[4 * nq + 1] = blk;
-    uint32_t *h32 = reinterpret_cast<uint32_t *>(h + 4 * nq + 2);
-    for (uint32_t p = 0; p < nd; p++) h32[p] = dense_q[p];
-    h32[nd] = nd;
-    for (size_t i = 0; i < nq; i++) h32[nd + 1 + i] = 0xFFFFFFFFu;
-    for (uint32_t p = 0; p < nd; p++) h32[nd + 1 + dense_q[p]] = p;
+    RaggedBatch b;
+    bool ok = true;
+    if (!upload_ragged_table(tab, d_doc_ids, d_counts, caps, nq32, tail, st, b, ok)) return -1;
     const uint32_t *d_dense_q = reinterpret_cast<const uint32_t *>(tab + 4 * nq + 2), *d_nd = d_dense_q + nd, *d_pos = d_nd + 1;
-    bool ok = cudaMemcpyAsync(tab, h, tab_elems * 8, cudaMemcpyHostToDevice, st) == cudaSuccess;
-    ok = ok && cudaEventRecord(slot->ev, st) == cudaSuccess;
-    const RaggedBatch b{reinterpret_cast<const uint32_t *const *>(tab), reinterpret_cast<const uint32_t *const *>(tab + nq), tab + 2 * nq, nq32};
     LaunchCounters lc;
     DenseRows dr;
     RaggedBatch bg = b; // the gather's batch: every query, or (dense route) the open ones
     if (nd) {
         // 1. row-space filter bitmaps of the dense queries; their queries packed to the front (fp32 for the rescoring, fp16 for the GEMM)
         ok = ok && cudaMemsetAsync(bm, 0, (size_t)nd * words * 4, st) == cudaSuccess;
-        ok = ok && launch_filter_bitmaps(b, d_dense_q, nd, max_cap, d_label_to_id_, (uint32_t)l2i_size_, bm, words, st, &lc) == cudaSuccess;
+        ok = ok && launch_filter_bitmaps(b, d_dense_q, nd, rc.max_cap, d_label_to_id_, (uint32_t)l2i_size_, bm, words, st, &lc) == cudaSuccess;
         ok = ok && launch_gather_queries(d_q, qpitch, nullptr, d_dense_q, d_nd, nd, q32, nullptr, st) == cudaSuccess;
-        ok = ok && launch_to_f16(q32, qpitch, (uint32_t)dim_, 0, nd, q16, q16_pitch, st) == cudaSuccess;
-        if (!unit) ok = ok && launch_row_stats(q32, qpitch, (uint32_t)dim_, 0, nd, d_qn2, nullptr, st) == cudaSuccess;
-        lc.launches += unit ? 2 : 3;
-        const CoarseOperands ops{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
-        const float eps = coarse_eps(CoarseF16);
-        const int l2 = mkind_ == MT_L2 ? 1 : 0;
-        // 2. sample pass over the filtered rows and the bound; 3. main pass; 4. exact rescoring + proof, selected by (distance, docId)
-        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nd, cps, cand_s, list_scratch, st, nullptr, nullptr, nullptr, bm, words) == cudaSuccess;
-        ok = ok && launch_threshold(cand_s, nd, cps.grid_x, cps.keep, ke, eps, d_qn2, shadow_max_norm_, (uint32_t)dim_, l2, d_thr, d_ovf, st) ==
-                       cudaSuccess;
-        cudaEventRecord(c->ev_start, st);
-        ok = ok && launch_coarse(ops, v.n_rows, v.dim, nd, cp, cand_m, list_scratch, st, nullptr, d_thr, d_ovf, bm, words) == cudaSuccess;
-        cudaEventRecord(c->ev_stop, st);
-        ok = ok && launch_refine(v, q32, qpitch, nd, cp.grid_x, cp.keep, ke, cand_m, eps, d_qn2, shadow_max_norm_, d_ok_d, out_d, nullptr, nullptr, st,
-                                 d_thr, d_ovf, d_id_to_label_) == cudaSuccess;
-        lc.launches += 4;
+        lc.launches++;
+        CoarseOperands ops{};
+        ok = ok && shadow_operands(q32, qpitch, nd, ks.q, ks.qn2, st, lc, ops);
+        // 2. sample pass over the filtered rows and the bound; 3. main pass; 4. exact rescoring + proof, selected by (distance, docId);
         // 5. second tier for the queries whose lists overflowed: adaptive lists of 128 over the filtered rows
-        if (tier2) {
-            ok = ok && launch_compact_unproven(d_ok_d, nd, d_idx, d_n2, st) == cudaSuccess;
-            ok = ok && launch_gather_queries(q16, q16_pitch, d_qn2, d_idx, d_n2, nd, q16_t2, d_qn2_t2, st) == cudaSuccess;
-            CoarseOperands ops2 = ops;
-            ops2.queries = q16_t2;
-            ops2.q_norm2 = d_qn2_t2;
-            ok = ok && launch_coarse(ops2, v.n_rows, v.dim, nd, cp2, cand_t2, list_scratch, st, d_n2, nullptr, nullptr, bm, words, d_idx) ==
-                           cudaSuccess;
-            ok = ok && launch_refine(v, q32, qpitch, nd, cp2.grid_x, cp2.keep, ke, cand_t2, eps, d_qn2_t2, shadow_max_norm_, d_ok_d, out_d, d_idx,
-                                     d_n2, st, nullptr, nullptr, d_id_to_label_) == cudaSuccess;
-            lc.launches += 4;
-        }
+        ok = ok && enqueue_knn_tiers(*c, v, CoarseF16, t, ks, ops, q32, qpitch, nd, ke, out_d, bm, words, d_id_to_label_, st, lc);
         // 6. the gather answers the ad-hoc queries and the dense ones still open; a proven query's count is 0
-        ok = ok && launch_hybrid_open(b, d_pos, d_ok_d, d_flags, d_live, d_live_ptr, st, &lc) == cudaSuccess;
+        ok = ok && launch_hybrid_open(b, d_pos, ks.ok, d_flags, d_live, d_live_ptr, st, &lc) == cudaSuccess;
         bg.counts = d_live_ptr;
         dr = DenseRows{out_d, d_pos, d_flags};
     } else {
@@ -2423,7 +2390,7 @@ int FlatIndex::hybrid_topk_batch_device(const void *d_q, size_t nq, size_t k, co
     }
     // with dense queries in the batch most chunks of the caps are empty: a grid of a few CTAs per SM strides over them
     const uint64_t max_grid = nd ? (uint64_t)device_sm_count() * 16 : 0;
-    ok = ok && launch_gather_ragged(v, d_q, qpitch, bg, tab + 3 * nq + 1, blocks, d_label_to_id_, (uint32_t)l2i_size_,
+    ok = ok && launch_gather_ragged(v, d_q, qpitch, bg, tab + 3 * nq + 1, rc.blocks, d_label_to_id_, (uint32_t)l2i_size_,
                                     multi_ ? d_label_rows_ : nullptr, scores, st, &lc, max_grid) == cudaSuccess;
     ok = ok && launch_topk_ragged(bg, scores, (uint32_t)k, parts, cand, out, st, &lc) == cudaSuccess;
     // 7. one unpack: gather rows map positions to docIds, proven dense rows carry them
@@ -2462,14 +2429,8 @@ int FlatIndex::hybrid_range_batch_device(const void *d_q, size_t nq, const float
         for (size_t i = 0; i < nq; i++) out_modes[i] = HYBRID_ADHOC_BF;
     last_mode_ = RANGE_QUERY;
     if (nq == 0) return 0;
-    size_t total = 0, max_cap = 0;
-    uint64_t blocks = 0;
-    for (size_t i = 0; i < nq; i++) {
-        if (caps[i] > 0xFFFFFFF0ull) return -2;
-        total += caps[i];
-        max_cap = std::max(max_cap, caps[i]);
-        blocks += ragged_blocks(caps[i]);
-    }
+    const RaggedCaps rc = scan_caps(caps, nq);
+    if (!rc.ok) return -2;
     if (!flush()) return -1;
     if (!sync_label_table()) return -2;
     if (!sync_labels_to_device()) return -1;
@@ -2486,15 +2447,11 @@ int FlatIndex::hybrid_range_batch_device(const void *d_q, size_t nq, const float
         const bool r32 = dtype_ == DT_F32 && cmode == 1 && !coarse_disabled_ && coarse_supported(v, nq32, 1, CoarseF16) &&
                          (nq >= kHybridRangeMinDense || single_query_takes_coarse(1));
         const double pass_bytes = (double)n * dim_ * (r8 ? 1 : 2); // the 8-bit rows, or the fp16 shadow
-        if ((r8 || r32) && (policy == HYBRID_BATCHES || hybrid_range_dense_pays(total, stored_bytes_, pass_bytes, nq, n))) {
+        if ((r8 || r32) && (policy == HYBRID_BATCHES || hybrid_range_dense_pays(rc.total, stored_bytes_, pass_bytes, nq, n))) {
             if (r8 && (!int_l2() || ensure_shadow(st))) {
                 path = 2;
-            } else if (r32 && ensure_shadow(st)) {
+            } else if (r32 && ensure_shadow(st) && shadow_values_in_range()) {
                 path = 1;
-                if (!unit_rows() && !(shadow_max_abs_ <= 60000.0f)) { // values outside the fp16 range: exact scans from now on
-                    disable_coarse();
-                    path = 0;
-                }
             }
         }
     }
@@ -2505,29 +2462,23 @@ int FlatIndex::hybrid_range_batch_device(const void *d_q, size_t nq, const float
     QueryCtx *c = dev_ctx_.get();
     if (!c) return -1;
     collect_dev_timing_locked();
-    const bool unit = unit_rows();
-    const CoarsePlan cp = path == 1   ? plan_coarse(v, nq32, CoarseF16, 1, 0, 1, 1, true)
-                          : path == 2 ? plan_coarse(v, nq32, CoarseDirect8, 1, 0, 1, 1, true)
-                                      : CoarsePlan{};
-    const size_t slots = (size_t)cp.grid_x * cp.keep, qpitch = query_pitch(), q16_pitch = (dim_ * 2 + 15) & ~(size_t)15;
+    const CoarseKind kind = path == 1 ? CoarseF16 : CoarseDirect8;
+    const CoarsePlan cp = path ? plan_coarse(v, nq32, kind, 1, 0, 1, 1, true) : CoarsePlan{};
+    const size_t qpitch = query_pitch();
     const uint32_t words = path ? (uint32_t)((n + 31) / 32) : 0;
-    // pinned table: [docId pointers nq][count pointers nq][score offsets nq + 1][first chunks nq + 1], then u32 [nq] = 0, 1, ..:
-    // a dense route runs over the whole batch, so its positions are the queries themselves
-    const size_t tab_elems = 4 * nq + 2 + (nq + 1) / 2;
-    uint64_t *tab, *cand, *list_scratch;
-    uint8_t *q16;
-    float *d_qn2, *d_thr;
-    uint32_t *d_ovf, *d_total, *d_ok, *d_flags, *d_live, *bm;
+    // u32 words after the pinned table: 0, 1, .. nq - 1.  A dense route runs over the whole batch, so its positions are the queries
+    // themselves
+    std::vector<uint32_t> iota(nq);
+    for (uint32_t i = 0; i < nq32; i++) iota[i] = i;
+    const size_t tab_elems = ragged_table_elems(nq, nq);
+    uint64_t *tab;
+    uint32_t *d_total, *d_ok, *d_flags, *d_live, *bm;
     const uint32_t **d_live_ptr;
+    RangeScratch rs;
     const auto layout = [&](void *base) {
         BatchScratch sc(base);
         tab = sc.take<uint64_t>(tab_elems);
-        cand = sc.take<uint64_t>(path ? nq * slots : 0);
-        list_scratch = sc.take<uint64_t>(path ? cp.scratch_elems : 0);
-        q16 = sc.take<uint8_t>(path == 1 ? nq * q16_pitch : 0);
-        d_qn2 = sc.take<float>((path == 1 && !unit) || (path == 2 && int_l2()) ? nq : 0); // |q|^2 (fp32), or int32 for 8-bit L2
-        d_thr = sc.take<float>(path == 1 ? nq : 0);
-        d_ovf = sc.take<uint32_t>(path ? nq : 0);
+        if (path) rs.take(sc, *this, kind, cp, nq32, false);
         d_total = sc.take<uint32_t>(1);
         d_ok = sc.take<uint32_t>(path ? nq : 0); // the route proved the query
         d_flags = sc.take<uint32_t>(nq);         // LastCoarseFlags
@@ -2538,60 +2489,20 @@ int FlatIndex::hybrid_range_batch_device(const void *d_q, size_t nq, const float
     };
     if (!c->need_cand(layout(nullptr))) return -1;
     layout(c->d_cand);
-    TableSlot *slot = table_slot(tab_elems);
-    if (!slot) return -1;
-    uint64_t *h = slot->h, off = 0, blk = 0;
-    for (size_t i = 0; i < nq; i++) {
-        h[i] = (uint64_t)(uintptr_t)d_doc_ids[i];
-        h[nq + i] = d_counts ? (uint64_t)(uintptr_t)d_counts[i] : 0;
-        h[2 * nq + i] = off;
-        h[3 * nq + 1 + i] = blk;
-        off += caps[i];
-        blk += ragged_blocks(caps[i]);
-    }
-    h[3 * nq] = off;
-    h[4 * nq + 1] = blk;
-    uint32_t *h32 = reinterpret_cast<uint32_t *>(h + 4 * nq + 2);
-    for (uint32_t i = 0; i < nq32; i++) h32[i] = i;
+    RaggedBatch b;
+    bool ok = true;
+    if (!upload_ragged_table(tab, d_doc_ids, d_counts, caps, nq32, iota, st, b, ok)) return -1;
     const uint32_t *d_iota = reinterpret_cast<const uint32_t *>(tab + 4 * nq + 2);
-    bool ok = cudaMemcpyAsync(tab, h, tab_elems * 8, cudaMemcpyHostToDevice, st) == cudaSuccess;
-    ok = ok && cudaEventRecord(slot->ev, st) == cudaSuccess;
     ok = ok && cudaMemsetAsync(d_counts_out, 0, nq * 4, st) == cudaSuccess;
-    const RaggedBatch b{reinterpret_cast<const uint32_t *const *>(tab), reinterpret_cast<const uint32_t *const *>(tab + nq), tab + 2 * nq, nq32};
     RaggedBatch bg = b; // the gather's batch: every query, or (dense route) the open ones
     LaunchCounters lc;
     uint64_t *comp = reinterpret_cast<uint64_t *>(d_labels);
     if (path) {
         // 1. row-space filter bitmaps; 2. range_device's route over the whole batch with them; 3. the open queries to the gather
         ok = ok && cudaMemsetAsync(bm, 0, (size_t)nq * words * 4, st) == cudaSuccess;
-        ok = ok && launch_filter_bitmaps(b, d_iota, nq32, max_cap, d_label_to_id_, (uint32_t)l2i_size_, bm, words, st, &lc) == cudaSuccess;
-        if (path == 1) {
-            ok = ok && launch_to_f16(d_q, qpitch, (uint32_t)dim_, 0, nq32, q16, q16_pitch, st) == cudaSuccess;
-            if (!unit) ok = ok && launch_row_stats(d_q, qpitch, (uint32_t)dim_, 0, nq32, d_qn2, nullptr, st) == cudaSuccess;
-            ok = ok && launch_range_bound(d_radii, nq32, kCoarseEpsF16, d_qn2, shadow_max_norm_, (uint32_t)dim_, mkind_ == MT_L2 ? 1 : 0, d_thr, d_ovf,
-                                          d_total, st) == cudaSuccess;
-            const CoarseOperands ops{d_shadow_, 0, q16, q16_pitch, 0, mkind_ == MT_L2 ? 1 : 0, d_norm2_, d_qn2};
-            cudaEventRecord(c->ev_start, st);
-            ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_thr, d_ovf, bm, words) == cudaSuccess;
-            cudaEventRecord(c->ev_stop, st);
-            ok = ok && launch_range_refine(v, d_q, qpitch, nq32, (uint32_t)slots, cand, d_radii, d_qn2, d_thr, d_ovf, comp, d_total, d_ok,
-                                           d_counts_out, nullptr, st, cap32) == cudaSuccess;
-            lc.launches += unit ? 4 : 5;
-        } else {
-            CoarseOperands ops{v.rows, v.pitch, d_q, qpitch, dtype_ == DT_I8 ? 1 : 0, mkind_ == MT_COS ? 1 : int_l2() ? 2 : 0, nullptr, nullptr};
-            ok = ok && cudaMemsetAsync(d_ovf, 0, nq * 4, st) == cudaSuccess;
-            if (int_l2()) {
-                ok = ok && launch_int_norm2(d_q, qpitch, v.dim, 0, nq32, dtype_ == DT_I8, reinterpret_cast<int32_t *>(d_qn2), st) == cudaSuccess;
-                ops.row_norm2 = reinterpret_cast<const float *>(d_norm2_); // int32 values (CoarseOperands)
-                ops.q_norm2 = d_qn2;
-                lc.launches++;
-            }
-            cudaEventRecord(c->ev_start, st);
-            ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq32, cp, cand, list_scratch, st, nullptr, d_radii, d_ovf, bm, words) == cudaSuccess;
-            cudaEventRecord(c->ev_stop, st);
-            ok = ok && launch_range_pack(cand, nq32, (uint32_t)slots, d_ovf, cap32, comp, d_counts_out, d_ok, st) == cudaSuccess;
-            lc.launches += 2;
-        }
+        ok = ok && launch_filter_bitmaps(b, d_iota, nq32, rc.max_cap, d_label_to_id_, (uint32_t)l2i_size_, bm, words, st, &lc) == cudaSuccess;
+        ok = ok && enqueue_range_route(*c, v, kind, cp, rs, d_q, qpitch, nq32, d_radii, bm, words,
+                                       RangeOut{comp, cap32, d_ok, d_counts_out, nullptr, d_total, nullptr}, st, lc);
         ok = ok && launch_hybrid_open(b, d_iota, d_ok, d_flags, d_live, d_live_ptr, st, &lc) == cudaSuccess;
         bg.counts = d_live_ptr;
     } else {
@@ -2599,7 +2510,7 @@ int FlatIndex::hybrid_range_batch_device(const void *d_q, size_t nq, const float
     }
     // after a dense route most chunks of the caps are empty: a grid of a few CTAs per SM strides over them
     const uint64_t max_grid = path ? (uint64_t)device_sm_count() * 16 : 0;
-    ok = ok && launch_gather_ragged_range(v, d_q, qpitch, bg, tab + 3 * nq + 1, blocks, d_label_to_id_, (uint32_t)l2i_size_,
+    ok = ok && launch_gather_ragged_range(v, d_q, qpitch, bg, tab + 3 * nq + 1, rc.blocks, d_label_to_id_, (uint32_t)l2i_size_,
                                           multi_ ? d_label_rows_ : nullptr, d_radii, cap32, comp, d_counts_out, st, &lc, max_grid) == cudaSuccess;
     ok = ok && launch_range_finish(d_labels, d_scores, d_counts_out, nq32, cap32, d_id_to_label_, order == BY_ID, st, &lc) == cudaSuccess;
     c->d_last_ok = d_flags;

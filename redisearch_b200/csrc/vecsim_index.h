@@ -7,6 +7,7 @@
 //   VS/algorithms/brute_force/bf_batch_iterator.h      (batch iterator state machine)
 #pragma once
 #include "../../include/vecsim_b200.h"
+#include "coarse_tc.h"
 #include "vecsim_kernels.h"
 
 #include <atomic>
@@ -39,6 +40,8 @@ struct VecSimDebugInfoIterator {
 };
 
 namespace rsb200 {
+
+class BatchScratch;
 
 struct Globals {
     std::atomic<timeoutCallbackFunction> timeout_cb{nullptr};
@@ -224,6 +227,7 @@ class FlatIndex {
     // kMaxFusedK; returns the number found or -1.
     long select_from_scores(QueryCtx &c, uint32_t n, bool has_cursor, uint64_t cursor, size_t want);
     size_t query_pitch() const { return (stored_bytes_ + 15) & ~(size_t)15; } // bytes between staged queries
+    size_t f16_query_pitch() const { return (dim_ * 2 + 15) & ~(size_t)15; } // bytes between the fp16 forms of fp32 queries
     // nq query blobs, `stride` bytes apart -> c.d_query, query_pitch() apart and zero-padded, then `tail_bytes` of `tail`.  raw:
     // the blobs are put in stored form (preprocess_query); else they are in stored form already
     bool stage_queries(QueryCtx &c, const void *blobs, size_t stride, size_t nq, bool raw, const void *tail = nullptr, size_t tail_bytes = 0);
@@ -236,6 +240,69 @@ class FlatIndex {
     // multi-value index: the first kl distinct labels per query (DESIGN.md §4.4); needs d_id_to_label_ in sync
     bool batch_scan_labels(QueryCtx &c, const void *d_q, size_t qpitch, uint32_t nq, uint32_t kl, cudaStream_t st, LaunchCounters &lc,
                            uint64_t **d_result, bool host_fallback = false);
+
+    // fp32 queries -> the operands of a pass over the fp16 shadow: their fp16 form in q16 (f16_query_pitch() apart) and, where d_qn2
+    // is not NULL (rows not all unit), |q|^2 in d_qn2
+    bool shadow_operands(const void *d_q, size_t qpitch, uint32_t nq, uint8_t *q16, float *d_qn2, cudaStream_t st, LaunchCounters &lc,
+                         CoarseOperands &ops);
+    // the operands of a pass over 8-bit rows; int8 / uint8 L2: the exact int32 |q|^2 into d_qn and the |row|^2 table (ensure_shadow)
+    bool direct8_operands(const void *d_q, size_t qpitch, uint32_t nq, int32_t *d_qn, cudaStream_t st, LaunchCounters &lc, CoarseOperands &ops);
+    // false when the fp32 rows hold values outside the fp16 range (or NaN): the index stays on the exact scans from now on
+    bool shadow_values_in_range();
+
+    // The fixed-bound range route (DESIGN.md §4.11) of one batch, over the fp16 shadow (CoarseF16), the stored 16-bit rows
+    // (CoarseDirect16) or the 8-bit rows (CoarseDirect8).  Its scratch is carved from the caller's batch layout by take().
+    struct RangeScratch {
+        uint64_t *cand = nullptr, *list_scratch = nullptr;
+        uint8_t *q16 = nullptr;
+        float *qn2 = nullptr, *thr = nullptr;
+        uint32_t *ovf = nullptr, *front = nullptr;
+        void take(BatchScratch &s, const FlatIndex &ix, CoarseKind kind, const CoarsePlan &cp, uint32_t nq, bool fold);
+    };
+    // Where the route writes its answers.  flags == NULL: the proven hits of query q, rows as (score key, row) composites, go to
+    // hits[q * cap, ...) with cnt[q] = their number (cap != 0), or packed at hits[off[q], ...) with *total = their sum (cap == 0;
+    // CoarseF16 only); ok[q] = 1 for a proven query.  flags != NULL (multi-value index): the label fold of launch_range_label_fold
+    // into hits[q * cap, ...), with LastCoarseFlags in flags.
+    struct RangeOut {
+        uint64_t *hits;
+        uint32_t cap;
+        uint32_t *ok, *cnt, *off, *total, *flags;
+    };
+    // the route's query operands, bound, main pass (timed by c's events) and rescoring or packing; bm / words (nullable): filter
+    // bitmaps of the batch's queries
+    bool enqueue_range_route(QueryCtx &c, const CorpusView &v, CoarseKind kind, const CoarsePlan &cp, const RangeScratch &r, const void *d_q,
+                             size_t qpitch, uint32_t nq, const float *d_radii, const uint32_t *bm, uint32_t words, const RangeOut &out,
+                             cudaStream_t st, LaunchCounters &lc);
+
+    // The plans of the shadow KNN tier chain (DESIGN.md §4.2, §4.5): the main pass (a fixed-bound pass after a sample pass when
+    // two_pass, else adaptive lists) and the second tier for the queries the first proof left open.
+    struct KnnTiers {
+        CoarsePlan main{}, sample{}, second{};
+        bool two_pass = false, tier2 = false;
+    };
+    // aim / tiles_per_k: the sample pass's stride (sample_stride); filt: the main pass runs with row filters
+    static KnnTiers plan_knn_tiers(const CorpusView &v, uint32_t nq, CoarseKind kind, uint32_t ke, double aim, double tiles_per_k, bool filt);
+    struct KnnScratch {
+        uint64_t *cand = nullptr, *cand_s = nullptr, *cand_t2 = nullptr, *list_scratch = nullptr;
+        uint8_t *q = nullptr, *q_t2 = nullptr; // the queries in the operand type of the copy, and tier 2's open ones
+        float *qn2 = nullptr, *qn2_t2 = nullptr, *qeps = nullptr, *qeps_t2 = nullptr, *thr = nullptr;
+        uint32_t *ok = nullptr, *idx = nullptr, *n2 = nullptr, *ovf = nullptr;
+        // q_pitch: bytes per operand query row; norms: |q|^2 per query (rows not all unit); q8: the int8 copy's eps per query
+        void take(BatchScratch &s, const KnnTiers &t, uint32_t nq, size_t q_pitch, bool norms, bool q8);
+    };
+    // sample pass, bound, main pass (timed by c's events), exact rescoring + proof into out [nq][ke] and ok, then the second tier.
+    // ops: the first tier's operands over the copy (their queries and |q|^2 in s); d_q32: the fp32 queries the rescoring reads.
+    // bm / words / row_label (nullable): filter bitmaps of the queries and the docId of each row (answers carry it, ties resolve by it)
+    bool enqueue_knn_tiers(QueryCtx &c, const CorpusView &v, CoarseKind kind, const KnnTiers &t, const KnnScratch &s, const CoarseOperands &ops,
+                           const void *d_q32, size_t qpitch, uint32_t nq, uint32_t ke, uint64_t *out, const uint32_t *bm, uint32_t words,
+                           const uint64_t *row_label, cudaStream_t st, LaunchCounters &lc);
+
+    // [docId pointers nq][count pointers nq][score offsets nq + 1][first chunks nq + 1], then the caller's u32 words `tail`: filled in a
+    // pinned table slot and uploaded to d_tab (ragged_table_elems(nq, tail.size()) words) on st.  False when no slot can be had;
+    // ok &= the upload was enqueued
+    static size_t ragged_table_elems(size_t nq, size_t tail_words) { return 4 * nq + 2 + (tail_words + 1) / 2; }
+    bool upload_ragged_table(uint64_t *d_tab, const uint32_t *const *d_doc_ids, const uint32_t *const *d_counts, const size_t *caps, uint32_t nq,
+                             const std::vector<uint32_t> &tail, cudaStream_t st, RaggedBatch &b, bool &ok);
     void finish_reply(VecSimQueryReply *rep, VecSimQueryReply_Order order) const;
 
     DType dtype_;
