@@ -588,17 +588,20 @@ constexpr int kQAccStride = kQN + 4;                            // accumulator t
 constexpr uint32_t kQAccBytes = kQM * kQAccStride * 4;
 // The fixed-bound pass (mode 1) runs two consumer warpgroups that take the CTA's tiles alternately: one warpgroup's
 // drain and bound test run under the other's MMAs instead of leaving the tensor pipe idle at every tile boundary
-// (DESIGN.md §4.2: 5,022 -> 4,294 clk per tile at 10M x 768).  The other modes keep one: their epilogue transposes
-// through shared memory and compacts lists, which a second warpgroup would have to double.
-__host__ __device__ constexpr int coarse_consumers(int mode) { return mode == 1 ? 2 : 1; }
-// Queries per CTA.  The fixed-bound pass over the int8 shadow (kOp 5, mode 1) holds 128: each consumer warpgroup owns 64 of
-// them and both run their MMAs against every ring stage, so a row tile is copied into shared memory once per 128 queries
-// instead of once per 64 (384 instead of 480 KB of shared-memory traffic per 128 queries x 128 rows, DESIGN.md §4.2), and
-// at a batch of 256 the two query groups of a row range form clusters of two, which fill all the SMs.  Its int8 queries
-// take 128 B per K block and query, so 128 of them leave at least three ring stages up to 1024 dimensions
-__host__ __device__ constexpr int coarse_cta_queries(bool q8, int mode) { return q8 && mode == 1 ? 2 * kQM : kQM; }
+// (DESIGN.md §4.2: 5,022 -> 4,294 clk per tile at 10M x 768).  The sample pass over the int8 shadow (kOp 5, mode 2) runs
+// two as well, on the wide CTA below: its epilogue reads the accumulator fragment too.  The other modes keep one: their
+// epilogue transposes through shared memory and compacts lists, which a second warpgroup would have to double.
+// The passes whose epilogue works on the accumulator fragment in registers (no transpose buffer)
+__host__ __device__ constexpr bool coarse_frag_epilogue(bool q8, int mode) { return mode == 1 || (q8 && mode == 2); }
+__host__ __device__ constexpr int coarse_consumers(bool q8, int mode) { return coarse_frag_epilogue(q8, mode) ? 2 : 1; }
+// Queries per CTA.  The fixed-bound and sample passes over the int8 shadow (kOp 5, modes 1 and 2) hold 128: each consumer
+// warpgroup owns 64 of them and both run their MMAs against every ring stage, so a row tile is copied into shared memory once
+// per 128 queries instead of once per 64 (384 instead of 480 KB of shared-memory traffic per 128 queries x 128 rows, DESIGN.md
+// §4.2), and at a batch of 256 the two query groups of a row range form clusters of two, which fill all the SMs.  Its int8
+// queries take 128 B per K block and query, so 128 of them leave at least three ring stages up to 1024 dimensions
+__host__ __device__ constexpr int coarse_cta_queries(bool q8, int mode) { return q8 && (mode == 1 || mode == 2) ? 2 * kQM : kQM; }
 // warp 0 produces, warps 1-3 idle, warps 4.. are the consumer warpgroups
-__host__ __device__ constexpr int coarse_threads(int mode) { return 128 * (1 + coarse_consumers(mode)); }
+__host__ __device__ constexpr int coarse_threads(bool q8, int mode) { return 128 * (1 + coarse_consumers(q8, mode)); }
 
 // bar.sync / bar.arrive on a named barrier (ids 1-3 in coarse_wgmma_kernel; 0 is __syncthreads)
 template <int kId, int kCount>
@@ -765,11 +768,16 @@ __device__ __forceinline__ int q8_dot_bound(float tdot, float rq, float rt) {
 //            a list that runs full sets overflow[q] (the query goes to the next tier).  fp32 route (kOp 0 / 3) and 16-bit
 //            corpora.  8-bit corpora (kOp 1 / 2 / 4): thr_fixed[q] is the radius of a range query and a row is kept iff its
 //            exact float distance d satisfies d <= thr_fixed[q] (range_int_bound for the pre-tests, DESIGN.md §4.11).
-//   kSample  the sample pass: no lists at all — every thread keeps the smallest approximate distance it has seen in each of
-//            8 interleaved slices of its row range (chunk of the tile x tile parity) and publishes those 8 values as
-//            keep = 8 composites per (query, row range).  The k-th smallest of a query's lists x 8 minima is an upper
-//            bound of its k-th best distance over the sample (k distinct rows are at or below it), which is all the
-//            fixed bound needs.
+//            list_count (nullable): list_count[q][blockIdx.x] = the entries of the published list (min(appends, keep)).
+//            The int8 shadow's pass (kOp 5) needs it and publishes only those entries, without the kEmptySlot padding:
+//            refine_kernel, its one reader, reads the counts.  Every other fixed pass pads its lists.
+//   kSample  the sample pass: no lists at all — per (query, row range) the smallest approximate distance of each of
+//            kCoarseSampleSlices = 32 disjoint slices of the range's sampled rows (32-row chunk of the tile x tile counter
+//            mod 8), published as keep = 32 composites.  Over the int8 shadow the slices follow the accumulator fragment
+//            instead: row 8 j + 2 (lane % 4) + c of the tile falls in slice (lane % 4, c, tile counter mod 4), so that every
+//            thread keeps its minima in registers.  Each minimum is the approximate distance of a distinct sampled row, so
+//            the k-th smallest of a query's lists x 32 minima is an upper bound of its k-th best distance over the sample (k
+//            distinct rows are at or below it), which is all the fixed bound needs.
 //   tile_stride > 1: only every tile_stride-th row tile is visited (the sample pass)
 //   kVar     operand type: 16-bit operands 1 = bfloat16 (else IEEE half); 8-bit 1 = int8 (else uint8).  A template parameter so
 //            that the MMA sequence of a stage is one straight run of wgmma instructions (no branch between them)
@@ -788,19 +796,21 @@ __device__ __forceinline__ int q8_dot_bound(float tdot, float rq, float rt) {
 //            which frees kRegKb x 8 KB for the ring (DESIGN.md §4.2).  The first kRegKb / kQKbPerStage stages of a tile take
 //            A from those registers; the MMA sequence in K is unchanged, so every distance is the same.  0 = all in sQ.
 template <bool kDirect, int kEpl, int kOp, int kMode, int kVar = 0, bool kFilt = false, int kRegKb = 0>
-__global__ void __launch_bounds__(coarse_threads(kMode), 1)
+__global__ void __launch_bounds__(coarse_threads(kOp == 5, kMode), 1)
 coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t *__restrict__ shadow, size_t row_pitch,
                     const uint8_t *__restrict__ q16, size_t q16_pitch, const float *__restrict__ row_norm2,
                     const float *__restrict__ q_norm2, uint32_t n_rows, uint32_t nq, uint32_t dim, uint32_t row_bytes,
                     uint32_t num_kb, uint32_t tiles_total, uint32_t keep, uint32_t nstages, uint32_t csize,
                     uint64_t *__restrict__ list_scratch, uint64_t *__restrict__ cand_out, const uint32_t *__restrict__ nq_dev,
                     uint32_t tile_stride, const float *__restrict__ thr_fixed, uint32_t *__restrict__ overflow,
-                    const uint32_t *__restrict__ filt, uint32_t filt_words, const uint32_t *__restrict__ filt_q) {
+                    const uint32_t *__restrict__ filt, uint32_t filt_words, const uint32_t *__restrict__ filt_q,
+                    uint32_t *__restrict__ list_count) {
     constexpr bool kFixed = kMode == 1, kSample = kMode == 2;
     constexpr bool kQ8 = kOp == 5;
     constexpr bool kInt = kOp == 1 || kOp == 2 || kOp == 4 || kQ8;
     constexpr int kOpE = kQ8 ? 0 : kOp; // the epilogue of kOp 5 past the integer bound test is kOp 0's
-    constexpr int kCons = coarse_consumers(kMode), kConsThreads = 128 * kCons;
+    constexpr bool kFrag = coarse_frag_epilogue(kQ8, kMode); // no transpose buffer
+    constexpr int kCons = coarse_consumers(kQ8, kMode), kConsThreads = 128 * kCons;
     // kWide: 128 queries per CTA, warpgroup cw takes the MMAs and the epilogue of queries 64 cw .. 64 cw + 63 of every tile
     constexpr int kCtaQ = coarse_cta_queries(kQ8, kMode);
     constexpr bool kWide = kCtaQ > kQM;
@@ -818,7 +828,11 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                   "register-held queries: the fixed-bound pass over the fp16 shadow, whole stages");
     // kFilt: the row-space bitmap of the query at position `pos` of this batch
     auto filt_row = [&](uint32_t pos) { return filt + (size_t)filt_words * (filt_q ? filt_q[pos] : pos); };
-    constexpr int kSliceSets = (int)kCoarseSampleSlices / (kQN / 32); // tiles i, i + kSliceSets, ... share a slice set
+    // the sample's slices: tiles i, i + kSliceSets, ... share a slice set of 4 chunks of 32 rows per tile.  kFrag: the slices
+    // (lane % 4, c, h) of the accumulator fragment, 4 x 2 x 4 (kSliceSets = 4 is then the number of 32-row chunks h)
+    constexpr int kSliceSets = (int)kCoarseSampleSlices / (kFrag ? 8 : kQN / 32);
+    static_assert(!kSample || kSliceSets * (kFrag ? 8 : kQN / 32) == (int)kCoarseSampleSlices, "whole slice sets");
+    static_assert(!(kSample && kFrag) || kSliceSets == kQN / 32, "kFrag: a slice per 32-row chunk and (lane % 4, c)");
     constexpr int kQListCap = kEpl * 32;
     if (nq_dev) { // second tier: the number of live queries is only known on the device; nothing to do = every CTA leaves
         nq = min(nq, *nq_dev);
@@ -832,8 +846,8 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
     uint8_t *sB = smem;                                                   // nstages x kQKbPerStage x [128 rows x 128B]
     // K blocks kRegKb .. num_kb - 1 x [64 queries x 128B], swizzled; kWide: two such 64-query halves per K block
     uint8_t *sQ = sB + (size_t)nstages * kQStageBytes;
-    uint32_t *sacc = reinterpret_cast<uint32_t *>(sQ + (size_t)(num_kb - kRegKb) * kQKbBytes); // [kQM][kQAccStride]; not kFixed
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sacc + (kFixed ? 0 : kQM * kQAccStride));
+    uint32_t *sacc = reinterpret_cast<uint32_t *>(sQ + (size_t)(num_kb - kRegKb) * kQKbBytes); // [kQM][kQAccStride]; not kFrag
+    uint64_t *bars = reinterpret_cast<uint64_t *>(sacc + (kFrag ? 0 : kQM * kQAccStride));
     uint64_t *full = bars, *empty = bars + kQMaxStages;
     uint32_t *qcount = reinterpret_cast<uint32_t *>(bars + 2 * kQMaxStages); // kFixed: [kCtaQ] appends per query
     // this CTA's candidate lists [kQListCap][kQListStride]
@@ -895,9 +909,11 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                         const uint8_t *src = shadow + ((size_t)tile * num_kb + kb0) * kQBlockBytes;
                         // fixed-bound pass: the same slice of the CTA's next tile into L2, so that its bulk copy waits on L2
                         // rather than HBM.  Only two of the ring's stages can load ahead of the MMAs, which is too little
-                        // to cover HBM latency (DESIGN.md §4.2); one tile ahead is 5.8 MB of L2 at 10M x 768, four thrash it
-                        if constexpr (kFixed) {
-                            if (i + 1 < my_tiles) bulk_prefetch_l2(src + (size_t)gx * num_kb * kQBlockBytes + crank * slice, slice);
+                        // to cover HBM latency (DESIGN.md §4.2); one tile ahead is 5.8 MB of L2 at 10M x 768, four thrash it.
+                        // The int8 sample pass likewise, its next tile tile_stride x gx tiles on
+                        if constexpr (kFixed || (kSample && kFrag)) {
+                            const size_t ahead = (size_t)gx * (kFixed ? 1u : tile_stride) * num_kb * kQBlockBytes;
+                            if (i + 1 < my_tiles) bulk_prefetch_l2(src + ahead + crank * slice, slice);
                         }
                         if (csize > 1) {
                             bulk_load_1d_mc(sB + (size_t)s * kQStageBytes + crank * slice, src + crank * slice, slice, &full[s], cmask);
@@ -1087,7 +1103,7 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
             // kOp 5, fixed bound: the tile's scale s_t, loaded before the MMAs so that the bound test after the drain does not
             // wait for it
             float q8_st = 0.0f;
-            if constexpr (kFixed && kQ8) q8_st = __ldg(row_norm2 + tile);
+            if constexpr (kFrag && kQ8) q8_st = __ldg(row_norm2 + tile);
             float2 rn[(kFixed && kOp == 3) ? kQN / 8 : 1];
             if constexpr (kFixed && kOp == 3) {
 #pragma unroll
@@ -1163,6 +1179,32 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
             release(prev);
             wg_fence_operands(acc);
             // accumulator fragment: acc[4j + 2 i2 + c] = (query 16 ew + lane / 4 + 8 i2, row 8 j + 2 (lane % 4) + c)
+            if constexpr (kSample && kQ8) {
+                // int8 sample pass: for each of its two queries, c and 32-row chunk h, the thread's 4 rows 8 j + 2 (lane % 4) + c
+                // (j = 4 h .. 4 h + 3) of the tile belong to slice (lane % 4, c, h).  The largest accumulator of the four has
+                // their smallest approximate distance 1 - fl(fl(s_q s_t) acc) (int -> float rounding and the product with
+                // s_q s_t >= 0 are monotone), so only that one is converted; smax[h][2 i2 + c] keeps the largest such dot
+                // product of the slice.  Rows past n_rows (zero or stale shadow bytes) never count.
+                const bool tail = tile * kQN + kQN > n_rows;
+#pragma unroll
+                for (int i2 = 0; i2 < 2; i2++) {
+                    const float sqt = __fmul_rn(fsq[i2], q8_st);
+#pragma unroll
+                    for (int c = 0; c < 2; c++)
+#pragma unroll
+                        for (int h = 0; h < kQN / 32; h++) {
+                            int v[4];
+#pragma unroll
+                            for (int u = 0; u < 4; u++) {
+                                const int j = 4 * h + u;
+                                v[u] = (!tail || rbase + 8 * j + c < n_rows) ? (int)acc[4 * j + 2 * i2 + c] : INT_MIN;
+                            }
+                            const int mx = max(__vimax3_s32(v[0], v[1], v[2]), v[3]);
+                            if (mx != INT_MIN) smax[h][2 * i2 + c] = fmaxf(smax[h][2 * i2 + c], __fmul_rn(sqt, __int2float_rn(mx)));
+                        }
+                }
+                continue;
+            }
             if constexpr (kFixed && kQ8) {
                 // int8 shadow: the bound dot > fthr_dot becomes one integer bound per query on this tile's accumulators
                 // (q8_dot_bound); the rare survivors take the float distance and the exact key comparison, as kOp 0
@@ -1523,11 +1565,32 @@ coarse_wgmma_kernel(const __grid_constant__ CUtensorMap map_rows, const uint8_t 
                 if (qq >= nq) break;
                 const uint32_t n = qcount[qs], c = min(n, (uint32_t)kQListCap);
                 uint64_t *dst = cand_out + ((size_t)qq * gx + bx) * keep;
-                for (uint32_t r = lane; r < keep; r += 32) dst[r] = r < c ? lists[r * kQListStride + qs] : kEmptySlot;
+                if constexpr (kQ8) { // the list's entries only: its reader takes their number from list_count
+                    for (uint32_t r = lane; r < c; r += 32) dst[r] = lists[r * kQListStride + qs];
+                } else {
+                    for (uint32_t r = lane; r < keep; r += 32) dst[r] = r < c ? lists[r * kQListStride + qs] : kEmptySlot;
+                }
+                if (lane == 0 && list_count) list_count[(size_t)qq * gx + bx] = c;
                 if (lane == 0 && n > (uint32_t)kQListCap) overflow[qq] = 1u;
             }
         }
-        if constexpr (kSample) { // keep == 8: the slice minima as composites (the row id is not needed by threshold_kernel)
+        if constexpr (kSample && kFrag) {
+            // the slice minima of the fragment's two queries: slice (lane % 4, c, h) at composite 8 (lane % 4) + 4 c + h
+#pragma unroll
+            for (int i2 = 0; i2 < 2; i2++) {
+                const uint32_t fq = qw + 16 * ew + (lane >> 2) + 8 * i2;
+                if (fq >= nq) continue;
+                uint64_t *dst = cand_out + ((size_t)fq * gx + bx) * keep + 8 * (lane & 3);
+#pragma unroll
+                for (int c = 0; c < 2; c++)
+#pragma unroll
+                    for (int h = 0; h < kQN / 32; h++) {
+                        const float m = smax[h][2 * i2 + c];
+                        dst[4 * c + h] = m > -__int_as_float(0x7f800000) ? (uint64_t)orderable_key(1.0f - m) << 32 : kEmptySlot;
+                    }
+            }
+        }
+        if constexpr (kSample && !kFrag) { // keep == 32: the slice minima as composites (the row id is not needed by threshold_kernel)
             if (live) {
                 uint64_t *dst = cand_out + ((size_t)q * gx + bx) * keep;
 #pragma unroll
@@ -1603,6 +1666,14 @@ __global__ void __launch_bounds__(256) to_f16_kernel(const uint8_t *__restrict__
 // ------------------------------------------------------------------------------------------------
 constexpr uint32_t kRefineMaxSurv = 2048;     // survivors rescored per query, k <= kCoarseMaxK
 constexpr uint32_t kRefineMaxSurvWide = 4096; // the same for k > kCoarseMaxK (32 KB)
+constexpr uint32_t kRefineMaxLists = 256;     // lists per query of a counted first tier (one per thread of the scan)
+// threads of refine_kernel: 16 warps share a query's survivors, each rescoring one row at a time, so that more rows are in
+// flight per SM (a row is a few dependent rounds of loads from a random place in the corpus)
+constexpr uint32_t kRefineThreads = 512;
+// candidates refine_kernel packs into shared memory: lists with kEmptySlot padding (the fp16 shadow's 96-entry lists), lists of
+// k > kCoarseMaxK, counted lists (the int8 shadow, DESIGN.md §4.2).  64 KB of packed candidates and the 19.5 KB of static
+// shared memory leave two CTAs per SM: a batch of 256 queries stays resident in one wave on 132 SMs
+constexpr uint32_t kRefineCapPadded = 2560, kRefineCapWide = 8192, kRefineCapCounted = 8192;
 
 // |approx - exact| bound of one query (see above); q_norm2 == NULL: unit vectors.  q_eps (the int8 shadow): the bound of each
 // query, computed with its quantization (quantize_queries_kernel)
@@ -1615,38 +1686,61 @@ __device__ __forceinline__ float query_eps(float eps, const float *q_norm2, uint
     if (l2) e = 2.0f * e + (float)(dim + 4) * 1.2e-7f * (max_norm * max_norm + qn2);
     return e * 1.0001f;
 }
-// k-th smallest key (high word) among the non-empty composites of mine[0, total) — block-wide radix select, 8 bits per
-// pass; 0xFFFFFFFF when there are fewer than k.  256 threads; hist[256] and ctl[4] in shared memory.
-__device__ __forceinline__ uint32_t block_kth_key(const uint64_t *mine, uint32_t total, uint32_t k, uint32_t *hist, uint32_t *ctl) {
+// inclusive prefix sum of v over the threads of the block (warp scans, then the warp totals in wsum[blockDim.x / 32], at most
+// 16); *total = the sum over the block.  Every thread must call it; wsum may be reused after the caller's next __syncthreads()
+__device__ __forceinline__ uint32_t block_incl_scan(uint32_t v, uint32_t *wsum, uint32_t *total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, v, o);
+        if (lane >= o) v += y;
+    }
+    if (lane == 31) wsum[warp] = v;
+    __syncthreads();
+    uint32_t base = 0, all = 0;
+    for (int w = 0; w < nw; w++) {
+        const uint32_t x = wsum[w];
+        if (w < warp) base += x;
+        all += x;
+    }
+    *total = all;
+    return v + base;
+}
+
+// k-th smallest key (high word) among the non-empty composites at(0), ..., at(total - 1) — block-wide radix select, 8 bits per
+// pass; 0xFFFFFFFF when there are fewer than k.  256 to 512 threads; hist[256 + 16] and ctl[4] in shared memory.  The bin of the
+// k-th key in each pass comes from a block-wide scan of the histogram: bin b is the one whose exclusive prefix is below the
+// rank still sought and whose inclusive prefix reaches it (the last bin when none does), as a walk over the bins in order
+// would find it.
+template <class At>
+__device__ __forceinline__ uint32_t block_kth_key(At at, uint32_t total, uint32_t k, uint32_t *hist, uint32_t *ctl) {
     const int lane = threadIdx.x & 31;
     if (threadIdx.x == 0) ctl[0] = 0, ctl[1] = k, ctl[2] = 0;
     __syncthreads();
     uint32_t cnt = 0;
-    for (uint32_t i = threadIdx.x; i < total; i += blockDim.x) cnt += mine[i] != kEmptySlot;
+    for (uint32_t i = threadIdx.x; i < total; i += blockDim.x) cnt += at(i) != kEmptySlot;
     cnt = __reduce_add_sync(0xFFFFFFFFu, cnt);
     if (lane == 0 && cnt) atomicAdd(&ctl[2], cnt);
     __syncthreads();
     if (ctl[2] < k) return 0xFFFFFFFFu;
     for (int shift = 24; shift >= 0; shift -= 8) {
-        hist[threadIdx.x] = 0;
+        if (threadIdx.x < 256) hist[threadIdx.x] = 0;
         __syncthreads();
-        const uint32_t prefix = ctl[0];
+        const uint32_t prefix = ctl[0], rem = ctl[1];
         const uint32_t hi_mask = shift == 24 ? 0u : ~((1u << (shift + 8)) - 1u);
         for (uint32_t i = threadIdx.x; i < total; i += blockDim.x) {
-            const uint64_t c = mine[i];
+            const uint64_t c = at(i);
             if (c == kEmptySlot) continue;
             const uint32_t key = (uint32_t)(c >> 32);
             if (((key ^ prefix) & hi_mask) == 0) atomicAdd(&hist[(key >> shift) & 255u], 1u);
         }
         __syncthreads();
-        if (threadIdx.x == 0) {
-            uint32_t rem = ctl[1], b = 0;
-            for (; b < 255; b++) {
-                if (hist[b] >= rem) break;
-                rem -= hist[b];
-            }
-            ctl[0] = prefix | (b << shift);
-            ctl[1] = rem;
+        const uint32_t h = threadIdx.x < 256 ? hist[threadIdx.x] : 0u; // threads past the bins never hold the k-th
+        uint32_t all;
+        const uint32_t incl = block_incl_scan(h, hist + 256, &all), excl = incl - h;
+        if (excl < rem && (incl >= rem || threadIdx.x == 255)) {
+            ctl[0] = prefix | (threadIdx.x << shift);
+            ctl[1] = rem - excl;
         }
         __syncthreads();
     }
@@ -1661,11 +1755,12 @@ __global__ void __launch_bounds__(256) threshold_kernel(const uint64_t *__restri
                                                         uint32_t keep, uint32_t k, float eps, const float *__restrict__ q_norm2,
                                                         float max_norm, uint32_t dim, int l2, float *__restrict__ thr_out,
                                                         uint32_t *__restrict__ overflow, const float *__restrict__ q_eps) {
-    __shared__ uint32_t hist[256];
+    __shared__ uint32_t hist[256 + 16];
     __shared__ uint32_t ctl[4];
     const uint32_t q = blockIdx.x;
     if (q >= nq) return;
-    const uint32_t ak = block_kth_key(cand + (size_t)q * lists_per_query * keep, lists_per_query * keep, k, hist, ctl);
+    const uint64_t *mine = cand + (size_t)q * lists_per_query * keep;
+    const uint32_t ak = block_kth_key([&](uint32_t i) { return mine[i]; }, lists_per_query * keep, k, hist, ctl);
     if (threadIdx.x == 0) {
         const float e = query_eps(eps, q_norm2, q, max_norm, dim, l2 != 0, q_eps);
         float T;
@@ -1686,22 +1781,25 @@ __global__ void __launch_bounds__(256) threshold_kernel(const uint64_t *__restri
 // kLab (hybrid batches, DESIGN.md §4.10): the exact composites carry the row's label row_label[row] instead of the row, so the
 //      answer is the k smallest (distance, docId) — the order of the ragged gather over an ascending filter
 template <int MT, uint32_t kSurv, bool kLab = false>
-__global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t pitch, uint32_t dim, const uint8_t *queries,
+__global__ void __launch_bounds__(kRefineThreads) refine_kernel(const uint8_t *rows, size_t pitch, uint32_t dim, const uint8_t *queries,
                                                      size_t qpitch, uint32_t nq, uint32_t lists_per_query, uint32_t keep, uint32_t k,
                                                      const uint64_t *__restrict__ cand, float eps, const float *__restrict__ q_norm2,
                                                      float max_norm, uint32_t *__restrict__ ok, uint32_t ok_value, uint64_t *__restrict__ out,
                                                      const uint32_t *__restrict__ q_index, const uint32_t *__restrict__ nq_dev,
                                                      const float *__restrict__ thr_T, const uint32_t *__restrict__ overflow,
-                                                     uint32_t smem_cap, const uint64_t *__restrict__ row_label, const float *__restrict__ q_eps) {
+                                                     uint32_t smem_cap, const uint64_t *__restrict__ row_label, const float *__restrict__ q_eps,
+                                                     const uint32_t *__restrict__ list_count) {
     using Tile = DistTile<DT_F32, MT, 1, 1>;
     __shared__ uint64_t surv[kSurv];
-    __shared__ uint32_t hist[256];
+    __shared__ uint32_t hist[256 + 16];
     __shared__ uint32_t ctl[4];
     __shared__ uint32_t s_nsurv, s_bad, s_ncomp;
+    __shared__ uint32_t s_off[kRefineMaxLists], s_cnt[kRefineMaxLists]; // list_count: offset and entries of each list
     if (nq_dev) nq = min(nq, *nq_dev);
     if (blockIdx.x >= nq) return;
     const uint32_t q = q_index ? q_index[blockIdx.x] : blockIdx.x; // query of the original batch
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    constexpr uint32_t kWarps = kRefineThreads / 32;
     const uint64_t *mine = cand + (size_t)blockIdx.x * lists_per_query * keep;
     uint32_t total = lists_per_query * keep;
     eps = query_eps(eps, q_norm2, blockIdx.x, max_norm, dim, MT == MT_L2, q_eps);
@@ -1710,33 +1808,55 @@ __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t
     // the lists are mostly empty slots (fixed-bound pass: ~15 of 96 per list): pack the real candidates into shared memory
     // once, so that the selection passes below do not re-read 57 KB of global memory five times per query
     extern __shared__ uint64_t s_cand[];
-    for (uint32_t i0 = 0; i0 < total; i0 += blockDim.x) {
-        const uint32_t i = i0 + threadIdx.x;
-        const uint64_t c = i < total ? mine[i] : kEmptySlot;
-        const uint32_t m = __ballot_sync(0xFFFFFFFFu, c != kEmptySlot);
-        uint32_t base = 0;
-        if (lane == 0 && m) base = atomicAdd(&s_ncomp, (uint32_t)__popc(m));
-        base = __shfl_sync(0xFFFFFFFFu, base, 0);
-        if (c != kEmptySlot) {
-            const uint32_t pos = base + __popc(m & ((1u << lane) - 1u));
-            if (pos < smem_cap) s_cand[pos] = c;
+    if (list_count) {
+        // counted lists (the int8 shadow's fixed pass): list l holds s_cnt[l] entries from its slot 0 and nothing after them.
+        // Their offsets in the packed buffer are an exclusive scan of the counts; each warp then copies whole lists, so the
+        // reads are coalesced and touch only the entries
+        const uint32_t cl = threadIdx.x < lists_per_query ? min(list_count[(size_t)blockIdx.x * lists_per_query + threadIdx.x], keep) : 0u;
+        uint32_t n_live;
+        const uint32_t incl = block_incl_scan(cl, hist + 256, &n_live);
+        if (threadIdx.x < lists_per_query) s_off[threadIdx.x] = incl - cl, s_cnt[threadIdx.x] = cl;
+        if (threadIdx.x == 0) s_ncomp = n_live;
+        __syncthreads();
+        if (n_live <= smem_cap) {
+            for (uint32_t l = warp; l < lists_per_query; l += kWarps) {
+                const uint64_t *src = mine + (size_t)l * keep;
+                uint64_t *dst = s_cand + s_off[l];
+                for (uint32_t j = lane; j < s_cnt[l]; j += 32) dst[j] = src[j];
+            }
+        }
+    } else {
+        for (uint32_t i0 = 0; i0 < total; i0 += blockDim.x) {
+            const uint32_t i = i0 + threadIdx.x;
+            const uint64_t c = i < total ? mine[i] : kEmptySlot;
+            const uint32_t m = __ballot_sync(0xFFFFFFFFu, c != kEmptySlot);
+            uint32_t base = 0;
+            if (lane == 0 && m) base = atomicAdd(&s_ncomp, (uint32_t)__popc(m));
+            base = __shfl_sync(0xFFFFFFFFu, base, 0);
+            if (c != kEmptySlot) {
+                const uint32_t pos = base + __popc(m & ((1u << lane) - 1u));
+                if (pos < smem_cap) s_cand[pos] = c;
+            }
         }
     }
     __syncthreads();
     const bool packed = s_ncomp <= smem_cap;
     const uint64_t *mine_all = mine; // the proof of the adaptive tier walks the lists as published
-    const uint32_t total_all = total;
-    if (packed) {
-        mine = s_cand;
-        total = s_ncomp;
-    }
+    if (packed) total = s_ncomp;
+    // candidate i: packed, from shared memory; else from the lists in global memory, where a counted list's slots past its
+    // entries are empty
+    auto at = [&](uint32_t i) -> uint64_t {
+        if (packed) return s_cand[i];
+        if (list_count) return i % keep < s_cnt[i / keep] ? mine[i] : kEmptySlot;
+        return mine[i];
+    };
     // a_k: k-th smallest approximate key; fewer than k candidates: everything survives
-    const uint32_t ak_key = block_kth_key(mine, total, k, hist, ctl);
+    const uint32_t ak_key = block_kth_key(at, total, k, hist, ctl);
     // survivors: approx <= a_k + 2 eps (rounded up)
     const float cut = ak_key == 0xFFFFFFFFu ? __int_as_float(0x7f800000) : key_to_float(ak_key) + (2.0f * eps) * 1.001f + 1e-30f;
     for (uint32_t i0 = 0; i0 < total; i0 += blockDim.x) {
         const uint32_t i = i0 + threadIdx.x;
-        const uint64_t c = i < total ? mine[i] : kEmptySlot;
+        const uint64_t c = i < total ? at(i) : kEmptySlot;
         const bool take = c != kEmptySlot && (ak_key == 0xFFFFFFFFu || key_to_float((uint32_t)(c >> 32)) <= cut);
         const uint32_t m = __ballot_sync(0xFFFFFFFFu, take);
         uint32_t base = 0;
@@ -1749,9 +1869,21 @@ __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t
     }
     __syncthreads();
     const uint32_t n_all = s_nsurv, n_surv = min(n_all, kSurv);
+    // Every survivor row is requested at once, one word of each of its 128-byte lines, spread over the block's threads: the
+    // rescoring below takes one row per warp and waits on a few rounds of loads per row, each a random row of the corpus (an
+    // address translation and an HBM round trip), and these loads have them in flight, or in L2, by then.  The words are only
+    // folded into `touch`, which the thread consumes at the very end, so nothing waits for them here
+    uint32_t touch = 0;
+    {
+        const uint32_t row_bytes = dim * (uint32_t)sizeof(float), lines = (row_bytes + 127) / 128;
+        for (uint32_t t = threadIdx.x; t < n_surv * lines; t += blockDim.x) {
+            const uint8_t *r = rows + (size_t)(uint32_t)surv[t / lines] * pitch;
+            touch ^= __ldcg(reinterpret_cast<const uint32_t *>(r + (t % lines) * 128));
+        }
+    }
     // exact distances of the survivors (one warp per row)
     const uint8_t *qb[1] = {queries + (size_t)q * qpitch};
-    for (uint32_t i = warp; i < n_surv; i += 8) {
+    for (uint32_t i = warp; i < n_surv; i += kWarps) {
         const uint32_t row = (uint32_t)surv[i];
         const uint8_t *rowb[1] = {rows + (size_t)row * pitch};
         float d[1];
@@ -1776,7 +1908,6 @@ __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t
     if (thr_T) {
         if (threadIdx.x == 0 && (overflow[blockIdx.x] != 0 || !have_k || !(thr_T[blockIdx.x] - eps > ek))) bad = true;
     } else {
-        (void)total_all;
         for (uint32_t l = threadIdx.x; l < lists_per_query; l += blockDim.x) {
             const uint64_t *lst = mine_all + (size_t)l * keep;
             uint32_t worst = 0;
@@ -1798,6 +1929,7 @@ __global__ void __launch_bounds__(256) refine_kernel(const uint8_t *rows, size_t
     if (bad) atomicOr(&s_bad, 1u);
     __syncthreads();
     if (threadIdx.x == 0) ok[q] = s_bad ? 0u : ok_value; // 1 = first tier, 2 = second tier (any non-zero = proven)
+    asm volatile("" ::"r"(touch));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2175,17 +2307,17 @@ static const void *wgmma_kernel_fn(CoarseKind kind, uint32_t epl, int epi, int m
     return epl == 3 ? (const void *)coarse_wgmma_kernel<false, 3, 0, 0> : (const void *)coarse_wgmma_kernel<false, 8, 0, 0>;
 }
 // shared memory of coarse_wgmma_kernel besides the ring: the resident queries (cta_q per CTA, less the reg_kb K blocks held in
-// registers), the accumulator transpose (the fixed-bound pass, mode 1, tests the accumulators in registers and keeps a counter
-// per query instead), the barriers
-static size_t wgmma_fixed_smem(uint32_t num_kb, int mode = 0, uint32_t reg_kb = 0, uint32_t cta_q = kQM) {
-    return 1024 + (size_t)(num_kb - reg_kb) * cta_q * 128 + (mode == 1 ? cta_q * 4 : kQAccBytes) + 2 * kQMaxStages * 8 + 64;
+// registers), the accumulator transpose (frag: the passes of coarse_frag_epilogue work on the accumulators in registers and
+// keep a counter per query instead), the barriers
+static size_t wgmma_fixed_smem(uint32_t num_kb, bool frag = false, uint32_t reg_kb = 0, uint32_t cta_q = kQM) {
+    return 1024 + (size_t)(num_kb - reg_kb) * cta_q * 128 + (frag ? cta_q * 4 : kQAccBytes) + 2 * kQMaxStages * 8 + 64;
 }
-static uint32_t wgmma_stages(uint32_t num_kb, int mode, uint32_t reg_kb, uint32_t cta_q = kQM) {
-    return (uint32_t)std::min<size_t>(kQMaxStages, (kSmemLimit - wgmma_fixed_smem(num_kb, mode, reg_kb, cta_q)) / kQStageBytes);
+static uint32_t wgmma_stages(uint32_t num_kb, bool frag, uint32_t reg_kb, uint32_t cta_q = kQM) {
+    return (uint32_t)std::min<size_t>(kQMaxStages, (kSmemLimit - wgmma_fixed_smem(num_kb, frag, reg_kb, cta_q)) / kQStageBytes);
 }
 // the 16/8-bit kernel needs at least two ring stages next to the resident queries (1024 fp16 dimensions fit)
 static bool wgmma_fits_bytes(uint32_t row_bytes, uint32_t cta_q = kQM) {
-    return wgmma_fixed_smem(coarse_kb(row_bytes), 0, 0, cta_q) + 2 * (size_t)kQStageBytes <= kSmemLimit;
+    return wgmma_fixed_smem(coarse_kb(row_bytes), false, 0, cta_q) + 2 * (size_t)kQStageBytes <= kSmemLimit;
 }
 static bool wgmma_fits(uint32_t dim) { return wgmma_fits_bytes(dim * 2); }
 
@@ -2252,7 +2384,8 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
         if (p.mode == 1 && (kind == CoarseDirect16 || kind == CoarseDirect8)) p.keep = kCoarseFixedCapDirect, p.epl = 8;
         if (p.mode == 1 && kind == CoarseQ8) p.keep = kCoarseFixedCapQ8, p.epl = 8;
         if (p.mode == 2) p.keep = kCoarseSampleSlices, p.epl = 3; // the slice minima
-        p.threads = (uint32_t)coarse_threads(p.mode);
+        p.threads = (uint32_t)coarse_threads(kind == CoarseQ8, p.mode);
+        const bool frag = coarse_frag_epilogue(kind == CoarseQ8, p.mode);
         const int epi = kind == CoarseQ8 ? 0 : kind == CoarseF16 ? (c.metric == MT_L2 ? 1 : 0) : c.metric == MT_COS ? 1 : (kind == CoarseDirect8 && c.metric == MT_L2) ? 2 : 0;
         // the fixed-bound pass over the shadow holds the leading K blocks of its queries in registers where that frees shared
         // memory for one more ring stage and leaves at least one stage of queries in shared memory
@@ -2264,11 +2397,11 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
         p.reg_kb = 0;
         if (kind == CoarseF16 && p.mode == 1) {
             const uint32_t rk = fixed_reg_kb(p.epl, epi != 0, filt);
-            if (rk && (int)rk <= rcap && p.num_kb >= rk + kQKbPerStage && wgmma_stages(p.num_kb, p.mode, rk) > wgmma_stages(p.num_kb, p.mode, 0))
+            if (rk && (int)rk <= rcap && p.num_kb >= rk + kQKbPerStage && wgmma_stages(p.num_kb, frag, rk) > wgmma_stages(p.num_kb, frag, 0))
                 p.reg_kb = rk;
         }
-        p.stages = wgmma_stages(p.num_kb, p.mode, p.reg_kb, cta_q);
-        p.smem_bytes = wgmma_fixed_smem(p.num_kb, p.mode, p.reg_kb, cta_q) + (size_t)p.stages * kQStageBytes;
+        p.stages = wgmma_stages(p.num_kb, frag, p.reg_kb, cta_q);
+        p.smem_bytes = wgmma_fixed_smem(p.num_kb, frag, p.reg_kb, cta_q) + (size_t)p.stages * kQStageBytes;
         // the query groups of a row range form a thread-block cluster (multicast of the row tiles).  128 queries per CTA: pairs at
         // most, which can fill all 132 SMs where clusters of four leave 12 idle (DESIGN.md §4.2)
         p.csize = 1;
@@ -2338,10 +2471,11 @@ static cudaError_t launch_coarse_t(const void *rows, size_t pitch, uint32_t n_ro
 
 cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim, uint32_t nq, const CoarsePlan &p, uint64_t *d_cand,
                           uint64_t *d_scratch, cudaStream_t s, const uint32_t *d_nq_dev, const float *d_thr_fixed, uint32_t *d_overflow,
-                          const uint32_t *d_filt, uint32_t filt_words, const uint32_t *d_filt_q) {
+                          const uint32_t *d_filt, uint32_t filt_words, const uint32_t *d_filt_q, uint32_t *d_list_count) {
     if (d_filt && p.kind != CoarseF16 && !(p.kind == CoarseDirect8 && p.mode == 1)) return cudaErrorInvalidValue;
     if (p.kind == CoarseF16 || p.kind == CoarseQ8 || p.kind == CoarseDirect16 || p.kind == CoarseDirect8) {
         if (p.mode == 1 && (!d_thr_fixed || !d_overflow)) return cudaErrorInvalidValue;
+        if (p.mode == 1 && p.kind == CoarseQ8 && !d_list_count) return cudaErrorInvalidValue; // its lists are not padded
         // operand variant: 16-bit 1 = bf16 (else fp16); 8-bit 1 = int8 (else uint8); the fp16 shadow of the fp32 route: 0
         const uint32_t ev = (p.kind == CoarseDirect16 || p.kind == CoarseDirect8) && o.elem_variant ? 1u : 0u;
         const void *kfn = wgmma_kernel_fn(p.kind, p.epl, o.epilogue, p.mode, ev, d_filt != nullptr, p.reg_kb);
@@ -2379,7 +2513,7 @@ cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim
                  a_st = p.stages, a_cs = p.csize, a_stride = p.tile_stride;
         void *args[] = {&mr,   &rows,    &rp,     &qs,   &qp,   &rn2,  &qn2,      &a_nrows, &a_nq,     &a_dim,       &a_rb, &a_kb,
                         &a_tiles, &a_keep, &a_st, &a_cs, &d_scratch, &d_cand, &d_nq_dev, &a_stride, &d_thr_fixed, &d_overflow,
-                        &d_filt, &filt_words, &d_filt_q};
+                        &d_filt, &filt_words, &d_filt_q, &d_list_count};
         const cudaError_t le = cudaLaunchKernelExC(&cfg, kfn, args);
         if (le != cudaSuccess)
             fprintf(stderr, "vecsim_b200: coarse pass launch failed (kind %d mode %d csize %u grid %u x %u smem %zu): %s\n", (int)p.kind,
@@ -2687,15 +2821,16 @@ cudaError_t launch_to_f16(const void *src, size_t spitch, uint32_t dim, uint32_t
 cudaError_t launch_refine(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t lists_per_query, uint32_t keep,
                           uint32_t k, const uint64_t *d_cand, float eps, const float *d_q_norm2, float max_norm, uint32_t *d_ok,
                           uint64_t *d_out, const uint32_t *d_q_index, const uint32_t *d_nq_dev, cudaStream_t s, const float *d_thr_T,
-                          const uint32_t *d_overflow, const uint64_t *d_row_label, const float *d_q_eps) {
+                          const uint32_t *d_overflow, const uint64_t *d_row_label, const float *d_q_eps, const uint32_t *d_list_count) {
     if (nq == 0) return cudaSuccess;
     const uint32_t okv = d_q_index ? 2u : 1u;
     const uint8_t *rows = static_cast<const uint8_t *>(c.rows), *qs = static_cast<const uint8_t *>(d_queries);
     // candidates packed in shared memory: as many slots as the lists have, up to 20 KB worth (k > kCoarseMaxK: 64 KB, two CTAs
-    // per SM next to the 32 KB survivor buffer)
+    // per SM next to the 32 KB survivor buffer; counted lists: 64 KB)
     const bool wide = k > kCoarseMaxK;
     if (k > kCoarseMaxKWide) return cudaErrorInvalidValue;
-    const uint32_t max_cap = wide ? 8192 : 2560;
+    if (d_list_count && (!d_thr_T || lists_per_query > kRefineMaxLists)) return cudaErrorInvalidValue;
+    const uint32_t max_cap = wide ? kRefineCapWide : d_list_count ? kRefineCapCounted : kRefineCapPadded;
     const uint32_t smem_cap = std::min<uint32_t>(lists_per_query * keep, max_cap);
     const size_t smem = (size_t)smem_cap * 8;
     const auto kern = d_row_label ? (c.metric == MT_L2 ? (wide ? refine_kernel<MT_L2, kRefineMaxSurvWide, true> : refine_kernel<MT_L2, kRefineMaxSurv, true>)
@@ -2703,17 +2838,18 @@ cudaError_t launch_refine(const CorpusView &c, const void *d_queries, size_t qpi
                     : c.metric == MT_L2 ? (wide ? refine_kernel<MT_L2, kRefineMaxSurvWide> : refine_kernel<MT_L2, kRefineMaxSurv>)
                                         : (wide ? refine_kernel<MT_IP, kRefineMaxSurvWide> : refine_kernel<MT_IP, kRefineMaxSurv>);
     // the 48 KB a launch gets without opting in cover static + dynamic shared memory (the wide survivor buffer alone is 32 KB).
-    // Opt in to the largest packing this instantiation can ask for, the same value every time: concurrent launches of the same
-    // kernel from other host threads never see the limit lowered under them
+    // Opt in to the largest packing any launch of an instantiation can ask for, the same value every time: concurrent launches
+    // of the same kernel from other host threads never see the limit lowered under them
+    constexpr uint32_t kOptIn = std::max(kRefineCapWide, kRefineCapCounted) * 8;
     cudaFuncAttributes fa{};
     cudaError_t e = cudaFuncGetAttributes(&fa, kern);
     if (e != cudaSuccess) return e;
-    if (fa.sharedSizeBytes + (size_t)max_cap * 8 > 48 * 1024) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(max_cap * 8));
+    if (fa.sharedSizeBytes + smem > 48 * 1024 && fa.maxDynamicSharedSizeBytes < (int)kOptIn) {
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kOptIn);
         if (e != cudaSuccess) return e;
     }
-    kern<<<nq, 256, smem, s>>>(rows, c.pitch, c.dim, qs, qpitch, nq, lists_per_query, keep, k, d_cand, eps, d_q_norm2, max_norm, d_ok, okv,
-                               d_out, d_q_index, d_nq_dev, d_thr_T, d_overflow, smem_cap, d_row_label, d_q_eps);
+    kern<<<nq, kRefineThreads, smem, s>>>(rows, c.pitch, c.dim, qs, qpitch, nq, lists_per_query, keep, k, d_cand, eps, d_q_norm2, max_norm, d_ok, okv,
+                               d_out, d_q_index, d_nq_dev, d_thr_T, d_overflow, smem_cap, d_row_label, d_q_eps, d_list_count);
     return cudaGetLastError();
 }
 

@@ -64,11 +64,12 @@ CoarsePlan plan_coarse(const CorpusView &c, uint32_t nq, CoarseKind kind, uint32
 // d_nq_dev (nullable): the number of live queries is read from device memory (min with nq); 0 = the kernel exits at once.
 // d_filt (nullable; CoarseF16, and CoarseDirect8 of mode 1): row filters of a hybrid batch, one bitmap of filt_words u32 per query
 // (bit r = row r); query i of the pass uses bitmap d_filt_q[i] (d_filt_q NULL: bitmap i).  Only filtered rows enter the lists and
-// the sample minima
+// the sample minima.  d_list_count (nullable; mode 1): [nq][grid_x], the entries of each published list.  Required by the fixed
+// pass over the int8 shadow (CoarseQ8, mode 1), whose lists carry those entries only, with no kEmptySlot padding
 cudaError_t launch_coarse(const CoarseOperands &o, uint32_t n_rows, uint32_t dim, uint32_t nq, const CoarsePlan &p, uint64_t *d_cand,
                           uint64_t *d_scratch, cudaStream_t s, const uint32_t *d_nq_dev = nullptr, const float *d_thr_fixed = nullptr,
                           uint32_t *d_overflow = nullptr, const uint32_t *d_filt = nullptr, uint32_t filt_words = 0,
-                          const uint32_t *d_filt_q = nullptr);
+                          const uint32_t *d_filt_q = nullptr, uint32_t *d_list_count = nullptr);
 // bound of the fixed pass from the sample pass's candidate lists: d_thr[q] = k-th smallest approximate distance + 2 eps;
 // clears d_overflow[q].  d_q_eps (nullable; the int8 shadow): eps of each query, in place of eps / d_q_norm2
 cudaError_t launch_threshold(const uint64_t *d_cand, uint32_t nq, uint32_t lists_per_query, uint32_t keep, uint32_t k, float eps,
@@ -101,11 +102,13 @@ cudaError_t launch_to_f16(const void *src, size_t spitch, uint32_t dim, uint32_t
 // d_q_index[i] = query of the original batch whose lists sit at position i (d_q_norm2 is indexed by position), *d_nq_dev
 // live positions.  d_row_label (nullable): the answer's composites carry row_label[row] (a docId) in place of the row, and ties
 // resolve by it.  d_q_eps (nullable; the int8 shadow): the bound of each query by position, in place of eps / d_q_norm2.
+// d_list_count (nullable; with d_thr_T): [nq][lists_per_query] entries of each list (launch_coarse's d_list_count), which
+// are read instead of the kEmptySlot padding.
 cudaError_t launch_refine(const CorpusView &c, const void *d_queries, size_t qpitch, uint32_t nq, uint32_t lists_per_query, uint32_t keep,
                           uint32_t k, const uint64_t *d_cand, float eps, const float *d_q_norm2, float max_norm, uint32_t *d_ok,
                           uint64_t *d_out, const uint32_t *d_q_index, const uint32_t *d_nq_dev, cudaStream_t s,
                           const float *d_thr_T = nullptr, const uint32_t *d_overflow = nullptr, const uint64_t *d_row_label = nullptr,
-                          const float *d_q_eps = nullptr);
+                          const float *d_q_eps = nullptr, const uint32_t *d_list_count = nullptr);
 // direct 16-bit route: d_ok[q] = d_overflow[q] ? 0 : 1
 cudaError_t launch_flags_from_overflow(const uint32_t *d_overflow, uint32_t nq, uint32_t *d_ok, cudaStream_t s);
 // second tier of the direct route: row i of src ([.][k] composites) -> row d_idx[i] of dst, d_ok[d_idx[i]] = 2, for i < *d_count

@@ -1054,6 +1054,8 @@ void FlatIndex::KnnScratch::take(BatchScratch &s, const KnnTiers &t, uint32_t nq
     n2 = s.take<uint32_t>(nq ? 1 : 0);  //         and their count
     thr = s.take<float>(nq);            // fixed bound per query
     ovf = s.take<uint32_t>(nq);         // a list of the main pass ran full
+    // entries of each list of the int8 copy's fixed pass, which publishes no padding
+    cnt = s.take<uint32_t>(q8 && t.two_pass ? (size_t)nq * t.main.grid_x : 0);
 }
 
 bool FlatIndex::enqueue_knn_tiers(QueryCtx &c, const CorpusView &v, CoarseKind kind, const KnnTiers &t, const KnnScratch &s,
@@ -1070,11 +1072,12 @@ bool FlatIndex::enqueue_knn_tiers(QueryCtx &c, const CorpusView &v, CoarseKind k
     const float *thr = t.two_pass ? s.thr : nullptr;
     uint32_t *ovf = t.two_pass ? s.ovf : nullptr;
     cudaEventRecord(c.ev_start, st);
-    ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq, t.main, s.cand, s.list_scratch, st, nullptr, thr, ovf, bm, words) == cudaSuccess;
+    ok = ok && launch_coarse(ops, v.n_rows, v.dim, nq, t.main, s.cand, s.list_scratch, st, nullptr, thr, ovf, bm, words, nullptr, s.cnt) ==
+                   cudaSuccess;
     cudaEventRecord(c.ev_stop, st);
     // exact rescoring of the few candidates that can still matter + exact top-k + proof, one CTA per query
     ok = ok && launch_refine(v, d_q32, qpitch, nq, t.main.grid_x, t.main.keep, ke, s.cand, eps, s.qn2, shadow_max_norm_, s.ok, out, nullptr,
-                             nullptr, st, thr, ovf, row_label, s.qeps) == cudaSuccess;
+                             nullptr, st, thr, ovf, row_label, s.qeps, s.cnt) == cudaSuccess;
     lc.launches += 2;
     if (!t.tier2) return ok;
     ok = ok && launch_compact_unproven(s.ok, nq, s.idx, s.n2, st) == cudaSuccess;

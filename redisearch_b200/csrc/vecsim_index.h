@@ -287,6 +287,7 @@ class FlatIndex {
         uint8_t *q = nullptr, *q_t2 = nullptr; // the queries in the operand type of the copy, and tier 2's open ones
         float *qn2 = nullptr, *qn2_t2 = nullptr, *qeps = nullptr, *qeps_t2 = nullptr, *thr = nullptr;
         uint32_t *ok = nullptr, *idx = nullptr, *n2 = nullptr, *ovf = nullptr;
+        uint32_t *cnt = nullptr; // [nq][main.grid_x] entries per list of the int8 copy's fixed pass (NULL on the other routes)
         // q_pitch: bytes per operand query row; norms: |q|^2 per query (rows not all unit); q8: the int8 copy's eps per query
         void take(BatchScratch &s, const KnnTiers &t, uint32_t nq, size_t q_pitch, bool norms, bool q8);
     };
